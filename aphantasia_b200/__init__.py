@@ -1,4 +1,4 @@
-"""aphantasia_b200 -- B200-native (sm_100a) hot path of eps696/aphantasia behind the reference's own
+"""aphantasia_b200 -- H100-native (sm_90a) hot path of eps696/aphantasia behind the reference's own
 Python entry points (fft_image, dwt_image, to_valid_rgb, slice_imgs, sim_func, clip model.encode_image).
 
 The package is host glue only: torch owns device memory / streams / autograd plumbing, all arithmetic of

@@ -2,7 +2,7 @@
 `clip.load(name, jit=False) -> (model, preprocess)`, `clip.tokenize`, `model.encode_image`, `model.encode_text`,
 `model.visual.input_resolution`.
 
-The image encoder (ViT-B/32, ViT-B/16) runs forward and data-gradient in libaphb200.so (csrc/vit.cu: tcgen05
+The image encoder (ViT-B/32, ViT-B/16) runs forward and data-gradient in libaphb200.so (csrc/vit.cu: wgmma
 GEMMs + fused kernels). Weights: an OpenAI state dict if `APH_CLIP_WEIGHTS=<file.pt>` is set, else seeded
 synthetic weights of the same architecture (there are no CLIP weights or network in this environment).
 The text encoder runs once before the optimisation loop and is not part of the hot path: without real weights
@@ -201,7 +201,7 @@ def tokenize(texts, context_length=77, truncate=False):
 def load(name, device=None, jit=False, download_root=None):
     """clip.load: returns (model, preprocess). `preprocess` is unused by the scripts (None)."""
     if name not in _MODELS:
-        raise RuntimeError('aphantasia_b200.clip: model %s not available (B200 hot path covers %s)' % (name, available_models()))
+        raise RuntimeError('aphantasia_b200.clip: model %s not available (the CUDA hot path covers %s)' % (name, available_models()))
     path = os.environ.get('APH_CLIP_WEIGHTS_' + name.replace('/', '').replace('-', '').upper(), os.environ.get('APH_CLIP_WEIGHTS'))
     if path and os.path.isfile(path):
         sd = torch.load(path, map_location='cpu')

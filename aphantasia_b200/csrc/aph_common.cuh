@@ -1,4 +1,4 @@
-// aph_common.cuh -- shared helpers for libaphb200.so (sm_100a only).
+// aph_common.cuh -- shared helpers for libaphb200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -41,11 +41,23 @@ inline void count_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_
     aph::count_launch();                                                                        \
   } while (0)
 
-constexpr int kNumSMs = 148;   // B200
+// SMs of the current device, queried once per device: sizes the persistent grids and the grid-stride launches
+// (132 on an H100 SXM, 114 on an H100 PCIe). A failed query only affects grid sizes, never results: it falls back to 132.
+inline int num_sms() {
+  static std::atomic<int> cache[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  int n = cache[dev].load(std::memory_order_relaxed);
+  if (n <= 0) {
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
+    cache[dev].store(n, std::memory_order_relaxed);
+  }
+  return n;
+}
 
 // Programmatic dependent launch: a kernel calls pdl_trigger() first thing (its dependents may start being scheduled as SMs
 // drain) and pdl_wait() before its first global-memory access (blocks until the preceding grid has completed and flushed).
-// The prologue in between (barrier init, TMEM allocation, descriptor prefetch, index setup) overlaps the predecessor's tail.
+// The prologue in between (barrier init, descriptor prefetch, index setup) overlaps the predecessor's tail.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 

@@ -199,7 +199,7 @@ k_sample_fwd(const float* __restrict__ canvas, int H, int W, int pad_top, int pa
   const TapTables tt = build_taps(A + ((n + 3) & ~3), p, size, H, W, pad_top, pad_left, scale);
   __syncthreads();
   // ---- stage 1: bicubic resize into shared memory (warp = output row), direct 16-tap form through the per-CTA tap tables.
-  // (A vertical-first per-warp strip variant was measured SLOWER here, 0.68 vs 0.51 ms, profiles/r1g: two extra warp barriers
+  // (A vertical-first per-warp strip variant was slower here: two extra warp barriers
   // and a dependent shared-memory round trip per chunk outweigh the saved L1 wavefronts; the backward keeps its strip.)
   for (int i = warp; i < size; i += nwarps) {
     const int4 yo = *reinterpret_cast<const int4*>(tt.yo + 4 * i);
@@ -1142,8 +1142,8 @@ static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int
                            int size, int kind, float* grad_canvas, float gscale, void* stream) {
   if (int e = check_sample_args("aph_sample_bwd", H, W, S, size, kind)) return e;
   APH_REQUIRE(grad_canvas, "aph_sample_bwd: null grad_canvas");
-  // Measured on B200 (profiles/r1e): the atomic scatter (0.99 ms @ C2) beats this gather (1.85 ms: per-(tile, crop) list
-  // building + 3 barriers dominate), so the gather is opt-in: APH_SAMPLE_BWD_GATHER=1 gives a bit-reproducible gradient.
+  // The atomic scatter is faster than this gather (per-(tile, crop) list building + 3 barriers dominate the gather),
+  // so the gather is opt-in: APH_SAMPLE_BWD_GATHER=1 gives a bit-reproducible gradient.
   static int force_scatter = -1;
   if (force_scatter < 0) { const char* e = getenv("APH_SAMPLE_BWD_GATHER"); force_scatter = (e && e[0] == '1') ? 0 : 1; }
   // (crops never upsample by more than 1/0.9 when min(H, W) >= size, which bounds the adjoint tap lists of the gather kernel)
@@ -1243,7 +1243,7 @@ static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int
   if (fixed) {
     k_sample_bwd<<<S * 3, 1024, smem, (cudaStream_t)stream>>>(grad_out, H, W, pad_top, pad_left, table, size, kind, grad_canvas);
     APH_LAUNCH_OK();
-    if (gscale != 1.f) { k_scale_inplace<<<kNumSMs * 4, 256, 0, (cudaStream_t)stream>>>(grad_canvas, (size_t)3 * H * W, gscale); APH_LAUNCH_OK(); }
+    if (gscale != 1.f) { k_scale_inplace<<<num_sms() * 4, 256, 0, (cudaStream_t)stream>>>(grad_canvas, (size_t)3 * H * W, gscale); APH_LAUNCH_OK(); }
     return 0;
   }
   k_sample_bwd_cas<<<S * 3, 1024, smem, (cudaStream_t)stream>>>(grad_out, H, W, pad_top, pad_left, table, size, kind, grad_canvas, gscale);

@@ -138,7 +138,7 @@ __global__ void __launch_bounds__(256) k_stats(const float* __restrict__ x, size
 }
 __global__ void k_fix_stats(double* stats, double n, double sigma) { stats[0] = 0.; stats[1] = sigma * sigma * (n - 1.0); stats[2] = 0.; }
 
-static inline int grid_for(size_t n) { return (int)std::min<size_t>((n + 255) / 256, (size_t)kNumSMs * 16); }
+static inline int grid_for(size_t n) { return (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16); }
 
 }  // namespace aph
 

@@ -459,7 +459,7 @@ extern "C" int aph_synth_fft_fwd(aph_fft_plan* plan, const float* params, const 
   k_row_c2r<<<3 * groups, 256, p->smem_row, st>>>(p->T, x_raw, stats, p->twW, H, W, Wh, p->rowP, norm, p->rw);
   APH_LAUNCH_OK();
   const size_t hw = (size_t)H * W;
-  const int blocks = (int)std::min<size_t>((hw + 255) / 256, (size_t)kNumSMs * 8);
+  const int blocks = (int)std::min<size_t>((hw + 255) / 256, (size_t)num_sms() * 8);
   k_finish<<<blocks, 256, 0, st>>>(x_raw, stats, out, hw, contrast, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
   return 0;
@@ -475,7 +475,7 @@ static int synth_fft_bwd_impl(aph_fft_plan* plan, const float* grad_out, const f
   const int H = p->H, W = p->W, Wh = p->Wh;
   const size_t hw = (size_t)H * W;
   APH_CUDA_OK(cudaMemsetAsync(stats + 2, 0, sizeof(double), st));
-  const int blocks = (int)std::min<size_t>((hw + 255) / 256, (size_t)kNumSMs * 8);
+  const int blocks = (int)std::min<size_t>((hw + 255) / 256, (size_t)num_sms() * 8);
   k_finish_bwd<<<blocks, 256, 0, st>>>(grad_out, out, x_raw, p->gimg, stats, hw, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
   const int groups = ((H + 1) / 2 + p->rowP - 1) / p->rowP;
@@ -526,7 +526,7 @@ __global__ void __launch_bounds__(256) k_rgb_fwd(const float* __restrict__ img, 
 
 extern "C" int aph_valid_rgb_fwd(const float* img, int64_t hw, const float* colmat_host, float* out, void* stream) {
   APH_REQUIRE(img && out && hw > 0, "aph_valid_rgb_fwd: bad arguments");
-  const int blocks = (int)std::min<size_t>(((size_t)hw + 255) / 256, (size_t)kNumSMs * 8);
+  const int blocks = (int)std::min<size_t>(((size_t)hw + 255) / 256, (size_t)num_sms() * 8);
   k_rgb_fwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(img, out, (size_t)hw, make_colmat(colmat_host));
   APH_LAUNCH_OK();
   return 0;
@@ -535,7 +535,7 @@ extern "C" int aph_valid_rgb_fwd(const float* img, int64_t hw, const float* colm
 extern "C" int aph_valid_rgb_bwd(const float* grad_out, const float* out, int64_t hw, const float* colmat_host,
                                  float* grad_img, void* stream) {
   APH_REQUIRE(grad_out && out && grad_img && hw > 0, "aph_valid_rgb_bwd: bad arguments");
-  const int blocks = (int)std::min<size_t>(((size_t)hw + 255) / 256, (size_t)kNumSMs * 8);
+  const int blocks = (int)std::min<size_t>(((size_t)hw + 255) / 256, (size_t)num_sms() * 8);
   k_finish_bwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(grad_out, out, nullptr, grad_img, nullptr, (size_t)hw,
                                                          make_colmat(colmat_host), 1);
   APH_LAUNCH_OK();

@@ -1,23 +1,15 @@
-// tc_gemm.cuh -- the tcgen05 / TMA / TMEM GEMM of the CLIP ViT encoder (sm_100a).
+// tc_gemm.cuh -- the wgmma / TMA GEMM of the CLIP ViT encoder (sm_90a).
 //
-//   C[M,N] = A[M,K] . B[N,K]^T      A, B bf16 row-major (K contiguous = "K-major"), fp32 accumulate in TMEM.
+//   C[M,N] = A[M,K] . B[N,K]^T      A, B bf16 row-major (K contiguous = "K-major"), fp32 accumulate in registers.
 //
-// Persistent, warp-specialised, one CTA per SM:
-//   warp 0 (1 lane)  TMA producer : cp.async.bulk.tensor.2d -> 128B-swizzled smem stages, mbarrier complete_tx
-//   warp 1 (1 lane)  MMA issuer   : tcgen05.mma.cta_group::1.kind::f16, M=128 x N=BLOCK_N x K=16 per instruction,
-//                                   tcgen05.commit releases smem stages / publishes the accumulator
-//   warp 2           TMEM allocator (2 accumulator stages x BLOCK_N columns)
-//   warps 4-7        epilogue     : tcgen05.ld 32x32b -> registers -> fused epilogue -> global
-// Fused epilogues (struct GemmEpi): +bias, QuickGELU (saving the pre-activation), x gelu'(h) for the MLP
-// backward, +fp32 residual, fp32 and/or bf16 outputs, and an NCHW "un-patchify" store for the patch-embed
-// data gradient. Rows >= M are zero-filled by TMA on load and clipped by TMA on store.
-//
-// Epilogue data path (all kinds but the un-patchify scatter): each epilogue warp owns a ring of 4 KB shared-memory tiles
-// (32 rows x 128 B, the TMA 128B-swizzle layout). Outputs are packed in registers (bf16 kinds: 64 columns per tile),
-// written once to a ring tile and leave through cp.async.bulk.tensor stores (one elected lane, bulk groups, L2 cache
-// hints per tensor); the global operands of the fused kinds (fp32 residual, saved bf16 pre-activation) ARRIVE through
-// TMA loads into the same ring, issued one item ahead -- also across tile boundaries, i.e. during the next tile's main
-// loop -- and are combined IN PLACE, so no epilogue warp ever waits on a global load or issues a global store itself.
+// Persistent, warp-specialised, one CTA of three warpgroups per SM, tile 128 x BN (BN = 128 or 256):
+//   warpgroup 0 (1 lane)  TMA producer : cp.async.bulk.tensor.2d -> 128B-swizzled smem stages, mbarrier complete_tx
+//   warpgroups 1, 2       consumers    : rows 0-63 / 64-127 of the tile; wgmma.mma_async m64nBNk16 with both operands read
+//                                        from shared memory through descriptors, then the fused epilogue from registers
+// The producer gives its registers to the consumers (setmaxnreg) and runs ahead into the next tile's stages while the
+// consumers store the current one. Fused epilogues (struct GemmEpi): +bias, QuickGELU (saving the pre-activation),
+// x gelu'(h) for the MLP backward, +fp32 residual, fp32 or bf16 outputs, and an NCHW "un-patchify" store for the
+// patch-embed data gradient. Rows >= M are zero-filled by TMA on load and not stored.
 #pragma once
 #include "aph_common.cuh"
 #include <cuda.h>
@@ -36,21 +28,16 @@ struct GemmEpi {
   int act = 0;                     // 1 = QuickGELU x*sigmoid(1.702x)
   int unpatch_p = 0;               // >0: out_f32 is [S,3,R,R]; row = s*g*g + gy*g + gx, col = c*p*p + py*p + px
   int unpatch_g = 0;
-  // remainder rows [tail_m0, tail_m) of a one-wave launch (BN = 384): computed by the epilogue warps with mma.sync (gemm_tail_task)
-  const bf16* tail_a = nullptr;    // A [tail_m, K]
-  const bf16* tail_b = nullptr;    // B [N, K]
-  int tail_m0 = 0, tail_m = 0;
 };
 
 struct GemmShape { int M, N, K; };
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;       // 64 bf16 = 128 B = one swizzle-128B row
-constexpr int GEMM_UK = 16;       // K per tcgen05.mma (kind::f16)
-constexpr int GEMM_EPI_WARPS = 8;      // 2 per SM sub-partition (16 measured identical: the epilogue is bound by the output stores, not by warp latency)
-constexpr int GEMM_THREADS = (4 + GEMM_EPI_WARPS) * 32;   // warps 0-3: TMA / MMA / TMEM alloc / spare; warps 4..: epilogue
+constexpr int GEMM_UK = 16;       // K per wgmma (bf16)
+constexpr int GEMM_THREADS = 3 * 128;   // warpgroup 0: TMA producer; warpgroups 1-2: MMA + epilogue
 
-// compile-time epilogue kinds (a runtime-flag epilogue was instruction-latency bound: 1 warp per scheduler, long predicated body)
+// compile-time epilogue kinds (a runtime-flag epilogue is a long predicated body in the hot loop)
 enum : int {
   EPI_F32 = 0,            // out_f32 = acc
   EPI_BF16 = 1,           // out_bf16 = acc
@@ -85,9 +72,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   } while (!done);
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
@@ -97,14 +81,12 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uin
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(x), "r"(y) : "memory");
 }
-
 // 3-D tile load (x = column, y = token, z = sample); out-of-bounds tokens are zero-filled
 __device__ __forceinline__ void tma_load_3d(uint32_t dst_saddr, const CUtensorMap* m, uint64_t* bar, int x, int y, int z) {
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                ::"r"(dst_saddr), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z) : "memory");
 }
-
-// same with an L2 eviction-priority hint (weights are re-read by every M tile: evict_last; streamed outputs must not evict them)
+// same with an L2 eviction-priority hint (weights are re-read by every M tile: evict_last)
 __device__ __forceinline__ void tma_load_2d_hint(void* dst, const CUtensorMap* m, uint64_t* bar, int x, int y, uint64_t policy) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
                ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(x), "r"(y), "l"(policy) : "memory");
@@ -114,96 +96,54 @@ __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
-__device__ __forceinline__ uint64_t l2_policy_evict_first() {
-  uint64_t p;
-  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
-  return p;
-}
 
-__device__ __forceinline__ void tmem_alloc(uint32_t* slot_in_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// D[tmem] (+)= A[smem desc] . B[smem desc]
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// 32 lanes x 32 consecutive fp32 columns -> 32 registers per thread (thread = TMEM lane = accumulator row)
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- CTA-pair (cta_group::2) helpers: two CTAs of a cluster share one 256-row accumulator tile; each loads its own 128 rows
-// of A and HALF of the B tile, the leader issues the MMAs for both, tcgen05.commit multicasts the barrier arrivals.
-__device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
-__device__ __forceinline__ void cluster_sync_all() { asm volatile("barrier.cluster.arrive.aligned;\n\tbarrier.cluster.wait.aligned;" ::: "memory"); }
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t saddr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load whose completion bytes are credited to an mbarrier that may live in the peer (leader) CTA
-__device__ __forceinline__ void tma_load_2d_2sm(void* dst, const CUtensorMap* m, uint32_t mbar_cluster_addr, int x, int y) {
-  asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(mbar_cluster_addr), "r"(x), "r"(y) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t* slot_in_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(slot_in_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16_cg2(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate) : "memory");
-}
-// arrive (after all previously issued MMAs retire) on the barrier at this offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(smem_u32(bar)), "h"(mask) : "memory");
-}
-
-// K-major, 128B-swizzled operand tile: rows of 128 B, 8-row groups 1024 B apart (SBO). sm_100 descriptor version 1.
+// K-major, 128B-swizzled operand tile: rows of 128 B, 8-row groups 1024 B apart (SBO). sm_90 wgmma descriptor.
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr & 0x3FFFF) >> 4);        // start address, bits [0,14)
-  d |= (uint64_t)0 << 16;                          // leading byte offset (unused for swizzled K-major)
+  d |= (uint64_t)1 << 16;                          // leading byte offset (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;                // stride byte offset, bits [32,46)
-  d |= (uint64_t)1 << 46;                          // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                          // layout type: SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                          // layout type: SWIZZLE_128B
   return d;
 }
-// kind::f16 instruction descriptor: D fp32, A/B bf16, both K-major, M=128, N=n
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int n, int m = GEMM_BM) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24);
-}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
+// D[64 x BN] (+)= A[64 x 16] . B[BN x 16]^T, fp32 accumulators d[BN/2] in the m64nNk16 fragment layout
+template <int BN> struct Wgmma;
+#define APH_WG_REGS8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+template <> struct Wgmma<128> {
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, int acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+        : APH_WG_REGS8(0), APH_WG_REGS8(8), APH_WG_REGS8(16), APH_WG_REGS8(24), APH_WG_REGS8(32), APH_WG_REGS8(40), APH_WG_REGS8(48), APH_WG_REGS8(56)
+        : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<256> {
+  static __device__ __forceinline__ void mma(float (&d)[128], uint64_t da, uint64_t db, int acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, "
+        "%72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, "
+        "%116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+        : APH_WG_REGS8(0), APH_WG_REGS8(8), APH_WG_REGS8(16), APH_WG_REGS8(24), APH_WG_REGS8(32), APH_WG_REGS8(40), APH_WG_REGS8(48), APH_WG_REGS8(56),
+          APH_WG_REGS8(64), APH_WG_REGS8(72), APH_WG_REGS8(80), APH_WG_REGS8(88), APH_WG_REGS8(96), APH_WG_REGS8(104), APH_WG_REGS8(112), APH_WG_REGS8(120)
+        : "l"(da), "l"(db), "r"(acc));
+  }
+};
+#undef APH_WG_REGS8
 
 // sigmoid(1.702 x) through ONE special-function op: 0.5 tanh(0.851 x) + 0.5 (tanh.approx: max rel. error 2^-11, far inside
 // the bf16 rounding of the value it feeds); the epilogues of the MLP GEMMs are MUFU-limited otherwise (exp + rcp per element)
@@ -217,421 +157,137 @@ __device__ __forceinline__ float quickgelu_grad(float x) {
   const float s = sigmoid1702(x);
   return s * (1.f + 1.702f * x * (1.f - s));
 }
-__device__ __forceinline__ void sts128(uint32_t saddr, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(saddr), "r"(a), "r"(b), "r"(c), "r"(d));
-}
-__device__ __forceinline__ float4 lds128(uint32_t saddr) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(saddr));
-  return v;
-}
-
-// ---- bulk-tensor stores (epilogue) ----------------------------------------------------------------------------------
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, uint32_t src_saddr, int x, int y) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(src_saddr), "r"(x), "r"(y) : "memory");
-}
-__device__ __forceinline__ void tma_store_2d_hint(const CUtensorMap* m, uint32_t src_saddr, int x, int y, uint64_t policy) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group.L2::cache_hint [%0, {%2, %3}], [%1], %4;"
-               ::"l"(reinterpret_cast<uint64_t>(m)), "r"(src_saddr), "r"(x), "r"(y), "l"(policy) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-// blocks until at most N of this thread's bulk groups still have to READ their shared-memory source
-template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-// 2-D tile load into this CTA's shared memory, completion on a local mbarrier (epilogue operands)
-__device__ __forceinline__ void tma_load_2d_cta(uint32_t dst_saddr, const CUtensorMap* m, uint64_t* bar, int x, int y) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-               ::"r"(dst_saddr), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(x), "r"(y) : "memory");
-}
-__device__ __forceinline__ uint4 lds128u(uint32_t saddr) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(saddr));
-  return v;
-}
 __device__ __forceinline__ uint32_t pack_bf16(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
-// ---- remainder rows of a "one-wave" GEMM ---------------------------------------------------------------------------------
-// The 384-wide pair tiles cover the first floor(M / 256) * 256 rows in exactly one wave; the last M % 256 (<= 64) rows -- 0.3 % of
-// the work at M = 9500 -- are computed by the epilogue warps of the same kernel while they would otherwise wait for the main loop:
-// one warp task = 8 output columns x 16 rows on the legacy tensor path (mma.sync m16n8k16), operands straight from global / L2
-// (no shared memory), 8 k-chunks x 3 x 16 B per lane in flight. K is consumed 32 at a time with ONE 16-byte load per operand row:
-// feeding the A and B fragments through the same k permutation leaves the dot products unchanged.
-__device__ __forceinline__ void mma16816_bf16(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
-}
-
-template <int EPI>
-__device__ __noinline__ void gemm_tail_task(int task, int lane, int N, int K, const GemmEpi& epi) {
-  const bf16* __restrict__ A = epi.tail_a; const bf16* __restrict__ B = epi.tail_b;
-  const int M = epi.tail_m, g = lane >> 2, t = lane & 3;
-  const int ncol = N / 8;
-  const int n0 = (task % ncol) * 8, m0 = epi.tail_m0 + (task / ncol) * 16;
-  const int r0 = m0 + g, r1 = r0 + 8;
-  const bf16* bp = B + (size_t)(n0 + g) * K + 8 * t;
-  const bf16* a0p = A + (size_t)min(r0, M - 1) * K + 8 * t;
-  const bf16* a1p = A + (size_t)min(r1, M - 1) * K + 8 * t;
-  float acc[4] = {0.f, 0.f, 0.f, 0.f};
-  constexpr int U = 8;
-  for (int k0 = 0; k0 < K; k0 += 32 * U) {
-    uint4 bq[U], al[U], ah[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int k = k0 + 32 * u;
-      const bool ok = k < K;
-      bq[u] = ok ? __ldg(reinterpret_cast<const uint4*>(bp + k)) : make_uint4(0u, 0u, 0u, 0u);
-      al[u] = ok ? __ldg(reinterpret_cast<const uint4*>(a0p + k)) : make_uint4(0u, 0u, 0u, 0u);
-      ah[u] = ok ? __ldg(reinterpret_cast<const uint4*>(a1p + k)) : make_uint4(0u, 0u, 0u, 0u);
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      mma16816_bf16(acc, al[u].x, ah[u].x, al[u].y, ah[u].y, bq[u].x, bq[u].y);
-      mma16816_bf16(acc, al[u].z, ah[u].z, al[u].w, ah[u].w, bq[u].z, bq[u].w);
-    }
-  }
-  const int col = n0 + 2 * t;
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int r = h ? r1 : r0;
-    if (r >= M) continue;                       // rows clamped on load are simply not stored
-    const float v0 = acc[2 * h], v1 = acc[2 * h + 1];
-    const size_t off = (size_t)r * N + col;
-    if (EPI == EPI_BIAS_RESID) {
-      const float2 bb = __ldg(reinterpret_cast<const float2*>(epi.bias + col)), rr = __ldg(reinterpret_cast<const float2*>(epi.resid + off));
-      *reinterpret_cast<float2*>(epi.out_f32 + off) = make_float2(v0 + bb.x + rr.x, v1 + bb.y + rr.y);
-    } else if (EPI == EPI_BF16) {
-      *reinterpret_cast<uint32_t*>(epi.out_bf16 + off) = pack_bf16(v0, v1);
-    }
-  }
-}
-
-constexpr int EPI_TILE_BYTES = 32 * 128;      // one ring tile: 32 rows x 128 B
-
-template <int BN, int STAGES, int CG, int NBUF>
-struct GemmSmem {
+template <int BN>
+struct GemmCfg {
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
-  static constexpr int B_BYTES = (BN / CG) * GEMM_BK * 2;      // a CTA pair splits the B tile
+  static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int EPI_OFFSET = STAGES * STAGE_BYTES;          // per epilogue warp: NBUF ring tiles
-  static constexpr int EPI_BYTES = GEMM_EPI_WARPS * NBUF * EPI_TILE_BYTES;
-  static constexpr int BAR_OFFSET = EPI_OFFSET + EPI_BYTES;
-  static constexpr int NUM_BARS = 2 * STAGES + 4 + GEMM_EPI_WARPS * NBUF;
-  static constexpr int TOTAL = BAR_OFFSET + NUM_BARS * 8 + 16 + 1024;   // + alignment slack
+  static constexpr int STAGES = (BN == 256) ? 4 : 6;              // 192 KB of operand stages either way
+  static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
+  static constexpr int SMEM = BAR_OFFSET + 2 * STAGES * 8 + 1024;  // + alignment slack
 };
 
-// compile-time properties of an epilogue kind
-template <int EPI> struct EpiTraits {
-  static constexpr bool OUT16 = (EPI == EPI_BF16 || EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_GELUGRAD_BF16);
-  static constexpr bool HAS_OP = (EPI == EPI_BIAS_RESID || EPI == EPI_GELUGRAD_BF16);      // a global operand arrives by TMA
-  static constexpr bool HAS_BIAS = (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_RESID);
-  static constexpr int NOUT = (EPI == EPI_BIAS_GELU) ? 2 : 1;
-  static constexpr int CW = OUT16 ? 64 : 32;                   // accumulator columns per ring tile
-  static constexpr int NBUF = (HAS_OP || NOUT == 2) ? 3 : 2;   // ring depth
-  static constexpr int STAGES = (NBUF == 3) ? 4 : 5;           // main-loop stages that still fit beside the ring (227 KB)
-};
+// two adjacent output columns (col, col + 1) of one row through the epilogue of kind EPI
+template <int EPI>
+__device__ __forceinline__ void epi_store2(const GemmEpi& epi, int N, int row, int col, float v0, float v1, float2 bb) {
+  const size_t off = (size_t)row * N + col;
+  if (EPI == EPI_F32) {
+    *reinterpret_cast<float2*>(epi.out_f32 + off) = make_float2(v0, v1);
+  } else if (EPI == EPI_BF16) {
+    *reinterpret_cast<uint32_t*>(epi.out_bf16 + off) = pack_bf16(v0, v1);
+  } else if (EPI == EPI_BIAS_BF16) {
+    *reinterpret_cast<uint32_t*>(epi.out_bf16 + off) = pack_bf16(v0 + bb.x, v1 + bb.y);
+  } else if (EPI == EPI_BIAS_GELU) {
+    v0 += bb.x; v1 += bb.y;
+    *reinterpret_cast<uint32_t*>(epi.out_pre + off) = pack_bf16(v0, v1);
+    *reinterpret_cast<uint32_t*>(epi.out_bf16 + off) = pack_bf16(quickgelu(v0), quickgelu(v1));
+  } else if (EPI == EPI_BIAS_RESID) {
+    const float2 r = __ldg(reinterpret_cast<const float2*>(epi.resid + off));
+    *reinterpret_cast<float2*>(epi.out_f32 + off) = make_float2(v0 + bb.x + r.x, v1 + bb.y + r.y);
+  } else if (EPI == EPI_GELUGRAD_BF16) {
+    const uint32_t u = __ldg(reinterpret_cast<const unsigned int*>(epi.gelu_in + off));
+    const float2 h = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u));
+    *reinterpret_cast<uint32_t*>(epi.out_bf16 + off) = pack_bf16(v0 * quickgelu_grad(h.x), v1 * quickgelu_grad(h.y));
+  } else {   // EPI_UNPATCH: col = c*p*p + py*p + px with p even, so (col, col + 1) are adjacent pixels of one image row
+    const int p = epi.unpatch_p, g = epi.unpatch_g, R = p * g;
+    const int ch = col / (p * p), rem = col - ch * p * p, py = rem / p, px = rem - py * p;
+    const int s = row / (g * g), pr = row - s * g * g, gy = pr / g, gx = pr - gy * g;
+    *reinterpret_cast<float2*>(epi.out_f32 + (((size_t)s * 3 + ch) * R + gy * p + py) * R + gx * p + px) = make_float2(v0, v1);
+  }
+}
 
-template <int BN, int STAGES, int EPI, int CG, int NBUF>
+template <int BN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
-               const __grid_constant__ CUtensorMap map_o1, const __grid_constant__ CUtensorMap map_o2,
-               const __grid_constant__ CUtensorMap map_op, GemmShape shp, GemmEpi epi) {
-  using L = GemmSmem<BN, STAGES, CG, NBUF>;
-  using E = EpiTraits<EPI>;
+k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, GemmShape shp, GemmEpi epi) {
+  using L = GemmCfg<BN>;
+  constexpr int STAGES = L::STAGES;
+  constexpr bool HAS_BIAS = (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_RESID);
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;     // [2] accumulator ready
-  uint64_t* tempty_bar = tfull_bar + 2;         // [2] accumulator drained
-  uint64_t* op_bar = tempty_bar + 2;            // [GEMM_EPI_WARPS][NBUF] epilogue operand landed
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(op_bar + GEMM_EPI_WARPS * NBUF);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t rank = (CG == 2) ? cluster_ctarank() : 0u;      // position inside the CTA pair (0 = leader)
-  // a "tile" is one accumulator of (128*CG) x BN: with CG = 2 the pair shares it, each CTA owning 128 of its rows
-  const int m_tiles = (shp.M + GEMM_BM * CG - 1) / (GEMM_BM * CG), n_tiles = shp.N / BN;
+  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
+  const int m_tiles = (shp.M + GEMM_BM - 1) / GEMM_BM, n_tiles = shp.N / BN;
   const int num_tiles = m_tiles * n_tiles, k_blocks = shp.K / GEMM_BK;
-  const int tile0 = blockIdx.x / CG, tile_step = gridDim.x / CG;
-  // BN = 384 ("one-wave" tiles for the N = 768 GEMMs: 37 x 2 pair tiles of 256 x 384 on the 74 SM pairs) holds ONE accumulator
-  // stage (384 of the 512 TMEM columns); the narrower tiles double-buffer theirs so a tile's epilogue overlaps the next main loop
-  constexpr int ACC = (BN == 384) ? 1 : 2;
-  // BN = 192 ("two exact waves" for the N = 768 GEMMs: floor(M/256) x 4 = 148 pair tiles on 74 pairs at M ~ 9500, remainder rows by the
-  // idle epilogue warps) keeps the double buffer: 2 x 192 = 384 columns of a 512-column allocation
-  constexpr uint32_t TMEM_COLS = (BN == 384 || BN == 192) ? 512 : 2 * BN;
-  static_assert(BN == 128 || BN == 256 || ((BN == 384 || BN == 192) && CG == 2), "tile widths: 128, 256, or 192 / 384 (CTA pair only)");
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a); tma_prefetch_desc(&map_b);
-    if (EPI != EPI_UNPATCH) tma_prefetch_desc(&map_o1);
-    if (E::NOUT == 2) tma_prefetch_desc(&map_o2);
-    if (E::HAS_OP) tma_prefetch_desc(&map_op);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], CG); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tfull_bar[i], 1); mbar_init(&tempty_bar[i], CG * GEMM_EPI_WARPS); }
-    for (int i = 0; i < GEMM_EPI_WARPS * NBUF; ++i) mbar_init(&op_bar[i], 1);
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }
     fence_barrier_init();
   }
-  if (warp == 2) { if (CG == 2) tmem_alloc_cg2(tmem_slot, TMEM_COLS); else tmem_alloc(tmem_slot, TMEM_COLS); }
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   pdl_wait();                  // everything above overlapped the previous kernel's tail; operands are read from here on
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (tid == 0) {
       // ===== TMA producer
       const uint64_t pol_b = l2_policy_evict_last();      // B = weights: shared by all M tiles
       uint32_t it = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step) {
-        const int m_blk = (tile / n_tiles) * CG + (int)rank, n_blk = tile % n_tiles;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
         for (int kb = 0; kb < k_blocks; ++kb, ++it) {
           const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
           mbar_wait(&empty_bar[s], ph ^ 1);
           uint8_t* sa = smem + s * L::STAGE_BYTES;
-          if (CG == 2) {
-            // both CTAs credit the LEADER's full barrier: the leader's MMA consumes the stage of both
-            const uint32_t lead_full = mapa_u32(smem_u32(&full_bar[s]), 0);
-            if (rank == 0) mbar_expect_tx(&full_bar[s], 2 * L::STAGE_BYTES); else mbar_arrive_cluster(lead_full);
-            tma_load_2d_2sm(sa, &map_a, lead_full, kb * GEMM_BK, m_blk * GEMM_BM);
-            if (BN == 384) {
-              // this CTA's half of the N = 256 instruction (128 rows of B) followed by its half of the N = 128 one (64 rows); 64-row boxes
-              const int n0 = n_blk * BN;
-              tma_load_2d_2sm(sa + L::A_BYTES, &map_b, lead_full, kb * GEMM_BK, n0 + (int)rank * 128);
-              tma_load_2d_2sm(sa + L::A_BYTES + 64 * 128, &map_b, lead_full, kb * GEMM_BK, n0 + (int)rank * 128 + 64);
-              tma_load_2d_2sm(sa + L::A_BYTES + 128 * 128, &map_b, lead_full, kb * GEMM_BK, n0 + 256 + (int)rank * 64);
-            } else {
-              tma_load_2d_2sm(sa + L::A_BYTES, &map_b, lead_full, kb * GEMM_BK, n_blk * BN + (int)rank * (BN / 2));
-            }
-          } else {
-            mbar_expect_tx(&full_bar[s], L::STAGE_BYTES);
-            tma_load_2d(sa, &map_a, &full_bar[s], kb * GEMM_BK, m_blk * GEMM_BM);
-            tma_load_2d_hint(sa + L::A_BYTES, &map_b, &full_bar[s], kb * GEMM_BK, n_blk * BN, pol_b);
-          }
+          mbar_expect_tx(&full_bar[s], L::STAGE_BYTES);
+          tma_load_2d(sa, &map_a, &full_bar[s], kb * GEMM_BK, m_blk * GEMM_BM);
+          tma_load_2d_hint(sa + L::A_BYTES, &map_b, &full_bar[s], kb * GEMM_BK, n_blk * BN, pol_b);
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {
-      // ===== MMA issuer (the leader CTA issues for the pair when CG = 2)
-      constexpr uint32_t idesc = make_idesc_bf16(BN == 384 ? 256 : BN, GEMM_BM * CG);
-      constexpr uint32_t idesc_b = make_idesc_bf16(128, GEMM_BM * CG);        // second instruction of a 384-wide tile
-      uint32_t it = 0, tile_iter = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step, ++tile_iter) {
-        const uint32_t as = tile_iter % ACC, aph_ = (tile_iter / ACC) & 1;
-        mbar_wait(&tempty_bar[as], aph_ ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + as * BN;
-        for (int kb = 0; kb < k_blocks; ++kb, ++it) {
-          const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
-          const uint64_t da = make_smem_desc(sa), db = make_smem_desc(sa + L::A_BYTES);
+  } else {
+    setmaxnreg_inc<232>();
+    // ===== consumer warpgroup: rows 64*(wg-1) .. +63 of each tile
+    const int warp = tid >> 5, lane = tid & 31;
+    const int row_in_tile = 64 * (wg - 1) + 16 * warp + (lane >> 2), col_in_tile = 2 * (lane & 3);
+    uint32_t it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
+      float d[BN / 2];
 #pragma unroll
-          for (int k = 0; k < GEMM_BK / GEMM_UK; ++k) {
-            // advance 16 bf16 = 32 B along K inside the swizzle atom: +2 in the (>>4) address field
-            if (CG == 2) umma_f16_cg2(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0);
-            else umma_f16(tmem_d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), idesc, (kb | k) != 0);
-            if (BN == 384)      // columns 256..383: B rows 128.. of this stage (16 KB further: +1024 in the >>4 address field)
-              umma_f16_cg2(tmem_d + 256, da + (uint64_t)(2 * k), db + (uint64_t)(1024 + 2 * k), idesc_b, (kb | k) != 0);
-          }
-          if (CG == 2) {
-            umma_commit_mc(&empty_bar[s], 0b11);                            // both CTAs' smem stages are free
-            if (kb == k_blocks - 1) umma_commit_mc(&tfull_bar[as], 0b11);   // both CTAs' epilogues may read TMEM
-          } else {
-            umma_commit(&empty_bar[s]);                                     // smem stage free once these MMAs retire
-            if (kb == k_blocks - 1) umma_commit(&tfull_bar[as]);            // accumulator complete
-          }
-        }
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < k_blocks; ++kb, ++it) {
+        const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
+        const uint64_t da = make_smem_desc(sa + (wg - 1) * (64 * 128)), db = make_smem_desc(sa + L::A_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GEMM_BK / GEMM_UK; ++k)      // advance 16 bf16 = 32 B along K inside the swizzle atom: +2 in the (>>4) address field
+          Wgmma<BN>::mma(d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) != 0);
+        wgmma_commit();
+        wgmma_wait<1>();                                 // the previous stage's MMAs have retired: hand that stage back
+        if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+        prev = (int)s;
       }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: 8 warps. Warp w reads TMEM lanes 32*(w%4) .. +31 (one accumulator row per lane) and owns the column
-    // groups half, half+2, ... (half = (w-4)/4) of every tile of this CTA.
-    const int ew = warp - 4, q = warp & 3, half = ew >> 2;
-    const uint32_t ring = smem_u32(smem + L::EPI_OFFSET + ew * (NBUF * EPI_TILE_BYTES));
-    if constexpr ((BN == 384 || BN == 192) && (EPI == EPI_BF16 || EPI == EPI_BIAS_RESID)) {
-      // remainder rows of a one-wave launch: warp tasks spread over all epilogue warps of the grid, done while the main loop runs
-      if (epi.tail_m > epi.tail_m0) {
-        const int ntasks = (shp.N / 8) * ((epi.tail_m - epi.tail_m0 + 15) / 16);
-        for (int task = (int)blockIdx.x * GEMM_EPI_WARPS + ew; task < ntasks; task += (int)gridDim.x * GEMM_EPI_WARPS)
-          gemm_tail_task<EPI>(task, lane, shp.N, shp.K, epi);
+      wgmma_wait<0>();
+      if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
+      // ---- epilogue straight from the accumulator fragments: d[4j + {0,1}] = (row, col + {0,1}), d[4j + {2,3}] = (row + 8, ...)
+      const int row0 = m_blk * GEMM_BM + row_in_tile, row1 = row0 + 8;
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n_blk * BN + 8 * j + col_in_tile;
+        const float2 bb = HAS_BIAS ? __ldg(reinterpret_cast<const float2*>(epi.bias + col)) : make_float2(0.f, 0.f);
+        if (row0 < shp.M) epi_store2<EPI>(epi, shp.N, row0, col, d[4 * j], d[4 * j + 1], bb);
+        if (row1 < shp.M) epi_store2<EPI>(epi, shp.N, row1, col, d[4 * j + 2], d[4 * j + 3], bb);
       }
-    }
-    if constexpr (EPI == EPI_UNPATCH) {
-      // ---- patch-embed data gradient: the NCHW destination of a 32-row tile is 32 scattered 128-byte segments (one per patch),
-      // not a TMA box: 32x32 fp32 chunks are transposed through one ring tile and stored row-contiguously by the lanes.
-      const int c4 = lane & 7, rsub = lane >> 3;
-      uint32_t tile_iter = 0;
-      for (int tile = tile0; tile < num_tiles; tile += tile_step, ++tile_iter) {
-        const int m_blk = (tile / n_tiles) * CG + (int)rank, n_blk = tile % n_tiles;
-        const uint32_t as = tile_iter % ACC, aph_ = (tile_iter / ACC) & 1;
-        mbar_wait(&tfull_bar[as], aph_);
-        tc_fence_after();
-        const int m_base = m_blk * GEMM_BM + q * 32;
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + as * BN;
-#pragma unroll 1
-        for (int c = half; c < BN / 32; c += GEMM_EPI_WARPS / 4) {
-          const int col = n_blk * BN + c * 32 + 4 * c4;
-          uint32_t r[32];
-          tmem_ld_32x32(taddr + c * 32, r);
-          tmem_wait_ld();
-          if (c + GEMM_EPI_WARPS / 4 >= BN / 32) {          // this warp's last read of the accumulator: hand the TMEM stage back
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { if (CG == 2) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty_bar[as]), 0)); else mbar_arrive(&tempty_bar[as]); }
-          }
-#pragma unroll
-          for (int i = 0; i < 8; ++i)      // lane = row: write its 32 columns as 8 swizzled 16-byte chunks
-            sts128(ring + lane * 128 + ((i ^ (lane & 7)) << 4), r[4 * i], r[4 * i + 1], r[4 * i + 2], r[4 * i + 3]);
-          __syncwarp();
-          const int p = epi.unpatch_p, g = epi.unpatch_g, R = p * g;
-          const int ch = col / (p * p), rem = col - ch * p * p, py = rem / p, px = rem - py * p;
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rr = it * 4 + rsub;
-            const int m = m_base + rr;
-            if (m >= shp.M) break;
-            const float4 v = lds128(ring + rr * 128 + ((c4 ^ (rr & 7)) << 4));
-            const int s = m / (g * g), pr = m - s * g * g, gy = pr / g, gx = pr - gy * g;
-            *reinterpret_cast<float4*>(epi.out_f32 + (((size_t)s * 3 + ch) * R + gy * p + py) * R + gx * p + px) = v;
-          }
-          __syncwarp();                    // staging tile is reused by this warp's next chunk
-        }
-      }
-    } else {
-      constexpr int CW = E::CW;
-      // items (ring tiles of CW accumulator columns) per warp per tile: column groups half, half+2, ... (an odd group count, BN = 192
-      // with 64-column items, gives the half-0 warps one more)
-      const int NI = (BN / CW - half + 1) / 2;
-      static_assert(BN / CW >= 2, "tile too narrow for the epilogue split");
-      uint64_t* my_bar = op_bar + ew * NBUF;
-      const int my_tiles = (tile0 < num_tiles) ? (num_tiles - tile0 + tile_step - 1) / tile_step : 0;
-      const int total_items = my_tiles * NI;
-      const uint64_t pol_stream = l2_policy_evict_first();
-      uint32_t slot = 0, ophase = 0;
-      // coordinates of item g: first row of this warp's 32-row slice and first column
-      auto coords = [&](int g, int& m0, int& col0) {
-        const int t = tile0 + (g / NI) * tile_step, i = g - (g / NI) * NI;
-        m0 = ((t / n_tiles) * CG + (int)rank) * GEMM_BM + q * 32;
-        col0 = (t % n_tiles) * BN + (half + 2 * i) * CW;
-      };
-      auto issue_operand = [&](int g) {             // lane 0 only: operand tile of item g -> ring tile g % NBUF
-        int m0, col0; coords(g, m0, col0);
-        if (m0 >= shp.M) return;                    // slice entirely past M: nothing to load (and nothing will be waited for)
-        const int b = g % NBUF;
-        mbar_expect_tx(&my_bar[b], EPI_TILE_BYTES);
-        tma_load_2d_cta(ring + b * EPI_TILE_BYTES, &map_op, &my_bar[b], col0, m0);
-      };
-      if (E::HAS_OP && total_items > 0 && lane == 0) issue_operand(0);
-#pragma unroll 1
-      for (int g = 0; g < total_items; ++g) {
-        const int tile_iter = g / NI, i = g - tile_iter * NI;
-        int m0, col0; coords(g, m0, col0);
-        const bool live = m0 < shp.M;               // warp-uniform
-        const uint32_t as = tile_iter % ACC, aph_ = (tile_iter / ACC) & 1;
-        if (E::HAS_OP) {
-          // next item's operand (possibly the next tile's: it then flies during that tile's main loop). Its ring tile was last
-          // read by the store of item g+1-NBUF: at most NBUF-2 younger stores may still be reading.
-          if (g + 1 < total_items && lane == 0) { bulk_wait_read<NBUF - 2>(); issue_operand(g + 1); }
-        }
-        if (i == 0) { mbar_wait(&tfull_bar[as], aph_); tc_fence_after(); }
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + as * BN + (half + 2 * i) * CW;
-        uint32_t b0, b1 = 0;                        // ring tiles of this item
-        if (E::HAS_OP) {
-          b0 = g % NBUF;
-          if (live) { mbar_wait(&my_bar[b0], (ophase >> b0) & 1u); ophase ^= 1u << b0; }
-        } else {
-          b0 = slot % NBUF; b1 = (slot + 1) % NBUF;
-          if (lane == 0) bulk_wait_read<NBUF - E::NOUT>();      // the ring tiles about to be overwritten are no longer being read
-          __syncwarp();
-        }
-        const uint32_t row0 = ring + b0 * EPI_TILE_BYTES + lane * 128, row1 = ring + b1 * EPI_TILE_BYTES + lane * 128;
-        const int sw = lane & 7;
-#pragma unroll
-        for (int h = 0; h < CW / 32; ++h) {          // 32 accumulator columns at a time
-          uint32_t r[32];
-          tmem_ld_32x32(taddr + h * 32, r);
-          tmem_wait_ld();
-          if (i == NI - 1 && h == CW / 32 - 1) {     // this warp's last read of the accumulator: hand the TMEM stage back
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) { if (CG == 2) mbar_arrive_cluster(mapa_u32(smem_u32(&tempty_bar[as]), 0)); else mbar_arrive(&tempty_bar[as]); }
-          }
-          const float* bias = epi.bias + col0 + h * 32;
-          if constexpr (!E::OUT16) {
-            // fp32 output: 8 chunks of 4 columns
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-              float4 v = make_float4(__uint_as_float(r[4 * c]), __uint_as_float(r[4 * c + 1]), __uint_as_float(r[4 * c + 2]), __uint_as_float(r[4 * c + 3]));
-              const uint32_t a = row0 + ((c ^ sw) << 4);
-              if (EPI == EPI_BIAS_RESID) {
-                const float4 bb = __ldg(reinterpret_cast<const float4*>(bias) + c);
-                const float4 o = lds128(a);
-                v.x += bb.x + o.x; v.y += bb.y + o.y; v.z += bb.z + o.z; v.w += bb.w + o.w;
-              }
-              sts128(a, __float_as_uint(v.x), __float_as_uint(v.y), __float_as_uint(v.z), __float_as_uint(v.w));
-            }
-          } else {
-            // bf16 output: this half fills 16-byte chunks 4h .. 4h+3 of the row (8 columns each)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              float v[8];
-#pragma unroll
-              for (int e = 0; e < 8; ++e) v[e] = __uint_as_float(r[8 * c + e]);
-              if (E::HAS_BIAS) {
-                const float4 b0v = __ldg(reinterpret_cast<const float4*>(bias) + 2 * c), b1v = __ldg(reinterpret_cast<const float4*>(bias) + 2 * c + 1);
-                v[0] += b0v.x; v[1] += b0v.y; v[2] += b0v.z; v[3] += b0v.w; v[4] += b1v.x; v[5] += b1v.y; v[6] += b1v.z; v[7] += b1v.w;
-              }
-              const uint32_t off = (uint32_t)(((4 * h + c) ^ sw) << 4);
-              if (EPI == EPI_BIAS_GELU) {
-                sts128(row1 + off, pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]), pack_bf16(v[6], v[7]));      // pre-activation
-#pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] = quickgelu(v[e]);
-              }
-              if (EPI == EPI_GELUGRAD_BF16) {
-                const uint4 u = lds128u(row0 + off);
-                const uint32_t uu[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                  const float2 hh = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&uu[e]));
-                  v[2 * e] *= quickgelu_grad(hh.x); v[2 * e + 1] *= quickgelu_grad(hh.y);
-                }
-              }
-              sts128(row0 + off, pack_bf16(v[0], v[1]), pack_bf16(v[2], v[3]), pack_bf16(v[4], v[5]), pack_bf16(v[6], v[7]));
-            }
-          }
-        }
-        fence_proxy_async();                         // generic-proxy writes of the ring tile -> visible to the bulk-tensor store
-        __syncwarp();
-        if (lane == 0 && live) {
-          tma_store_2d(&map_o1, ring + b0 * EPI_TILE_BYTES, col0, m0);
-          bulk_commit();
-          if (E::NOUT == 2) { tma_store_2d_hint(&map_o2, ring + b1 * EPI_TILE_BYTES, col0, m0, pol_stream); bulk_commit(); }   // saved for backward only
-        }
-        slot += E::NOUT;
-      }
-      if (lane == 0) bulk_wait_read<0>();            // shared memory must stay valid until the last store has read it
     }
   }
-  __syncwarp();               // single-lane roles rejoin their warp before the (warp-aligned) cluster barrier
-  tc_fence_before();
-  if (CG == 2) cluster_sync_all(); else __syncthreads();
-  if (warp == 2) { if (CG == 2) tmem_dealloc_cg2(tmem_base, TMEM_COLS); else tmem_dealloc(tmem_base, TMEM_COLS); }
 }
 
 // ---- host side ---------------------------------------------------------------------------------
 // 2-D bf16 tensor map: tensor [rows, K] row-major, box [box_rows, 64] with 128B swizzle.
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int K, int box_rows);
 int make_tmap_bf16_tokens(CUtensorMap* out, const void* base, int cols, int T, int S, int box_rows);
-// epilogue ring-tile map: tensor [rows, cols] row-major of 2- or 4-byte elements, box 32 rows x 128 bytes, 128B swizzle
-int make_tmap_epi(CUtensorMap* out, const void* base, int rows, int cols, int elem_bytes);
 // Launches the GEMM on `st`. A: [M,K], B: [N,K] device bf16. Requires K % 64 == 0, N % 128 == 0.
 int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st);
 

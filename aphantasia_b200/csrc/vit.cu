@@ -1,5 +1,5 @@
 // vit.cu -- CLIP ViT-B image encoder handle: packed bf16 weights, activation arena, forward and
-// data-gradient backward built from the tcgen05 GEMM (tc_gemm.cuh) and the kernels of vit_ops.cuh.
+// data-gradient backward built from the wgmma GEMM (tc_gemm.cuh) and the kernels of vit_ops.cuh.
 //
 // Restates OpenAI clip/model.py VisionTransformer.forward (third-party, SURVEY.md A5):
 //   conv1 (patch-embed GEMM) -> [cls; tok] + pos -> ln_pre -> 12 x { x += out_proj(MHA(ln_1 x)); x += c_proj(QuickGELU(c_fc(ln_2 x))) }
@@ -8,7 +8,6 @@
 // LayerNorm backward can recompute x-hat. No weight gradients (the reference computes and discards them).
 #include "vit_ops.cuh"
 #include "vit_attn_tc.cuh"
-#include "vit_attn_umma.cuh"
 #include <stdlib.h>
 #include <string>
 #include <vector>
@@ -154,7 +153,7 @@ __global__ void __launch_bounds__(256) k_pack_weight(const float* __restrict__ i
 
 static int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st) {
   const size_t n = (size_t)rows * cols;
-  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)kNumSMs * 16);
+  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16);
   k_pack_weight<<<blocks, 256, 0, st>>>(src, dst, rows, cols, transpose);
   APH_LAUNCH_OK();
   return 0;
@@ -180,13 +179,6 @@ static inline int rows_grid(int rows) { return (rows * 32 + 255) / 256; }
 static bool attn_simt() {
   static int v = -1;
   if (v < 0) { const char* e = getenv("APH_ATTN_SIMT"); v = (e && e[0] == '1') ? 1 : 0; }
-  return v == 1;
-}
-
-// APH_ATTN_UMMA=0 falls back to the mma.sync forward for T <= 64 (default: the tcgen05 / TMEM kernel of vit_attn_umma.cuh)
-static bool attn_umma() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("APH_ATTN_UMMA"); v = (e && e[0] == '0') ? 0 : 1; }
   return v == 1;
 }
 
@@ -346,7 +338,7 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, float* emb, in
   if (images) {
     const int g = v->g, Mp = S * g * g;
     const size_t n8 = (size_t)Mp * v->Kp / 8;
-    APH_CUDA_OK(launch_k(k_patchify, dim3((unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)kNumSMs * 16)), dim3(256), (size_t)0, st, 1, images, v->patches, S, v->cfg.patch, g));
+    APH_CUDA_OK(launch_k(k_patchify, dim3((unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1, images, v->patches, S, v->cfg.patch, g));
     APH_LAUNCH_OK();
   }
   const int rc = run_cached(v->fwd_graphs, v->warm_fwd, v->stamp, v->graph_misses, nullptr, nullptr, S, save_for_bwd, st, [&]() -> int {
@@ -372,7 +364,6 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, float* emb, in
     { GemmEpi ep; ep.bias = w.b_qkv; ep.out_bf16 = v->qkv[l];
       if ((e = launch_gemm(v->ln_out, w.w_qkv, GemmShape{M, 3 * D, D}, ep, st))) return e; }
     if (attn_simt()) { k_attn_fwd<<<S * H, 256, attn_fwd_smem(T), st>>>(v->qkv[l], v->attn_out, T, D, H); APH_LAUNCH_OK(); }
-    else if (T <= 64 && attn_umma()) { if ((e = attn_fwd_umma_launch(v->qkv[l], v->attn_out, S, T, D, H, st))) return e; }
     else if ((e = attn_dispatch(true, v->qkv[l], nullptr, v->attn_out, S, T, D, H, st))) return e;
     { GemmEpi ep; ep.bias = w.b_o; ep.resid = x_in; ep.out_f32 = x_mid;
       if ((e = launch_gemm(v->attn_out, w.w_o, GemmShape{M, D, D}, ep, st))) return e; }
@@ -406,7 +397,7 @@ extern "C" int aph_vit_bwd(aph_vit* vit, const float* grad_emb, int S, float* gr
   cudaStream_t st = (cudaStream_t)stream;
   {   // caller-owned input: converted outside the cached graph (see aph_vit_fwd)
     const size_t n = (size_t)S * v->cfg.out_dim;
-    APH_CUDA_OK(launch_k(k_f32_to_bf16, dim3((int)std::min<size_t>((n + 255) / 256, (size_t)kNumSMs * 8)), dim3(256), (size_t)0, st, 1, grad_emb, v->d_emb, n));
+    APH_CUDA_OK(launch_k(k_f32_to_bf16, dim3((int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8)), dim3(256), (size_t)0, st, 1, grad_emb, v->d_emb, n));
     APH_LAUNCH_OK();
   }
   const int rc = run_cached(v->bwd_graphs, v->warm_bwd, v->stamp, v->graph_misses, nullptr, nullptr, S, 0, st, [&]() -> int {

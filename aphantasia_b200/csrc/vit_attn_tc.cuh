@@ -357,7 +357,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 4 ? 3 : 1) k_attn_bwd_tc(const 
 // strided list of (sample, head) items and prefetches the NEXT item's tiles into the other half of a double buffer while it
 // computes the current one. The tiles are fetched by TMA (one thread, 3-4 cp.async.bulk.tensor.3d per item, completion on an
 // mbarrier) from a [S][T][cols] view of the token matrix whose out-of-range token rows arrive zero-filled; the per-thread
-// cp.async loop this replaced was 20 % of the backward kernel's instructions (profiles/r1l_ncu_full_summary.md).
+// cp.async loop this replaced was 20 % of the backward kernel's instructions (measured in an earlier version).
 template <int NT2>
 __global__ void __launch_bounds__(128) k_attn_fwd_tc1(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_q,
                                                       bf16* __restrict__ out, int T, int D, int heads, int items) {
@@ -583,12 +583,12 @@ static int attn_launch1(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_o
   if (int e = make_tmap_bf16_tokens(&tm_q, qkv, 3 * D, T, S, 64)) return e;
   if (fwd) {
     const int per_sm = (int)(220 * 1024 / smem_f) < 6 ? (int)(220 * 1024 / smem_f) : 6;
-    const int grid = items < kNumSMs * per_sm ? items : kNumSMs * per_sm;
+    const int grid = items < num_sms() * per_sm ? items : num_sms() * per_sm;
     APH_CUDA_OK(launch_k(k_attn_fwd_tc1<NT2>, dim3(grid), dim3(128), smem_f, st, 1, tm_kv, tm_q, out_or_dqkv, T, D, heads, items));
   } else {
     if (int e = make_tmap_bf16_tokens(&tm_do, dout, D, T, S, 64)) return e;
     const int per_sm = (int)(220 * 1024 / smem_b) < 3 ? (int)(220 * 1024 / smem_b) : 3;
-    const int grid = items < kNumSMs * per_sm ? items : kNumSMs * per_sm;
+    const int grid = items < num_sms() * per_sm ? items : num_sms() * per_sm;
     APH_CUDA_OK(launch_k(k_attn_bwd_tc1<NT2>, dim3(grid), dim3(128), smem_b, st, 1, tm_kv, tm_q, tm_do, out_or_dqkv, T, D, heads, items));
   }
   APH_LAUNCH_OK();

@@ -1,10 +1,9 @@
-// vit_gemm.cu -- host side of the tcgen05 GEMM (tensor-map encoding, launch) + the exported test entry.
+// vit_gemm.cu -- host side of the wgmma GEMM (tensor-map encoding, launch) + the exported test entry.
 #include "tc_gemm.cuh"
 #include <atomic>
 #include <mutex>
 #include <vector>
 #include <utility>
-#include <stdlib.h>
 
 namespace aph {
 
@@ -56,63 +55,34 @@ int make_tmap_bf16_tokens(CUtensorMap* out, const void* base, int cols, int T, i
   return 0;
 }
 
-int make_tmap_epi(CUtensorMap* out, const void* base, int rows, int cols, int elem_bytes) {
-  EncodeTiledFn enc = get_encode();
-  APH_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
-  APH_REQUIRE(elem_bytes == 2 || elem_bytes == 4, "epilogue tensor map: element size %d", elem_bytes);
-  APH_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && ((size_t)cols * elem_bytes) % 16 == 0, "epilogue tensor map: base/stride not 16-byte aligned");
-  const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  const cuuint64_t gstride[1] = {(cuuint64_t)cols * elem_bytes};
-  const cuuint32_t box[2] = {(cuuint32_t)(128 / elem_bytes), 32u};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = enc(out, elem_bytes == 2 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base),
-                         gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  APH_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (epilogue) failed: CUresult %d (rows=%d cols=%d elem=%d)", (int)r, rows, cols, elem_bytes);
-  return 0;
-}
-
 // ---- optional per-launch event timing (bench.py's roofline: the GEMM kernel's real time inside a step)
 static bool g_prof = false;
 bool gemm_profiling_on() { return g_prof; }
 static std::vector<std::pair<cudaEvent_t, cudaEvent_t>> g_prof_ev;
 static std::vector<double> g_prof_flops;
 
-// launches per (tile variant, epilogue kind): variant 0 = 128x128 single CTA, 1 = 128x256 single CTA, 2 = 256x256 CTA pair.
+// launches per (tile variant, epilogue kind): variant 0 = 128x128 tiles, 1 = 128x256 tiles.
 // Read by the tests to prove which kernel a shape really ran (aph_gemm_variant_launches).
-static std::atomic<long long> g_variant_launches[4][EPI_KINDS];
+static std::atomic<long long> g_variant_launches[2][EPI_KINDS];
 
-template <int BN, int EPI, int CG>
+template <int BN, int EPI>
 static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st) {
-  using E = EpiTraits<EPI>;
-  // 384-wide stages are 40 KB; 192-wide ones 28 KB (5 stages beside a 2-deep ring, 4 beside a 3-deep one)
-  constexpr int STAGES = (BN == 384) ? 4 : (BN == 192 ? (E::NBUF == 3 ? 4 : 5) : E::STAGES), NBUF = (BN == 384) ? 2 : E::NBUF;
-  using L = GemmSmem<BN, STAGES, CG, NBUF>;
-  static_assert(L::TOTAL <= 227 * 1024, "GEMM shared-memory budget");
-  g_variant_launches[BN == 384 ? 3 : (BN == 192 ? 1 : (CG == 2 ? 2 : 0))][EPI].fetch_add(1, std::memory_order_relaxed);
+  using L = GemmCfg<BN>;
+  static_assert(L::SMEM <= 227 * 1024, "GEMM shared-memory budget");
+  g_variant_launches[BN == 256 ? 1 : 0][EPI].fetch_add(1, std::memory_order_relaxed);
   static bool configured = false;
   if (!configured) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_gemm_bf16_tn<BN, STAGES, EPI, CG, NBUF>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::TOTAL));
+    APH_CUDA_OK(cudaFuncSetAttribute(k_gemm_bf16_tn<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM));
     configured = true;
   }
-  CUtensorMap ma, mb, mo1, mo2, mop;
+  CUtensorMap ma, mb;
   if (int e = make_tmap_bf16(&ma, A, shp.M, shp.K, GEMM_BM)) return e;
-  if (int e = make_tmap_bf16(&mb, B, shp.N, shp.K, BN == 384 ? 64 : BN / CG)) return e;
-  mo1 = ma; mo2 = ma; mop = ma;                       // placeholders for the maps a kind does not use
-  if (EPI != EPI_UNPATCH) {
-    if (E::OUT16) { if (int e = make_tmap_epi(&mo1, epi.out_bf16, shp.M, shp.N, 2)) return e; }
-    else { if (int e = make_tmap_epi(&mo1, epi.out_f32, shp.M, shp.N, 4)) return e; }
-  }
-  if (EPI == EPI_BIAS_GELU) { if (int e = make_tmap_epi(&mo2, epi.out_pre, shp.M, shp.N, 2)) return e; }
-  if (EPI == EPI_BIAS_RESID) { if (int e = make_tmap_epi(&mop, epi.resid, shp.M, shp.N, 4)) return e; }
-  if (EPI == EPI_GELUGRAD_BF16) { if (int e = make_tmap_epi(&mop, epi.gelu_in, shp.M, shp.N, 2)) return e; }
-  const int tiles = ((shp.M + GEMM_BM * CG - 1) / (GEMM_BM * CG)) * (shp.N / BN);
-  const int slots = kNumSMs / CG;
-  const int groups = tiles < slots ? tiles : slots;
-  const int grid = CG * groups;
+  if (int e = make_tmap_bf16(&mb, B, shp.N, shp.K, BN)) return e;
+  const int tiles = ((shp.M + GEMM_BM - 1) / GEMM_BM) * (shp.N / BN);
+  const int grid = tiles < num_sms() ? tiles : num_sms();
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (g_prof) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, st); }
-  APH_CUDA_OK(launch_k(k_gemm_bf16_tn<BN, STAGES, EPI, CG, NBUF>, dim3(grid), dim3(GEMM_THREADS), (size_t)L::TOTAL, st, CG, ma, mb, mo1, mo2, mop, shp, epi));
+  APH_CUDA_OK(launch_k(k_gemm_bf16_tn<BN, EPI>, dim3(grid), dim3(GEMM_THREADS), (size_t)L::SMEM, st, 1, ma, mb, shp, epi));
   APH_LAUNCH_OK();
   if (g_prof) { cudaEventRecord(e1, st); g_prof_ev.emplace_back(e0, e1); g_prof_flops.push_back(2.0 * shp.M * shp.N * shp.K); }
   return 0;
@@ -133,52 +103,10 @@ int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi,
   else if (f && !h && b && r && !gi && !pre && !act) kind = EPI_BIAS_RESID;
   else if (h && !f && !b && !r && gi && !pre && !act) kind = EPI_GELUGRAD_BF16;
   APH_REQUIRE(kind >= 0, "gemm: unsupported epilogue combination");
-  // CTA-pair tiles (cta_group::2, 256 x 256 accumulator per pair, B tile split across the pair) for problems that fill the
-  // 74 SM pairs; smaller problems keep the finer 128 x 128 single-CTA tiling. APH_GEMM_2CTA=0 forces single-CTA tiles.
-  static int pair = -1;
-  if (pair < 0) { const char* e = getenv("APH_GEMM_2CTA"); pair = (e && e[0] == '0') ? 0 : 1; }
-  // (threshold: from ~40 pair tiles on, one partial round of 256 x 256 pair tiles beats two rounds of 128 x 128 single-CTA tiles, whose
-  // A + B operand reads per MMA exceed the shared-memory bandwidth: the N = 768 GEMMs of a 95-crop shard (N = 2 ranks) have 57)
-  const bool use_pair = pair && shp.N % 256 == 0 && ((shp.M + 255) / 256) * (shp.N / 256) >= 40;
-  // "two exact waves": N = 768-like shapes whose floor(M/256) x N/192 pair tiles of 256 x 192 fill the 74 SM pairs an integral number of
-  // times where 256-wide tiles leave the last wave half empty (M = 9500, N = 768: 37 x 4 = 148 = 2 x 74 instead of 38 x 3 = 114); the
-  // <= 64 remainder rows are computed inside the same kernel by its epilogue warps on the legacy mma.sync path while the main loop runs.
-  // Kinds: the two the N = 768 GEMMs of the encoder use (bf16 out; +bias +fp32 residual).
-  // MEASURED (profiles/README.md, r2m): not a win -- 174.4 vs 176.2 steps/s at C2, the five N = 768 GEMMs within +-3 % of the 256-wide
-  // tiles: an N = 192 instruction needs ~146 B/clk of shared-memory operand reads against 128 available, which eats the 25 % saved
-  // by the exact second wave. Opt-in experiment (APH_GEMM_192=1); parity-tested either way.
-  static int w192 = -1, onewave = -1;
-  if (w192 < 0) { const char* e = getenv("APH_GEMM_192"); w192 = (e && e[0] == '1') ? 1 : 0; }
-  if (onewave < 0) { const char* e = getenv("APH_GEMM_ONEWAVE"); onewave = (e && e[0] == '1') ? 1 : 0; }
-  if (w192 && !onewave && pair && (kind == EPI_BF16 || kind == EPI_BIAS_RESID) && shp.N % 192 == 0 && shp.N % 256 == 0) {
-    const int mt = shp.M / 256, rem = shp.M - mt * 256;
-    const int t192 = mt * (shp.N / 192), t256 = ((shp.M + 255) / 256) * (shp.N / 256), slots = kNumSMs / 2;
-    const int cost192 = ((t192 + slots - 1) / slots) * 192, cost256 = ((t256 + slots - 1) / slots) * 256;
-    if (mt >= 1 && rem <= 64 && t256 >= 40 && cost192 * 100 < cost256 * 88) {       // the narrower instruction reads ~14 % more shared memory per flop
-      GemmShape main_shp{mt * 256, shp.N, shp.K};
-      GemmEpi e2 = epi;
-      e2.tail_a = reinterpret_cast<const bf16*>(A); e2.tail_b = reinterpret_cast<const bf16*>(B); e2.tail_m0 = mt * 256; e2.tail_m = shp.M;
-      return (kind == EPI_BF16) ? launch_cfg<192, EPI_BF16, 2>(A, B, main_shp, e2, st) : launch_cfg<192, EPI_BIAS_RESID, 2>(A, B, main_shp, e2, st);
-    }
-  }
-  // "one-wave" tiles: N a multiple of 384 and floor(M/256) * N/384 pair tiles that fit the 74 SM pairs at once (the N = 768 GEMMs of
-  // ViT-B at M ~ 9500: 37 x 2 = 74). Two 256-wide waves with the second 54 % full become one; the <= 64 remainder rows are computed
-  // inside the same kernel by its epilogue warps (idle during the main loop) on the legacy mma.sync path.
-  // MEASURED (profiles/README.md, r2g): not a win -- 165.0 vs 168.1 steps/s at C2. One 384-wide tile per pair has 25 % less main-loop
-  // work than two 256-wide rounds but its epilogue is fully exposed, the N = 128 second instruction re-reads A from shared memory and
-  // only 4 stages fit. Kept as an opt-in experiment (APH_GEMM_ONEWAVE=1); parity-tested either way.
-  if (onewave && pair && (kind == EPI_BF16 || kind == EPI_BIAS_RESID) && shp.N % 384 == 0) {
-    const int mt = shp.M / 256, rem = shp.M - mt * 256, tiles = mt * (shp.N / 384);
-    if (mt >= 1 && tiles <= kNumSMs / 2 && 2 * tiles > kNumSMs / 2 && rem <= 64) {
-      // the main kernel covers rows [0, mt*256) with TMA-clipped tensor maps; its epilogue warps compute the remainder rows with
-      // mma.sync while the main loop runs (tc_gemm.cuh: gemm_tail_task)
-      GemmShape main_shp{mt * 256, shp.N, shp.K};
-      GemmEpi e2 = epi;
-      e2.tail_a = reinterpret_cast<const bf16*>(A); e2.tail_b = reinterpret_cast<const bf16*>(B); e2.tail_m0 = mt * 256; e2.tail_m = shp.M;
-      return (kind == EPI_BF16) ? launch_cfg<384, EPI_BF16, 2>(A, B, main_shp, e2, st) : launch_cfg<384, EPI_BIAS_RESID, 2>(A, B, main_shp, e2, st);
-    }
-  }
-#define APH_GEMM_CASE(K) case K: return use_pair ? launch_cfg<256, K, 2>(A, B, shp, epi, st) : launch_cfg<128, K, 1>(A, B, shp, epi, st);
+  // 128 x 256 tiles halve the B-operand shared-memory reads per MMA against 128 x 128; they are chosen when there are at least as
+  // many of them as SMs, so that no SM idles (the encoder GEMMs at M ~ 9500 token rows); smaller problems keep the finer tiling.
+  const bool wide = shp.N % 256 == 0 && ((shp.M + GEMM_BM - 1) / GEMM_BM) * (shp.N / 256) >= num_sms();
+#define APH_GEMM_CASE(K) case K: return wide ? launch_cfg<256, K>(A, B, shp, epi, st) : launch_cfg<128, K>(A, B, shp, epi, st);
   switch (kind) {
     APH_GEMM_CASE(EPI_F32) APH_GEMM_CASE(EPI_BF16) APH_GEMM_CASE(EPI_BIAS_BF16) APH_GEMM_CASE(EPI_BIAS_GELU)
     APH_GEMM_CASE(EPI_BIAS_RESID) APH_GEMM_CASE(EPI_GELUGRAD_BF16) APH_GEMM_CASE(EPI_UNPATCH)
@@ -210,10 +138,10 @@ extern "C" int aph_gemm_epi_test(const void* A, const void* B, int M, int N, int
   return launch_gemm(A, B, GemmShape{M, N, K}, epi, (cudaStream_t)stream);
 }
 
-// launches so far of tile variant `variant` (0: 128x128 single CTA, 1: 256x192 pair (two exact waves), 2: 256x256 cta_group::2 pair, 3: 256x384 one-wave pair) with
+// launches so far of tile variant `variant` (0: 128x128 tiles, 1: 128x256 tiles) with
 // epilogue kind `epi` (EPI_* order of tc_gemm.cuh: 0 f32, 1 bf16, 2 bias-bf16, 3 bias-gelu, 4 bias-resid, 5 gelugrad, 6 unpatch; -1 = all)
 extern "C" int64_t aph_gemm_variant_launches(int variant, int epi) {
-  if (variant < 0 || variant > 3 || epi >= EPI_KINDS) return -1;
+  if (variant < 0 || variant > 1 || epi >= EPI_KINDS) return -1;
   long long n = 0;
   for (int k = 0; k < EPI_KINDS; ++k) if (epi < 0 || epi == k) n += g_variant_launches[variant][k].load();
   return (int64_t)n;

@@ -122,7 +122,7 @@ def resume_fft(resume=None, shape=None, decay=None, colors=1.6, sd=0.01):
     elif isinstance(resume, str):
         if os.path.isfile(resume):
             if os.path.splitext(resume)[1].lower()[1:] in ['jpg', 'png', 'tif', 'bmp']:
-                raise NotImplementedError('aphantasia_b200: resuming from an image file (img2fft) is not on the B200 hot path')
+                raise NotImplementedError('aphantasia_b200: resuming from an image file (img2fft) is not on the CUDA hot path')
             params = torch.load(resume)
             if isinstance(params, list): params = params[0]
             params = params.detach().cuda()
@@ -334,7 +334,7 @@ def dwt_image(shape, wave='coif2', sharp=0.3, colors=1., resume=None):
         if not os.path.isfile(resume):
             print(' Snapshot not found:', resume); exit()
         if os.path.splitext(resume)[1].lower()[1:] in ['jpg', 'png', 'tif', 'bmp']:
-            raise NotImplementedError('aphantasia_b200: resuming from an image file (img2dwt) is not on the B200 hot path')
+            raise NotImplementedError('aphantasia_b200: resuming from an image file (img2dwt) is not on the CUDA hot path')
         Ys = [y.detach().cuda() for y in torch.load(resume)]
     else:
         Ys = [y.cuda() for y in resume]

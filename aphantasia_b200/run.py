@@ -1,4 +1,4 @@
-"""Launcher: run an UNMODIFIED reference script (clip_fft.py, illustra.py, ...) against the B200 drop-in.
+"""Launcher: run an UNMODIFIED reference script (clip_fft.py, illustra.py, ...) against the CUDA drop-in.
 
     python -m aphantasia_b200.run /path/to/aphantasia/clip_fft.py -t "red square" --size 1280-720 --samples 200 -nv
     python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 --master-port 29511 \

@@ -3,7 +3,7 @@
 In the reference these are Python closures applied per crop. Here `transforms_fast` and `normalize()` are
 *spec-carrying* callables: slice_imgs recognises them and runs the whole pipeline inside the fused CUDA
 sampler (csrc/sample.cu). The kornia-based pipelines (custom / elastic / lucent / openai) are outside the
-B200 hot path (SURVEY.md section 2.1) and raise when selected.
+CUDA hot path (SURVEY.md section 2.1) and raise when selected.
 """
 import torch
 
@@ -42,7 +42,7 @@ class _Unsupported:
         self.name = name
 
     def __call__(self, x):
-        raise NotImplementedError('aphantasia_b200: transform "%s" needs kornia and is outside the B200 hot path; '
+        raise NotImplementedError('aphantasia_b200: transform "%s" needs kornia and is outside the CUDA hot path; '
                                   'use --transform fast (default) or none' % self.name)
 
 

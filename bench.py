@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- optimisation steps/sec of the Aphantasia hot path (BASELINE.json metric).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (BASELINE.json configs[1]): clip_fft.py --size 1280-720 --samples 200 ViT-B/32 FFT -> S = int(200*0.95) = 190
@@ -14,6 +14,9 @@ data-gradient -> sample bwd -> [all-reduce] -> synth bwd -> Adam.
           model.encode_image / sim_func + loss.backward() + torch.optim.Adam), including per step the host RNG replay,
           the pinned H2D copy of the crop table and a D2H read of the loss.
   --impl reference : the CPU oracle port of the reference path (oracle/restate.py) on the host cores.
+  --dump-outputs DIR : after the timed steps, writes what the last timed device-resident step computed as DIR/<name>.npy
+          (float32): the step's loss, the crop embeddings, the rendered RGB canvas, d loss / d spectrum and the spectrum after
+          the Adam update. Inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 import os as _os
 if _os.environ.get('NCCL_DEBUG', 'VERSION').upper() == 'VERSION':
@@ -36,12 +39,12 @@ sys.path.insert(0, ROOT)
 H, W, SAMPLES_FLAG, MODEL, PATCH = 720, 1280, 200, 'ViT-B/32', 32
 S_TOTAL = int(SAMPLES_FLAG * 0.95)
 F_VIT = {32: 8.8176e9, 16: 35.1269e9}      # forward FLOPs per image (SURVEY.md 8d)
-# one workload string for BOTH arms (the driver compares config.workload of the two lines)
+# one workload string for BOTH arms, so that their result lines can be compared
 WORKLOAD = 'clip_fft.py --size 1280-720 --samples 200 ViT-B/32 FFT: S=190 crops/step, transforms_fast, mix loss, Adam'
 
 
 def vit_gemm_shapes(S, patch=32, D=768, layers=12, out=512, res=224):
-    """(M, N, K) of every tcgen05 GEMM launch of one step (forward + data-gradient)."""
+    """(M, N, K) of every wgmma GEMM launch of one step (forward + data-gradient)."""
     g = res // patch; T = g * g + 1; M = S * T; Mp = S * g * g; Kp = 3 * patch * patch
     fwd = [(Mp, D, Kp)] + layers * [(M, 3 * D, D), (M, D, D), (M, 4 * D, D), (M, D, 4 * D)] + [(S, out, D)]
     bwd = [(S, D, out)] + layers * [(M, 4 * D, D), (M, D, 4 * D), (M, D, D), (M, D, 3 * D)] + [(Mp, Kp, D)]
@@ -49,9 +52,9 @@ def vit_gemm_shapes(S, patch=32, D=768, layers=12, out=512, res=224):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = 'clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,' \
-        'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap'
+        'clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit'
 
     def __init__(self, index=0):
         self.rows, self.proc = [], None
@@ -68,16 +71,18 @@ class ClockSampler:
 
     def stop(self):
         if self.proc is None:
-            return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': ['nvidia-smi unavailable']}
+            return {'sm_mhz': None, 'sm_max_mhz': None, 'power_limit_w': None, 'reasons': ['nvidia-smi unavailable']}
         time.sleep(0.15)
         self.proc.terminate()
-        rows = [r for r in self.rows if len(r) >= 7]
+        self.proc.wait(timeout=5)
+        rows = [r for r in self.rows if len(r) >= 8]
         if not rows:
-            return {'sm_mhz': None, 'sm_max_mhz': None, 'reasons': ['no samples']}
+            return {'sm_mhz': None, 'sm_max_mhz': None, 'power_limit_w': None, 'reasons': ['no samples']}
         sm = sorted(float(r[0]) for r in rows)
         names = ['hw_slowdown', 'hw_thermal_slowdown', 'sw_thermal_slowdown', 'sw_power_cap']
         reasons = [n for i, n in enumerate(names) if any(r[3 + i].lower().startswith('active') for r in rows)]
         return {'sm_mhz': sm[len(sm) // 2], 'sm_max_mhz': float(rows[0][1]), 'power_w_max': max(float(r[2]) for r in rows),
+                'power_limit_w': float(rows[0][7]),
                 'samples': len(rows), 'reasons': reasons}
 
 
@@ -358,6 +363,8 @@ def run_ours(args):
     t_dev = timed(ds.step, K, Wm, barrier)
     launches = (_lib.lib().aph_launch_count() - l0) * K // (K + Wm)
     clk = clocks.stop() if clocks else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(ds, args.dump_outputs)
     # per-stage split + GEMM-kernel timing, measured live right after the timed region (same process, same buffers)
     ds.ev = []
     for i in range(3):
@@ -417,16 +424,15 @@ def run_ours(args):
         for ops in (1, 50):
             d = tempfile.mkdtemp(prefix='aph_bench_')
             try:
-                n = max(K, 50) * (2 if ops == 50 else 1)      # opt_step 50: two previews in the window (one made the 50-step leg noisy)
-                for i in range(5):
+                for i in range(Wm):
                     api.script_step(i, ops, d)
                 _drain_saves(); torch.cuda.synchronize()
                 t0 = time.perf_counter()
-                for i in range(n):
+                for i in range(K):
                     api.script_step(i, ops, d)
                 torch.cuda.synchronize(); _drain_saves()
                 dt = time.perf_counter() - t0
-                script['opt_step_%d' % ops] = {'value': n / dt, 'unit': 'steps/s', 'steps': n, 'frames_written': len(os.listdir(d))}
+                script['opt_step_%d' % ops] = {'value': K / dt, 'unit': 'steps/s', 'steps': K, 'frames_written': len(os.listdir(d))}
             finally:
                 shutil.rmtree(d, ignore_errors=True)
 
@@ -438,36 +444,26 @@ def run_ours(args):
         dist.destroy_process_group()
     if rank != 0:
         return
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json')))
-    except Exception:
-        pass
-    peak_tf = peaks.get('bf16_tflops_sustained', 1400.0)
-    peak_src = 'MEASURED_PEAKS.json bf16_tflops_sustained' if peaks else 'fallback 1.4 PFLOP/s sustained (B200_PROFILING.md)'
+    peak_tf = 989.0
+    peak_src = 'NVIDIA H100 SXM data sheet, dense BF16 at up to 700 W (a ceiling, not a measured rate)'
     flops_vit = 2.0 * (hi - lo) * F_VIT[PATCH]
-    traffic = None
-    try:        # DRAM bytes per launch of the same kernel from the committed ncu capture (cannot be measured outside a profiler)
-        traffic = json.load(open(os.path.join(ROOT, 'profiles', 'r2p_gemm_traffic.json')))['traffic_bytes_per_launch']
-    except Exception:
-        pass
     out = {
         'metric': 'optimization steps/sec @1280x720 FFT, 200 samples, ViT-B/32', 'value': K / t_dev, 'unit': 'steps/s',
         'n_gpus': world, 'steps': K, 'warmup': Wm, 'ms_per_step': 1e3 * t_dev / K, 'higher_is_better': True, 'scaling': 'strong',
         'vs_baseline': None, 'dtype': 'bf16', 'data': 'synthetic (seeded spectrum, seeded synthetic ViT-B/32 weights, seeded text embedding)',
         'config': {'workload': WORKLOAD,
                    'parallelism': ('samples sharded over %d GPU(s), one all-reduce of dRGB per step (%s)' % (world, collective)) if world > 1 else 'single GPU',
-                   'l2': 'working set per step (~1.9 GB of saved activations) exceeds the 126 MB L2; no explicit flush'},
+                   'l2': 'working set per step (~1.9 GB of saved activations) exceeds the 50 MB L2; no explicit flush'},
         'e2e': {'value': K / t_api, 'unit': 'steps/s', 'h2d_bytes_per_step': (hi - lo) * 24 * 4, 'd2h_bytes_per_step': 4,
                 'ms_per_step': 1e3 * t_api / K, 'path': 'fft_image/to_valid_rgb/slice_imgs/encode_image/sim_func + backward + torch.optim.Adam'},
         'e2e_fused_adam': e2e_fused,
         'e2e_script': script or None,
         'gpu_launches': int(launches),
         'clocks': clk,
-        'roofline': {'bound': 'tensor', 'kernel': 'k_gemm_bf16_tn (tcgen05): all %d launches of one step, CUDA-event pair around each launch '
+        'gpu': torch.cuda.get_device_name(local),
+        'roofline': {'bound': 'tensor', 'kernel': 'k_gemm_bf16_tn (wgmma): all %d launches of one step, CUDA-event pair around each launch '
                                                   'inside the running step (real fused epilogues)' % gemm_live['launches'],
-                     'achieved': gemm_live['tflops'], 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': gemm_live['tflops'] / peak_tf, 'traffic': traffic,
-                     'traffic_source': 'profiles/r2p_gemm_traffic.json (ncu --set full: dram__bytes_read+write of the 8 GEMM launches of one transformer layer inside a C2 step, per launch; algorithmic operand+output bytes of the same launches = 87 MB per launch, the difference is absorbed by the 126 MB L2 between consecutive kernels)',
+                     'achieved': gemm_live['tflops'], 'peak': peak_tf, 'unit': 'TFLOP/s', 'frac': gemm_live['tflops'] / peak_tf,
                      'peak_source': peak_src, 'gemm_ms_per_step': gemm_live['ms'],
                      'isolated_plain_epilogue': {'tflops': gemm['tflops'], 'ms_per_step': gemm['ms'], 'per_shape_ms': gemm.get('per_shape_ms')},
                      'vit_step_frac': (flops_vit / (1e-3 * (stages.get('vit_fwd', 0) + stages.get('vit_bwd', 0)) + 1e-12)) / 1e12 / peak_tf},
@@ -491,7 +487,7 @@ def run_ours(args):
 
 
 def time_gemms(ds, S):
-    """Average duration of the step's tcgen05 GEMM launches: each shape of the step replayed on the handle's own
+    """Average duration of the step's wgmma GEMM launches: each shape of the step replayed on the handle's own
     operand-sized buffers with CUDA events on the launching stream (after warm-up)."""
     from aphantasia_b200 import _lib
     lib, ck = _lib.lib(), _lib.check
@@ -515,6 +511,15 @@ def time_gemms(ds, S):
     fl = sum(2.0 * m * n * k for (m, n, k) in shapes)
     return {'ms': ms, 'tflops': fl / (ms * 1e-3) / 1e12, 'launches': len(shapes),
             'per_shape_ms': {'%dx%dx%d' % s: round(v, 4) for s, v in per.items()}}
+
+
+def dump_outputs(ds, out_dir):
+    """What the last step of `ds` computed, as a caller of the device-resident path receives it: DIR/<name>.npy, float32 (~34 MB)."""
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {'loss': -ds.loss.reshape(1), 'embeddings': ds.emb, 'rgb': ds.rgb, 'spectrum_grad': ds.g_params, 'spectrum': ds.params}
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + '.npy'), t.detach().float().cpu().numpy())
 
 
 # =============================================================================================== reference arm
@@ -584,6 +589,7 @@ def _main():
     ap.add_argument('--warmup', type=int, default=3)
     ap.add_argument('--impl', default='ours', choices=['ours', 'reference'])
     ap.add_argument('--config', default='c2', choices=sorted(CONFIGS), help='c2 = the bench line (default); others: supplementary e2e runs')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None, help='write the last timed step\'s outputs as DIR/<name>.npy (float32)')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == 'ours' else args.warmup
     if args.impl == 'ours' and args.config != 'c2':

@@ -1,4 +1,4 @@
-/* aphb200.h -- C ABI of libaphb200.so: the B200-native (sm_100a) hot path of eps696/aphantasia.
+/* aphb200.h -- C ABI of libaphb200.so: the H100-native (sm_90a) hot path of eps696/aphantasia.
  *
  * Drop-in boundary (SURVEY.md section 8b). Plain pointers and sizes only; no torch types. Every compute entry
  * point is asynchronous on the caller's `stream` (pass torch.cuda.current_stream().cuda_stream as void*),
@@ -176,16 +176,15 @@ int aph_vit_bwd(aph_vit* vit, const float* grad_emb, int S, float* grad_images, 
 /* bytes of device memory owned by the handle (weights + activation arena)                          */
 int64_t aph_vit_bytes(const aph_vit* vit);
 
-/* Stand-alone tcgen05 GEMM used by the encoder (exported for tests / profiling):
+/* Stand-alone wgmma GEMM used by the encoder (exported for tests / profiling):
  * C[M,N] (fp32) = A[M,K] (bf16, row-major) . B[N,K]^T (bf16, row-major). K % 64 == 0, N % 128 == 0. */
 int aph_gemm_bf16_tn(const void* A, const void* B, float* C, int M, int N, int K, void* stream);
 
 /* Test entries. aph_gemm_epi_test: the same GEMM with the encoder's fused epilogues on caller-supplied operands
  * (NULL = unused; the combination selects the kind as the encoder's own calls do: +bias, QuickGELU saving the
  * pre-activation (act=1, out_pre), x gelu'(gelu_in), +fp32 resid, fp32 / bf16 outputs, NCHW un-patchify).
- * aph_gemm_variant_launches: launches so far of tile variant 0 (128x128, one CTA), 1 (256x192 pair tiles, two exact waves at
- * N = 768, remainder rows in-kernel), 2 (256x256, cta_group::2 pair) or 3 (256x384 one-wave pair tiles) with epilogue kind epi (0 f32, 1 bf16, 2 bias-bf16, 3 bias-gelu, 4 bias-resid,
- * 5 gelu-grad, 6 un-patchify; -1 = any).                                                             */
+ * aph_gemm_variant_launches: launches so far of tile variant 0 (128x128 tiles) or 1 (128x256 tiles) with epilogue kind epi
+ * (0 f32, 1 bf16, 2 bias-bf16, 3 bias-gelu, 4 bias-resid, 5 gelu-grad, 6 un-patchify; -1 = any).                                                             */
 int aph_gemm_epi_test(const void* A, const void* B, int M, int N, int K, const float* bias, const float* resid,
                       const void* gelu_in, int act, float* out_f32, void* out_bf16, void* out_pre,
                       int unpatch_p, int unpatch_g, void* stream);

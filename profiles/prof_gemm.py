@@ -1,4 +1,4 @@
-"""Stand-alone launcher for ncu captures of the tcgen05 GEMM on the step's shapes (profiles/*.md cite its output)."""
+"""Stand-alone launcher of the wgmma GEMM on the step's shapes: prints time and TFLOP/s per shape (and is a small target for profilers)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

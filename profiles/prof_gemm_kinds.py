@@ -1,10 +1,10 @@
-"""Per-shape / per-epilogue timing of the tcgen05 GEMM against cuBLASLt (torch) on the same shapes, isolated launches.
+"""Per-shape / per-epilogue timing of the wgmma GEMM against cuBLASLt (torch) on the same shapes, isolated launches.
 
-    python profiles/prof_gemm_kinds.py > gpurun_out/gemm_kinds.json
+    python profiles/prof_gemm_kinds.py > gemm_kinds.json
 
 Every GEMM launch of one C2 step (ViT-B/32, S=190: M=9500 token rows) with its real fused epilogue, through the test entry
 aph_gemm_epi_test, 20 timed repetitions after 3 warm-ups (CUDA events on the launching stream). Between repetitions a 256 MB
-buffer is written so the operands do not sit in the 126 MB L2 (flush=1) -- and once more without the flush (what back-to-back
+buffer is written so the operands do not sit in the 50 MB L2 (flush=1) -- and once more without the flush (what back-to-back
 kernels of the step see). The cuBLASLt column is torch's bf16 matmul (+ the UNFUSED epilogue as separate torch ops, which is
 what the reference's PyTorch path launches).
 """

@@ -1,6 +1,6 @@
 """Times the spectrum -> RGB synthesis (forward and backward, C ABI calls on resident buffers) at the BASELINE canvas sizes.
 
-    python profiles/prof_synth.py > gpurun_out/synth_times.json
+    python profiles/prof_synth.py > synth_times.json
 Algorithmic HBM bytes (DESIGN.md 4): forward = params + scale read, x_raw + out written (+ the complex intermediate T written and
 read once, L2-resident at 720p); backward = grad_out + out + x_raw read, grad_params written (+ g_img and T round trips)."""
 import ctypes as C

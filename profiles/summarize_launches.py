@@ -1,7 +1,7 @@
 """Aggregates an `ncu --metrics gpu__time_duration.sum --csv` launch list into per-kernel totals (markdown on stdout).
 
-    python profiles/summarize_launches.py gpurun_out/r2e/launches.csv [steps_in_window]
-Durations are cold-cache, serialised replays: compare SHARES, not absolutes (B200_PROFILING.md)."""
+    python profiles/summarize_launches.py launches.csv [steps_in_window]
+Durations are cold-cache, serialised replays: compare SHARES, not absolutes."""
 import csv
 import re
 import sys

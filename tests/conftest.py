@@ -20,7 +20,7 @@ def _usable_cpus():
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run with -m gpu on the B200 box)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run with -m gpu on an H100)')
     # the oracle runs on the host: a box that shows 100+ cores but grants a small cgroup quota makes torch's default
     # thread pool thrash (one GPU-box run of this suite took 8 min instead of 30 s)
     import torch
@@ -30,4 +30,8 @@ def pytest_configure(config):
 @pytest.fixture(scope='session')
 def golden():
     import numpy as np
-    return np.load(os.path.join(ROOT, 'tests', 'golden', 'reference_golden.npz'))
+    out = {}
+    for name in ('reference_golden.npz', 'reference_golden_sampler.npz'):
+        with np.load(os.path.join(ROOT, 'tests', 'golden', name)) as z:
+            out.update({k: z[k] for k in z.files})
+    return out

@@ -1,12 +1,12 @@
 """Not a pytest module: times the oracle restatement of the reference step as plain PyTorch-eager CUDA ops on the GPU box.
 
-BASELINE.md section 3, item 5 ("second baseline"): the reference has no Blackwell kernels of its own; on a GPU it runs
-as a few hundred ATen launches per crop plus cuBLAS/cuDNN inside CLIP. /root/reference cannot travel to the GPU box, so
+BASELINE.md section 3, item 5 ("second baseline"): the reference has no GPU kernels of its own; on a GPU it runs
+as a few hundred ATen launches per crop plus cuBLAS/cuDNN inside CLIP. the original project is not part of this repository, so
 the op sequence executed here is oracle/restate.py (same per-crop interpolate / grid_sample / normalise loop, same CLIP
 module layout), placed on the device with torch.set_default_device('cuda') -- the device-context mode costs about a
 microsecond per op, small against the ~10 us of an eager launch. CLIP runs in fp16 as clip.load() does on a GPU.
 
-    python tests/eager_gpu_baseline.py [steps] > gpurun_out/eager_gpu_baseline.json
+    python tests/eager_gpu_baseline.py [steps] > eager_gpu_baseline.json
 """
 import json
 import os

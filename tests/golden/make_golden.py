@@ -173,9 +173,12 @@ def main():
     g['chain_grad'] = params[0].grad.numpy().copy()
     g['chain_emb'] = emb.detach().numpy()
 
-    path = os.path.join(OUT, 'reference_golden.npz')
-    np.savez_compressed(path, **g)
-    print('wrote', path, os.path.getsize(path) // 1024, 'KiB,', len(g), 'arrays')
+    # the sampler fixtures go to a file of their own: each file stays under 1 MB
+    for name, keep in (('reference_golden.npz', lambda k: not k.startswith('smp_')), ('reference_golden_sampler.npz', lambda k: k.startswith('smp_'))):
+        path = os.path.join(OUT, name)
+        part = {k: v for k, v in g.items() if keep(k)}
+        np.savez_compressed(path, **part)
+        print('wrote', path, os.path.getsize(path) // 1024, 'KiB,', len(part), 'arrays')
 
 
 if __name__ == '__main__':

@@ -1,9 +1,9 @@
 """GPU parity at the BENCHMARK configuration: the kernels bench.py actually times (VERDICT r1 items 2a-2e).
 
-At S=190 ViT-B/32 (M = 9500 token rows) and S=47 ViT-B/16 (M = 9259) launch_gemm selects the cta_group::2 CTA-pair tiles
-<256,6,K,2> with fused epilogues and the forward / backward launch chains are replayed from the CUDA-graph cache; the
-small-shape tests of test_gpu_parity.py never reach those code paths. Reference call sites: /root/reference/clip_fft.py:254
-(encode_image at S=190), :240 (slice_imgs), :235-295 (whole step). Tolerances: north_star (1e-3 fp32, 2e-2 bf16), norm-wise.
+At S=190 ViT-B/32 (M = 9500 token rows) and S=47 ViT-B/16 (M = 9259) launch_gemm selects the 128 x 256 tiles with fused
+epilogues and the forward / backward launch chains are replayed from the CUDA-graph cache; the small-shape tests of
+test_gpu_parity.py never reach those code paths. Reference call sites: clip_fft.py:254 (encode_image at S=190), :240
+(slice_imgs), :235-295 (whole step). Tolerances: north_star (1e-3 fp32, 2e-2 bf16), norm-wise.
 """
 import ctypes as C
 import os
@@ -46,13 +46,13 @@ def _quickgelu_grad(x):
     return s * (1. + 1.702 * x * (1. - s))
 
 
-# ---------------------------------------------------------------------------------------------- (b) every epilogue kind, pair tiles
+# ---------------------------------------------------------------------------------------------- (b) every epilogue kind, wide tiles
 @pytest.mark.parametrize('kind,M,N,K', [
     ('f32', 9500, 768, 3072),            # d fc1 (ViT-B/32 data-gradient)
     ('bf16', 9500, 768, 768),            # d out_proj
     ('bf16', 9500, 768, 3072),           # d fc1 (bf16 gradient into the LayerNorm backward)
     ('bf16', 9500, 768, 2304),           # d qkv
-    ('bf16', 9259, 768, 768),            # ViT-B/16 batch: 36 x 2 one-wave tiles + 43 remainder rows
+    ('bf16', 9259, 768, 768),            # ViT-B/16 batch: tail tile of 43 rows
     ('bias_bf16', 9500, 2304, 768),      # qkv
     ('bias_gelu', 9500, 3072, 768),      # fc1 + QuickGELU (saves the pre-activation)
     ('bias_resid', 9500, 768, 3072),     # fc2 + residual
@@ -63,6 +63,7 @@ def _quickgelu_grad(x):
     ('gelugrad', 9259, 3072, 768),
     ('unpatch', 9212, 768, 768),         # ViT-B/16: 47 x 196 patches, p=16
 ])
+# test id kept stable across the port: the large-tile variant it checks is now the 128x256 wgmma tile
 def test_pair_gemm_epilogue_kinds_at_bench_size(L, kind, M, N, K):
     lib = L.lib()
     _seed(M + N + K + EPI[kind])
@@ -74,8 +75,8 @@ def test_pair_gemm_epilogue_kinds_at_bench_size(L, kind, M, N, K):
     resid = torch.randn(M, N, device=dev)
     hpre = torch.randn(M, N, device=dev).bfloat16()
     nul = None
-    pair_launches = lambda: sum(lib.aph_gemm_variant_launches(v, EPI[kind]) for v in (1, 2, 3))     # 256x192 / 256x256 / 256x384 pair tiles
-    before = pair_launches()
+    wide_launches = lambda: lib.aph_gemm_variant_launches(1, EPI[kind])     # 128x256 tiles
+    before = wide_launches()
     st = L.stream_ptr()
     if kind == 'f32':
         out = torch.full((M, N), float('nan'), device=dev)
@@ -109,11 +110,7 @@ def test_pair_gemm_epilogue_kinds_at_bench_size(L, kind, M, N, K):
         ref = acc.reshape(S, g, g, 3, p, p).permute(0, 3, 1, 4, 2, 5).reshape(S, 3, 224, 224)
         checks = [(out, ref, 1e-5)]
     torch.cuda.synchronize()
-    assert pair_launches() == before + 1, 'this shape did not run a cta_group::2 pair kernel'
-    if kind in ('bf16', 'bias_resid') and N == 768 and os.environ.get('APH_GEMM_ONEWAVE') == '1':
-        assert lib.aph_gemm_variant_launches(3, EPI[kind]) >= 1, 'N = 768 at this M should take the one-wave 256x384 tiles (+ in-kernel remainder rows)'
-    elif kind in ('bf16', 'bias_resid') and N == 768 and os.environ.get('APH_GEMM_192') == '1':
-        assert lib.aph_gemm_variant_launches(1, EPI[kind]) >= 1, 'N = 768 at this M should take the 256x192 pair tiles (two exact waves + in-kernel remainder rows)'
+    assert wide_launches() == before + 1, 'this shape did not run the 128x256-tile kernel'
     for got, want, tol in checks:
         assert torch.isfinite(got).all()
         assert _rel(got, want) < tol, (kind, M, N, K, _rel(got, want))
@@ -139,8 +136,8 @@ def test_vit_at_bench_batch_vs_oracle_incl_graph_replay(L, patch, S):
     (eo * cot).sum().backward()
     xc, gc = x.cuda(), cot.cuda()
     emb = torch.empty(S, 512, device='cuda'); gx = torch.empty(S, 3, 224, 224, device='cuda')
-    pairs = lambda: sum(lib.aph_gemm_variant_launches(v, -1) for v in (1, 2, 3))
-    pair_before = pairs()
+    wides = lambda: lib.aph_gemm_variant_launches(1, -1)
+    wide_before = wides()
     errs = []
     for it in range(3):
         emb.fill_(float('nan')); gx.fill_(float('nan'))
@@ -148,7 +145,7 @@ def test_vit_at_bench_batch_vs_oracle_incl_graph_replay(L, patch, S):
         L.check(lib.aph_vit_bwd(vis.handle, gc.data_ptr(), S, gx.data_ptr(), L.stream_ptr()), 'vit_bwd')
         torch.cuda.synchronize()
         if it == 0:
-            assert pairs() - pair_before >= 90, 'the cta_group::2 pair kernels were not selected at this batch'
+            assert wides() - wide_before >= 90, 'the 128x256-tile kernels were not selected at this batch'
         errs.append((_rel(emb, eo), _rel(gx, xo.grad)))
     print('vit B/%d S=%d: rel err (emb, grad) eager %s capture %s replay %s' % (patch, S, errs[0], errs[1], errs[2]))
     for e_emb, e_grad in errs:

@@ -34,7 +34,7 @@ def L():
 
 # ---------------------------------------------------------------------------------------------- GEMM
 @pytest.mark.parametrize('M,N,K', [(128, 128, 64), (256, 256, 128), (300, 384, 192), (1000, 768, 3072), (9500, 2304, 768), (190, 512, 768)])
-def test_tcgen05_gemm(L, M, N, K):
+def test_tcgen05_gemm(L, M, N, K):     # test id kept stable across the port; the kernel under test is the wgmma GEMM
     _seed(M + N + K)
     a = torch.randn(M, K, device='cuda').bfloat16()
     b = torch.randn(N, K, device='cuda').bfloat16()

@@ -194,11 +194,14 @@ def test_launcher_shadows_a_package_sitting_next_to_the_script(tmp_path):
     assert 'aphantasia -> %s' % os.path.join(ROOT, 'dropin', 'aphantasia') in out.stderr
 
 
-@pytest.mark.skipif(not os.path.isfile('/root/reference/clip_fft.py'), reason='the reference tree only exists in the build container')
+_REF_TREE = os.path.join(ROOT, 'oracle', '_ref')        # the original clip_fft.py + aphantasia/ as build() staged them
+
+
+@pytest.mark.skipif(not os.path.isfile(os.path.join(_REF_TREE, 'clip_fft.py')), reason='no copy of the original project: build() stages one into oracle/_ref/')
 def test_launcher_runs_the_real_clip_fft_imports():
-    """The unmodified /root/reference/clip_fft.py, started from INSIDE the reference tree: all of its top-level imports
-    (clip_fft.py:1-31) must resolve through the drop-in (argparse --help exits before any GPU work)."""
-    out = _run_launcher('/root/reference/clip_fft.py', ['--help'], cwd='/root/reference')
+    """The unmodified clip_fft.py, started from INSIDE a tree with the original `aphantasia/` package beside it: all of its
+    top-level imports (clip_fft.py:1-31) must resolve through the drop-in (argparse --help exits before any GPU work)."""
+    out = _run_launcher(os.path.join(_REF_TREE, 'clip_fft.py'), ['--help'], cwd=_REF_TREE)
     assert out.returncode == 0, out.stderr[-3000:]
     assert '--samples' in out.stdout and '--dualmod' in out.stdout
     assert 'aphantasia -> %s' % os.path.join(ROOT, 'dropin', 'aphantasia') in out.stderr

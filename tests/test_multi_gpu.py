@@ -1,6 +1,6 @@
 """Multi-GPU parity (SURVEY.md 4 "distributed" row, 8e): an N-rank run (crops sharded, one all-reduce of dRGB) must reproduce the
 1-rank run on the same seeds -- loss, d loss / d spectrum and the spectrum after two Adam steps. Needs >= 2 GPUs
-(`gpurun --gpus N -- python -m pytest tests/test_multi_gpu.py -m gpu`); skipped on a one-GPU box.
+(`python -m pytest tests/test_multi_gpu.py -m gpu` on a machine with N GPUs); skipped on a one-GPU machine.
 
 Tolerances. A rank's loss is the mean over ITS crops, so its backward runs with gradients S/S_local times larger than the 1-rank
 run's and is rescaled afterwards. With EVEN shards and a power-of-two rank count that factor is a power of two: every bf16

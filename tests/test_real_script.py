@@ -1,7 +1,7 @@
-"""GPU integration: the UNMODIFIED reference script /root/reference/clip_fft.py executed end to end against libaphb200.so
-through the launcher (python -m aphantasia_b200.run), SURVEY.md 8(b). /root/reference does not exist on the GPU box: for a
-gpurun call the file is staged, untracked, as scratch_ref/clip_fft.py (`mkdir -p scratch_ref && cp /root/reference/clip_fft.py
-scratch_ref/`; scratch_ref/ is git-ignored, never committed). Skipped when no copy of the script is reachable."""
+"""GPU integration: the UNMODIFIED clip_fft.py of eps696/aphantasia executed end to end against libaphb200.so through the
+launcher (python -m aphantasia_b200.run), SURVEY.md 8(b). The script belongs to the original project and is not part of this
+repository: build() stages a copy into the git-ignored oracle/_ref/ (oracle/stage_ref.py) when the original project is readable,
+APH_REF_SCRIPT may name another copy, and without either these tests are skipped."""
 import glob
 import json
 import os
@@ -12,9 +12,8 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-_CANDIDATES = [os.environ.get('APH_REF_SCRIPT'), '/root/reference/clip_fft.py', os.path.join(ROOT, 'scratch_ref', 'clip_fft.py')]
-SCRIPT = next((p for p in _CANDIDATES if p and os.path.isfile(p)), None)
-needs_script = pytest.mark.skipif(SCRIPT is None, reason='no copy of the reference clip_fft.py reachable (stage it under scratch_ref/)')
+SCRIPT = os.environ.get('APH_REF_SCRIPT') or os.path.join(ROOT, 'oracle', '_ref', 'clip_fft.py')
+needs_script = pytest.mark.skipif(not os.path.isfile(SCRIPT), reason='no copy of the original clip_fft.py: build() stages one into oracle/_ref/')
 
 
 def _run(tmp_path, args, env_add=None, nproc=1):
