@@ -3,20 +3,24 @@
 `model.visual.input_resolution`.
 
 The image encoder (ViT-B/32, ViT-B/16) runs forward and data-gradient in libaphb200.so (csrc/vit.cu: wgmma
-GEMMs + fused kernels). Weights: an OpenAI state dict if `APH_CLIP_WEIGHTS=<file.pt>` is set, else seeded
-synthetic weights of the same architecture (there are no CLIP weights or network in this environment).
-The text encoder runs once before the optimisation loop and is not part of the hot path: without real weights
-`encode_text` returns a deterministic seeded embedding per prompt (loudly).
+GEMMs + fused kernels). Weights: an OpenAI state dict if `APH_CLIP_WEIGHTS=<file.pt>` is set (a TorchScript archive as
+OpenAI ships them, or a plain state dict), else seeded synthetic weights of the same architecture.
+The text encoder (csrc/text.cu, forward only) runs once per prompt before the optimisation loop when the weights hold
+the text tower; `tokenize` uses CLIP's BPE vocabulary from `APH_CLIP_BPE=<bpe_simple_vocab_16e6.txt.gz>` or from that
+file next to the weights. Without text weights `encode_text` returns a deterministic seeded embedding per prompt, and
+without a vocabulary `tokenize` encodes the prompt's UTF-8 bytes (both loudly).
 """
 import ctypes as C
 import hashlib
 import os
+import zipfile
 from collections import OrderedDict
 
 import torch
 
 from .. import _patchlink, _pool, _trace
-from .._lib import VitConfig, check, lib, require_cuda, stream_ptr
+from .._lib import TextConfig, VitConfig, check, lib, require_cuda, stream_ptr
+from ._bpe import SimpleTokenizer
 
 _MODELS = {'ViT-B/32': dict(patch=32, width=768, layers=12, heads=12, out_dim=512, res=224),
            'ViT-B/16': dict(patch=16, width=768, layers=12, heads=12, out_dim=512, res=224)}
@@ -57,6 +61,102 @@ def synthetic_visual_state_dict(patch=32, width=768, layers=12, heads=12, out_di
         sd[p + 'mlp.c_proj.bias'] = uni((width,), (4 * width) ** -0.5)
         sd[p + 'ln_2.weight'] = torch.ones(width); sd[p + 'ln_2.bias'] = torch.zeros(width)
     return sd
+
+
+_TEXT_KEYS = ('token_embedding.weight', 'positional_embedding', 'ln_final.weight', 'ln_final.bias', 'text_projection')
+
+
+def synthetic_text_state_dict(width=512, layers=12, heads=8, out_dim=512, context=77, vocab=49408, seed=0):
+    """Seeded synthetic text-tower weights in the OpenAI key layout (OpenAI's init scales; LayerNorm affines perturbed so that
+    a swapped or dropped LayerNorm shows in a comparison)."""
+    assert heads * 64 == width, 'the text tower has head dim 64'
+    g = torch.Generator().manual_seed(seed)
+
+    def uni(shape, bound):
+        return (torch.rand(shape, generator=g) * 2 - 1) * bound
+
+    def nrm(shape, std):
+        return torch.randn(shape, generator=g) * std
+    sd = OrderedDict()
+    sd['token_embedding.weight'] = nrm((vocab, width), 0.02)
+    sd['positional_embedding'] = nrm((context, width), 0.01)
+    sd['text_projection'] = nrm((width, out_dim), width ** -0.5)
+    sd['ln_final.weight'] = 1 + uni((width,), 0.1); sd['ln_final.bias'] = uni((width,), 0.1)
+    for i in range(layers):
+        p = 'transformer.resblocks.%d.' % i
+        sd[p + 'attn.in_proj_weight'] = uni((3 * width, width), (6. / (4 * width)) ** 0.5)
+        sd[p + 'attn.in_proj_bias'] = uni((3 * width,), 0.02)
+        sd[p + 'attn.out_proj.weight'] = uni((width, width), width ** -0.5)
+        sd[p + 'attn.out_proj.bias'] = uni((width,), 0.02)
+        sd[p + 'ln_1.weight'] = 1 + uni((width,), 0.1); sd[p + 'ln_1.bias'] = uni((width,), 0.1)
+        sd[p + 'mlp.c_fc.weight'] = uni((4 * width, width), width ** -0.5)
+        sd[p + 'mlp.c_fc.bias'] = uni((4 * width,), width ** -0.5)
+        sd[p + 'mlp.c_proj.weight'] = uni((width, 4 * width), (4 * width) ** -0.5)
+        sd[p + 'mlp.c_proj.bias'] = uni((width,), (4 * width) ** -0.5)
+        sd[p + 'ln_2.weight'] = 1 + uni((width,), 0.1); sd[p + 'ln_2.bias'] = uni((width,), 0.1)
+    return sd
+
+
+def has_text_tower(state_dict):
+    return all(k in state_dict for k in _TEXT_KEYS) and 'transformer.resblocks.0.attn.in_proj_weight' in state_dict
+
+
+class TextTransformer:
+    """Handle-owning forward of clip.model.CLIP's text tower (token embedding -> causal transformer -> ln_final at the
+    end-of-text position -> text_projection) through the C ABI. The handle is created on the first call (constructing a
+    CLIP needs no GPU) and re-created when a call brings more prompts than it was sized for."""
+
+    def __init__(self, state_dict):
+        sd = {k: v for k, v in state_dict.items() if k in _TEXT_KEYS or k.startswith('transformer.resblocks.')}
+        self.vocab, self.width = sd['token_embedding.weight'].shape
+        self.context = sd['positional_embedding'].shape[0]
+        self.layers = len([k for k in sd if k.endswith('.attn.in_proj_weight')])
+        self.heads = self.width // 64
+        self.output_dim = sd['text_projection'].shape[1]
+        self._sd = {k: v.detach().float().contiguous() for k, v in sd.items()}
+        self.handle, self.max_batch = None, 0
+
+    def _ensure(self, n):
+        if self.handle is not None and n <= self.max_batch:
+            return
+        self.close()
+        cfg = TextConfig(self.width, self.layers, self.heads, self.output_dim, self.context, self.vocab, int(n), 0)
+        h = C.c_void_p()
+        check(lib().aph_text_create(C.byref(h), C.byref(cfg)), 'aph_text_create')
+        self.handle = h            # owned from here on: a failed load below still frees it in close()
+        st = stream_ptr()
+        for k, v in self._sd.items():
+            d = v.cuda()
+            check(lib().aph_text_load_tensor(h, k.encode(), d.data_ptr(), d.numel(), st), 'aph_text_load_tensor(%s)' % k)
+        torch.cuda.current_stream().synchronize()      # staging copies `d` die with this scope
+        check(lib().aph_text_finalize(h), 'aph_text_finalize')
+        self.max_batch = int(n)
+
+    def close(self):
+        if self.handle is not None:
+            lib().aph_text_destroy(self.handle)
+            self.handle, self.max_batch = None, 0
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @torch.no_grad()
+    def __call__(self, tokens):
+        require_cuda(tokens, 'encode_text tokens')
+        if tokens.dim() != 2 or tokens.shape[1] != self.context:
+            raise ValueError('encode_text: tokens must be [n, %d], got %s' % (self.context, tuple(tokens.shape)))
+        t = tokens.detach().to(torch.int64).contiguous()
+        lo, hi = (int(v) for v in torch.stack((t.min(), t.max())).cpu())     # one host read per prompt batch, before the loop
+        if lo < 0 or hi >= self.vocab:
+            raise ValueError('encode_text: token ids must lie in [0, %d), got [%d, %d]' % (self.vocab, lo, hi))
+        n = t.shape[0]
+        self._ensure(n)
+        emb = torch.empty(n, self.output_dim, device=t.device, dtype=torch.float32)
+        check(lib().aph_text_fwd(self.handle, t.data_ptr(), n, emb.data_ptr(), stream_ptr()), 'aph_text_fwd')
+        return emb
 
 
 class _EncodeImage(torch.autograd.Function):
@@ -163,12 +263,18 @@ class CLIP:
         self.name, self.synthetic = name, synthetic
         self.visual = VisionTransformer(state_dict)
         self.embed_dim = self.visual.output_dim
+        self.transformer = TextTransformer(state_dict) if has_text_tower(state_dict) else None
+        _trace.text_tower('cuda' if self.transformer is not None else 'stand-in')
 
     def encode_image(self, image):
         return self.visual(image)
 
     def encode_text(self, tokens):
-        """Deterministic seeded stand-in (no text-tower weights / BPE vocab in this environment), unit norm x 10."""
+        """With text-tower weights: the CLIP text encoder on the GPU (tokens: CUDA [n, context]) -> [n, embed_dim] fp32, no
+        grad. Without them: a deterministic seeded stand-in per token row set, unit norm x 10."""
+        _trace.encode_text()
+        if self.transformer is not None:
+            return self.transformer(tokens)
         dev = tokens.device
         digest = hashlib.sha256(tokens.detach().cpu().numpy().tobytes() + self.name.encode()).digest()
         g = torch.Generator().manual_seed(int.from_bytes(digest[:7], 'little'))
@@ -186,28 +292,91 @@ class CLIP:
         return self
 
 
+VOCAB_FILE = 'bpe_simple_vocab_16e6.txt.gz'
+_weights_dir = None          # directory of the weights file load() used last: its VOCAB_FILE is the default vocabulary
+_tokenizers = {}
+
+
+def vocab_path():
+    """The BPE vocabulary in use: APH_CLIP_BPE, else VOCAB_FILE next to the loaded weights, else None (byte-level stand-in)."""
+    p = os.environ.get('APH_CLIP_BPE')
+    if p:
+        if not os.path.isfile(p):
+            raise RuntimeError('aphantasia_b200.clip: APH_CLIP_BPE=%s is not a file' % p)
+        return p
+    if _weights_dir is not None and os.path.isfile(os.path.join(_weights_dir, VOCAB_FILE)):
+        return os.path.join(_weights_dir, VOCAB_FILE)
+    return None
+
+
+def _tokenizer():
+    p = vocab_path()
+    if p is None:
+        return None
+    if p not in _tokenizers:
+        _tokenizers[p] = SimpleTokenizer(p)
+    return _tokenizers[p]
+
+
 def tokenize(texts, context_length=77, truncate=False):
-    """Byte-level stand-in for clip.tokenize: LongTensor [n, 77] (start 49406, bytes, end 49407, zero padded)."""
+    """clip.tokenize: LongTensor [n, context_length] = [sot] + BPE ids + [eot], zero padded. RuntimeError when a prompt does
+    not fit and truncate is False; truncate=True cuts it and ends it with eot.
+    Without a vocabulary (see vocab_path): the byte-level stand-in (start 49406, UTF-8 bytes, end 49407, cut to fit)."""
     if isinstance(texts, str):
         texts = [texts]
+    tok = _tokenizer()
     out = torch.zeros(len(texts), context_length, dtype=torch.long)
+    if tok is None:
+        for i, t in enumerate(texts):
+            b = list(t.encode('utf-8'))[:context_length - 2]
+            toks = [49406] + b + [49407]
+            out[i, :len(toks)] = torch.tensor(toks)
+        return out
     for i, t in enumerate(texts):
-        b = list(t.encode('utf-8'))[:context_length - 2]
-        toks = [49406] + b + [49407]
+        toks = [tok.sot] + tok.encode(t) + [tok.eot]
+        if len(toks) > context_length:
+            if not truncate:
+                raise RuntimeError('Input %s is too long for context length %d' % (t, context_length))
+            toks = toks[:context_length]
+            toks[-1] = tok.eot
         out[i, :len(toks)] = torch.tensor(toks)
     return out
 
 
+def _read_weights(path):
+    """OpenAI's TorchScript archive (torch.load refuses those under weights_only) or a plain state dict -> fp32 state dict
+    without the JIT model's non-tensor attributes."""
+    if _is_torchscript(path):
+        sd = torch.jit.load(path, map_location='cpu').state_dict()
+    else:
+        sd = torch.load(path, map_location='cpu')
+        if hasattr(sd, 'state_dict'):
+            sd = sd.state_dict()
+    return OrderedDict((k, v.float() if v.is_floating_point() else v) for k, v in sd.items()
+                       if k not in ('input_resolution', 'context_length', 'vocab_size'))
+
+
+def _is_torchscript(path):
+    """torch.jit.save archives carry compiled code and a constants table; torch.save archives do not."""
+    if not zipfile.is_zipfile(path):
+        return False
+    with zipfile.ZipFile(path) as z:
+        return any(n.endswith('/constants.pkl') for n in z.namelist())
+
+
 def load(name, device=None, jit=False, download_root=None):
     """clip.load: returns (model, preprocess). `preprocess` is unused by the scripts (None)."""
+    global _weights_dir
     if name not in _MODELS:
         raise RuntimeError('aphantasia_b200.clip: model %s not available (the CUDA hot path covers %s)' % (name, available_models()))
     path = os.environ.get('APH_CLIP_WEIGHTS_' + name.replace('/', '').replace('-', '').upper(), os.environ.get('APH_CLIP_WEIGHTS'))
     if path and os.path.isfile(path):
-        sd = torch.load(path, map_location='cpu')
-        if hasattr(sd, 'state_dict'):
-            sd = sd.state_dict()
+        sd = _read_weights(path)
         synthetic = False
+        _weights_dir = os.path.dirname(os.path.abspath(path))
+        if has_text_tower(sd) and vocab_path() is None:
+            print(' [aphantasia_b200.clip] WARNING: no BPE vocabulary (set APH_CLIP_BPE=<%s> or put it next to %s): prompts will be '
+                  'byte-tokenized and the text encoder will not see CLIP tokens' % (VOCAB_FILE, path))
     else:
         sd = synthetic_visual_state_dict(seed=int(os.environ.get('APH_CLIP_SEED', '0')), **_MODELS[name])
         synthetic = True

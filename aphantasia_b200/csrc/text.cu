@@ -1,0 +1,279 @@
+// text.cu -- CLIP text encoder handle (forward only): fp32 token embedding, packed bf16 layer weights, one set of
+// activation buffers, built from the image tower's pieces (wgmma GEMM with fused epilogues, k_ln_fwd, tensor-core attention).
+//
+// Restates OpenAI clip/model.py CLIP.encode_text (third-party, SURVEY.md A5):
+//   x = token_embedding[ids] + positional_embedding -> layers x { x += out_proj(causal MHA(ln_1 x)); x += c_proj(QuickGELU(c_fc(ln_2 x))) }
+//   -> ln_final(x[s, argmax(ids[s])]) @ text_projection
+// It runs a handful of times per script run (once per prompt, before the optimisation loop): no CUDA graph, nothing is
+// saved for a backward pass, and each layer overwrites the previous one's activations.
+#include "vit_ops.cuh"
+#include "vit_attn_tc.cuh"
+#include <stdlib.h>
+#include <string.h>
+#include <map>
+#include <string>
+#include <vector>
+
+namespace aph {
+
+int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st);   // vit.cu
+int copy_f32(const float* src, float* dst, size_t n, cudaStream_t st);                      // vit.cu
+
+namespace {
+
+struct TextLayer {
+  float *ln1_w = nullptr, *ln1_b = nullptr, *ln2_w = nullptr, *ln2_b = nullptr;
+  float *b_qkv = nullptr, *b_o = nullptr, *b_fc = nullptr, *b_proj = nullptr;
+  bf16 *w_qkv = nullptr, *w_o = nullptr, *w_fc = nullptr, *w_proj = nullptr;   // forward B operands [N, K]
+};
+
+struct TextImpl {
+  aph_text_config cfg;
+  int64_t bytes = 0;
+  std::vector<void*> allocs;
+  // weights
+  float* tok_emb = nullptr;      // [vocab, D] fp32: a gather reads n*ctx rows of it once per call
+  float* pos = nullptr;          // [ctx, D]
+  float *lnf_w = nullptr, *lnf_b = nullptr;
+  bf16* w_out = nullptr;         // text_projection^T [out, D]
+  std::vector<TextLayer> L;
+  std::map<std::string, bool> loaded;
+  bool finalized = false;
+  // activations, sized for max_batch * ctx rows
+  float *x = nullptr, *x_mid = nullptr;   // residual stream fp32 [M, D], ping-pong within a layer
+  bf16* ln_out = nullptr;        // [M, D]
+  bf16* qkv = nullptr;           // [M, 3D]
+  bf16* attn_out = nullptr;      // [M, D]
+  bf16* h_pre = nullptr;         // [M, 4D] (the fused QuickGELU epilogue always writes its pre-activation)
+  bf16* h_act = nullptr;         // [M, 4D]
+  float *mean = nullptr, *rstd = nullptr;  // [M] LayerNorm statistics (written by k_ln_fwd, unused here)
+  int* eot = nullptr;            // [max_batch] pooling position per sequence
+  bf16* pooled = nullptr;        // [max_batch, D] ln_final of the pooled rows
+};
+
+template <typename Tp>
+int dev_alloc(TextImpl* t, Tp** p, size_t count) {
+  void* q = nullptr;
+  APH_CUDA_OK(cudaMalloc(&q, count * sizeof(Tp)));
+  t->allocs.push_back(q);
+  t->bytes += (int64_t)(count * sizeof(Tp));
+  *p = reinterpret_cast<Tp*>(q);
+  return 0;
+}
+
+inline int rows_grid(int rows) { return (rows * 32 + 255) / 256; }
+
+// x[row] = token_embedding[ids[row]] + positional_embedding[row % ctx]; one warp per token row.
+// An id outside [0, vocab) contributes a zero row instead of reading out of bounds.
+template <int NCH>
+__global__ void __launch_bounds__(256) k_text_embed(const int64_t* __restrict__ ids, const float* __restrict__ tok_emb,
+                                                    const float* __restrict__ pos, float* __restrict__ x, int rows, int ctx, int D, int vocab) {
+  pdl_trigger(); pdl_wait();
+  const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (row >= rows) return;
+  constexpr int N = 4 * NCH;
+  const long long id = ids[row];
+  float v[N], pz[N];
+  load_row(pos + (size_t)(row % ctx) * D, pz, lane);
+  if (id >= 0 && id < vocab) load_row(tok_emb + (size_t)id * D, v, lane);
+  else {
+#pragma unroll
+    for (int i = 0; i < N; ++i) v[i] = 0.f;
+  }
+#pragma unroll
+  for (int i = 0; i < N; ++i) v[i] += pz[i];
+  store_row_f32(x + (size_t)row * D, v, lane);
+}
+
+// eot[s] = first position of the largest id of sequence s (torch.argmax semantics); one warp per sequence.
+__global__ void __launch_bounds__(256) k_text_eot(const int64_t* __restrict__ ids, int* __restrict__ eot, int n, int ctx) {
+  pdl_trigger(); pdl_wait();
+  const int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (s >= n) return;
+  long long best = ids[(size_t)s * ctx];
+  int bi = 0;
+  for (int t = lane; t < ctx; t += 32) {
+    const long long v = ids[(size_t)s * ctx + t];
+    if (v > best) { best = v; bi = t; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const long long ob = __shfl_xor_sync(0xffffffffu, best, o);
+    const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+    if (ob > best || (ob == best && oi < bi)) { best = ob; bi = oi; }
+  }
+  if (lane == 0) eot[s] = bi;
+}
+
+// y[s] = ln_final(x[s * ctx + eot[s]]) as bf16 (the A operand of the projection GEMM); one warp per sequence.
+template <int NCH>
+__global__ void __launch_bounds__(256) k_text_pool_ln(const float* __restrict__ x, const int* __restrict__ eot, const float* __restrict__ gamma,
+                                                      const float* __restrict__ beta, bf16* __restrict__ y, int n, int ctx, int D) {
+  pdl_trigger(); pdl_wait();
+  const int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (s >= n) return;
+  constexpr int N = 4 * NCH;
+  float v[N], gm[N], bt[N];
+  load_row(x + ((size_t)s * ctx + eot[s]) * D, v, lane);
+  const RowStats st = row_stats(v, D);
+  load_row(gamma, gm, lane); load_row(beta, bt, lane);
+#pragma unroll
+  for (int i = 0; i < N; ++i) v[i] = (v[i] - st.mean) * st.rstd * gm[i] + bt[i];
+  store_row_bf16(y + (size_t)s * D, v, lane);
+}
+
+// causal tensor-core attention: the image tower's forward kernel with the mask compiled in
+template <int NW, int NT2>
+int attn_causal_launch(const bf16* qkv, bf16* out, int S, int T, int D, int heads, cudaStream_t st) {
+  static bool cfg = false;
+  if (!cfg) {
+    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd_tc<NW, NT2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_tc_fwd_smem<NW, NT2>()));
+    cfg = true;
+  }
+  APH_CUDA_OK(launch_k(k_attn_fwd_tc<NW, NT2, true>, dim3(S * heads), dim3(NW * 32), attn_tc_fwd_smem<NW, NT2>(), st, 1, qkv, out, T, D, heads));
+  APH_LAUNCH_OK();
+  return 0;
+}
+
+int attn_causal(const bf16* qkv, bf16* out, int S, int T, int D, int heads, cudaStream_t st) {
+  if (T <= 32) return attn_causal_launch<4, 2>(qkv, out, S, T, D, heads, st);
+  if (T <= 64) return attn_causal_launch<4, 4>(qkv, out, S, T, D, heads, st);
+  if (T <= 112) return attn_causal_launch<8, 7>(qkv, out, S, T, D, heads, st);
+  set_error("text attention: context %d > 112 unsupported", T);
+  return 2;
+}
+
+}  // namespace
+}  // namespace aph
+
+using namespace aph;
+
+extern "C" int aph_text_create(aph_text** out, const aph_text_config* cfg) {
+  APH_REQUIRE(out && cfg, "aph_text_create: null argument");
+  const int w128 = cfg->width / 128;
+  APH_REQUIRE(cfg->width % 128 == 0 && (w128 == 1 || w128 == 2 || w128 == 4 || w128 == 6 || w128 == 8),
+              "aph_text_create: width %d unsupported (128, 256, 512, 768, 1024)", cfg->width);
+  APH_REQUIRE(cfg->heads * 64 == cfg->width, "aph_text_create: head dim must be 64 (width %d, heads %d)", cfg->width, cfg->heads);
+  APH_REQUIRE(cfg->context > 0 && cfg->context <= 112, "aph_text_create: context %d outside [1, 112]", cfg->context);
+  APH_REQUIRE(cfg->out_dim > 0 && cfg->out_dim % 128 == 0, "aph_text_create: out_dim %d must be a multiple of 128", cfg->out_dim);
+  APH_REQUIRE(cfg->vocab > 0 && cfg->max_batch > 0 && cfg->layers > 0, "aph_text_create: vocab %d, max_batch %d, layers %d must be positive",
+              cfg->vocab, cfg->max_batch, cfg->layers);
+  TextImpl* t = new TextImpl();
+  t->cfg = *cfg;
+  const int D = cfg->width, O = cfg->out_dim, B = cfg->max_batch;
+  const size_t M = (size_t)B * cfg->context;
+  int e = 0;
+  e |= dev_alloc(t, &t->tok_emb, (size_t)cfg->vocab * D); e |= dev_alloc(t, &t->pos, (size_t)cfg->context * D);
+  e |= dev_alloc(t, &t->lnf_w, D); e |= dev_alloc(t, &t->lnf_b, D); e |= dev_alloc(t, &t->w_out, (size_t)O * D);
+  t->L.resize(cfg->layers);
+  for (auto& l : t->L) {
+    e |= dev_alloc(t, &l.ln1_w, D); e |= dev_alloc(t, &l.ln1_b, D); e |= dev_alloc(t, &l.ln2_w, D); e |= dev_alloc(t, &l.ln2_b, D);
+    e |= dev_alloc(t, &l.b_qkv, 3 * D); e |= dev_alloc(t, &l.b_o, D); e |= dev_alloc(t, &l.b_fc, 4 * D); e |= dev_alloc(t, &l.b_proj, D);
+    e |= dev_alloc(t, &l.w_qkv, (size_t)3 * D * D); e |= dev_alloc(t, &l.w_o, (size_t)D * D);
+    e |= dev_alloc(t, &l.w_fc, (size_t)4 * D * D); e |= dev_alloc(t, &l.w_proj, (size_t)4 * D * D);
+  }
+  e |= dev_alloc(t, &t->x, M * D); e |= dev_alloc(t, &t->x_mid, M * D); e |= dev_alloc(t, &t->ln_out, M * D);
+  e |= dev_alloc(t, &t->qkv, M * 3 * D); e |= dev_alloc(t, &t->attn_out, M * D);
+  e |= dev_alloc(t, &t->h_pre, M * 4 * D); e |= dev_alloc(t, &t->h_act, M * 4 * D);
+  e |= dev_alloc(t, &t->mean, M); e |= dev_alloc(t, &t->rstd, M);
+  e |= dev_alloc(t, &t->eot, (size_t)B); e |= dev_alloc(t, &t->pooled, (size_t)B * D);
+  if (e) { aph_text_destroy(reinterpret_cast<aph_text*>(t)); return 1; }
+  *out = reinterpret_cast<aph_text*>(t);
+  return 0;
+}
+
+extern "C" int aph_text_destroy(aph_text* text) {
+  if (!text) return 0;
+  TextImpl* t = reinterpret_cast<TextImpl*>(text);
+  for (void* p : t->allocs) cudaFree(p);
+  delete t;
+  return 0;
+}
+
+extern "C" int64_t aph_text_bytes(const aph_text* text) { return text ? reinterpret_cast<const TextImpl*>(text)->bytes : 0; }
+
+extern "C" int aph_text_load_tensor(aph_text* text, const char* key, const float* data, int64_t numel, void* stream) {
+  APH_REQUIRE(text && key && data, "aph_text_load_tensor: null argument");
+  TextImpl* t = reinterpret_cast<TextImpl*>(text);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = t->cfg.width, O = t->cfg.out_dim, C = t->cfg.context;
+  const std::string k(key);
+  auto need = [&](int64_t n) -> int { APH_REQUIRE(numel == n, "aph_text_load_tensor(%s): expected %lld elements, got %lld", key, (long long)n, (long long)numel); return 0; };
+  int e = 0;
+  if (k == "token_embedding.weight") { if ((e = need((int64_t)t->cfg.vocab * D))) return e; e = copy_f32(data, t->tok_emb, (size_t)t->cfg.vocab * D, st); }
+  else if (k == "positional_embedding") { if ((e = need((int64_t)C * D))) return e; e = copy_f32(data, t->pos, (size_t)C * D, st); }
+  else if (k == "ln_final.weight") { if ((e = need(D))) return e; e = copy_f32(data, t->lnf_w, D, st); }
+  else if (k == "ln_final.bias") { if ((e = need(D))) return e; e = copy_f32(data, t->lnf_b, D, st); }
+  else if (k == "text_projection") { if ((e = need((int64_t)D * O))) return e; e = pack(data, t->w_out, D, O, 1, st); }   // [D, out] -> [out, D]
+  else if (k.rfind("transformer.resblocks.", 0) == 0) {
+    const char* rest = k.c_str() + strlen("transformer.resblocks.");
+    char* endp = nullptr;
+    const long li = strtol(rest, &endp, 10);
+    APH_REQUIRE(endp && *endp == '.' && li >= 0 && li < t->cfg.layers, "aph_text_load_tensor: bad layer index in %s", key);
+    TextLayer& l = t->L[li];
+    const std::string f(endp + 1);
+    if (f == "ln_1.weight") { if ((e = need(D))) return e; e = copy_f32(data, l.ln1_w, D, st); }
+    else if (f == "ln_1.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.ln1_b, D, st); }
+    else if (f == "ln_2.weight") { if ((e = need(D))) return e; e = copy_f32(data, l.ln2_w, D, st); }
+    else if (f == "ln_2.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.ln2_b, D, st); }
+    else if (f == "attn.in_proj_weight") { if ((e = need((int64_t)3 * D * D))) return e; e = pack(data, l.w_qkv, 3 * D, D, 0, st); }
+    else if (f == "attn.in_proj_bias") { if ((e = need(3 * D))) return e; e = copy_f32(data, l.b_qkv, 3 * D, st); }
+    else if (f == "attn.out_proj.weight") { if ((e = need((int64_t)D * D))) return e; e = pack(data, l.w_o, D, D, 0, st); }
+    else if (f == "attn.out_proj.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.b_o, D, st); }
+    else if (f == "mlp.c_fc.weight") { if ((e = need((int64_t)4 * D * D))) return e; e = pack(data, l.w_fc, 4 * D, D, 0, st); }
+    else if (f == "mlp.c_fc.bias") { if ((e = need(4 * D))) return e; e = copy_f32(data, l.b_fc, 4 * D, st); }
+    else if (f == "mlp.c_proj.weight") { if ((e = need((int64_t)4 * D * D))) return e; e = pack(data, l.w_proj, D, 4 * D, 0, st); }
+    else if (f == "mlp.c_proj.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.b_proj, D, st); }
+    else { set_error("aph_text_load_tensor: unknown tensor %s", key); return 2; }
+  } else { set_error("aph_text_load_tensor: unknown tensor %s", key); return 2; }
+  if (e) return e;
+  t->loaded[k] = true;
+  return 0;
+}
+
+extern "C" int aph_text_finalize(aph_text* text) {
+  APH_REQUIRE(text, "aph_text_finalize: null handle");
+  TextImpl* t = reinterpret_cast<TextImpl*>(text);
+  std::vector<std::string> want = {"token_embedding.weight", "positional_embedding", "ln_final.weight", "ln_final.bias", "text_projection"};
+  const char* per[] = {"ln_1.weight", "ln_1.bias", "ln_2.weight", "ln_2.bias", "attn.in_proj_weight", "attn.in_proj_bias",
+                       "attn.out_proj.weight", "attn.out_proj.bias", "mlp.c_fc.weight", "mlp.c_fc.bias", "mlp.c_proj.weight", "mlp.c_proj.bias"};
+  for (int i = 0; i < t->cfg.layers; ++i)
+    for (const char* p : per) want.push_back("transformer.resblocks." + std::to_string(i) + "." + p);
+  for (const auto& w : want) APH_REQUIRE(t->loaded.count(w), "aph_text_finalize: tensor %s was never loaded", w.c_str());
+  t->finalized = true;
+  return 0;
+}
+
+extern "C" int aph_text_fwd(aph_text* text, const int64_t* tokens, int n, float* emb, void* stream) {
+  APH_REQUIRE(text && tokens && emb, "aph_text_fwd: null argument");
+  TextImpl* t = reinterpret_cast<TextImpl*>(text);
+  APH_REQUIRE(t->finalized, "aph_text_fwd: weights not finalized");
+  APH_REQUIRE(n > 0 && n <= t->cfg.max_batch, "aph_text_fwd: n=%d outside (0, max_batch=%d]", n, t->cfg.max_batch);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int D = t->cfg.width, C = t->cfg.context, H = t->cfg.heads, O = t->cfg.out_dim;
+  const int M = n * C;
+  int e;
+  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_text_embed<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, tokens, t->tok_emb, t->pos, t->x, M, C, D, t->cfg.vocab)));
+  APH_LAUNCH_OK();
+  APH_CUDA_OK(launch_k(k_text_eot, dim3(rows_grid(n)), dim3(256), (size_t)0, st, 1, tokens, t->eot, n, C));
+  APH_LAUNCH_OK();
+  for (const TextLayer& w : t->L) {
+    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, t->x, (size_t)D, w.ln1_w, w.ln1_b, t->ln_out, t->mean, t->rstd, M, D)));
+    APH_LAUNCH_OK();
+    { GemmEpi ep; ep.bias = w.b_qkv; ep.out_bf16 = t->qkv;
+      if ((e = launch_gemm(t->ln_out, w.w_qkv, GemmShape{M, 3 * D, D}, ep, st))) return e; }
+    if ((e = attn_causal(t->qkv, t->attn_out, n, C, D, H, st))) return e;
+    { GemmEpi ep; ep.bias = w.b_o; ep.resid = t->x; ep.out_f32 = t->x_mid;
+      if ((e = launch_gemm(t->attn_out, w.w_o, GemmShape{M, D, D}, ep, st))) return e; }
+    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, t->x_mid, (size_t)D, w.ln2_w, w.ln2_b, t->ln_out, t->mean, t->rstd, M, D)));
+    APH_LAUNCH_OK();
+    { GemmEpi ep; ep.bias = w.b_fc; ep.out_pre = t->h_pre; ep.act = 1; ep.out_bf16 = t->h_act;
+      if ((e = launch_gemm(t->ln_out, w.w_fc, GemmShape{M, 4 * D, D}, ep, st))) return e; }
+    { GemmEpi ep; ep.bias = w.b_proj; ep.resid = t->x_mid; ep.out_f32 = t->x;
+      if ((e = launch_gemm(t->h_act, w.w_proj, GemmShape{M, D, 4 * D}, ep, st))) return e; }
+  }
+  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_text_pool_ln<NCH>, dim3(rows_grid(n)), dim3(256), (size_t)0, st, 1, t->x, t->eot, t->lnf_w, t->lnf_b, t->pooled, n, C, D)));
+  APH_LAUNCH_OK();
+  GemmEpi ep; ep.out_f32 = emb;
+  return launch_gemm(t->pooled, t->w_out, GemmShape{n, O, D}, ep, st);
+}

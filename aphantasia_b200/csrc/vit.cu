@@ -151,7 +151,8 @@ __global__ void __launch_bounds__(256) k_pack_weight(const float* __restrict__ i
   }
 }
 
-static int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st) {
+// (also used by text.cu)
+int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st) {
   const size_t n = (size_t)rows * cols;
   const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16);
   k_pack_weight<<<blocks, 256, 0, st>>>(src, dst, rows, cols, transpose);
@@ -159,19 +160,10 @@ static int pack(const float* src, bf16* dst, int rows, int cols, int transpose, 
   return 0;
 }
 
-static int copy_f32(const float* src, float* dst, size_t n, cudaStream_t st) {
+int copy_f32(const float* src, float* dst, size_t n, cudaStream_t st) {
   APH_CUDA_OK(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
   return 0;
 }
-
-#define NCH_DISPATCH(D, ...)                                                           \
-  switch ((D) / 128) {                                                                 \
-    case 1: { constexpr int NCH = 1; __VA_ARGS__; } break;                             \
-    case 2: { constexpr int NCH = 2; __VA_ARGS__; } break;                             \
-    case 6: { constexpr int NCH = 6; __VA_ARGS__; } break;                             \
-    case 8: { constexpr int NCH = 8; __VA_ARGS__; } break;                             \
-    default: set_error("vit: unsupported width %d", (D)); return 2;                    \
-  }
 
 static inline int rows_grid(int rows) { return (rows * 32 + 255) / 256; }
 

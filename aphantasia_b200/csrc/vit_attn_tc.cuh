@@ -80,7 +80,8 @@ __device__ __forceinline__ void av_step(float (&acc)[8][4], const uint32_t (&a)[
 }
 
 // ---------------------------------------------------------------------------------------------
-template <int NW, int NT2>
+// CAUSAL (the CLIP text tower): query row i attends to keys j <= i only; forward only.
+template <int NW, int NT2, bool CAUSAL = false>
 __global__ void __launch_bounds__(NW * 32) k_attn_fwd_tc(const bf16* __restrict__ qkv, bf16* __restrict__ out, int T, int D, int heads) {
   pdl_trigger(); pdl_wait();
   extern __shared__ __align__(128) uint8_t sm[];
@@ -113,8 +114,12 @@ __global__ void __launch_bounds__(NW * 32) k_attn_fwd_tc(const bf16* __restrict_
       for (int u = 0; u < 2; ++u) {
         const int col = n2 * 16 + u * 8 + 2 * t;
         float* cc = c[2 * n2 + u];
-        cc[0] = (col < T) ? cc[0] * kAttnScaleLog2 : -INFINITY; cc[1] = (col + 1 < T) ? cc[1] * kAttnScaleLog2 : -INFINITY;
-        cc[2] = (col < T) ? cc[2] * kAttnScaleLog2 : -INFINITY; cc[3] = (col + 1 < T) ? cc[3] * kAttnScaleLog2 : -INFINITY;
+        // causal: this lane's query rows are q0 + r0 + g (cc[0], cc[1]) and that + 8 (cc[2], cc[3]); key 0 always survives
+        const int qa0 = q0 + r0 + g, qa1 = qa0 + 8;
+        cc[0] = (col < T && (!CAUSAL || col <= qa0)) ? cc[0] * kAttnScaleLog2 : -INFINITY;
+        cc[1] = (col + 1 < T && (!CAUSAL || col + 1 <= qa0)) ? cc[1] * kAttnScaleLog2 : -INFINITY;
+        cc[2] = (col < T && (!CAUSAL || col <= qa1)) ? cc[2] * kAttnScaleLog2 : -INFINITY;
+        cc[3] = (col + 1 < T && (!CAUSAL || col + 1 <= qa1)) ? cc[3] * kAttnScaleLog2 : -INFINITY;
         m0 = fmaxf(m0, fmaxf(cc[0], cc[1])); m1 = fmaxf(m1, fmaxf(cc[2], cc[3]));
       }
     }

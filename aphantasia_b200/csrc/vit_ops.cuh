@@ -4,14 +4,26 @@
 // stride = kernel is an im2col permutation), cls/pos embedding + ln_pre, LayerNorm (fp32 statistics),
 // multi-head attention core softmax(QK^T/sqrt(64))V, and their backward passes (no weight gradients).
 // Token rows are sample-major: row = s*T + t.  Width D = 128*NCH (template), so rows live in registers.
+// Included by vit.cu and text.cu: the non-template kernels are static so that each translation unit has its own copy.
 #pragma once
 #include "tc_gemm.cuh"
 
 namespace aph {
 
+// Runs the statement with `constexpr int NCH = D / 128` for the row-in-registers kernels below (width 512 is the text tower's).
+#define NCH_DISPATCH(D, ...)                                                           \
+  switch ((D) / 128) {                                                                 \
+    case 1: { constexpr int NCH = 1; __VA_ARGS__; } break;                             \
+    case 2: { constexpr int NCH = 2; __VA_ARGS__; } break;                             \
+    case 4: { constexpr int NCH = 4; __VA_ARGS__; } break;                             \
+    case 6: { constexpr int NCH = 6; __VA_ARGS__; } break;                             \
+    case 8: { constexpr int NCH = 8; __VA_ARGS__; } break;                             \
+    default: set_error("vit: unsupported width %d", (D)); return 2;                    \
+  }
+
 // ---------------------------------------------------------------------------------------------
 // images fp32 [S,3,R,R] -> patches bf16 [S*g*g, 3*p*p], col = c*p*p + py*p + px  (conv1 weight layout)
-__global__ void __launch_bounds__(256) k_patchify(const float* __restrict__ img, bf16* __restrict__ out, int S, int p, int g) {
+static __global__ void __launch_bounds__(256) k_patchify(const float* __restrict__ img, bf16* __restrict__ out, int S, int p, int g) {
   pdl_trigger(); pdl_wait();
   const int R = p * g, Kp = 3 * p * p;
   const size_t total = (size_t)S * g * g * Kp / 8;
@@ -30,7 +42,7 @@ __global__ void __launch_bounds__(256) k_patchify(const float* __restrict__ img,
   }
 }
 
-__global__ void __launch_bounds__(256) k_f32_to_bf16(const float* __restrict__ in, bf16* __restrict__ out, size_t n) {
+static __global__ void __launch_bounds__(256) k_f32_to_bf16(const float* __restrict__ in, bf16* __restrict__ out, size_t n) {
   pdl_trigger(); pdl_wait();
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     out[i] = __float2bfloat16_rn(in[i]);
@@ -193,7 +205,7 @@ __global__ void __launch_bounds__(256) k_ln_bwd(const DY* __restrict__ dy, const
 // Forward: warp per query row; lanes own keys for the scores, dims for the output.
 constexpr int HD = 64;
 
-__global__ void __launch_bounds__(256) k_attn_fwd(const bf16* __restrict__ qkv, bf16* __restrict__ out, int T, int D, int heads) {
+static __global__ void __launch_bounds__(256) k_attn_fwd(const bf16* __restrict__ qkv, bf16* __restrict__ out, int T, int D, int heads) {
   extern __shared__ uint8_t sm_raw[];
   const int Tp = (T + 31) & ~31;
   const int Tq = Tp + 2;                                 // padded leading dim of transposed arrays (bank spread)
@@ -251,7 +263,7 @@ __global__ void __launch_bounds__(256) k_attn_fwd(const bf16* __restrict__ qkv, 
 
 // Backward: pass 1 (warp per query row) -> dQ and the row statistics (max, 1/sum, delta);
 //           pass 2 (warp per key) recomputes its column of P / dS and reduces dK, dV without atomics.
-__global__ void __launch_bounds__(256) k_attn_bwd(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, bf16* __restrict__ dqkv,
+static __global__ void __launch_bounds__(256) k_attn_bwd(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, bf16* __restrict__ dqkv,
                                                   int T, int D, int heads) {
   extern __shared__ uint8_t sm_raw[];
   const int Tp = (T + 31) & ~31;

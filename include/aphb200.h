@@ -176,6 +176,35 @@ int aph_vit_bwd(aph_vit* vit, const float* grad_emb, int S, float* grad_images, 
 /* bytes of device memory owned by the handle (weights + activation arena)                          */
 int64_t aph_vit_bytes(const aph_vit* vit);
 
+/* ================= CLIP text encoder (forward only) ===========================================
+ * Replaces clip.model.CLIP.encode_text (third-party OpenAI clip; call site clip_fft.py:150), run once per prompt
+ * before the optimisation loop: token_embedding[ids] + positional_embedding -> layers x pre-LN residual block with
+ * CAUSAL attention -> ln_final(x[s, argmax(ids[s])]) @ text_projection. Same kernels as the image tower.          */
+typedef struct aph_text aph_text;
+typedef struct {
+  int32_t width;      /* 512 (multiple of 128, <= 1024)              */
+  int32_t layers;     /* 12                                           */
+  int32_t heads;      /* 8 (head dim must be 64)                      */
+  int32_t out_dim;    /* 512 (multiple of 128)                        */
+  int32_t context;    /* 77 (<= 112)                                  */
+  int32_t vocab;      /* 49408                                        */
+  int32_t max_batch;  /* largest n a call will pass                   */
+  int32_t reserved;
+} aph_text_config;
+int aph_text_create(aph_text** t, const aph_text_config* cfg);
+int aph_text_destroy(aph_text* t);
+/* One tensor of the OpenAI state dict by its key (token_embedding.weight, positional_embedding,
+ * transformer.resblocks.N.{ln_1,attn,ln_2,mlp}.*, ln_final.weight / bias, text_projection), fp32 DEVICE pointer.
+ * token_embedding stays fp32 on the device; the layer matrices are packed to bf16. aph_text_finalize checks
+ * every tensor arrived.                                                                                          */
+int aph_text_load_tensor(aph_text* t, const char* key, const float* data, int64_t numel, void* stream);
+int aph_text_finalize(aph_text* t);
+/* tokens int64 [n, context] DEVICE -> emb [n, out_dim] fp32. Pooling row = first position of the largest id
+ * (torch.argmax). Ids outside [0, vocab) read no memory out of bounds (they embed as zeros); callers reject them. */
+int aph_text_fwd(aph_text* t, const int64_t* tokens, int n, float* emb, void* stream);
+/* bytes of device memory owned by the handle (weights + activations)                              */
+int64_t aph_text_bytes(const aph_text* t);
+
 /* Stand-alone wgmma GEMM used by the encoder (exported for tests / profiling):
  * C[M,N] (fp32) = A[M,K] (bf16, row-major) . B[N,K]^T (bf16, row-major). K % 64 == 0, N % 128 == 0. */
 int aph_gemm_bf16_tn(const void* A, const void* B, float* C, int M, int N, int K, void* stream);
