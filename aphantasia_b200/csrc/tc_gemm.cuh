@@ -4,12 +4,18 @@
 //
 // Persistent, warp-specialised, one CTA of three warpgroups per SM, tile 128 x BN (BN = 128 or 256):
 //   warpgroup 0 (1 lane)  TMA producer : cp.async.bulk.tensor.2d -> 128B-swizzled smem stages, mbarrier complete_tx
-//   warpgroups 1, 2       consumers    : rows 0-63 / 64-127 of the tile; wgmma.mma_async m64nBNk16 with both operands read
-//                                        from shared memory through descriptors, then the fused epilogue from registers
-// The producer gives its registers to the consumers (setmaxnreg) and runs ahead into the next tile's stages while the
-// consumers store the current one. Fused epilogues (struct GemmEpi): +bias, QuickGELU (saving the pre-activation),
-// x gelu'(h) for the MLP backward, +fp32 residual, fp32 or bf16 outputs, and an NCHW "un-patchify" store for the
-// patch-embed data gradient. Rows >= M are zero-filled by TMA on load and not stored.
+//   warpgroups 1, 2       consumers    : wgmma.mma_async with both operands read from shared memory through descriptors,
+//                                        then the fused epilogue from registers
+// Two consumer schedules (launch_gemm picks one from the shape):
+//   cooperative  both consumers work on every tile, rows 0-63 / 64-127 (m64nBNk16); the producer runs ahead into the next
+//                tile's stages while they store the current one. BN = 256 for large problems with long K, BN = 128 for
+//                small problems.
+//   ping-pong    BN = 128; each consumer owns every other tile whole (two m64n128k16 per k16) and the two take turns in the
+//                main loop, so one stores its tile while the other's MMAs run (large problems with short K).
+// The producer gives its registers to the consumers (setmaxnreg). Fused epilogues (struct GemmEpi): +bias, QuickGELU (saving
+// the pre-activation), x gelu'(h) for the MLP backward, +fp32 residual, fp32 or bf16 outputs, and an NCHW "un-patchify" store
+// for the patch-embed data gradient. bf16 outputs are stored 16 B per lane after an exchange inside each quad of lanes.
+// Rows >= M are zero-filled by TMA on load and not stored.
 #pragma once
 #include "aph_common.cuh"
 #include <cuda.h>
@@ -172,27 +178,24 @@ struct GemmCfg {
   static constexpr int SMEM = BAR_OFFSET + 2 * STAGES * 8 + 1024;  // + alignment slack
 };
 
-// two adjacent output columns (col, col + 1) of one row through the epilogue of kind EPI
+// named barriers of the two consumer warpgroups (256 threads; id 0 is __syncthreads): consumer c syncs on 1 + c before its
+// mainloop, the other consumer arrives on it
+__device__ __forceinline__ void consumer_bar_sync(int id) { asm volatile("bar.sync %0, 256;" ::"r"(id) : "memory"); }
+__device__ __forceinline__ void consumer_bar_arrive(int id) { asm volatile("bar.arrive %0, 256;" ::"r"(id) : "memory"); }
+
+// epilogue kinds with bf16 outputs: stored 8 columns (16 B) per lane after a transpose inside each quad of lanes
+template <int EPI>
+constexpr bool epi_bf16_out() { return EPI == EPI_BF16 || EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_GELUGRAD_BF16; }
+
+// two adjacent output columns (col, col + 1) of one row through an fp32-output epilogue of kind EPI
 template <int EPI>
 __device__ __forceinline__ void epi_store2(const GemmEpi& epi, int N, int row, int col, float v0, float v1, float2 bb) {
   const size_t off = (size_t)row * N + col;
   if (EPI == EPI_F32) {
     *reinterpret_cast<float2*>(epi.out_f32 + off) = make_float2(v0, v1);
-  } else if (EPI == EPI_BF16) {
-    *reinterpret_cast<uint32_t*>(epi.out_bf16 + off) = pack_bf16(v0, v1);
-  } else if (EPI == EPI_BIAS_BF16) {
-    *reinterpret_cast<uint32_t*>(epi.out_bf16 + off) = pack_bf16(v0 + bb.x, v1 + bb.y);
-  } else if (EPI == EPI_BIAS_GELU) {
-    v0 += bb.x; v1 += bb.y;
-    *reinterpret_cast<uint32_t*>(epi.out_pre + off) = pack_bf16(v0, v1);
-    *reinterpret_cast<uint32_t*>(epi.out_bf16 + off) = pack_bf16(quickgelu(v0), quickgelu(v1));
   } else if (EPI == EPI_BIAS_RESID) {
     const float2 r = __ldg(reinterpret_cast<const float2*>(epi.resid + off));
     *reinterpret_cast<float2*>(epi.out_f32 + off) = make_float2(v0 + bb.x + r.x, v1 + bb.y + r.y);
-  } else if (EPI == EPI_GELUGRAD_BF16) {
-    const uint32_t u = __ldg(reinterpret_cast<const unsigned int*>(epi.gelu_in + off));
-    const float2 h = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&u));
-    *reinterpret_cast<uint32_t*>(epi.out_bf16 + off) = pack_bf16(v0 * quickgelu_grad(h.x), v1 * quickgelu_grad(h.y));
   } else {   // EPI_UNPATCH: col = c*p*p + py*p + px with p even, so (col, col + 1) are adjacent pixels of one image row
     const int p = epi.unpatch_p, g = epi.unpatch_g, R = p * g;
     const int ch = col / (p * p), rem = col - ch * p * p, py = rem / p, px = rem - py * p;
@@ -201,11 +204,78 @@ __device__ __forceinline__ void epi_store2(const GemmEpi& epi, int N, int row, i
   }
 }
 
-template <int BN, int EPI>
+// one 16-byte store (written out: the compiler splits a uint4 assignment through a bf16 pointer into four 4-byte stores)
+__device__ __forceinline__ void st_global_16(void* p, const uint32_t (&w)[4]) {
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]) : "memory");
+}
+
+// 4 x 4 transpose of 32-bit words over the 4 lanes of a quad (lane q = lane & 3): lane q's w[t] <-> lane t's w[q].
+// In the accumulator layout lane q holds columns 8 t + 2 q, +1 (t = 0..3) of a 32-column chunk; after the transpose it holds the
+// 8 contiguous columns 8 q .. 8 q + 7, and the reverse. Two exchange steps, one per bit of (q, t).
+__device__ __forceinline__ void quad_transpose(uint32_t (&w)[4], int q) {
+  const bool b0 = q & 1, b1 = q & 2;
+#pragma unroll
+  for (int p = 0; p < 2; ++p) {
+    const uint32_t r = __shfl_xor_sync(0xffffffffu, b0 ? w[2 * p] : w[2 * p + 1], 1);
+    if (b0) w[2 * p] = r; else w[2 * p + 1] = r;
+  }
+#pragma unroll
+  for (int p = 0; p < 2; ++p) {
+    const uint32_t r = __shfl_xor_sync(0xffffffffu, b1 ? w[p] : w[p + 2], 2);
+    if (b1) w[p] = r; else w[p + 2] = r;
+  }
+}
+
+// A 32-column chunk of one row through a bf16-output epilogue of kind EPI. v[2 t + {0,1}] = accumulators at columns
+// col0 + 8 t + 2 q + {0,1}, bb[t] their bias. The math per element is that of the pairwise store; only the stores (and the
+// gelu_in loads) are 16 B per lane, so that a warp writes whole 32 B sectors. All 32 lanes must call it (shuffles); rows >= M
+// load and store nothing.
+template <int EPI>
+__device__ __forceinline__ void epi_store_bf16x32(const GemmEpi& epi, int N, int row, bool valid, int col0, int q, const float* v,
+                                                  const float2* bb) {
+  const size_t off = (size_t)row * N + col0 + 8 * q;          // this lane's 8 columns after the transpose
+  uint32_t w[4], w2[4];
+  if constexpr (EPI == EPI_GELUGRAD_BF16) {
+    uint4 g = make_uint4(0u, 0u, 0u, 0u);
+    if (valid) g = __ldg(reinterpret_cast<const uint4*>(epi.gelu_in + off));
+    w2[0] = g.x; w2[1] = g.y; w2[2] = g.z; w2[3] = g.w;
+    quad_transpose(w2, q);                                     // back to the accumulator layout
+  }
+#pragma unroll
+  for (int t = 0; t < 4; ++t) {
+    float v0 = v[2 * t], v1 = v[2 * t + 1];
+    if (EPI == EPI_BF16) {
+      w[t] = pack_bf16(v0, v1);
+    } else if (EPI == EPI_BIAS_BF16) {
+      w[t] = pack_bf16(v0 + bb[t].x, v1 + bb[t].y);
+    } else if (EPI == EPI_BIAS_GELU) {
+      v0 += bb[t].x; v1 += bb[t].y;
+      w2[t] = pack_bf16(v0, v1);
+      w[t] = pack_bf16(quickgelu(v0), quickgelu(v1));
+    } else {   // EPI_GELUGRAD_BF16
+      const float2 h = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w2[t]));
+      w[t] = pack_bf16(v0 * quickgelu_grad(h.x), v1 * quickgelu_grad(h.y));
+    }
+  }
+  quad_transpose(w, q);
+  if (valid) st_global_16(epi.out_bf16 + off, w);
+  if constexpr (EPI == EPI_BIAS_GELU) {
+    quad_transpose(w2, q);
+    if (valid) st_global_16(epi.out_pre + off, w2);
+  }
+}
+
+// PINGPONG = false ("cooperative"): both consumer warpgroups work on every tile, rows 0-63 / 64-127, one m64nBNk16 per k16.
+// PINGPONG = true: consumer warpgroup c owns the whole 128 x 128 tiles i = c, c + 2, ... of this CTA's schedule (two m64n128k16
+// per k16: rows 0-63 and 64-127). Two named barriers hand the mainloop back and forth, so one warpgroup issues the MMAs of tile
+// i while the other stores tile i - 1: the tensor pipe and the epilogue's HBM traffic overlap instead of taking turns.
+template <int BN, bool PINGPONG, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, GemmShape shp, GemmEpi epi) {
+  static_assert(BN == 128 || !PINGPONG, "the ping-pong schedule runs 128 x 128 tiles");
   using L = GemmCfg<BN>;
   constexpr int STAGES = L::STAGES;
+  constexpr int MMAS = PINGPONG ? 2 : 1;          // m64 row blocks per consumer warpgroup and tile
   constexpr bool HAS_BIAS = (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_RESID);
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
@@ -219,7 +289,7 @@ k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a); tma_prefetch_desc(&map_b);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }
+    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], PINGPONG ? 1 : 2); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -228,7 +298,7 @@ k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
   if (wg == 0) {
     setmaxnreg_dec<40>();
     if (tid == 0) {
-      // ===== TMA producer
+      // ===== TMA producer: fills the stage ring in tile order (both schedules)
       const uint64_t pol_b = l2_policy_evict_last();      // B = weights: shared by all M tiles
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
@@ -245,40 +315,71 @@ k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     }
   } else {
     setmaxnreg_inc<232>();
-    // ===== consumer warpgroup: rows 64*(wg-1) .. +63 of each tile
-    const int warp = tid >> 5, lane = tid & 31;
-    const int row_in_tile = 64 * (wg - 1) + 16 * warp + (lane >> 2), col_in_tile = 2 * (lane & 3);
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
-      float d[BN / 2];
+    // ===== consumer warpgroup c
+    const int c = wg - 1, warp = tid >> 5, lane = tid & 31;
+    const int row_in_tile = (PINGPONG ? 0 : 64 * c) + 16 * warp + (lane >> 2), col_in_tile = 2 * (lane & 3);
+    // this CTA's tiles are blockIdx.x + i * gridDim.x, i = 0, 1, ...; their stages follow each other in the ring (`it`)
+    uint32_t it = PINGPONG ? c * k_blocks : 0;
+    const int tile_step = (PINGPONG ? 2 : 1) * gridDim.x;
+    // (the loop bounds compare rows with shp.M, a kernel parameter, rather than keep num_tiles in a register)
+    for (int tile = blockIdx.x + (PINGPONG ? c * gridDim.x : 0); tile / n_tiles * GEMM_BM < shp.M; tile += tile_step) {
+      // Ping-pong: wait until the other warpgroup has issued the previous tile. This also keeps every full-barrier wait below at
+      // most one phase ahead of the barrier (the stage's previous use, in that tile or earlier, has already been waited for).
+      if (PINGPONG && tile != (int)blockIdx.x) consumer_bar_sync(1 + c);
+      float d[MMAS][BN / 2];
 #pragma unroll
-      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
-      int prev = -1;
+      for (int h = 0; h < MMAS; ++h)
+#pragma unroll
+        for (int r = 0; r < BN / 2; ++r) d[h][r] = 0.f;
       for (int kb = 0; kb < k_blocks; ++kb, ++it) {
         const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
         mbar_wait(&full_bar[s], ph);
-        const uint32_t sa = smem_u32(smem + s * L::STAGE_BYTES);
-        const uint64_t da = make_smem_desc(sa + (wg - 1) * (64 * 128)), db = make_smem_desc(sa + L::A_BYTES);
+        // one descriptor for the stage; offsets go into its (address >> 4) field: +2 per 16 bf16 along K inside the swizzle atom,
+        // +512 per 64 rows of A, +A_BYTES / 16 for B
+        const uint64_t ds = make_smem_desc(smem_u32(smem + s * L::STAGE_BYTES));
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < GEMM_BK / GEMM_UK; ++k)      // advance 16 bf16 = 32 B along K inside the swizzle atom: +2 in the (>>4) address field
-          Wgmma<BN>::mma(d, da + (uint64_t)(2 * k), db + (uint64_t)(2 * k), (kb | k) != 0);
+        for (int k = 0; k < GEMM_BK / GEMM_UK; ++k)
+#pragma unroll
+          for (int h = 0; h < MMAS; ++h)
+            Wgmma<BN>::mma(d[h], ds + (uint64_t)((PINGPONG ? h : c) * 512 + 2 * k), ds + (uint64_t)(L::A_BYTES / 16 + 2 * k), (kb | k) != 0);
         wgmma_commit();
         wgmma_wait<1>();                                 // the previous stage's MMAs have retired: hand that stage back
-        if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
-        prev = (int)s;
+        if (kb > 0 && tid == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
       }
+      if (PINGPONG && (tile + (int)gridDim.x) / n_tiles * GEMM_BM < shp.M) consumer_bar_arrive(1 + (c ^ 1));    // the other warpgroup may issue the next tile
       wgmma_wait<0>();
-      if (prev >= 0 && tid == 0) mbar_arrive(&empty_bar[prev]);
-      // ---- epilogue straight from the accumulator fragments: d[4j + {0,1}] = (row, col + {0,1}), d[4j + {2,3}] = (row + 8, ...)
-      const int row0 = m_blk * GEMM_BM + row_in_tile, row1 = row0 + 8;
+      if (tid == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+      if (PINGPONG) it += k_blocks;                    // skip the other warpgroup's tile
+      const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
+      // ---- epilogue straight from the accumulator fragments: d[h][4j + {0,1}] = (row, col + {0,1}), d[h][4j + {2,3}] = (row + 8, ...)
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int col = n_blk * BN + 8 * j + col_in_tile;
-        const float2 bb = HAS_BIAS ? __ldg(reinterpret_cast<const float2*>(epi.bias + col)) : make_float2(0.f, 0.f);
-        if (row0 < shp.M) epi_store2<EPI>(epi, shp.N, row0, col, d[4 * j], d[4 * j + 1], bb);
-        if (row1 < shp.M) epi_store2<EPI>(epi, shp.N, row1, col, d[4 * j + 2], d[4 * j + 3], bb);
+      for (int h = 0; h < MMAS; ++h) {
+        const int row0 = m_blk * GEMM_BM + 64 * h + row_in_tile, row1 = row0 + 8;
+        if constexpr (epi_bf16_out<EPI>()) {
+#pragma unroll
+          for (int j0 = 0; j0 < BN / 8; j0 += 4) {        // 32-column chunks
+            const int col0 = n_blk * BN + 8 * j0;
+            float2 bb[4];
+            float v0[8], v1[8];
+#pragma unroll
+            for (int t = 0; t < 4; ++t) {
+              bb[t] = HAS_BIAS ? __ldg(reinterpret_cast<const float2*>(epi.bias + col0 + 8 * t + col_in_tile)) : make_float2(0.f, 0.f);
+              v0[2 * t] = d[h][4 * (j0 + t)]; v0[2 * t + 1] = d[h][4 * (j0 + t) + 1];
+              v1[2 * t] = d[h][4 * (j0 + t) + 2]; v1[2 * t + 1] = d[h][4 * (j0 + t) + 3];
+            }
+            epi_store_bf16x32<EPI>(epi, shp.N, row0, row0 < shp.M, col0, lane & 3, v0, bb);
+            epi_store_bf16x32<EPI>(epi, shp.N, row1, row1 < shp.M, col0, lane & 3, v1, bb);
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            const int col = n_blk * BN + 8 * j + col_in_tile;
+            const float2 bb = HAS_BIAS ? __ldg(reinterpret_cast<const float2*>(epi.bias + col)) : make_float2(0.f, 0.f);
+            if (row0 < shp.M) epi_store2<EPI>(epi, shp.N, row0, col, d[h][4 * j], d[h][4 * j + 1], bb);
+            if (row1 < shp.M) epi_store2<EPI>(epi, shp.N, row1, col, d[h][4 * j + 2], d[h][4 * j + 3], bb);
+          }
+        }
       }
     }
   }

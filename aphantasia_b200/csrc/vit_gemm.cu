@@ -61,18 +61,19 @@ bool gemm_profiling_on() { return g_prof; }
 static std::vector<std::pair<cudaEvent_t, cudaEvent_t>> g_prof_ev;
 static std::vector<double> g_prof_flops;
 
-// launches per (tile variant, epilogue kind): variant 0 = 128x128 tiles, 1 = 128x256 tiles.
+// launches per (kernel variant, epilogue kind): variant 0 = the small-problem kernel (cooperative, 128 x 128 tiles),
+// 1 = the large-problem kernels (ping-pong 128 x 128 tiles, or cooperative 128 x 256 tiles for long K).
 // Read by the tests to prove which kernel a shape really ran (aph_gemm_variant_launches).
 static std::atomic<long long> g_variant_launches[2][EPI_KINDS];
 
-template <int BN, int EPI>
+template <int BN, bool PINGPONG, int EPI>
 static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st) {
   using L = GemmCfg<BN>;
   static_assert(L::SMEM <= 227 * 1024, "GEMM shared-memory budget");
-  g_variant_launches[BN == 256 ? 1 : 0][EPI].fetch_add(1, std::memory_order_relaxed);
+  g_variant_launches[(PINGPONG || BN == 256) ? 1 : 0][EPI].fetch_add(1, std::memory_order_relaxed);
   static bool configured = false;
   if (!configured) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_gemm_bf16_tn<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM));
+    APH_CUDA_OK(cudaFuncSetAttribute(k_gemm_bf16_tn<BN, PINGPONG, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM));
     configured = true;
   }
   CUtensorMap ma, mb;
@@ -82,7 +83,7 @@ static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi
   const int grid = tiles < num_sms() ? tiles : num_sms();
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (g_prof) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, st); }
-  APH_CUDA_OK(launch_k(k_gemm_bf16_tn<BN, EPI>, dim3(grid), dim3(GEMM_THREADS), (size_t)L::SMEM, st, 1, ma, mb, shp, epi));
+  APH_CUDA_OK(launch_k(k_gemm_bf16_tn<BN, PINGPONG, EPI>, dim3(grid), dim3(GEMM_THREADS), (size_t)L::SMEM, st, 1, ma, mb, shp, epi));
   APH_LAUNCH_OK();
   if (g_prof) { cudaEventRecord(e1, st); g_prof_ev.emplace_back(e0, e1); g_prof_flops.push_back(2.0 * shp.M * shp.N * shp.K); }
   return 0;
@@ -103,10 +104,17 @@ int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi,
   else if (f && !h && b && r && !gi && !pre && !act) kind = EPI_BIAS_RESID;
   else if (h && !f && !b && !r && gi && !pre && !act) kind = EPI_GELUGRAD_BF16;
   APH_REQUIRE(kind >= 0, "gemm: unsupported epilogue combination");
-  // 128 x 256 tiles halve the B-operand shared-memory reads per MMA against 128 x 128; they are chosen when there are at least as
-  // many of them as SMs, so that no SM idles (the encoder GEMMs at M ~ 9500 token rows); smaller problems keep the finer tiling.
-  const bool wide = shp.N % 256 == 0 && ((shp.M + GEMM_BM - 1) / GEMM_BM) * (shp.N / 256) >= num_sms();
-#define APH_GEMM_CASE(K) case K: return wide ? launch_cfg<256, K>(A, B, shp, epi, st) : launch_cfg<128, K>(A, B, shp, epi, st);
+  const uintptr_t bf16_ptrs = reinterpret_cast<uintptr_t>(epi.out_bf16) | reinterpret_cast<uintptr_t>(epi.out_pre) | reinterpret_cast<uintptr_t>(epi.gelu_in);
+  APH_REQUIRE((bf16_ptrs & 15) == 0, "gemm: bf16 epilogue operands must be 16-byte aligned (8 columns are stored per lane)");
+  // The ping-pong kernel overlaps one consumer's epilogue with the other's mainloop, which needs two tiles per SM in flight. It is
+  // chosen when there are at least twice as many 128 x 128 tiles as SMs and K is short (K = 768 in the encoder), so that the
+  // epilogue is a large share of a tile's time. With long K the mainloop dominates and the cooperative 128 x 256 tile wins: its
+  // m64n256 MMAs read less shared memory per FLOP. Smaller problems (the final projection, the text tower) keep 128 x 128 tiles.
+  const int m_tiles = (shp.M + GEMM_BM - 1) / GEMM_BM;
+  const bool pingpong = m_tiles * (shp.N / 128) >= 2 * num_sms() && shp.K <= 1024;
+  const bool wide = !pingpong && shp.N % 256 == 0 && m_tiles * (shp.N / 256) >= num_sms();
+#define APH_GEMM_CASE(K) case K: return pingpong ? launch_cfg<128, true, K>(A, B, shp, epi, st) \
+                                                 : wide ? launch_cfg<256, false, K>(A, B, shp, epi, st) : launch_cfg<128, false, K>(A, B, shp, epi, st);
   switch (kind) {
     APH_GEMM_CASE(EPI_F32) APH_GEMM_CASE(EPI_BF16) APH_GEMM_CASE(EPI_BIAS_BF16) APH_GEMM_CASE(EPI_BIAS_GELU)
     APH_GEMM_CASE(EPI_BIAS_RESID) APH_GEMM_CASE(EPI_GELUGRAD_BF16) APH_GEMM_CASE(EPI_UNPATCH)
@@ -138,7 +146,7 @@ extern "C" int aph_gemm_epi_test(const void* A, const void* B, int M, int N, int
   return launch_gemm(A, B, GemmShape{M, N, K}, epi, (cudaStream_t)stream);
 }
 
-// launches so far of tile variant `variant` (0: 128x128 tiles, 1: 128x256 tiles) with
+// launches so far of kernel variant `variant` (0: the small-problem kernel, 1: the large-problem kernels) with
 // epilogue kind `epi` (EPI_* order of tc_gemm.cuh: 0 f32, 1 bf16, 2 bias-bf16, 3 bias-gelu, 4 bias-resid, 5 gelugrad, 6 unpatch; -1 = all)
 extern "C" int64_t aph_gemm_variant_launches(int variant, int epi) {
   if (variant < 0 || variant > 1 || epi >= EPI_KINDS) return -1;

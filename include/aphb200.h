@@ -212,7 +212,9 @@ int aph_gemm_bf16_tn(const void* A, const void* B, float* C, int M, int N, int K
 /* Test entries. aph_gemm_epi_test: the same GEMM with the encoder's fused epilogues on caller-supplied operands
  * (NULL = unused; the combination selects the kind as the encoder's own calls do: +bias, QuickGELU saving the
  * pre-activation (act=1, out_pre), x gelu'(gelu_in), +fp32 resid, fp32 / bf16 outputs, NCHW un-patchify).
- * aph_gemm_variant_launches: launches so far of tile variant 0 (128x128 tiles) or 1 (128x256 tiles) with epilogue kind epi
+ * bf16 operands of the epilogue (out_bf16, out_pre, gelu_in) must be 16-byte aligned.
+ * aph_gemm_variant_launches: launches so far of kernel variant 0 (the small-problem kernel) or 1 (the large-problem kernels:
+ * ping-pong 128x128 tiles for short K, cooperative 128x256 tiles for long K) with epilogue kind epi
  * (0 f32, 1 bf16, 2 bias-bf16, 3 bias-gelu, 4 bias-resid, 5 gelu-grad, 6 un-patchify; -1 = any).                                                             */
 int aph_gemm_epi_test(const void* A, const void* B, int M, int N, int K, const float* bias, const float* resid,
                       const void* gelu_in, int act, float* out_f32, void* out_bf16, void* out_pre,
