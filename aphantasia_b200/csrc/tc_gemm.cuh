@@ -15,7 +15,8 @@
 // The producer gives its registers to the consumers (setmaxnreg). Fused epilogues (struct GemmEpi): +bias, QuickGELU (saving
 // the pre-activation), x gelu'(h) for the MLP backward, +fp32 residual, fp32 or bf16 outputs, and an NCHW "un-patchify" store
 // for the patch-embed data gradient. bf16 outputs are stored 16 B per lane after an exchange inside each quad of lanes.
-// Rows >= M are zero-filled by TMA on load and not stored.
+// Rows >= M are zero-filled by TMA on load and not stored. A, the residual and the outputs may have a row stride larger than
+// their width (the encoder's last block reads and writes the class-token rows s*T of token-major matrices in place).
 #pragma once
 #include "aph_common.cuh"
 #include <cuda.h>
@@ -34,6 +35,10 @@ struct GemmEpi {
   int act = 0;                     // 1 = QuickGELU x*sigmoid(1.702x)
   int unpatch_p = 0;               // >0: out_f32 is [S,3,R,R]; row = s*g*g + gy*g + gx, col = c*p*p + py*p + px
   int unpatch_g = 0;
+  // row strides in elements, 0 = N (dense). ld_out covers out_f32 / out_bf16 / out_pre and gelu_in, which has the output's rows.
+  // A strided output leaves the rows between its rows untouched (the encoder's last block writes only the class-token rows).
+  int ld_resid = 0;
+  int ld_out = 0;
 };
 
 struct GemmShape { int M, N, K; };
@@ -187,14 +192,16 @@ __device__ __forceinline__ void consumer_bar_arrive(int id) { asm volatile("bar.
 template <int EPI>
 constexpr bool epi_bf16_out() { return EPI == EPI_BF16 || EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_GELUGRAD_BF16; }
 
-// two adjacent output columns (col, col + 1) of one row through an fp32-output epilogue of kind EPI
+// two adjacent output columns (col, col + 1) of one row through an fp32-output epilogue of kind EPI (launch_gemm has resolved the
+// strides: epi.ld_out and epi.ld_resid are never 0 here). out_row / res_row: the row's offsets, computed once per row and tile.
 template <int EPI>
-__device__ __forceinline__ void epi_store2(const GemmEpi& epi, int N, int row, int col, float v0, float v1, float2 bb) {
-  const size_t off = (size_t)row * N + col;
+__device__ __forceinline__ void epi_store2(const GemmEpi& epi, size_t out_row, size_t res_row, int row, int col, float v0, float v1,
+                                           float2 bb) {
+  const size_t off = out_row + col;
   if (EPI == EPI_F32) {
     *reinterpret_cast<float2*>(epi.out_f32 + off) = make_float2(v0, v1);
   } else if (EPI == EPI_BIAS_RESID) {
-    const float2 r = __ldg(reinterpret_cast<const float2*>(epi.resid + off));
+    const float2 r = __ldg(reinterpret_cast<const float2*>(epi.resid + res_row + col));
     *reinterpret_cast<float2*>(epi.out_f32 + off) = make_float2(v0 + bb.x + r.x, v1 + bb.y + r.y);
   } else {   // EPI_UNPATCH: col = c*p*p + py*p + px with p even, so (col, col + 1) are adjacent pixels of one image row
     const int p = epi.unpatch_p, g = epi.unpatch_g, R = p * g;
@@ -231,9 +238,9 @@ __device__ __forceinline__ void quad_transpose(uint32_t (&w)[4], int q) {
 // gelu_in loads) are 16 B per lane, so that a warp writes whole 32 B sectors. All 32 lanes must call it (shuffles); rows >= M
 // load and store nothing.
 template <int EPI>
-__device__ __forceinline__ void epi_store_bf16x32(const GemmEpi& epi, int N, int row, bool valid, int col0, int q, const float* v,
+__device__ __forceinline__ void epi_store_bf16x32(const GemmEpi& epi, int row, bool valid, int col0, int q, const float* v,
                                                   const float2* bb) {
-  const size_t off = (size_t)row * N + col0 + 8 * q;          // this lane's 8 columns after the transpose
+  const size_t off = (size_t)row * epi.ld_out + col0 + 8 * q;  // this lane's 8 columns after the transpose
   uint32_t w[4], w2[4];
   if constexpr (EPI == EPI_GELUGRAD_BF16) {
     uint4 g = make_uint4(0u, 0u, 0u, 0u);
@@ -368,16 +375,18 @@ k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
               v0[2 * t] = d[h][4 * (j0 + t)]; v0[2 * t + 1] = d[h][4 * (j0 + t) + 1];
               v1[2 * t] = d[h][4 * (j0 + t) + 2]; v1[2 * t + 1] = d[h][4 * (j0 + t) + 3];
             }
-            epi_store_bf16x32<EPI>(epi, shp.N, row0, row0 < shp.M, col0, lane & 3, v0, bb);
-            epi_store_bf16x32<EPI>(epi, shp.N, row1, row1 < shp.M, col0, lane & 3, v1, bb);
+            epi_store_bf16x32<EPI>(epi, row0, row0 < shp.M, col0, lane & 3, v0, bb);
+            epi_store_bf16x32<EPI>(epi, row1, row1 < shp.M, col0, lane & 3, v1, bb);
           }
         } else {
+          const size_t out0 = (size_t)row0 * epi.ld_out, out1 = out0 + 8 * (size_t)epi.ld_out;
+          const size_t res0 = (EPI == EPI_BIAS_RESID) ? (size_t)row0 * epi.ld_resid : 0, res1 = res0 + 8 * (size_t)epi.ld_resid;
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
             const int col = n_blk * BN + 8 * j + col_in_tile;
             const float2 bb = HAS_BIAS ? __ldg(reinterpret_cast<const float2*>(epi.bias + col)) : make_float2(0.f, 0.f);
-            if (row0 < shp.M) epi_store2<EPI>(epi, shp.N, row0, col, d[h][4 * j], d[h][4 * j + 1], bb);
-            if (row1 < shp.M) epi_store2<EPI>(epi, shp.N, row1, col, d[h][4 * j + 2], d[h][4 * j + 3], bb);
+            if (row0 < shp.M) epi_store2<EPI>(epi, out0, res0, row0, col, d[h][4 * j], d[h][4 * j + 1], bb);
+            if (row1 < shp.M) epi_store2<EPI>(epi, out1, res1, row1, col, d[h][4 * j + 2], d[h][4 * j + 3], bb);
           }
         }
       }
@@ -386,10 +395,11 @@ k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 }
 
 // ---- host side ---------------------------------------------------------------------------------
-// 2-D bf16 tensor map: tensor [rows, K] row-major, box [box_rows, 64] with 128B swizzle.
-int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int K, int box_rows);
+// 2-D bf16 tensor map: tensor [rows, K] with rows `row_stride` elements apart (K when 0), box [box_rows, 64] with 128B swizzle.
+int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int K, int box_rows, int64_t row_stride = 0);
 int make_tmap_bf16_tokens(CUtensorMap* out, const void* base, int cols, int T, int S, int box_rows);
-// Launches the GEMM on `st`. A: [M,K], B: [N,K] device bf16. Requires K % 64 == 0, N % 128 == 0.
-int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st);
+// Launches the GEMM on `st`. A: [M,K] with rows `lda` elements apart (K when 0), B: [N,K] device bf16. Requires K % 64 == 0,
+// N % 128 == 0, and row strides that are multiples of 16 bytes.
+int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st, int lda = 0);
 
 }  // namespace aph

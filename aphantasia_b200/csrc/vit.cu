@@ -41,23 +41,30 @@ struct VitImpl {
   bf16* patches = nullptr;       // [S*g*g, Kp]
   float* tok = nullptr;          // [S*g*g, D]
   float* e = nullptr;            // [M, D] pre-ln_pre
-  std::vector<float*> xs;        // 2*layers+1 residual-stream snapshots, fp32 [M, D]
+  // Everything the caller gets comes from the cls rows s*T of the last block's output (ln_post reads x[:, 0]). So past its
+  // attention (whose keys and values come from every token) the last block runs on the S cls rows only: its x_mid, x_out and
+  // h_pre are compact [S, ...] and its residual gradient is dxc / dxc_bf.
+  std::vector<float*> xs;        // 2*layers+1 residual-stream snapshots, fp32 [M, D]; the last two are [S, D]
   bf16* ln_out = nullptr;        // [M, D]
   std::vector<bf16*> qkv;        // per layer [M, 3D]
   bf16* attn_out = nullptr;      // [M, D]
-  std::vector<bf16*> h_pre;      // per layer [M, 4D]
+  std::vector<bf16*> h_pre;      // per layer [M, 4D]; the last layer's is [S, 4D]
   bf16* h_act = nullptr;         // [M, 4D]
-  float *st_mean = nullptr, *st_rstd = nullptr;   // [(2*layers+2)][M]
+  float *st_mean = nullptr, *st_rstd = nullptr;   // LayerNorm statistics, slots of stat_off()
   bf16* cls_ln = nullptr;        // [S, D]
   float* emb_int = nullptr;      // [S, out] (copied to the caller's buffer outside the graph)
   // backward scratch
   bf16* d_emb = nullptr;         // [S, out]
   float* d_cls = nullptr;        // [S, D]
+  float* dxc = nullptr;          // [S, D] residual gradient of the last block (cls rows)
+  bf16* dxc_bf = nullptr;        // [S, D]
   float* dx = nullptr;           // [M, D]
   bf16* dx_bf = nullptr;         // [M, D]
   bf16* dh = nullptr;            // [M, 4D]
   bf16* d_ln = nullptr;          // [M, D] gradient entering a LayerNorm backward (bf16: it is the output of a bf16-operand GEMM and is consumed once)
   bf16* d_attn = nullptr;        // [M, D]
+  bf16* d_attn_last = nullptr;   // [M, D] the last block's attention-output gradient: zeroed at creation, only rows s*T are ever
+                                 // written, so every other row stays exactly zero (layers below overwrite all rows of d_attn)
   bf16* d_qkv = nullptr;         // [M, 3D]
   bf16* d_tok = nullptr;         // [S*g*g, D]
   int last_S = -1;
@@ -69,6 +76,13 @@ struct VitImpl {
   unsigned long long stamp = 0;
   int graph_misses = 0;          // captures in a row that were never replayed (e.g. the caller re-allocates its tensors every step)
 };
+
+// LayerNorm statistics slot k: 0 = ln_pre, 1 + 2l / 2 + 2l = ln_1 / ln_2 of layer l, 2 layers + 1 = ln_post. The slots below
+// 2 layers hold max_batch*T rows; the last two (ln_2 of the last block and ln_post, cls rows only) hold max_batch rows.
+static size_t stat_off(const VitImpl* v, int k) {
+  const size_t Mmax = (size_t)v->cfg.max_batch * v->T, k2 = 2 * (size_t)v->cfg.layers;
+  return (size_t)k < k2 ? k * Mmax : k2 * Mmax + (k - k2) * (size_t)v->cfg.max_batch;
+}
 
 bool gemm_profiling_on();      // vit_gemm.cu
 
@@ -208,17 +222,21 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
   }
   // activations
   e |= dev_alloc(v, &v->patches, Mp * v->Kp); e |= dev_alloc(v, &v->tok, Mp * D); e |= dev_alloc(v, &v->e, M * D);
-  v->xs.resize(2 * Ly + 1); for (auto& x : v->xs) e |= dev_alloc(v, &x, M * D);
+  v->xs.resize(2 * Ly + 1);
+  for (int i = 0; i <= 2 * Ly; ++i) e |= dev_alloc(v, &v->xs[i], (i >= 2 * Ly - 1 ? (size_t)S : M) * D);
   e |= dev_alloc(v, &v->ln_out, M * D); e |= dev_alloc(v, &v->attn_out, M * D); e |= dev_alloc(v, &v->h_act, M * 4 * D);
   v->qkv.resize(Ly); v->h_pre.resize(Ly);
-  for (int i = 0; i < Ly; ++i) { e |= dev_alloc(v, &v->qkv[i], M * 3 * D); e |= dev_alloc(v, &v->h_pre[i], M * 4 * D); }
-  e |= dev_alloc(v, &v->st_mean, (size_t)(2 * Ly + 2) * M); e |= dev_alloc(v, &v->st_rstd, (size_t)(2 * Ly + 2) * M);
+  for (int i = 0; i < Ly; ++i) { e |= dev_alloc(v, &v->qkv[i], M * 3 * D); e |= dev_alloc(v, &v->h_pre[i], (i == Ly - 1 ? (size_t)S : M) * 4 * D); }
+  e |= dev_alloc(v, &v->st_mean, stat_off(v, 2 * Ly + 2)); e |= dev_alloc(v, &v->st_rstd, stat_off(v, 2 * Ly + 2));
   e |= dev_alloc(v, &v->cls_ln, (size_t)S * D); e |= dev_alloc(v, &v->emb_int, (size_t)S * O);
   e |= dev_alloc(v, &v->d_emb, (size_t)S * O); e |= dev_alloc(v, &v->d_cls, (size_t)S * D);
+  e |= dev_alloc(v, &v->dxc, (size_t)S * D); e |= dev_alloc(v, &v->dxc_bf, (size_t)S * D);
   e |= dev_alloc(v, &v->dx, M * D); e |= dev_alloc(v, &v->dx_bf, M * D); e |= dev_alloc(v, &v->dh, M * 4 * D);
-  e |= dev_alloc(v, &v->d_ln, M * D); e |= dev_alloc(v, &v->d_attn, M * D); e |= dev_alloc(v, &v->d_qkv, M * 3 * D);
-  e |= dev_alloc(v, &v->d_tok, Mp * D);
+  e |= dev_alloc(v, &v->d_ln, M * D); e |= dev_alloc(v, &v->d_attn, M * D); e |= dev_alloc(v, &v->d_attn_last, M * D);
+  e |= dev_alloc(v, &v->d_qkv, M * 3 * D); e |= dev_alloc(v, &v->d_tok, Mp * D);
   if (e) { aph_vit_destroy(reinterpret_cast<aph_vit*>(v)); return 1; }
+  APH_CUDA_OK(cudaMemset(v->d_attn_last, 0, M * D * sizeof(bf16)));
+  APH_CUDA_OK(cudaDeviceSynchronize());     // the zeros are in place before any caller stream (blocking or not) can read them
   APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_fwd_smem(T)));
   APH_CUDA_OK(cudaFuncSetAttribute(k_attn_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_bwd_smem(T)));
   *out = reinterpret_cast<aph_vit*>(v);
@@ -336,7 +354,6 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, float* emb, in
   const int rc = run_cached(v->fwd_graphs, v->warm_fwd, v->stamp, v->graph_misses, nullptr, nullptr, S, save_for_bwd, st, [&]() -> int {
   const int D = v->D, T = v->T, g = v->g, Ly = v->cfg.layers, O = v->cfg.out_dim, H = v->cfg.heads;
   const int M = S * T, Mp = S * g * g;
-  const size_t Mmax = (size_t)v->cfg.max_batch * T;
   int e;
   // patch embedding
   {
@@ -348,27 +365,30 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, float* emb, in
   }
   for (int l = 0; l < Ly; ++l) {
     const LayerW& w = v->L[l];
+    // the last block runs on the cls rows after attention: out_proj reads rows s*T of attn_out and x_in (stride T*D)
+    const bool last = l == Ly - 1;
+    const int Mr = last ? S : M, ld_tok = last ? T * D : 0;
     float* x_in = v->xs[2 * l]; float* x_mid = v->xs[2 * l + 1]; float* x_out = v->xs[2 * l + 2];
-    float* mean1 = v->st_mean + (size_t)(1 + 2 * l) * Mmax; float* rstd1 = v->st_rstd + (size_t)(1 + 2 * l) * Mmax;
-    float* mean2 = mean1 + Mmax; float* rstd2 = rstd1 + Mmax;
+    float* mean1 = v->st_mean + stat_off(v, 1 + 2 * l); float* rstd1 = v->st_rstd + stat_off(v, 1 + 2 * l);
+    float* mean2 = v->st_mean + stat_off(v, 2 + 2 * l); float* rstd2 = v->st_rstd + stat_off(v, 2 + 2 * l);
     NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, x_in, (size_t)D, w.ln1_w, w.ln1_b, v->ln_out, mean1, rstd1, M, D)));
     APH_LAUNCH_OK();
     { GemmEpi ep; ep.bias = w.b_qkv; ep.out_bf16 = v->qkv[l];
       if ((e = launch_gemm(v->ln_out, w.w_qkv, GemmShape{M, 3 * D, D}, ep, st))) return e; }
     if (attn_simt()) { k_attn_fwd<<<S * H, 256, attn_fwd_smem(T), st>>>(v->qkv[l], v->attn_out, T, D, H); APH_LAUNCH_OK(); }
     else if ((e = attn_dispatch(true, v->qkv[l], nullptr, v->attn_out, S, T, D, H, st))) return e;
-    { GemmEpi ep; ep.bias = w.b_o; ep.resid = x_in; ep.out_f32 = x_mid;
-      if ((e = launch_gemm(v->attn_out, w.w_o, GemmShape{M, D, D}, ep, st))) return e; }
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, x_mid, (size_t)D, w.ln2_w, w.ln2_b, v->ln_out, mean2, rstd2, M, D)));
+    { GemmEpi ep; ep.bias = w.b_o; ep.resid = x_in; ep.ld_resid = ld_tok; ep.out_f32 = x_mid;
+      if ((e = launch_gemm(v->attn_out, w.w_o, GemmShape{Mr, D, D}, ep, st, ld_tok))) return e; }
+    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(Mr)), dim3(256), (size_t)0, st, 1, x_mid, (size_t)D, w.ln2_w, w.ln2_b, v->ln_out, mean2, rstd2, Mr, D)));
     APH_LAUNCH_OK();
     { GemmEpi ep; ep.bias = w.b_fc; ep.out_pre = v->h_pre[l]; ep.act = 1; ep.out_bf16 = v->h_act;
-      if ((e = launch_gemm(v->ln_out, w.w_fc, GemmShape{M, 4 * D, D}, ep, st))) return e; }
+      if ((e = launch_gemm(v->ln_out, w.w_fc, GemmShape{Mr, 4 * D, D}, ep, st))) return e; }
     { GemmEpi ep; ep.bias = w.b_proj; ep.resid = x_mid; ep.out_f32 = x_out;
-      if ((e = launch_gemm(v->h_act, w.w_proj, GemmShape{M, D, 4 * D}, ep, st))) return e; }
+      if ((e = launch_gemm(v->h_act, w.w_proj, GemmShape{Mr, D, 4 * D}, ep, st))) return e; }
   }
   {
-    float* meanp = v->st_mean + (size_t)(2 * Ly + 1) * Mmax; float* rstdp = v->st_rstd + (size_t)(2 * Ly + 1) * Mmax;
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(S)), dim3(256), (size_t)0, st, 1, v->xs[2 * Ly], (size_t)T * D, v->lnpost_w, v->lnpost_b, v->cls_ln,
+    float* meanp = v->st_mean + stat_off(v, 2 * Ly + 1); float* rstdp = v->st_rstd + stat_off(v, 2 * Ly + 1);
+    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(S)), dim3(256), (size_t)0, st, 1, v->xs[2 * Ly], (size_t)D, v->lnpost_w, v->lnpost_b, v->cls_ln,
                                                                  meanp, rstdp, S, D)));
     APH_LAUNCH_OK();
     GemmEpi ep; ep.out_f32 = v->emb_int;
@@ -395,42 +415,48 @@ extern "C" int aph_vit_bwd(aph_vit* vit, const float* grad_emb, int S, float* gr
   const int rc = run_cached(v->bwd_graphs, v->warm_bwd, v->stamp, v->graph_misses, nullptr, nullptr, S, 0, st, [&]() -> int {
   const int D = v->D, T = v->T, Ly = v->cfg.layers, O = v->cfg.out_dim, H = v->cfg.heads;
   const int M = S * T;
-  const size_t Mmax = (size_t)v->cfg.max_batch * T;
   int e;
   {
     GemmEpi ep; ep.out_f32 = v->d_cls;
     if ((e = launch_gemm(v->d_emb, v->w_out_t, GemmShape{S, D, O}, ep, st))) return e;
-    APH_CUDA_OK(cudaMemsetAsync(v->dx, 0, (size_t)M * D * sizeof(float), st));
-    APH_CUDA_OK(cudaMemsetAsync(v->dx_bf, 0, (size_t)M * D * sizeof(bf16), st));
-    float* meanp = v->st_mean + (size_t)(2 * Ly + 1) * Mmax; float* rstdp = v->st_rstd + (size_t)(2 * Ly + 1) * Mmax;
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH>, dim3(rows_grid(S)), dim3(256), (size_t)0, st, 1, v->d_cls, v->xs[2 * Ly], meanp, rstdp, v->lnpost_w, v->dx, v->dx_bf,
-                                                                 S, T, D, 1, 0)));
+    // ln_post: the gradient reaching the last block is non-zero on its cls rows only; it is kept compact in dxc / dxc_bf
+    float* meanp = v->st_mean + stat_off(v, 2 * Ly + 1); float* rstdp = v->st_rstd + stat_off(v, 2 * Ly + 1);
+    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH>, dim3(rows_grid(S)), dim3(256), (size_t)0, st, 1, v->d_cls, v->xs[2 * Ly], meanp, rstdp, v->lnpost_w, v->dxc, v->dxc_bf,
+                                                                 S, T, D, 0, 0, (const float*)nullptr)));
     APH_LAUNCH_OK();
   }
   for (int l = Ly - 1; l >= 0; --l) {
     const LayerW& w = v->L[l];
+    // the last block's MLP and out_proj run on its S cls rows: their gradient is dxc; d out_proj lands on rows s*T of d_attn_last
+    const bool last = l == Ly - 1;
+    const int Mr = last ? S : M;
+    float* gx = last ? v->dxc : v->dx; bf16* gx_bf = last ? v->dxc_bf : v->dx_bf; bf16* d_attn = last ? v->d_attn_last : v->d_attn;
     float* x_in = v->xs[2 * l]; float* x_mid = v->xs[2 * l + 1];
-    float* mean1 = v->st_mean + (size_t)(1 + 2 * l) * Mmax; float* rstd1 = v->st_rstd + (size_t)(1 + 2 * l) * Mmax;
-    float* mean2 = mean1 + Mmax; float* rstd2 = rstd1 + Mmax;
+    float* mean1 = v->st_mean + stat_off(v, 1 + 2 * l); float* rstd1 = v->st_rstd + stat_off(v, 1 + 2 * l);
+    float* mean2 = v->st_mean + stat_off(v, 2 + 2 * l); float* rstd2 = v->st_rstd + stat_off(v, 2 + 2 * l);
     // MLP branch: dh = (dx . W_proj) * gelu'(h); d_ln2 = dh . W_fc
     { GemmEpi ep; ep.gelu_in = v->h_pre[l]; ep.out_bf16 = v->dh;
-      if ((e = launch_gemm(v->dx_bf, w.w_proj_t, GemmShape{M, 4 * D, D}, ep, st))) return e; }
+      if ((e = launch_gemm(gx_bf, w.w_proj_t, GemmShape{Mr, 4 * D, D}, ep, st))) return e; }
     { GemmEpi ep; ep.out_bf16 = v->d_ln;
-      if ((e = launch_gemm(v->dh, w.w_fc_t, GemmShape{M, D, 4 * D}, ep, st))) return e; }
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH, bf16>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, v->d_ln, x_mid, mean2, rstd2, w.ln2_w, v->dx, v->dx_bf, M, T, D, 0, 1)));
+      if ((e = launch_gemm(v->dh, w.w_fc_t, GemmShape{Mr, D, 4 * D}, ep, st))) return e; }
+    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH, bf16>, dim3(rows_grid(Mr)), dim3(256), (size_t)0, st, 1, v->d_ln, x_mid, mean2, rstd2, w.ln2_w, gx, gx_bf, Mr, T, D, 0, 1,
+                                         (const float*)nullptr)));
     APH_LAUNCH_OK();
     // attention branch: d_attn = dx . W_o; (dq,dk,dv) = attn'(...); d_ln1 = d_qkv . W_qkv
-    { GemmEpi ep; ep.out_bf16 = v->d_attn;
-      if ((e = launch_gemm(v->dx_bf, w.w_o_t, GemmShape{M, D, D}, ep, st))) return e; }
-    if (attn_simt()) { k_attn_bwd<<<S * H, 256, attn_bwd_smem(T), st>>>(v->qkv[l], v->d_attn, v->d_qkv, T, D, H); APH_LAUNCH_OK(); }
-    else if ((e = attn_dispatch(false, v->qkv[l], v->d_attn, v->d_qkv, S, T, D, H, st))) return e;
+    { GemmEpi ep; ep.out_bf16 = d_attn; ep.ld_out = last ? T * D : 0;
+      if ((e = launch_gemm(gx_bf, w.w_o_t, GemmShape{Mr, D, D}, ep, st))) return e; }
+    if (attn_simt()) { k_attn_bwd<<<S * H, 256, attn_bwd_smem(T), st>>>(v->qkv[l], d_attn, v->d_qkv, T, D, H); APH_LAUNCH_OK(); }
+    else if ((e = attn_dispatch(false, v->qkv[l], d_attn, v->d_qkv, S, T, D, H, st))) return e;
     { GemmEpi ep; ep.out_bf16 = v->d_ln;
       if ((e = launch_gemm(v->d_qkv, w.w_qkv_t, GemmShape{M, D, 3 * D}, ep, st))) return e; }
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH, bf16>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, v->d_ln, x_in, mean1, rstd1, w.ln1_w, v->dx, v->dx_bf, M, T, D, 0, 1)));
+    // ln_1: back to all M rows; in the last block dx is written here for the first time (+ dxc on the cls rows)
+    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH, bf16>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, v->d_ln, x_in, mean1, rstd1, w.ln1_w, v->dx, v->dx_bf, M, T, D,
+                                         last ? 1 : 0, 1, (const float*)(last ? v->dxc : nullptr))));
     APH_LAUNCH_OK();
   }
   // ln_pre backward (cls rows dropped) and patch-embed data gradient scattered back to NCHW
-  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, v->dx, v->e, v->st_mean, v->st_rstd, v->lnpre_w, nullptr, v->d_tok, M, T, D, 2, 0)));
+  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, v->dx, v->e, v->st_mean, v->st_rstd, v->lnpre_w, nullptr, v->d_tok, M, T, D, 2, 0,
+                                       (const float*)nullptr)));
   APH_LAUNCH_OK();
   return 0;
   });

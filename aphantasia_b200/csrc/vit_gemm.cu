@@ -23,12 +23,14 @@ static EncodeTiledFn get_encode() {
   return fn;
 }
 
-int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int K, int box_rows) {
+int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int K, int box_rows, int64_t row_stride) {
   EncodeTiledFn enc = get_encode();
   APH_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
-  APH_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && K % 8 == 0, "tensor map: base/stride not 16-byte aligned");
+  if (row_stride == 0) row_stride = K;
+  APH_REQUIRE(row_stride >= K, "tensor map: row stride %lld < K=%d", (long long)row_stride, K);
+  APH_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && row_stride % 8 == 0, "tensor map: base/stride not 16-byte aligned");
   const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  const cuuint64_t gstride[1] = {(cuuint64_t)K * 2};
+  const cuuint64_t gstride[1] = {(cuuint64_t)row_stride * 2};
   const cuuint32_t box[2] = {(cuuint32_t)GEMM_BK, (cuuint32_t)box_rows};
   const cuuint32_t estr[2] = {1, 1};
   const CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
@@ -67,7 +69,7 @@ static std::vector<double> g_prof_flops;
 static std::atomic<long long> g_variant_launches[2][EPI_KINDS];
 
 template <int BN, bool PINGPONG, int EPI>
-static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st) {
+static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st, int lda) {
   using L = GemmCfg<BN>;
   static_assert(L::SMEM <= 227 * 1024, "GEMM shared-memory budget");
   g_variant_launches[(PINGPONG || BN == 256) ? 1 : 0][EPI].fetch_add(1, std::memory_order_relaxed);
@@ -77,7 +79,7 @@ static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi
     configured = true;
   }
   CUtensorMap ma, mb;
-  if (int e = make_tmap_bf16(&ma, A, shp.M, shp.K, GEMM_BM)) return e;
+  if (int e = make_tmap_bf16(&ma, A, shp.M, shp.K, GEMM_BM, lda)) return e;
   if (int e = make_tmap_bf16(&mb, B, shp.N, shp.K, BN)) return e;
   const int tiles = ((shp.M + GEMM_BM - 1) / GEMM_BM) * (shp.N / BN);
   const int grid = tiles < num_sms() ? tiles : num_sms();
@@ -89,13 +91,20 @@ static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi
   return 0;
 }
 
-int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st) {
+int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi_in, cudaStream_t st, int lda) {
   APH_REQUIRE(A && B && shp.M > 0, "gemm: null operand or empty M");
   APH_REQUIRE(shp.K % GEMM_BK == 0 && shp.K > 0, "gemm: K=%d must be a positive multiple of %d", shp.K, GEMM_BK);
   APH_REQUIRE(shp.N % 128 == 0 && shp.N > 0, "gemm: N=%d must be a positive multiple of 128", shp.N);
+  APH_REQUIRE(lda == 0 || lda >= shp.K, "gemm: lda=%d < K=%d", lda, shp.K);
+  APH_REQUIRE((epi_in.ld_out == 0 || epi_in.ld_out >= shp.N) && (epi_in.ld_resid == 0 || epi_in.ld_resid >= shp.N),
+              "gemm: output / residual row stride below N=%d", shp.N);
+  GemmEpi epi = epi_in;                       // the kernel reads resolved strides
+  if (epi.ld_out == 0) epi.ld_out = shp.N;
+  if (epi.ld_resid == 0) epi.ld_resid = shp.N;
   // map the requested fusion onto one of the compiled epilogue kinds
   int kind = -1;
   const bool b = epi.bias, r = epi.resid, gi = epi.gelu_in, f = epi.out_f32, h = epi.out_bf16, pre = epi.out_pre, act = epi.act == 1, un = epi.unpatch_p > 0;
+  APH_REQUIRE(!un || epi.ld_out == shp.N, "gemm: the un-patchify store takes no output stride");
   if (un && f && !b && !r && !gi && !h && !pre && !act) kind = EPI_UNPATCH;
   else if (f && !h && !b && !r && !gi && !pre && !act) kind = EPI_F32;
   else if (h && !f && !b && !r && !gi && !pre && !act) kind = EPI_BF16;
@@ -105,7 +114,9 @@ int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi,
   else if (h && !f && !b && !r && gi && !pre && !act) kind = EPI_GELUGRAD_BF16;
   APH_REQUIRE(kind >= 0, "gemm: unsupported epilogue combination");
   const uintptr_t bf16_ptrs = reinterpret_cast<uintptr_t>(epi.out_bf16) | reinterpret_cast<uintptr_t>(epi.out_pre) | reinterpret_cast<uintptr_t>(epi.gelu_in);
-  APH_REQUIRE((bf16_ptrs & 15) == 0, "gemm: bf16 epilogue operands must be 16-byte aligned (8 columns are stored per lane)");
+  APH_REQUIRE((bf16_ptrs & 15) == 0 && ((size_t)epi.ld_out * (f ? 4 : 2)) % 16 == 0 && ((size_t)epi.ld_resid * 4) % 16 == 0 &&
+              ((size_t)lda * 2) % 16 == 0,
+              "gemm: bf16 epilogue operands and row strides must be 16-byte aligned (8 columns are stored per lane)");
   // The ping-pong kernel overlaps one consumer's epilogue with the other's mainloop, which needs two tiles per SM in flight. It is
   // chosen when there are at least twice as many 128 x 128 tiles as SMs and K is short (K = 768 in the encoder), so that the
   // epilogue is a large share of a tile's time. With long K the mainloop dominates and the cooperative 128 x 256 tile wins: its
@@ -113,8 +124,8 @@ int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi,
   const int m_tiles = (shp.M + GEMM_BM - 1) / GEMM_BM;
   const bool pingpong = m_tiles * (shp.N / 128) >= 2 * num_sms() && shp.K <= 1024;
   const bool wide = !pingpong && shp.N % 256 == 0 && m_tiles * (shp.N / 256) >= num_sms();
-#define APH_GEMM_CASE(K) case K: return pingpong ? launch_cfg<128, true, K>(A, B, shp, epi, st) \
-                                                 : wide ? launch_cfg<256, false, K>(A, B, shp, epi, st) : launch_cfg<128, false, K>(A, B, shp, epi, st);
+#define APH_GEMM_CASE(K) case K: return pingpong ? launch_cfg<128, true, K>(A, B, shp, epi, st, lda) \
+                                                 : wide ? launch_cfg<256, false, K>(A, B, shp, epi, st, lda) : launch_cfg<128, false, K>(A, B, shp, epi, st, lda);
   switch (kind) {
     APH_GEMM_CASE(EPI_F32) APH_GEMM_CASE(EPI_BF16) APH_GEMM_CASE(EPI_BIAS_BF16) APH_GEMM_CASE(EPI_BIAS_GELU)
     APH_GEMM_CASE(EPI_BIAS_RESID) APH_GEMM_CASE(EPI_GELUGRAD_BF16) APH_GEMM_CASE(EPI_UNPATCH)
@@ -144,6 +155,17 @@ extern "C" int aph_gemm_epi_test(const void* A, const void* B, int M, int N, int
   epi.out_f32 = out_f32; epi.out_bf16 = reinterpret_cast<bf16*>(out_bf16); epi.out_pre = reinterpret_cast<bf16*>(out_pre);
   epi.unpatch_p = unpatch_p; epi.unpatch_g = unpatch_g;
   return launch_gemm(A, B, GemmShape{M, N, K}, epi, (cudaStream_t)stream);
+}
+
+// Same with row strides in elements (0 = dense) for A, the residual and the outputs (tests/test_vit_last_block_gpu.py).
+extern "C" int aph_gemm_epi_strided_test(const void* A, int lda, const void* B, int M, int N, int K, const float* bias,
+                                         const float* resid, int ld_resid, const void* gelu_in, int act, float* out_f32,
+                                         void* out_bf16, void* out_pre, int ld_out, void* stream) {
+  GemmEpi epi;
+  epi.bias = bias; epi.resid = resid; epi.gelu_in = reinterpret_cast<const bf16*>(gelu_in); epi.act = act;
+  epi.out_f32 = out_f32; epi.out_bf16 = reinterpret_cast<bf16*>(out_bf16); epi.out_pre = reinterpret_cast<bf16*>(out_pre);
+  epi.ld_resid = ld_resid; epi.ld_out = ld_out;
+  return launch_gemm(A, B, GemmShape{M, N, K}, epi, (cudaStream_t)stream, lda);
 }
 
 // launches so far of kernel variant `variant` (0: the small-problem kernel, 1: the large-problem kernels) with

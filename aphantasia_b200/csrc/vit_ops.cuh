@@ -165,36 +165,36 @@ __device__ __forceinline__ void ln_bwd_row(float (&v)[N], const float (&xv)[N], 
   }
 }
 
-// mode 0: all rows: dx[row] (+)= LNbwd(dy[row]); writes dx (fp32) and dx_bf16.        (ln_1 / ln_2)
-// mode 1: ln_post: dy has S rows (cls only); dx[s*T] = LNbwd, other rows were zeroed by the caller.
+// mode 0: all rows: dx[row] (+)= LNbwd(dy[row]); writes dx (fp32) and dx_bf16.        (ln_1 / ln_2, ln_post on its S rows)
+// mode 1: ln_1 of the last block, whose residual gradient lives on the cls rows only, compact in dcls [S, D]:
+//         dx[row] = LNbwd(dy[row]) + (row = s*T ? dcls[s] : 0); writes every row of dx and dx_bf16, reads no dx.
 // mode 2: ln_pre : dy = dx itself (all rows); writes only non-cls rows as bf16 into dtok [S*(T-1), D].
 template <int NCH, typename DY = float>
 __global__ void __launch_bounds__(256) k_ln_bwd(const DY* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ mean,
                                                 const float* __restrict__ rstd, const float* __restrict__ gamma,
                                                 float* __restrict__ dx, bf16* __restrict__ dx_bf16, int rows, int T, int D,
-                                                int mode, int accumulate) {
+                                                int mode, int accumulate, const float* __restrict__ dcls) {
   pdl_trigger(); pdl_wait();
   const int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (r >= rows) return;
   constexpr int N = 4 * NCH;
-  const size_t row = (mode == 1) ? (size_t)r * T : (size_t)r;      // token row in x / dx
+  const size_t row = (size_t)r;
   if (mode == 2 && (r % T) == 0) return;                           // the cls row has no patch behind it
   float v[N], xv[N], gm[N];
-  load_row(dy + (size_t)r * D, v, lane);
+  load_row(dy + row * D, v, lane);
   load_row(x + row * D, xv, lane);
   load_row(gamma, gm, lane);
-  const int sidx = (mode == 1) ? r : (int)row;
-  ln_bwd_row(v, xv, gm, mean[sidx], rstd[sidx], D);
+  ln_bwd_row(v, xv, gm, mean[row], rstd[row], D);
   if (mode == 2) {
     const int s = r / T, t = r - s * T;
     store_row_bf16(dx_bf16 + ((size_t)s * (T - 1) + (t - 1)) * D, v, lane);
     return;
   }
-  if (accumulate) {
+  if (mode == 1 ? (r % T) == 0 : accumulate != 0) {
     float a[N];
-    load_row(dx + row * D, a, lane);
+    load_row(mode == 1 ? dcls + (size_t)(r / T) * D : dx + row * D, a, lane);
     #pragma unroll
-  for (int i = 0; i < N; ++i) v[i] += a[i];
+    for (int i = 0; i < N; ++i) v[i] += a[i];
   }
   store_row_f32(dx + row * D, v, lane);
   store_row_bf16(dx_bf16 + row * D, v, lane);

@@ -219,6 +219,12 @@ int aph_gemm_bf16_tn(const void* A, const void* B, float* C, int M, int N, int K
 int aph_gemm_epi_test(const void* A, const void* B, int M, int N, int K, const float* bias, const float* resid,
                       const void* gelu_in, int act, float* out_f32, void* out_bf16, void* out_pre,
                       int unpatch_p, int unpatch_g, void* stream);
+/* aph_gemm_epi_strided_test: the same without un-patchify, with row strides in elements (0 = dense) for A (lda), the residual
+ * (ld_resid) and the outputs and gelu_in (ld_out), as the encoder's last block reads and writes its class-token rows.
+ * Strides must be multiples of 16 bytes; rows between the strided output rows are not written.                      */
+int aph_gemm_epi_strided_test(const void* A, int lda, const void* B, int M, int N, int K, const float* bias,
+                              const float* resid, int ld_resid, const void* gelu_in, int act, float* out_f32,
+                              void* out_bf16, void* out_pre, int ld_out, void* stream);
 int64_t aph_gemm_variant_launches(int variant, int epi);
 
 /* Profiling aid: enable=1 records a CUDA-event pair around every GEMM launch of this library; enable=0 stops and returns
