@@ -58,6 +58,10 @@ _SIGS = {
     'aph_gemm_epi_strided_test': (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, C.c_int, C.c_void_p,
                                             C.c_int, c_f32p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     'aph_gemm_variant_launches': (C.c_int64, [C.c_int, C.c_int]),
+    'aph_attn_test': (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    'aph_ln_fwd_test': (C.c_int, [c_f32p, c_f32p, c_f32p, C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, C.c_void_p]),
+    'aph_ln_bwd_test': (C.c_int, [C.c_void_p, C.c_int, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                  C.c_int, c_f32p, C.c_void_p]),
     'aph_prof_gemm': (C.c_int, [C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int)]),
     'aph_sim_fwd': (C.c_int, [c_f32p, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, c_f32p, C.c_void_p]),
     'aph_derivat_fwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p, c_f32p, C.c_void_p]),

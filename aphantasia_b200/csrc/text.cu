@@ -144,6 +144,11 @@ int attn_causal(const bf16* qkv, bf16* out, int S, int T, int D, int heads, cuda
 }
 
 }  // namespace
+
+// the text tower's causal attention, for the test entry aph_attn_test (vit.cu)
+int attn_causal_test(const bf16* qkv, bf16* out, int S, int T, int D, int heads, cudaStream_t st) {
+  return attn_causal(qkv, out, S, T, D, heads, st);
+}
 }  // namespace aph
 
 using namespace aph;

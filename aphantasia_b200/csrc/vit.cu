@@ -467,3 +467,46 @@ extern "C" int aph_vit_bwd(aph_vit* vit, const float* grad_emb, int S, float* gr
     if (int e = launch_gemm(v->d_tok, v->w_conv_t, GemmShape{Mp, v->Kp, v->D}, ep, st)) return e; }
   return 0;
 }
+
+namespace aph { int attn_causal_test(const bf16* qkv, bf16* out, int S, int T, int D, int heads, cudaStream_t st); }   // text.cu
+
+// Test entries (tests/test_encoder_kernels_gpu.py): the encoder's attention and LayerNorm kernels on caller-supplied operands,
+// dispatched exactly as the encoder (and, for causal attention, the text tower) dispatches them.
+extern "C" int aph_attn_test(int fwd, int causal, const void* qkv, const void* dout, void* out, int S, int T, int D, int heads, void* stream) {
+  APH_REQUIRE(qkv && out && (fwd || dout), "aph_attn_test: null argument");
+  APH_REQUIRE(S > 0 && T > 0 && heads > 0 && D == 64 * heads, "aph_attn_test: S=%d T=%d D=%d heads=%d (head dim must be 64)", S, T, D, heads);
+  const bf16* q = reinterpret_cast<const bf16*>(qkv);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (causal) {
+    APH_REQUIRE(fwd, "aph_attn_test: causal attention has no backward");
+    return attn_causal_test(q, reinterpret_cast<bf16*>(out), S, T, D, heads, st);
+  }
+  return attn_dispatch(fwd != 0, q, reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(out), S, T, D, heads, st);
+}
+
+extern "C" int aph_ln_fwd_test(const float* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows, int D,
+                               void* stream) {
+  APH_REQUIRE(x && gamma && beta && y && mean && rstd && rows > 0 && D % 128 == 0, "aph_ln_fwd_test: null argument or rows=%d D=%d", rows, D);
+  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(rows)), dim3(256), (size_t)0, (cudaStream_t)stream, 1, x, (size_t)D, gamma,
+                                       beta, reinterpret_cast<bf16*>(y), mean, rstd, rows, D)));
+  APH_LAUNCH_OK();
+  return 0;
+}
+
+extern "C" int aph_ln_bwd_test(const void* dy, int dy_bf16, const float* x, const float* mean, const float* rstd, const float* gamma, float* dx,
+                               void* dx_bf16, int rows, int T, int D, int mode, int accumulate, const float* dcls, void* stream) {
+  APH_REQUIRE(dy && x && mean && rstd && gamma && dx_bf16 && rows > 0 && T > 0 && D % 128 == 0, "aph_ln_bwd_test: null argument or rows=%d T=%d D=%d",
+              rows, T, D);
+  APH_REQUIRE(mode >= 0 && mode <= 2 && (mode == 2 || dx) && (mode != 1 || dcls), "aph_ln_bwd_test: mode %d needs dx%s", mode,
+              mode == 1 ? " and dcls" : "");
+  cudaStream_t st = (cudaStream_t)stream;
+  bf16* dxb = reinterpret_cast<bf16*>(dx_bf16);
+  if (dy_bf16)
+    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH, bf16>, dim3(rows_grid(rows)), dim3(256), (size_t)0, st, 1, reinterpret_cast<const bf16*>(dy), x,
+                                         mean, rstd, gamma, dx, dxb, rows, T, D, mode, accumulate, dcls)))
+  else
+    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH>, dim3(rows_grid(rows)), dim3(256), (size_t)0, st, 1, reinterpret_cast<const float*>(dy), x,
+                                         mean, rstd, gamma, dx, dxb, rows, T, D, mode, accumulate, dcls)))
+  APH_LAUNCH_OK();
+  return 0;
+}

@@ -226,6 +226,19 @@ int aph_gemm_epi_strided_test(const void* A, int lda, const void* B, int M, int 
                               const float* resid, int ld_resid, const void* gelu_in, int act, float* out_f32,
                               void* out_bf16, void* out_pre, int ld_out, void* stream);
 int64_t aph_gemm_variant_launches(int variant, int epi);
+/* aph_attn_test: the encoder's attention core on caller operands. qkv bf16 [S*T, 3*D] (q | k | v), D = 64*heads.
+ * fwd = 1: out bf16 [S*T, D]; fwd = 0: dout bf16 [S*T, D] in, out = dqkv bf16 [S*T, 3*D]. causal = 0 runs the image
+ * tower's dispatch (T <= 256), causal = 1 the text tower's causal forward (T <= 112; there is no causal backward).
+ * Unsupported shapes return an error and launch nothing.
+ * aph_ln_fwd_test: k_ln_fwd on x fp32 [rows, D] (row stride D) -> y bf16 [rows, D], mean / rstd fp32 [rows].
+ * aph_ln_bwd_test: k_ln_bwd with dy fp32 (dy_bf16 = 0) or bf16 (dy_bf16 = 1) [rows, D]; mode 0: dx (+)= LN'(dy) (fp32 dx and
+ * bf16 dx_bf16, accumulate = 1 adds to dx); mode 1: dx = LN'(dy) + dcls[s] on rows s*T (dcls fp32 [rows/T, D]); mode 2:
+ * the non-class rows into dx_bf16 = dtok bf16 [rows/T*(T-1), D], dx unused. D in {128, 256, 512, 768, 1024}.            */
+int aph_attn_test(int fwd, int causal, const void* qkv, const void* dout, void* out, int S, int T, int D, int heads, void* stream);
+int aph_ln_fwd_test(const float* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows, int D,
+                    void* stream);
+int aph_ln_bwd_test(const void* dy, int dy_bf16, const float* x, const float* mean, const float* rstd, const float* gamma, float* dx,
+                    void* dx_bf16, int rows, int T, int D, int mode, int accumulate, const float* dcls, void* stream);
 
 /* Profiling aid: enable=1 records a CUDA-event pair around every GEMM launch of this library; enable=0 stops and returns
  * the summed kernel time (ms), FLOPs (sum of 2MNK) and launch count since enabling (bench.py's roofline).            */
