@@ -45,6 +45,8 @@ _SIGS = {
     'aph_vit_patch_operand': (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     'aph_vit_fwd_prepatched': (C.c_int, [C.c_void_p, C.c_int, c_f32p, C.c_int, C.c_void_p]),
     'aph_vit_bwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, c_f32p, C.c_void_p]),
+    'aph_vit_fwd_sized': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, C.c_void_p]),
+    'aph_vit_bwd_sized': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     'aph_vit_bytes': (C.c_int64, [C.c_void_p]),
     'aph_text_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p]),
     'aph_text_destroy': (C.c_int, [C.c_void_p]),

@@ -19,12 +19,17 @@ def register(vis):
     _consumers.add(vis)
 
 
-def target(size):
-    """The one live encoder that will consume [*,3,size,size] batches, or None."""
+def target(size, windowed=False):
+    """The one live encoder that will consume [*,3,size,size] batches, or None. windowed: the batch may be larger than the
+    encoder's input resolution r by less than one patch (r <= size < r + patch, the size + 8 batches of transforms_custom /
+    transforms_elastic): conv1 reads its top-left r x r window, and that window is the operand."""
     if os.environ.get('APH_PATCH_FUSE', '1') == '0':
         return None
     live = list(_consumers)
-    if len(live) != 1 or live[0].input_resolution != size:
+    if len(live) != 1:
+        return None
+    r = live[0].input_resolution
+    if not (r == size or (windowed and r <= size < r + live[0].patch_size)):
         return None
     return live[0]
 

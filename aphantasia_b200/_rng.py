@@ -26,10 +26,17 @@ F_PERSP = 4          # 8 floats a..h  (output -> input mapping, torchvision conv
 F_ER_I, F_ER_J, F_ER_H, F_ER_W = 12, 13, 14, 15
 F_ROT = 16           # theta00, theta01, theta10, theta11 (inverse affine matrix, float32)
 F_ANGLE = 20         # degrees (informational)
-FLAG_PERSP, FLAG_ERASE, FLAG_ROT = 1, 2, 4
+F_JIT_DX, F_JIT_DY = 21, 22    # custom / elastic: integer jitter shift
+FLAG_PERSP, FLAG_ERASE, FLAG_ROT, FLAG_JITTER, FLAG_ELASTIC = 1, 2, 4, 8, 16
 
 # transform kinds understood by the fused sampler
-TF_NONE, TF_NORMALIZE, TF_FAST = 0, 1, 2
+TF_NONE, TF_NORMALIZE, TF_FAST, TF_CUSTOM, TF_ELASTIC = 0, 1, 2, 3, 4
+KORNIA_PAD = 4       # pad(4) of transforms_custom / transforms_elastic: their output side is size + 8
+
+
+def out_side(size, kind):
+    """Side of the crops slice_imgs returns for transform `kind`."""
+    return size + 2 * KORNIA_PAD if kind in (TF_CUSTOM, TF_ELASTIC) else size
 
 FAST_ANGLES = list(range(-30, 30)) + 20 * [0]   # reference transforms.py:168
 PERSP_DISTORTION, PERSP_P = 0.33, 0.2           # reference transforms.py:166
@@ -55,6 +62,53 @@ def inverse_rotation_matrix(angle):
     return [d, -b, -c, a]
 
 
+def kornia_inverse_rotation(angle):
+    """Pixel-space inverse of kornia's get_rotation_matrix2d (OpenCV convention: positive = counter-clockwise on screen):
+    source = c + [[cos, -sin], [sin, cos]] (dest - c), as [r00, r01, r10, r11]."""
+    rot = math.radians(angle)
+    return [math.cos(rot), -math.sin(rot), math.sin(rot), math.cos(rot)]
+
+
+def draw_erase(row, side):
+    """RandomErasing(p=0.2), value=0 (torchvision transforms.py:1697-1727) on an image of side `side`: FLAG_ERASE or 0."""
+    if not torch.rand(1) < ERASE_P:
+        return 0
+    area = side * side
+    log_ratio = torch.log(torch.tensor(ERASE_RATIO))
+    for _ in range(10):
+        erase_area = area * torch.empty(1).uniform_(ERASE_SCALE[0], ERASE_SCALE[1]).item()
+        aspect = torch.exp(torch.empty(1).uniform_(log_ratio[0], log_ratio[1])).item()
+        h = int(round(math.sqrt(erase_area * aspect)))
+        w = int(round(math.sqrt(erase_area / aspect)))
+        if not (h < side and w < side):
+            continue
+        i = torch.randint(0, side - h + 1, size=(1,)).item()
+        j = torch.randint(0, side - w + 1, size=(1,)).item()
+        row[F_ER_I], row[F_ER_J], row[F_ER_H], row[F_ER_W] = i, j, h, w
+        return FLAG_ERASE
+    return 0
+
+
+def draw_kornia(row, size, elastic):
+    """Draws one crop's transforms_custom / transforms_elastic parameters into `row` (reference transforms.py:147-163, in order):
+    elastic only: RandomErasing on the padded (size + 8) image (torch); random_rotate: np.random.choice(angles); elastic only:
+    random_elastic's rand(2), randint(8, 64), rand() (zero noise: drawn, without effect on the output); jitter(8): dx, dy."""
+    flags = FLAG_ROT | FLAG_JITTER
+    if elastic:
+        flags |= draw_erase(row, size + 2 * KORNIA_PAD)
+    angle = float(np.random.choice(FAST_ANGLES))
+    row[F_ROT:F_ROT + 4] = kornia_inverse_rotation(angle)
+    row[F_ANGLE] = angle
+    if elastic:
+        np.random.rand(2)
+        np.random.randint(8, 64)
+        np.random.rand()
+        flags |= FLAG_ELASTIC
+    row[F_JIT_DX] = np.random.choice(8)
+    row[F_JIT_DY] = np.random.choice(8)
+    return flags
+
+
 def draw_fast(row, size):
     """Draws one crop's transforms_fast parameters into `row` (numpy float32 view), reference order."""
     flags = 0
@@ -70,22 +124,7 @@ def draw_fast(row, size):
         start = [[0, 0], [size - 1, 0], [size - 1, size - 1], [0, size - 1]]
         row[F_PERSP:F_PERSP + 8] = perspective_coeffs(start, [tl, tr, br, bl])
         flags |= FLAG_PERSP
-    # RandomErasing(p=0.2), value=0
-    if torch.rand(1) < ERASE_P:
-        area = size * size
-        log_ratio = torch.log(torch.tensor(ERASE_RATIO))
-        for _ in range(10):
-            erase_area = area * torch.empty(1).uniform_(ERASE_SCALE[0], ERASE_SCALE[1]).item()
-            aspect = torch.exp(torch.empty(1).uniform_(log_ratio[0], log_ratio[1])).item()
-            h = int(round(math.sqrt(erase_area * aspect)))
-            w = int(round(math.sqrt(erase_area / aspect)))
-            if not (h < size and w < size):
-                continue
-            i = torch.randint(0, size - h + 1, size=(1,)).item()
-            j = torch.randint(0, size - w + 1, size=(1,)).item()
-            row[F_ER_I], row[F_ER_J], row[F_ER_H], row[F_ER_W] = i, j, h, w
-            flags |= FLAG_ERASE
-            break
+    flags |= draw_erase(row, size)
     # random_rotate_fast: always executed, even for angle 0
     angle = float(np.random.choice(FAST_ANGLES))
     row[F_ROT:F_ROT + 4] = inverse_rotation_matrix(angle)
@@ -204,6 +243,8 @@ def draw_crop_table_py(count, canvas_hw, size=224, kind=TF_FAST, align='uniform'
             flags = 0
             if kind == TF_FAST:
                 flags = draw_fast(row, size)
+            elif kind in (TF_CUSTOM, TF_ELASTIC):
+                flags = draw_kornia(row, size, kind == TF_ELASTIC)
             row[F_FLAGS] = flags
         tables.append(tab)
     return tables, (pad_top, pad_left, fh, fw)

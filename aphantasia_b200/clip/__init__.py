@@ -173,7 +173,7 @@ class _EncodeImage(torch.autograd.Function):
             vis.prepatched_forwards += 1
         else:
             vis._patch_gen += 1                 # k_patchify overwrites the operand buffer: outstanding stamps are void
-            check(lib().aph_vit_fwd(vis.handle, xi.data_ptr(), S, emb.data_ptr(), int(need_bwd), stream_ptr()), 'aph_vit_fwd')
+            vis._fwd(xi, S, emb, int(need_bwd))
         _trace.encode()
         ctx.vis, ctx.S, ctx.shape = vis, S, tuple(xi.shape)
         if need_bwd:
@@ -196,11 +196,15 @@ class _EncodeImage(torch.autograd.Function):
             vis._ensure(ctx.S)
             scratch = torch.empty(ctx.S, vis.output_dim, device=g.device, dtype=torch.float32)
             vis._patch_gen += 1
-            check(lib().aph_vit_fwd(vis.handle, xi.data_ptr(), ctx.S, scratch.data_ptr(), 1, stream_ptr()), 'aph_vit_fwd (recompute)')
+            vis._fwd(xi, ctx.S, scratch, 1)
             vis._generation += 1            # the arena now belongs to this call; any other pending backward must recompute too
             vis.recomputes += 1
         gi = _pool.empty(ctx.shape)
-        check(lib().aph_vit_bwd(vis.handle, g.data_ptr(), ctx.S, gi.data_ptr(), stream_ptr()), 'aph_vit_bwd')
+        side = ctx.shape[-1]
+        if side == vis.input_resolution:
+            check(lib().aph_vit_bwd(vis.handle, g.data_ptr(), ctx.S, gi.data_ptr(), stream_ptr()), 'aph_vit_bwd')
+        else:
+            check(lib().aph_vit_bwd_sized(vis.handle, g.data_ptr(), ctx.S, side, gi.data_ptr(), stream_ptr()), 'aph_vit_bwd_sized')
         return gi, None, None
 
 
@@ -252,7 +256,24 @@ class VisionTransformer:
         except Exception:
             pass
 
+    def _fwd(self, xi, S, emb, save_for_bwd):
+        side = xi.shape[-1]
+        if side == self.input_resolution:
+            check(lib().aph_vit_fwd(self.handle, xi.data_ptr(), S, emb.data_ptr(), save_for_bwd, stream_ptr()), 'aph_vit_fwd')
+        else:
+            check(lib().aph_vit_fwd_sized(self.handle, xi.data_ptr(), S, side, emb.data_ptr(), save_for_bwd, stream_ptr()),
+                  'aph_vit_fwd_sized')
+
+    def check_input(self, x):
+        """conv1 (kernel = stride = patch, no padding) takes [S,3,side,side] with r <= side < r + patch (r = input_resolution) and
+        reads its top-left r x r window: the size + 8 batches of transforms_custom / transforms_elastic. Anything else is refused."""
+        r, p = self.input_resolution, self.patch_size
+        if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != x.shape[3] or not r <= x.shape[2] < r + p:
+            raise ValueError('encode_image: expected images [S, 3, side, side] with %d <= side < %d, got %s' % (r, r + p, tuple(x.shape)))
+
     def __call__(self, x):
+        require_cuda(x, 'encode_image input')
+        self.check_input(x)
         return _EncodeImage.apply(x, self, _patchlink.matches(x, self))
 
 

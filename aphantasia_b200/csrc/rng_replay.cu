@@ -67,6 +67,10 @@ struct NumpyGen {      // legacy RandomState: key[624], pos
     do { v = next32() & mask; } while (v > rng);
     return v;
   }
+  inline double rand53() {                         // legacy random_sample / rand(): 53-bit double from two 32-bit draws
+    const uint32_t a = next32() >> 5, b = next32() >> 6;
+    return (a * 67108864.0 + b) / 9007199254740992.0;
+  }
 };
 
 // 8x8 linear solve in double (partial pivoting); the system is the one torchvision's _get_perspective_coeffs builds.
@@ -87,6 +91,51 @@ static bool solve8(double a[8][8], double b[8], double x[8]) {
     x[r] = acc / a[r][r];
   }
   return true;
+}
+
+// RandomErasing(p = 0.2, scale (0.02, 0.33), ratio (0.3, 3.3), value 0) on an image of side `side`: APH_FLAG_ERASE or 0
+static int draw_erase(TorchGen& tg, float* row, int side) {
+  if (!(tg.rand01() < 0.2f)) return 0;
+  const double area = (double)side * side;
+  const float lr0 = logf(0.3f), lr1 = logf(3.3f);          // torch.log(torch.tensor((0.3, 3.3))) in float32
+  for (int it = 0; it < 10; ++it) {
+    const double erase_area = area * (double)tg.uniform(0.02f, 0.33f);
+    const double aspect = (double)(float)exp((double)tg.uniform(lr0, lr1));     // torch.exp on a float32 tensor
+    const int h = (int)nearbyint(sqrt(erase_area * aspect)), w = (int)nearbyint(sqrt(erase_area / aspect));
+    if (!(h < side && w < side)) continue;
+    const int i = (int)tg.randint(0, side - h + 1), j = (int)tg.randint(0, side - w + 1);
+    row[APH_F_ER_I] = (float)i; row[APH_F_ER_J] = (float)j; row[APH_F_ER_H] = (float)h; row[APH_F_ER_W] = (float)w;
+    return APH_FLAG_ERASE;
+  }
+  return 0;
+}
+
+// np.random.choice(list(range(-30, 30)) + 20 * [0]) (transforms.py:160, 168): degrees
+static double draw_angle(NumpyGen& ng) {
+  const uint32_t idx = ng.bounded_masked(79);
+  return idx < 60 ? (double)((int)idx - 30) : 0.0;
+}
+
+// transforms_custom / transforms_elastic (transforms.py:147-163) after slice_imgs' macro draw: [RandomErasing on the padded
+// image (torch)], random_rotate's angle, [random_elastic: rand(2), randint(8, 64), rand()], jitter(8): dx, dy (all NumPy)
+static void draw_kornia(TorchGen& tg, NumpyGen& ng, float* row, int size, bool elastic) {
+  const int s = size + 8;
+  int flags = APH_FLAG_ROT | APH_FLAG_JITTER;
+  if (elastic) flags |= draw_erase(tg, row, s);
+  const double angle = draw_angle(ng);
+  const double rot = angle * (M_PI / 180.0);
+  // kornia get_rotation_matrix2d (OpenCV convention) inverted: source = c + [[cos, -sin], [sin, cos]] (dest - c)
+  row[APH_F_ROT] = (float)cos(rot); row[APH_F_ROT + 1] = (float)(-sin(rot)); row[APH_F_ROT + 2] = (float)sin(rot); row[APH_F_ROT + 3] = (float)cos(rot);
+  row[APH_F_ANGLE] = (float)angle;
+  if (elastic) {        // the noise is zero: alpha, kernel size and sigma are drawn but do not change the output
+    ng.rand53(); ng.rand53();
+    ng.bounded_masked(55);
+    ng.rand53();
+    flags |= APH_FLAG_ELASTIC;
+  }
+  row[APH_F_JIT_DX] = (float)ng.bounded_masked(7);
+  row[APH_F_JIT_DY] = (float)ng.bounded_masked(7);
+  row[APH_F_FLAGS] = (float)flags;
 }
 
 static void draw_fast(TorchGen& tg, NumpyGen& ng, float* row, int size) {
@@ -110,24 +159,9 @@ static void draw_fast(TorchGen& tg, NumpyGen& ng, float* row, int size) {
     }
     if (solve8(a, b, x)) { for (int i = 0; i < 8; ++i) row[APH_F_PERSP + i] = (float)x[i]; flags |= APH_FLAG_PERSP; }
   }
-  // RandomErasing(p = 0.2, scale (0.02, 0.33), ratio (0.3, 3.3), value 0)
-  if (tg.rand01() < 0.2f) {
-    const double area = (double)size * size;
-    const float lr0 = logf(0.3f), lr1 = logf(3.3f);          // torch.log(torch.tensor((0.3, 3.3))) in float32
-    for (int it = 0; it < 10; ++it) {
-      const double erase_area = area * (double)tg.uniform(0.02f, 0.33f);
-      const double aspect = (double)(float)exp((double)tg.uniform(lr0, lr1));     // torch.exp on a float32 tensor
-      const int h = (int)nearbyint(sqrt(erase_area * aspect)), w = (int)nearbyint(sqrt(erase_area / aspect));
-      if (!(h < size && w < size)) continue;
-      const int i = (int)tg.randint(0, size - h + 1), j = (int)tg.randint(0, size - w + 1);
-      row[APH_F_ER_I] = (float)i; row[APH_F_ER_J] = (float)j; row[APH_F_ER_H] = (float)h; row[APH_F_ER_W] = (float)w;
-      flags |= APH_FLAG_ERASE;
-      break;
-    }
-  }
+  flags |= draw_erase(tg, row, size);
   // random_rotate_fast: np.random.choice(list(range(-30, 30)) + 20 * [0]), always applied
-  const uint32_t idx = ng.bounded_masked(79);
-  const double angle = idx < 60 ? (double)((int)idx - 30) : 0.0;
+  const double angle = draw_angle(ng);
   const double rot = angle * (M_PI / 180.0);
   row[APH_F_ROT] = (float)cos(rot); row[APH_F_ROT + 1] = (float)sin(rot); row[APH_F_ROT + 2] = (float)(-sin(rot)); row[APH_F_ROT + 3] = (float)cos(rot);
   row[APH_F_ANGLE] = (float)angle;
@@ -167,6 +201,7 @@ extern "C" int aph_rng_crop_tables(uint8_t* torch_state, int64_t torch_state_byt
       row[APH_F_OFFY] = (float)(int)(py + 0.0f); row[APH_F_OFFX] = (float)(int)(px + 0.0f); row[APH_F_CSIZE] = (float)csize;
       row[APH_F_ROT] = 1.f; row[APH_F_ROT + 3] = 1.f;
       if (kind == APH_TF_FAST) draw_fast(tg, ng, row, size);
+      else if (kind == APH_TF_CUSTOM || kind == APH_TF_ELASTIC) draw_kornia(tg, ng, row, size, kind == APH_TF_ELASTIC);
     }
   }
   tg.store();

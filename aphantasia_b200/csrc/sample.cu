@@ -25,6 +25,7 @@
 #include "aph_common.cuh"
 #include <stdlib.h>
 #include <stdint.h>
+#include <type_traits>
 
 namespace aph {
 
@@ -76,13 +77,21 @@ __device__ __forceinline__ void cubic_taps(int i, float scale, int cs, int idx[4
 
 // bilinear grid_sample taps (align_corners=False, zeros padding) for normalised coords (gx, gy).
 struct Bilin { int x0, y0; float w00, w01, w10, w11; };   // wYX; taps (y0,x0) (y0,x0+1) (y0+1,x0) (y0+1,x0+1)
+template <typename T> __device__ __forceinline__ Bilin pix_taps(T ix, T iy, int size);
 __device__ __forceinline__ Bilin bilin_taps(float gx, float gy, int size) {
   const float ix = ((gx + 1.f) * (float)size - 1.f) * 0.5f;
   const float iy = ((gy + 1.f) * (float)size - 1.f) * 0.5f;
-  const float fx = floorf(ix), fy = floorf(iy);
+  return pix_taps<float>(ix, iy, size);
+}
+
+// bilinear taps at pixel-index coordinates (ix, iy); taps outside [0, size) get weight 0 (zeros padding, no renormalisation).
+// T = double: the kornia stages' positions, whose fractions a float near 200 would quantise to 1.5e-5 pixel
+template <typename T>
+__device__ __forceinline__ Bilin pix_taps(T ix, T iy, int size) {
+  const T fx = floor(ix), fy = floor(iy);
   Bilin b;
   b.x0 = (int)fx; b.y0 = (int)fy;
-  const float tx = ix - fx, ty = iy - fy;
+  const float tx = (float)(ix - fx), ty = (float)(iy - fy);
   b.w00 = (1.f - tx) * (1.f - ty); b.w01 = tx * (1.f - ty);
   b.w10 = (1.f - tx) * ty;         b.w11 = tx * ty;
   const bool xin0 = b.x0 >= 0 && b.x0 < size, xin1 = b.x0 + 1 >= 0 && b.x0 + 1 < size;
@@ -320,9 +329,9 @@ k_resize(const float* __restrict__ canvas, int H, int W, int pad_top, int pad_le
       const float4 wx = *reinterpret_cast<const float4*>(xw + 4 * j);
       float acc = wx.x * strip[xo.x];
       acc += wx.y * strip[xo.y]; acc += wx.z * strip[xo.z]; acc += wx.w * strip[xo.w];
-      const float v = (kind == APH_TF_FAST) ? acc : fmaf(acc, na, nb);
+      const float v = (kind >= APH_TF_FAST) ? acc : fmaf(acc, na, nb);
       o[i * size + j] = v;
-      if (kind != APH_TF_FAST && po.base) po.base[patch_index(po, crop, ch, i, j)] = __float2bfloat16_rn(v);
+      if (kind < APH_TF_FAST && po.base) po.base[patch_index(po, crop, ch, i, j)] = __float2bfloat16_rn(v);
     }
     __syncwarp();
   }
@@ -401,6 +410,101 @@ k_compose(const float* __restrict__ Ag, const float* __restrict__ table, int siz
   }
   else if (er) compose3<false, true>(A, n, p, i, j, size, o, po, crop);
   else compose3<false, false>(A, n, p, i, j, size, o, po, crop);
+}
+
+// ---------------------------------------------------------------------------------------------
+// transforms_custom / transforms_elastic (reference transforms.py:147-163, kornia stages restated; DESIGN §1). On the resized crop
+// A [3,size,size] and s = size + 8, c = (s - 1) / 2, every stage a resampling of an s x s image:
+//   P = pad(4, 0.5) of A, then (elastic) the erase rectangle -> 0        (F.pad; torchvision RandomErasing on the padded image)
+//   R(x, y) = bilinear(P, c + Rot (x - c, y - c)), zeros outside          (kornia warp_affine, align_corners=True: pixel space)
+//   E(x, y) = bilinear(R, x k - 1/2, y k - 1/2), k = s / (s - 1)          (elastic_transform2d with zero noise: grid_sample,
+//                                                                          align_corners=False, of the align_corners=True mesh)
+//   J(x, y) = E(x - dx, y - dy), zeros outside                           (kornia translate by an integer shift)
+//   out = (J - mean) / std
+// k_compose_kornia evaluates the chain by exact tap composition for the three channels of one output pixel, as k_compose does for
+// transforms_fast; nothing between A and the output is materialised.
+constexpr int KPAD = 4;
+
+// pixel of the padded (and erased) image P
+__device__ __forceinline__ void padded3(const float* __restrict__ A, int n, const CropParams& p, int y, int x, int size, float w, float (&acc)[3]) {
+  if (erased(p, y, x)) return;
+  const int u = y - KPAD, v = x - KPAD;
+  if ((unsigned)u >= (unsigned)size || (unsigned)v >= (unsigned)size) { acc[0] += 0.5f * w; acc[1] += 0.5f * w; acc[2] += 0.5f * w; return; }
+  const int o = u * size + v;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) acc[c] += w * __ldg(A + c * n + o);
+}
+
+// where pixel (yr, xr) of R samples P: the same expression rot_gather3 inverts in the backward
+__device__ __forceinline__ Bilin kornia_rot_taps(const CropParams& p, int yr, int xr, int s) {
+  const double off = 0.5 * s - 0.5;
+  const double bx = xr - off, by = yr - off;
+  return pix_taps<double>(fma(bx, (double)p.r00, fma(by, (double)p.r01, off)), fma(bx, (double)p.r10, fma(by, (double)p.r11, off)), s);
+}
+
+__device__ __forceinline__ void rotated3(const float* __restrict__ A, int n, const CropParams& p, int yr, int xr, int size, float w, float (&acc)[3]) {
+  const int s = size + 2 * KPAD;
+  const Bilin b = kornia_rot_taps(p, yr, xr, s);
+  if (b.w00 != 0.f) padded3(A, n, p, b.y0, b.x0, size, w * b.w00, acc);
+  if (b.w01 != 0.f) padded3(A, n, p, b.y0, b.x0 + 1, size, w * b.w01, acc);
+  if (b.w10 != 0.f) padded3(A, n, p, b.y0 + 1, b.x0, size, w * b.w10, acc);
+  if (b.w11 != 0.f) padded3(A, n, p, b.y0 + 1, b.x0 + 1, size, w * b.w11, acc);
+}
+
+// the elastic stretch along one axis: output index j samples x0 (weight w0) and x0 + 1 (weight w1); out-of-range taps weigh 0
+__device__ __forceinline__ void stretch_taps(int j, int s, int& x0, float& w0, float& w1) {
+  const double src = (double)j * s / (s - 1) - 0.5;
+  const double f = floor(src);
+  const float t = (float)(src - f);
+  x0 = (int)f;
+  w0 = ((unsigned)x0 < (unsigned)s) ? 1.f - t : 0.f;
+  w1 = ((unsigned)(x0 + 1) < (unsigned)s) ? t : 0.f;
+}
+
+template <bool ELASTIC>
+__global__ void __launch_bounds__(256)
+k_compose_kornia(const float* __restrict__ Ag, const float* __restrict__ table, int size, float* __restrict__ out, PatchOut po) {
+  const int s = size + 2 * KPAD;
+  const int crop = blockIdx.y, tiles_x = (s + 15) >> 4;
+  const int ti = blockIdx.x / tiles_x, tj = blockIdx.x - ti * tiles_x;
+  const int i = ti * 16 + (threadIdx.x >> 4), j = tj * 16 + (threadIdx.x & 15);
+  __shared__ CropParams sp;
+  __shared__ int sd[2];
+  if (threadIdx.x == 0) {
+    const float* row = table + (size_t)crop * APH_CROP_PARAM_FLOATS;
+    sp = load_params(row); sd[0] = (int)row[APH_F_JIT_DX]; sd[1] = (int)row[APH_F_JIT_DY];
+  }
+  __syncthreads();
+  const CropParams p = sp;
+  if (i >= s || j >= s) return;
+  const int n = size * size;
+  const float* A = Ag + (size_t)crop * 3 * n;
+  float acc[3] = {0.f, 0.f, 0.f};
+  const int ye = i - sd[1], xe = j - sd[0];                 // jitter: J(i, j) = E(i - dy, j - dx)
+  if ((unsigned)ye < (unsigned)s && (unsigned)xe < (unsigned)s) {
+    if (ELASTIC) {
+      int y0, x0; float wy0, wy1, wx0, wx1;
+      stretch_taps(ye, s, y0, wy0, wy1);
+      stretch_taps(xe, s, x0, wx0, wx1);
+      if (wy0 * wx0 != 0.f) rotated3(A, n, p, y0, x0, size, wy0 * wx0, acc);
+      if (wy0 * wx1 != 0.f) rotated3(A, n, p, y0, x0 + 1, size, wy0 * wx1, acc);
+      if (wy1 * wx0 != 0.f) rotated3(A, n, p, y0 + 1, x0, size, wy1 * wx0, acc);
+      if (wy1 * wx1 != 0.f) rotated3(A, n, p, y0 + 1, x0 + 1, size, wy1 * wx1, acc);
+    } else {
+      rotated3(A, n, p, ye, xe, size, 1.f, acc);
+    }
+  }
+  const int sn = s * s, pix = i * s + j;
+  float* o = out + (size_t)crop * 3 * sn;
+  // the encoder's patch operand holds the top-left (g p)^2 window: conv1 (kernel = stride = p) never reads the rest
+  const bool in_window = po.base && i < po.p * po.g && j < po.p * po.g;
+  const size_t pi = in_window ? patch_index(po, crop, 0, i, j) : 0;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float v = fmaf(acc[c], c_inv_std[c], c_shift[c]);
+    o[c * sn + pix] = v;
+    if (in_window) po.base[pi + (size_t)c * po.p * po.p] = __float2bfloat16_rn(v);
+  }
 }
 
 // Shared-memory accumulation cell. fp32 atomicAdd on shared memory is a compare-and-swap loop on this architecture
@@ -771,30 +875,35 @@ __device__ __forceinline__ bool rigid_rot(const CropParams& p) {
 }
 
 // gradient with respect to B(y, x) (the post-perspective, post-erase image the rotate stage samples) of sum(go * rotate(B)),
-// unnormalised (no 1/std), for the three channels; go = this crop's [3, size, size] block of grad_out
+// unnormalised (no 1/std), for the three channels; go = this crop's [3, size, size] block of grad_out.
+// COVER: torchvision's rotate multiplies by the coverage of the [img; ones] stack; kornia's warp_affine (COVER = false) does not.
+template <bool COVER = true>
 __device__ __forceinline__ void rot_gather3(const float* __restrict__ go, int n, const CropParams& p, int y, int x, int size, float (&acc)[3]) {
-  const float off = 0.5f * (float)size - 0.5f, fs = (float)size;
-  const float sx = (float)x - off, sy = (float)y - off;
+  using P = typename std::conditional<COVER, float, double>::type;      // kornia's positions in double (see pix_taps)
+  const P off = (P)0.5 * (P)size - (P)0.5;
+  const float fs = (float)size;
+  const P sx = (P)x - off, sy = (P)y - off;
+  const P r00 = p.r00, r01 = p.r01, r10 = p.r10, r11 = p.r11;
   // centre of the footprint in output coordinates: the forward samples at R b + off, b = (j, i) - off; R^-1 = R^T
-  const int jr = __float2int_rn(fmaf(p.r00, sx, fmaf(p.r10, sy, off))), ir = __float2int_rn(fmaf(p.r01, sx, fmaf(p.r11, sy, off)));
+  const int jr = (int)rint(fma(r00, sx, fma(r10, sy, off))), ir = (int)rint(fma(r01, sx, fma(r11, sy, off)));
   acc[0] = acc[1] = acc[2] = 0.f;
 #pragma unroll
   for (int di = -1; di <= 1; ++di) {
     const int i = ir + di;
     if ((unsigned)i >= (unsigned)size) continue;
-    const float by = (float)i - off;
-    const float cx = fmaf(by, p.r01, off), cy = fmaf(by, p.r11, off);
+    const P by = (P)i - off;
+    const P cx = fma(by, r01, off), cy = fma(by, r11, off);
 #pragma unroll
     for (int dj = -1; dj <= 1; ++dj) {
       const int j = jr + dj;
       if ((unsigned)j >= (unsigned)size) continue;
-      const float bx = (float)j - off;
-      const float ix = fmaf(bx, p.r00, cx), iy = fmaf(bx, p.r10, cy);              // where output pixel (i, j) samples B
-      const float wx = 1.f - fabsf(ix - (float)x), wy = 1.f - fabsf(iy - (float)y);
+      const P bx = (P)j - off;
+      const P ix = fma(bx, r00, cx), iy = fma(bx, r10, cy);                        // where output pixel (i, j) samples B
+      const float wx = (float)(1 - fabs(ix - (P)x)), wy = (float)(1 - fabs(iy - (P)y));
       if (wx > 0.f && wy > 0.f) {
         // coverage of (i, j): sum of its in-bounds tap weights (zeros padding of the [img; ones] stack), separable
-        const float mx = __saturatef(fminf(ix + 1.f, fs - ix)), my = __saturatef(fminf(iy + 1.f, fs - iy));
-        const float w = wx * wy * mx * my;
+        float w = wx * wy;
+        if (COVER) { w *= __saturatef(fminf((float)ix + 1.f, fs - (float)ix)); w *= __saturatef(fminf((float)iy + 1.f, fs - (float)iy)); }
         const int o = i * size + j;
         acc[0] = fmaf(w, __ldg(go + o), acc[0]); acc[1] = fmaf(w, __ldg(go + n + o), acc[1]); acc[2] = fmaf(w, __ldg(go + 2 * n + o), acc[2]);
       }
@@ -879,6 +988,55 @@ k_bwd_warp_adjoint(const float* __restrict__ grad_out, const float* __restrict__
   }
 }
 
+// transforms_custom / _elastic, backward first stage: the adjoints of normalise, jitter and (elastic) the stretch, as a gather into
+// gR [S,3,s,s] = d loss / d R (the rotated image). The rest -- rotation adjoint, erase mask, pad border, bicubic adjoint -- runs in
+// k_bwd_bicubic3 (mode 4). Every element of gR is written: the scratch carries nothing from one call to the next.
+// Output index j of the stretch taps x0(j) and x0(j) + 1 with x0(j) in {j - 1, j}: R index r is reached from j in {r - 1, r, r + 1}.
+__device__ __forceinline__ int stretch_adjoint(int r, int s, int (&js)[3], float (&ws)[3]) {
+  int m = 0;
+#pragma unroll
+  for (int d = -1; d <= 1; ++d) {
+    const int j = r + d;
+    if ((unsigned)j >= (unsigned)s) continue;
+    int x0; float w0, w1;
+    stretch_taps(j, s, x0, w0, w1);
+    const float w = (x0 == r ? w0 : 0.f) + (x0 + 1 == r ? w1 : 0.f);
+    if (w != 0.f) { js[m] = j; ws[m] = w; ++m; }
+  }
+  return m;
+}
+
+template <bool ELASTIC>
+__global__ void __launch_bounds__(256)
+k_bwd_kornia_stage(const float* __restrict__ grad_out, const float* __restrict__ table, int size, float gscale, float* __restrict__ gR_all) {
+  const int s = size + 2 * KPAD, sn = s * s, crop = blockIdx.y;
+  const float* row = table + (size_t)crop * APH_CROP_PARAM_FLOATS;
+  const int dx = (int)row[APH_F_JIT_DX], dy = (int)row[APH_F_JIT_DY];
+  const float* go = grad_out + (size_t)crop * 3 * sn;
+  float* gR = gR_all + (size_t)crop * 3 * sn;
+  const float k0 = c_inv_std[0] * gscale, k1 = c_inv_std[1] * gscale, k2 = c_inv_std[2] * gscale;
+  for (int pix = blockIdx.x * blockDim.x + threadIdx.x; pix < sn; pix += gridDim.x * blockDim.x) {
+    const int yr = pix / s, xr = pix - yr * s;
+    float a0 = 0.f, a1 = 0.f, a2 = 0.f;
+    int jy[3], jx[3]; float wy[3], wx[3];
+    int my = 1, mx = 1;
+    if (ELASTIC) { my = stretch_adjoint(yr, s, jy, wy); mx = stretch_adjoint(xr, s, jx, wx); }
+    else { jy[0] = yr; jx[0] = xr; wy[0] = wx[0] = 1.f; }
+    for (int a = 0; a < my; ++a) {
+      const int y = jy[a] + dy;                             // output row the jitter moved E's row jy to
+      if ((unsigned)y >= (unsigned)s) continue;
+      for (int b = 0; b < mx; ++b) {
+        const int x = jx[b] + dx;
+        if ((unsigned)x >= (unsigned)s) continue;
+        const float w = wy[a] * wx[b];
+        const int o = y * s + x;
+        a0 = fmaf(w, __ldg(go + o), a0); a1 = fmaf(w, __ldg(go + sn + o), a1); a2 = fmaf(w, __ldg(go + 2 * sn + o), a2);
+      }
+    }
+    gR[pix] = a0 * k0; gR[sn + pix] = a1 * k1; gR[2 * sn + pix] = a2 * k2;
+  }
+}
+
 __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float c, float d) {
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" :: "l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
@@ -912,15 +1070,19 @@ k_bwd_bicubic3(const float* __restrict__ grad_out, float* __restrict__ gA_all, i
   for (int x = lane; x < 3 * STRIP; x += 32) strip[x] = 0.f;       // re-zeroed as they are drained
   __syncthreads();
   // where this crop's gradient rows come from (CTA-uniform)
-  int mode;                                                        // 0: grad_out * pre, 1: + erase mask, 2: rotation gather inline, 3: scratch
+  // 0: grad_out * pre, 1: + erase mask, 2: rotation gather inline, 3: scratch, 4: kornia rotation gather from gR (grad_out is
+  // k_bwd_kornia_stage's [S,3,size+8,size+8] output) at the padded pixel, erase mask
+  int mode;
   float pre[3];
-  if (kind != APH_TF_FAST) { mode = 0; for (int c = 0; c < 3; ++c) pre[c] = (kind == APH_TF_NORMALIZE ? c_inv_std[c] : 1.f) * gscale; }
+  if (kind >= APH_TF_CUSTOM) { mode = 4; pre[0] = pre[1] = pre[2] = 1.f; }
+  else if (kind != APH_TF_FAST) { mode = 0; for (int c = 0; c < 3; ++c) pre[c] = (kind == APH_TF_NORMALIZE ? c_inv_std[c] : 1.f) * gscale; }
   else {
     for (int c = 0; c < 3; ++c) pre[c] = c_inv_std[c] * gscale;
     if (via_scratch(p)) { mode = 3; pre[0] = pre[1] = pre[2] = 1.f; }
     else mode = identity_rot(p) ? 1 : 2;
   }
-  const float* src = grad_out + (size_t)crop * 3 * n;
+  const int ks = size + 2 * KPAD;
+  const float* src = grad_out + (size_t)crop * 3 * (mode == 4 ? ks * ks : n);
   float* scr = gA_all + (size_t)crop * 3 * n;
   const bool can_strip = (pad_top == 0 && pad_left == 0);
   const size_t plane = (size_t)H * W;
@@ -942,6 +1104,8 @@ k_bwd_bicubic3(const float* __restrict__ grad_out, float* __restrict__ gA_all, i
           if (g[2] != 0.f) scr[2 * n + o] = 0.f;
         } else if (mode == 2) {
           if (!erased(p, i, j)) rot_gather3(src, n, p, i, j, size, g);
+        } else if (mode == 4) {
+          if (!erased(p, i + KPAD, j + KPAD)) rot_gather3<false>(src, ks * ks, p, i + KPAD, j + KPAD, ks, g);
         } else if (!(mode == 1 && erased(p, i, j))) {
           g[0] = __ldg(src + o); g[1] = __ldg(src + n + o); g[2] = __ldg(src + 2 * n + o);
         }
@@ -1033,7 +1197,7 @@ using namespace aph;
 static int check_sample_args(const char* who, int H, int W, int S, int size, int kind) {
   APH_REQUIRE(H > 0 && W > 0 && S >= 0 && size > 0, "%s: bad shape H=%d W=%d S=%d size=%d", who, H, W, S, size);
   APH_REQUIRE(((size_t)size * size + 4 + 16 * (size_t)size + 32 * STRIP) * sizeof(float) <= 227 * 1024, "%s: size=%d does not fit one CTA's shared memory (max 224)", who, size);
-  APH_REQUIRE(kind >= APH_TF_NONE && kind <= APH_TF_FAST, "%s: unknown transform kind %d", who, kind);
+  APH_REQUIRE(kind >= APH_TF_NONE && kind <= APH_TF_ELASTIC, "%s: unknown transform kind %d", who, kind);
   return 0;
 }
 
@@ -1051,10 +1215,13 @@ extern "C" int aph_sample_fwd(const float* canvas, int H, int W, int pad_top, in
 extern "C" int aph_sample_fwd_patches(const float* canvas, int H, int W, int pad_top, int pad_left, const float* table, int S,
                                       int size, int kind, float* out, void* patches_bf16, int patch, int* patches_written, void* stream) {
   APH_REQUIRE(patches_bf16 && patches_written, "aph_sample_fwd_patches: null pointer");
-  APH_REQUIRE(patch > 0 && size % patch == 0, "aph_sample_fwd_patches: size=%d is not a multiple of patch=%d", size, patch);
+  APH_REQUIRE(patch > 0, "aph_sample_fwd_patches: patch=%d", patch);
+  // the kornia kinds write size + 8: the operand is the top-left (grid * patch)^2 window conv1 reads
+  const int side = size + (kind >= APH_TF_CUSTOM ? 2 * KPAD : 0);
+  APH_REQUIRE(kind >= APH_TF_CUSTOM ? side >= patch : size % patch == 0, "aph_sample_fwd_patches: size=%d does not fit patch=%d", size, patch);
   *patches_written = 0;
   return sample_fwd_impl(canvas, H, W, pad_top, pad_left, table, S, size, kind, out,
-                         PatchOut{reinterpret_cast<__nv_bfloat16*>(patches_bf16), patch, size / patch}, patches_written, stream);
+                         PatchOut{reinterpret_cast<__nv_bfloat16*>(patches_bf16), patch, side / patch}, patches_written, stream);
 }
 
 static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int pad_left, const float* table, int S,
@@ -1069,10 +1236,13 @@ static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int p
     if (old_path < 0) { const char* e = getenv("APH_SAMPLE_FWD_OLD"); old_path = (e && e[0] == '1') ? 1 : 0; }
     const int cap = ((H + 2 * pad_top < W + 2 * pad_left ? H + 2 * pad_top : W + 2 * pad_left) + 1 + 3) & ~3;     // crops never exceed the short side of the frame
     const size_t smem2 = ((size_t)8 * size + (size_t)8 * cap) * sizeof(float);
-    if (!old_path && smem2 <= 200 * 1024) {
+    // the kornia kinds exist in this form only (APH_SAMPLE_FWD_OLD does not apply to them)
+    const bool kornia = kind >= APH_TF_CUSTOM;
+    APH_REQUIRE(!kornia || smem2 <= 200 * 1024, "aph_sample_fwd: a %dx%d frame is too large for transform kind %d", H + 2 * pad_top, W + 2 * pad_left, kind);
+    if ((!old_path || kornia) && smem2 <= 200 * 1024) {
       cudaStream_t st = (cudaStream_t)stream;
       float* dst = out;
-      if (kind == APH_TF_FAST) {
+      if (kind >= APH_TF_FAST) {
         const size_t need = (size_t)S * 3 * size * size * sizeof(float);
         if (need > g_A_bytes) {
           APH_CUDA_OK(cudaStreamSynchronize(st));
@@ -1097,6 +1267,11 @@ static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int p
       if (kind == APH_TF_FAST) {
         const int tiles = ((size + 15) / 16) * ((size + 15) / 16);
         k_compose<<<dim3(tiles, S), 256, 0, st>>>(g_A, table, size, out, po);
+        APH_LAUNCH_OK();
+      } else if (kornia) {
+        const int s = size + 2 * KPAD, tiles = ((s + 15) / 16) * ((s + 15) / 16);
+        if (kind == APH_TF_ELASTIC) k_compose_kornia<true><<<dim3(tiles, S), 256, 0, st>>>(g_A, table, size, out, po);
+        else k_compose_kornia<false><<<dim3(tiles, S), 256, 0, st>>>(g_A, table, size, out, po);
         APH_LAUNCH_OK();
       }
       if (patches_written) *patches_written = 1;
@@ -1124,6 +1299,8 @@ static float* g_gW = nullptr;          // warp-stage adjoint scratch [S,3,size,s
 static size_t g_gW_bytes = 0;
 static float* g_gA = nullptr;          // stage-1 scratch [S,3,size,size] (library-owned: survives torch.cuda.empty_cache())
 static size_t g_gA_bytes = 0;
+static float* g_gR = nullptr;          // kornia kinds: d loss / d rotated image [S,3,size+8,size+8], rewritten by every backward
+static size_t g_gR_bytes = 0;
 
 static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int pad_left, const float* table, int S,
                            int size, int kind, float* grad_canvas, float gscale, void* stream);
@@ -1147,7 +1324,9 @@ static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int
   static int force_scatter = -1;
   if (force_scatter < 0) { const char* e = getenv("APH_SAMPLE_BWD_GATHER"); force_scatter = (e && e[0] == '1') ? 0 : 1; }
   // (crops never upsample by more than 1/0.9 when min(H, W) >= size, which bounds the adjoint tap lists of the gather kernel)
-  if (S > 0 && pad_top == 0 && pad_left == 0 && !force_scatter && (H < W ? H : W) >= size) {
+  // The kornia kinds run the default kernels only: APH_SAMPLE_BWD_GATHER / _OLD / _FIXED do not apply to them.
+  const bool kornia = kind >= APH_TF_CUSTOM;
+  if (S > 0 && pad_top == 0 && pad_left == 0 && !force_scatter && !kornia && (H < W ? H : W) >= size) {
     // ---- atomic-free path: (stage 1) + tile gather
     APH_REQUIRE(grad_out && table, "aph_sample_bwd: null pointer");
     cudaStream_t st = (cudaStream_t)stream;
@@ -1186,7 +1365,7 @@ static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int
   // default: the two-kernel form (k_bwd_warp_adjoint + k_bwd_bicubic3); APH_SAMPLE_BWD_OLD=1 keeps the one-kernel form
   static int old_bwd = -1;
   if (old_bwd < 0) { const char* e = getenv("APH_SAMPLE_BWD_OLD"); const char* f = getenv("APH_SAMPLE_BWD_FIXED"); old_bwd = ((e && e[0] == '1') || (f && f[0] == '1')) ? 1 : 0; }
-  if (!old_bwd) {
+  if (!old_bwd || kornia) {
     cudaStream_t st = (cudaStream_t)stream;
     const size_t smem3 = ((size_t)8 * size + 8 * 3 * STRIP) * sizeof(float);
     static size_t configured3 = 48 * 1024;
@@ -1202,7 +1381,25 @@ static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int
     // strips in integer fixed point (native shared atomic add) by default; APH_SAMPLE_STRIP_FP32=1: fp32 strips (compare-and-swap loops)
     static int fp32_strips = -1;
     if (fp32_strips < 0) { const char* e = getenv("APH_SAMPLE_STRIP_FP32"); fp32_strips = (e && e[0] == '1') ? 1 : 0; }
-#define APH_BB(V, F, STREAM) k_bwd_bicubic3<V, F><<<g3, 256, smem3, STREAM>>>(grad_out, g_gW, H, W, pad_top, pad_left, table, size, kind, gscale, grad_canvas)
+    const float* bb_src = grad_out;
+    if (kornia) {
+      // adjoints of normalise, jitter and the elastic stretch into gR (fully overwritten), then the rest in k_bwd_bicubic3 (mode 4)
+      const int s = size + 2 * KPAD;
+      const size_t need = (size_t)S * 3 * s * s * sizeof(float);
+      if (need > g_gR_bytes) {
+        APH_CUDA_OK(cudaStreamSynchronize(st));
+        if (g_gR) cudaFree(g_gR);
+        g_gR = nullptr; g_gR_bytes = 0;
+        APH_CUDA_OK(cudaMalloc(&g_gR, need));
+        g_gR_bytes = need;
+      }
+      const dim3 gk((s * s + 1023) / 1024, S);
+      if (kind == APH_TF_ELASTIC) k_bwd_kornia_stage<true><<<gk, 256, 0, st>>>(grad_out, table, size, gscale, g_gR);
+      else k_bwd_kornia_stage<false><<<gk, 256, 0, st>>>(grad_out, table, size, gscale, g_gR);
+      APH_LAUNCH_OK();
+      bb_src = g_gR;
+    }
+#define APH_BB(V, F, STREAM) k_bwd_bicubic3<V, F><<<g3, 256, smem3, STREAM>>>(bb_src, g_gW, H, W, pad_top, pad_left, table, size, kind, gscale, grad_canvas)
 #define APH_BB_ANY(STREAM)                                                                           \
     do {                                                                                             \
       if (vec) { if (fp32_strips) APH_BB(true, false, STREAM); else APH_BB(true, true, STREAM); }    \

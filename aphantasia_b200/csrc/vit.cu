@@ -314,11 +314,33 @@ extern "C" int aph_vit_finalize(aph_vit* vit) {
   return 0;
 }
 
-static int vit_fwd_impl(aph_vit* vit, const float* images, int S, float* emb, int save_for_bwd, void* stream);
+static int vit_fwd_impl(aph_vit* vit, const float* images, int S, int side, float* emb, int save_for_bwd, void* stream);
+static float* g_win = nullptr;         // aph_vit_bwd_sized: the R x R window gradient before k_window_expand (grown on demand)
+static size_t g_win_bytes = 0;
+static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, float* grad_images, void* stream);
 
 extern "C" int aph_vit_fwd(aph_vit* vit, const float* images, int S, float* emb, int save_for_bwd, void* stream) {
   APH_REQUIRE(vit && images && emb, "aph_vit_fwd: null argument");
-  return vit_fwd_impl(vit, images, S, emb, save_for_bwd, stream);
+  return vit_fwd_impl(vit, images, S, reinterpret_cast<VitImpl*>(vit)->cfg.res, emb, save_for_bwd, stream);
+}
+
+// images of side res <= side < res + patch (the 232-pixel batches of transforms_custom / _elastic): conv1 sees the top-left window
+static int check_side(const aph_vit* vit, int side, const char* who) {
+  const VitImpl* v = reinterpret_cast<const VitImpl*>(vit);
+  APH_REQUIRE(side >= v->cfg.res && side < v->cfg.res + v->cfg.patch, "%s: side=%d outside [%d, %d)", who, side, v->cfg.res, v->cfg.res + v->cfg.patch);
+  return 0;
+}
+
+extern "C" int aph_vit_fwd_sized(aph_vit* vit, const float* images, int S, int side, float* emb, int save_for_bwd, void* stream) {
+  APH_REQUIRE(vit && images && emb, "aph_vit_fwd_sized: null argument");
+  if (int e = check_side(vit, side, "aph_vit_fwd_sized")) return e;
+  return vit_fwd_impl(vit, images, S, side, emb, save_for_bwd, stream);
+}
+
+extern "C" int aph_vit_bwd_sized(aph_vit* vit, const float* grad_emb, int S, int side, float* grad_images, void* stream) {
+  APH_REQUIRE(vit && grad_emb && grad_images, "aph_vit_bwd_sized: null argument");
+  if (int e = check_side(vit, side, "aph_vit_bwd_sized")) return e;
+  return vit_bwd_impl(vit, grad_emb, S, side, grad_images, stream);
 }
 
 // The sampler can write the patch-embedding operand itself (aph_sample_fwd_patches): this is where it goes ...
@@ -334,10 +356,10 @@ extern "C" int aph_vit_patch_operand(aph_vit* vit, int S, void** patches_bf16, i
 // ... and the forward that consumes it as it is (no k_patchify: the fp32 images are not read)
 extern "C" int aph_vit_fwd_prepatched(aph_vit* vit, int S, float* emb, int save_for_bwd, void* stream) {
   APH_REQUIRE(vit && emb, "aph_vit_fwd_prepatched: null argument");
-  return vit_fwd_impl(vit, nullptr, S, emb, save_for_bwd, stream);
+  return vit_fwd_impl(vit, nullptr, S, 0, emb, save_for_bwd, stream);
 }
 
-static int vit_fwd_impl(aph_vit* vit, const float* images, int S, float* emb, int save_for_bwd, void* stream) {
+static int vit_fwd_impl(aph_vit* vit, const float* images, int S, int side, float* emb, int save_for_bwd, void* stream) {
   VitImpl* v = reinterpret_cast<VitImpl*>(vit);
   APH_REQUIRE(v->finalized, "aph_vit_fwd: weights not finalized");
   APH_REQUIRE(S > 0 && S <= v->cfg.max_batch, "aph_vit_fwd: S=%d outside (0, max_batch=%d]", S, v->cfg.max_batch);
@@ -348,7 +370,7 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, float* emb, in
   if (images) {
     const int g = v->g, Mp = S * g * g;
     const size_t n8 = (size_t)Mp * v->Kp / 8;
-    APH_CUDA_OK(launch_k(k_patchify, dim3((unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1, images, v->patches, S, v->cfg.patch, g));
+    APH_CUDA_OK(launch_k(k_patchify, dim3((unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1, images, v->patches, S, v->cfg.patch, g, side));
     APH_LAUNCH_OK();
   }
   const int rc = run_cached(v->fwd_graphs, v->warm_fwd, v->stamp, v->graph_misses, nullptr, nullptr, S, save_for_bwd, st, [&]() -> int {
@@ -404,6 +426,10 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, float* emb, in
 
 extern "C" int aph_vit_bwd(aph_vit* vit, const float* grad_emb, int S, float* grad_images, void* stream) {
   APH_REQUIRE(vit && grad_emb && grad_images, "aph_vit_bwd: null argument");
+  return vit_bwd_impl(vit, grad_emb, S, reinterpret_cast<VitImpl*>(vit)->cfg.res, grad_images, stream);
+}
+
+static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, float* grad_images, void* stream) {
   VitImpl* v = reinterpret_cast<VitImpl*>(vit);
   APH_REQUIRE(v->last_S == S, "aph_vit_bwd: no saved forward for S=%d (last saved S=%d)", S, v->last_S);
   cudaStream_t st = (cudaStream_t)stream;
@@ -462,9 +488,29 @@ extern "C" int aph_vit_bwd(aph_vit* vit, const float* grad_emb, int S, float* gr
   });
   if (rc) return rc;
   // caller-owned output: the patch-embed data gradient (un-patchify epilogue writes NCHW) is launched outside the graph
-  { const int g = v->g, Mp = S * g * g;
-    GemmEpi ep; ep.out_f32 = grad_images; ep.unpatch_p = v->cfg.patch; ep.unpatch_g = g;
-    if (int e = launch_gemm(v->d_tok, v->w_conv_t, GemmShape{Mp, v->Kp, v->D}, ep, st)) return e; }
+  { const int g = v->g, Mp = S * g * g, R = v->cfg.res;
+    // a larger image (aph_vit_bwd_sized): the epilogue writes the R x R window into a scratch image, k_window_expand places it
+    // and zeroes the margin, which conv1 never reads
+    const bool sized = side != R;
+    if (sized) {
+      const size_t need = (size_t)S * 3 * R * R * sizeof(float);
+      if (need > g_win_bytes) {
+        APH_CUDA_OK(cudaStreamSynchronize(st));
+        if (g_win) cudaFree(g_win);
+        g_win = nullptr; g_win_bytes = 0;
+        APH_CUDA_OK(cudaMalloc(&g_win, need));
+        g_win_bytes = need;
+      }
+    }
+    GemmEpi ep; ep.out_f32 = sized ? g_win : grad_images; ep.unpatch_p = v->cfg.patch; ep.unpatch_g = g;
+    if (int e = launch_gemm(v->d_tok, v->w_conv_t, GemmShape{Mp, v->Kp, v->D}, ep, st)) return e;
+    if (sized) {
+      const size_t n = (size_t)S * 3 * side * side;
+      APH_CUDA_OK(launch_k(k_window_expand, dim3((unsigned)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1,
+                           (const float*)g_win, grad_images, S * 3, R, side));
+      APH_LAUNCH_OK();
+    }
+  }
   return 0;
 }
 

@@ -22,10 +22,11 @@ namespace aph {
   }
 
 // ---------------------------------------------------------------------------------------------
-// images fp32 [S,3,R,R] -> patches bf16 [S*g*g, 3*p*p], col = c*p*p + py*p + px  (conv1 weight layout)
-static __global__ void __launch_bounds__(256) k_patchify(const float* __restrict__ img, bf16* __restrict__ out, int S, int p, int g) {
+// images fp32 [S,3,side,side] -> patches bf16 [S*g*g, 3*p*p], col = c*p*p + py*p + px  (conv1 weight layout); side >= R = p*g:
+// conv1 reads the top-left R x R window
+static __global__ void __launch_bounds__(256) k_patchify(const float* __restrict__ img, bf16* __restrict__ out, int S, int p, int g, int side) {
   pdl_trigger(); pdl_wait();
-  const int R = p * g, Kp = 3 * p * p;
+  const int R = side, Kp = 3 * p * p;
   const size_t total = (size_t)S * g * g * Kp / 8;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
     const size_t e = idx * 8;
@@ -33,12 +34,28 @@ static __global__ void __launch_bounds__(256) k_patchify(const float* __restrict
     const int s = row / (g * g), pr = row - s * g * g, gy = pr / g, gx = pr - gy * g;
     const int c = col / (p * p), rem = col - c * p * p, py = rem / p, px = rem - py * p;
     const float* src = img + (((size_t)s * 3 + c) * R + gy * p + py) * R + gx * p + px;
-    const float4 a = __ldg(reinterpret_cast<const float4*>(src)), b = __ldg(reinterpret_cast<const float4*>(src) + 1);
+    float4 a, b;
+    if ((R & 3) == 0) { a = __ldg(reinterpret_cast<const float4*>(src)); b = __ldg(reinterpret_cast<const float4*>(src) + 1); }
+    else {                                          // rows of a side that is not a multiple of 4 are not 16-byte aligned
+      a = make_float4(__ldg(src), __ldg(src + 1), __ldg(src + 2), __ldg(src + 3));
+      b = make_float4(__ldg(src + 4), __ldg(src + 5), __ldg(src + 6), __ldg(src + 7));
+    }
     __nv_bfloat162 p0 = __floats2bfloat162_rn(a.x, a.y), p1 = __floats2bfloat162_rn(a.z, a.w);
     __nv_bfloat162 p2 = __floats2bfloat162_rn(b.x, b.y), p3 = __floats2bfloat162_rn(b.z, b.w);
     uint4 u; u.x = *reinterpret_cast<uint32_t*>(&p0); u.y = *reinterpret_cast<uint32_t*>(&p1);
     u.z = *reinterpret_cast<uint32_t*>(&p2); u.w = *reinterpret_cast<uint32_t*>(&p3);
     *reinterpret_cast<uint4*>(out + e) = u;
+  }
+}
+
+// planes [n,R,R] -> [n,side,side] (side >= R): the window at the top left, zeros in the margin
+static __global__ void __launch_bounds__(256) k_window_expand(const float* __restrict__ src, float* __restrict__ dst, int n, int R, int side) {
+  pdl_trigger(); pdl_wait();
+  const size_t total = (size_t)n * side * side;
+  for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
+    const size_t plane = idx / ((size_t)side * side);
+    const int rem = (int)(idx - plane * side * side), y = rem / side, x = rem - y * side;
+    dst[idx] = (y < R && x < R) ? __ldg(src + (plane * R + y) * R + x) : 0.f;
   }
 }
 

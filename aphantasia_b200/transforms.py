@@ -1,9 +1,11 @@
 """Augmentation pipelines -- drop-in for /root/reference/aphantasia/transforms.py (names clip_fft.py reads).
 
-In the reference these are Python closures applied per crop. Here `transforms_fast` and `normalize()` are
-*spec-carrying* callables: slice_imgs recognises them and runs the whole pipeline inside the fused CUDA
-sampler (csrc/sample.cu). The kornia-based pipelines (custom / elastic / lucent / openai) are outside the
-CUDA hot path (SURVEY.md section 2.1) and raise when selected.
+In the reference these are Python closures applied per crop. Here `transforms_fast`, `transforms_custom`,
+`transforms_elastic` and `normalize()` are *spec-carrying* callables: slice_imgs recognises them and runs the whole
+pipeline inside the fused CUDA sampler (csrc/sample.cu). `transforms_custom` and `transforms_elastic` pad each crop
+by 4 pixels, so slice_imgs returns [count, 3, size + 8, size + 8] with them, as the reference does; the reference
+builds their rotation, elastic and jitter stages on kornia, which the sampler restates (DESIGN.md section 1).
+`transforms_lucent` / `transforms_openai` are selected by no script and raise.
 """
 import torch
 
@@ -35,6 +37,10 @@ def normalize():
 
 # transforms.py:165-170: RandomPerspective(0.33, .2) -> RandomErasing(.2) -> random_rotate_fast -> normalize
 transforms_fast = SamplerTransform(_rng.TF_FAST, 'fast')
+# transforms.py:156-163: pad(4, constant 0.5) -> random_rotate -> jitter(8) -> normalize
+transforms_custom = SamplerTransform(_rng.TF_CUSTOM, 'custom')
+# transforms.py:147-154: pad(4, constant 0.5) -> RandomErasing(.2) -> random_rotate -> random_elastic -> jitter(8) -> normalize
+transforms_elastic = SamplerTransform(_rng.TF_ELASTIC, 'elastic')
 
 
 class _Unsupported:
@@ -42,12 +48,10 @@ class _Unsupported:
         self.name = name
 
     def __call__(self, x):
-        raise NotImplementedError('aphantasia_b200: transform "%s" needs kornia and is outside the CUDA hot path; '
-                                  'use --transform fast (default) or none' % self.name)
+        raise NotImplementedError('aphantasia_b200: transform "%s" is not implemented in the fused sampler; '
+                                  'use --transform fast (default), custom, elastic or none' % self.name)
 
 
-transforms_custom = _Unsupported('custom')
-transforms_elastic = _Unsupported('elastic')
 transforms_lucent = _Unsupported('lucent')
 transforms_openai = _Unsupported('openai')
 device = torch.device('cuda:0' if torch.cuda.is_available() else 'cpu')

@@ -23,7 +23,8 @@ class _SliceImgs(torch.autograd.Function):
     def forward(ctx, canvas, table_dev, meta, vis=None):
         H, W, pad_top, pad_left, S, size, kind, scale = meta
         x = canvas.detach().contiguous().float()
-        out = _tpool.empty((S, 3, size, size))
+        side = _rng.out_side(size, kind)
+        out = _tpool.empty((S, 3, side, side))
         if vis is not None and S > 0:
             # the encoder that will consume this batch takes its patch operand straight from the sampler's last stage (_patchlink)
             vis._ensure(S)
@@ -62,8 +63,8 @@ def _transform_kind(transform):
         return _rng.TF_NONE
     kind = getattr(transform, 'kind', None)
     if kind is None:
-        raise NotImplementedError('aphantasia_b200.slice_imgs: only transform=None, transforms.normalize() and '
-                                  'transforms.transforms_fast run in the fused sampler (got %r)' % (transform,))
+        raise NotImplementedError('aphantasia_b200.slice_imgs: only transform=None, transforms.normalize(), transforms_fast, '
+                                  'transforms_custom and transforms_elastic run in the fused sampler (got %r)' % (transform,))
     return kind
 
 
@@ -94,8 +95,9 @@ def _table_to_device(tab, device):
 
 
 def slice_imgs(imgs, count, size=224, transform=None, align='uniform', macro=0.):
-    """Drop-in for utils.py:218-254. Returns a list with one [count_local,3,size,size] tensor per input image
-    (count_local == count on one GPU; the contiguous shard of this rank under torchrun)."""
+    """Drop-in for utils.py:218-254. Returns a list with one [count_local,3,side,side] tensor per input image
+    (count_local == count on one GPU; the contiguous shard of this rank under torchrun). side = size, or size + 8 for
+    transforms_custom / transforms_elastic, whose pad(4) the reference applies after the resize."""
     _dist.init()
     kind = _transform_kind(transform)
     for img in imgs:
@@ -110,7 +112,8 @@ def slice_imgs(imgs, count, size=224, transform=None, align='uniform', macro=0.)
         local = np.ascontiguousarray(tab[lo:hi])
         tdev = _table_to_device(local, img.device)
         meta = (hw[0], hw[1], pad_top, pad_left, hi - lo, size, kind, float(hi - lo) / float(count))
-        vis = _patchlink.target(size) if len(imgs) == 1 else None
+        side = _rng.out_side(size, kind)
+        vis = _patchlink.target(side, windowed=side != size) if len(imgs) == 1 else None
         gen0 = vis._patch_gen if vis is not None else 0
         out = _SliceImgs.apply(img, tdev, meta, vis)
         if vis is not None and vis._patch_gen != gen0 and vis._patch_written:
@@ -122,7 +125,7 @@ def slice_imgs(imgs, count, size=224, transform=None, align='uniform', macro=0.)
 def apply_transform_standalone(x, transform):
     """transform(x) outside slice_imgs: every image of the batch is an identity crop (csize == size). As in the reference
     (torchvision draws get_params ONCE per call, transforms.py:165-170), one parameter row is drawn per call and applied to
-    every image of the batch."""
+    every image of the batch. transforms_custom / transforms_elastic return [N,3,s+8,s+8]."""
     require_cuda(x, 'transform input')
     n, c, h, w = x.shape
     assert c == 3 and h == w, 'fused transforms expect [N,3,s,s]'
@@ -131,6 +134,8 @@ def apply_transform_standalone(x, transform):
     tab[0, _rng.F_ROT:_rng.F_ROT + 4] = (1., 0., 0., 1.)
     if transform.kind == _rng.TF_FAST:
         tab[0, _rng.F_FLAGS] = _rng.draw_fast(tab[0], h)
+    elif transform.kind in (_rng.TF_CUSTOM, _rng.TF_ELASTIC):
+        tab[0, _rng.F_FLAGS] = _rng.draw_kornia(tab[0], h, transform.kind == _rng.TF_ELASTIC)
     tdev = torch.from_numpy(tab).to(x.device)
     meta = (h, w, 0, 0, 1, h, transform.kind, 1.)
     return torch.cat([_SliceImgs.apply(x[i:i + 1], tdev, meta, None) for i in range(n)], 0)

@@ -27,22 +27,32 @@ extern "C" {
 #define APH_F_OFFY   0   /* crop top-left y in the sampling frame (integer-valued)   utils.py:247 */
 #define APH_F_OFFX   1   /* crop top-left x                                          utils.py:246 */
 #define APH_F_CSIZE  2   /* crop side in canvas pixels                                utils.py:245 */
-#define APH_F_FLAGS  3   /* bit0 perspective, bit1 erase, bit2 rotate                              */
+#define APH_F_FLAGS  3   /* bit0 perspective, bit1 erase, bit2 rotate, bit3 jitter, bit4 elastic    */
 #define APH_F_PERSP  4   /* 8 coeffs a..h, output->input (torchvision _get_perspective_coeffs)     */
 #define APH_F_ER_I   12  /* erase rect top, left, height, width (torchvision RandomErasing)        */
 #define APH_F_ER_J   13
 #define APH_F_ER_H   14
 #define APH_F_ER_W   15
-#define APH_F_ROT    16  /* theta00, theta01, theta10, theta11 of the inverse affine matrix        */
+#define APH_F_ROT    16  /* theta00, theta01, theta10, theta11 of the inverse affine matrix. For APH_TF_CUSTOM /
+                          * APH_TF_ELASTIC: the pixel-space inverse rotation of kornia's warp_affine about
+                          * c = (s-1)/2, s = size + 8: source = c + [[r00, r01], [r10, r11]] (dest - c), (x, y) order */
 #define APH_F_ANGLE  20  /* degrees, informational                                                 */
-#define APH_FLAG_PERSP 1
-#define APH_FLAG_ERASE 2
-#define APH_FLAG_ROT   4
+#define APH_F_JIT_DX 21  /* APH_TF_CUSTOM / APH_TF_ELASTIC: integer jitter shift (kornia translate): */
+#define APH_F_JIT_DY 22  /*   out(x, y) = in(x - dx, y - dy), zero outside                          */
+#define APH_FLAG_PERSP   1
+#define APH_FLAG_ERASE   2   /* for APH_TF_ELASTIC the rectangle is in the padded (size + 8) image  */
+#define APH_FLAG_ROT     4
+#define APH_FLAG_JITTER  8
+#define APH_FLAG_ELASTIC 16  /* kornia elastic_transform2d with zero noise: a 1-D bilinear stretch per axis */
 
 /* sampler transform kinds (what `transform=` of slice_imgs was)                                  */
 #define APH_TF_NONE      0   /* bicubic resize only                                                */
 #define APH_TF_NORMALIZE 1   /* + transforms.normalize()            transforms.py:102-109          */
 #define APH_TF_FAST      2   /* transforms.transforms_fast          transforms.py:165-170          */
+/* The next two write [S,3,size+8,size+8]: pad(4, 0.5) -> [erase] -> rotate (bilinear, zeros) -> [elastic stretch]
+ * -> jitter(8) -> normalise, each stage a resampling of the (size+8)^2 image.                                       */
+#define APH_TF_CUSTOM    3   /* transforms.transforms_custom        transforms.py:156-163          */
+#define APH_TF_ELASTIC   4   /* transforms.transforms_elastic       transforms.py:147-154          */
 
 /* similarity kinds (sim_func `type`)                                         utils.py:276-295    */
 #define APH_SIM_COS 0
@@ -112,12 +122,15 @@ int aph_valid_rgb_bwd(const float* grad_out, const float* out, int64_t hw, const
  * (bilinear, zeros, x coverage) -> erase -> rotate (bilinear, zeros, x coverage) -> normalise.
  * canvas [3,H,W]; the sampling frame is the canvas wrap-padded by (pad_top, pad_left)
  * ('over*' aligns, utils.py:152-187; 0,0 otherwise); table: DEVICE [S, APH_CROP_PARAM_FLOATS];
- * out [S,3,size,size]. the resized crop, its tap tables and the per-warp strips must fit one CTA's shared memory (size <= 224).           */
+ * out [S,3,size,size] ([S,3,size+8,size+8] for APH_TF_CUSTOM / APH_TF_ELASTIC). the resized crop, its tap tables and
+ * the per-warp strips must fit one CTA's shared memory (size <= 224).                                               */
 int aph_sample_fwd(const float* canvas, int H, int W, int pad_top, int pad_left,
                    const float* table, int S, int size, int kind, float* out, void* stream);
 /* Same, and the last stage also writes the batch as the encoder's patch operand (bf16, patch-major: see
- * aph_vit_patch_operand below); size must be a multiple of patch. *patches_written = 1 when it did (0: the one-kernel
- * fallback form ran and the caller has to use aph_vit_fwd on `out`).                                 */
+ * aph_vit_patch_operand below); the output side (size, or size + 8) must be a multiple of patch, or lie in
+ * [res, res + patch) of an encoder with input resolution res = grid * patch: then the operand is the top-left res x res
+ * window, as conv1 reads it. *patches_written = 1 when it did (0: the one-kernel fallback form ran and the caller has
+ * to use aph_vit_fwd on `out`).                                                                                      */
 int aph_sample_fwd_patches(const float* canvas, int H, int W, int pad_top, int pad_left,
                            const float* table, int S, int size, int kind, float* out,
                            void* patches_bf16, int patch, int* patches_written, void* stream);
@@ -173,6 +186,11 @@ int aph_vit_fwd_prepatched(aph_vit* vit, int S, float* emb, int save_for_bwd, vo
 /* grad_emb [S,out_dim] -> grad_images [S,3,res,res] (overwritten). Uses activations of the last
  * aph_vit_fwd(save_for_bwd=1) with the same S.                                                     */
 int aph_vit_bwd(aph_vit* vit, const float* grad_emb, int S, float* grad_images, void* stream);
+/* The same for images of side `side` in [res, res + patch): conv1 (kernel = stride = patch, no padding) reads only the
+ * top-left res x res window, so the forward reads that window through a row stride and the backward writes grad_images
+ * [S,3,side,side] with an exactly zero margin (rows and columns >= res). side == res is aph_vit_fwd / aph_vit_bwd.     */
+int aph_vit_fwd_sized(aph_vit* vit, const float* images, int S, int side, float* emb, int save_for_bwd, void* stream);
+int aph_vit_bwd_sized(aph_vit* vit, const float* grad_emb, int S, int side, float* grad_images, void* stream);
 /* bytes of device memory owned by the handle (weights + activation arena)                          */
 int64_t aph_vit_bytes(const aph_vit* vit);
 
