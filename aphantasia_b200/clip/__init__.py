@@ -101,10 +101,42 @@ def has_text_tower(state_dict):
     return all(k in state_dict for k in _TEXT_KEYS) and 'transformer.resblocks.0.attn.in_proj_weight' in state_dict
 
 
-class TextTransformer:
+class _Tower:
+    """A tower's device handle, built through the C ABI's `<api>_create`, `_load_tensor` and `_finalize` from `self._sd`.
+    The handle is owned from its creation on: when a load or the finalize fails, close() still frees it."""
+    _api = None
+    handle, max_batch = None, 0
+
+    def _build(self, cfg, max_batch, prefix=''):
+        self.close()
+        h = C.c_void_p()
+        check(getattr(lib(), self._api + '_create')(C.byref(h), C.byref(cfg)), self._api + '_create')
+        self.handle = h
+        load, st = getattr(lib(), self._api + '_load_tensor'), stream_ptr()
+        for k, v in self._sd.items():
+            d = v.cuda()
+            check(load(h, (prefix + k).encode(), d.data_ptr(), d.numel(), st), '%s_load_tensor(%s)' % (self._api, k))
+        torch.cuda.current_stream().synchronize()      # staging copies `d` die with this scope
+        check(getattr(lib(), self._api + '_finalize')(h), self._api + '_finalize')
+        self.max_batch = int(max_batch)
+
+    def close(self):
+        if self.handle is not None:
+            getattr(lib(), self._api + '_destroy')(self.handle)
+            self.handle, self.max_batch = None, 0
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+class TextTransformer(_Tower):
     """Handle-owning forward of clip.model.CLIP's text tower (token embedding -> causal transformer -> ln_final at the
     end-of-text position -> text_projection) through the C ABI. The handle is created on the first call (constructing a
     CLIP needs no GPU) and re-created when a call brings more prompts than it was sized for."""
+    _api = 'aph_text'
 
     def __init__(self, state_dict):
         sd = {k: v for k, v in state_dict.items() if k in _TEXT_KEYS or k.startswith('transformer.resblocks.')}
@@ -114,34 +146,11 @@ class TextTransformer:
         self.heads = self.width // 64
         self.output_dim = sd['text_projection'].shape[1]
         self._sd = {k: v.detach().float().contiguous() for k, v in sd.items()}
-        self.handle, self.max_batch = None, 0
 
     def _ensure(self, n):
         if self.handle is not None and n <= self.max_batch:
             return
-        self.close()
-        cfg = TextConfig(self.width, self.layers, self.heads, self.output_dim, self.context, self.vocab, int(n), 0)
-        h = C.c_void_p()
-        check(lib().aph_text_create(C.byref(h), C.byref(cfg)), 'aph_text_create')
-        self.handle = h            # owned from here on: a failed load below still frees it in close()
-        st = stream_ptr()
-        for k, v in self._sd.items():
-            d = v.cuda()
-            check(lib().aph_text_load_tensor(h, k.encode(), d.data_ptr(), d.numel(), st), 'aph_text_load_tensor(%s)' % k)
-        torch.cuda.current_stream().synchronize()      # staging copies `d` die with this scope
-        check(lib().aph_text_finalize(h), 'aph_text_finalize')
-        self.max_batch = int(n)
-
-    def close(self):
-        if self.handle is not None:
-            lib().aph_text_destroy(self.handle)
-            self.handle, self.max_batch = None, 0
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+        self._build(TextConfig(self.width, self.layers, self.heads, self.output_dim, self.context, self.vocab, int(n), 0), n)
 
     @torch.no_grad()
     def __call__(self, tokens):
@@ -208,8 +217,9 @@ class _EncodeImage(torch.autograd.Function):
         return gi, None, None
 
 
-class VisionTransformer:
+class VisionTransformer(_Tower):
     """Handle-owning mirror of clip.model.VisionTransformer (forward only through the C ABI)."""
+    _api = 'aph_vit'
 
     def __init__(self, state_dict, max_batch=None):
         sd = {k[len('visual.'):]: v for k, v in state_dict.items() if k.startswith('visual.')}
@@ -221,7 +231,6 @@ class VisionTransformer:
         self.heads = self.width // 64
         self.output_dim = sd['proj'].shape[1]
         self._sd = {k: v.detach().float().contiguous() for k, v in sd.items()}
-        self.handle, self.max_batch = None, 0
         self._generation, self.recomputes, self._handle_epoch = 0, 0, 0        # see _EncodeImage
         self._patch_gen, self._patch_written, self.prepatched_forwards = 0, False, 0      # see _patchlink
         _patchlink.register(self)
@@ -232,29 +241,9 @@ class VisionTransformer:
         """(Re)creates the device handle so that its activation arena holds S samples."""
         if self.handle is not None and S <= self.max_batch:
             return
-        self.close()
-        cfg = VitConfig(self.patch_size, self.width, self.layers, self.heads, self.output_dim, self.input_resolution, int(S), 0)
-        h = C.c_void_p()
-        check(lib().aph_vit_create(C.byref(h), C.byref(cfg)), 'aph_vit_create')
-        st = stream_ptr()
-        for k, v in self._sd.items():
-            d = v.cuda()
-            check(lib().aph_vit_load_tensor(h, ('visual.' + k).encode(), d.data_ptr(), d.numel(), st), 'aph_vit_load_tensor(%s)' % k)
-        torch.cuda.current_stream().synchronize()      # staging copies `d` die with this scope
-        check(lib().aph_vit_finalize(h), 'aph_vit_finalize')
-        self.handle, self.max_batch = h, int(S)
+        self._build(VitConfig(self.patch_size, self.width, self.layers, self.heads, self.output_dim, self.input_resolution, int(S), 0),
+                    S, 'visual.')
         self._handle_epoch += 1
-
-    def close(self):
-        if self.handle is not None:
-            lib().aph_vit_destroy(self.handle)
-            self.handle = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
     def _fwd(self, xi, S, emb, save_for_bwd):
         side = xi.shape[-1]

@@ -55,6 +55,22 @@ inline int num_sms() {
   return n;
 }
 
+// Library-owned device scratch (it survives torch.cuda.empty_cache()) that grows on demand. Growing waits for `st` first: work
+// already queued there may still use the old buffer.
+struct Scratch {
+  float* p = nullptr;
+  size_t bytes = 0;
+  int grow(size_t need, cudaStream_t st) {
+    if (need <= bytes) return 0;
+    APH_CUDA_OK(cudaStreamSynchronize(st));
+    if (p) cudaFree(p);
+    p = nullptr; bytes = 0;
+    APH_CUDA_OK(cudaMalloc(&p, need));
+    bytes = need;
+    return 0;
+  }
+};
+
 // Programmatic dependent launch: a kernel calls pdl_trigger() first thing (its dependents may start being scheduled as SMs
 // drain) and pdl_wait() before its first global-memory access (blocks until the preceding grid has completed and flushed).
 // The prologue in between (barrier init, descriptor prefetch, index setup) overlaps the predecessor's tail.

@@ -1201,8 +1201,7 @@ static int check_sample_args(const char* who, int H, int W, int S, int size, int
   return 0;
 }
 
-static float* g_A = nullptr;           // resized crops [S,3,size,size] between k_resize and k_compose (library-owned scratch)
-static size_t g_A_bytes = 0;
+static Scratch g_A;                    // resized crops [S,3,size,size] between k_resize and k_compose
 
 static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int pad_left, const float* table, int S,
                            int size, int kind, float* out, PatchOut po, int* patches_written, void* stream);
@@ -1243,15 +1242,8 @@ static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int p
       cudaStream_t st = (cudaStream_t)stream;
       float* dst = out;
       if (kind >= APH_TF_FAST) {
-        const size_t need = (size_t)S * 3 * size * size * sizeof(float);
-        if (need > g_A_bytes) {
-          APH_CUDA_OK(cudaStreamSynchronize(st));
-          if (g_A) cudaFree(g_A);
-          g_A = nullptr; g_A_bytes = 0;
-          APH_CUDA_OK(cudaMalloc(&g_A, need));
-          g_A_bytes = need;
-        }
-        dst = g_A;
+        if (int e = g_A.grow((size_t)S * 3 * size * size * sizeof(float), st)) return e;
+        dst = g_A.p;
       }
       static size_t conf = 0;
       if (smem2 > conf) {
@@ -1266,12 +1258,12 @@ static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int p
       APH_LAUNCH_OK();
       if (kind == APH_TF_FAST) {
         const int tiles = ((size + 15) / 16) * ((size + 15) / 16);
-        k_compose<<<dim3(tiles, S), 256, 0, st>>>(g_A, table, size, out, po);
+        k_compose<<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
         APH_LAUNCH_OK();
       } else if (kornia) {
         const int s = size + 2 * KPAD, tiles = ((s + 15) / 16) * ((s + 15) / 16);
-        if (kind == APH_TF_ELASTIC) k_compose_kornia<true><<<dim3(tiles, S), 256, 0, st>>>(g_A, table, size, out, po);
-        else k_compose_kornia<false><<<dim3(tiles, S), 256, 0, st>>>(g_A, table, size, out, po);
+        if (kind == APH_TF_ELASTIC) k_compose_kornia<true><<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
+        else k_compose_kornia<false><<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
         APH_LAUNCH_OK();
       }
       if (patches_written) *patches_written = 1;
@@ -1295,12 +1287,9 @@ __global__ void __launch_bounds__(256) k_scale_inplace(float* __restrict__ p, si
 }
 }  // namespace aph
 
-static float* g_gW = nullptr;          // warp-stage adjoint scratch [S,3,size,size] of the default backward (all-zero between calls)
-static size_t g_gW_bytes = 0;
-static float* g_gA = nullptr;          // stage-1 scratch [S,3,size,size] (library-owned: survives torch.cuda.empty_cache())
-static size_t g_gA_bytes = 0;
-static float* g_gR = nullptr;          // kornia kinds: d loss / d rotated image [S,3,size+8,size+8], rewritten by every backward
-static size_t g_gR_bytes = 0;
+static Scratch g_gW;                   // warp-stage adjoint scratch [S,3,size,size] of the default backward (all-zero between calls)
+static Scratch g_gA;                   // stage-1 scratch [S,3,size,size]
+static Scratch g_gR;                   // kornia kinds: d loss / d rotated image [S,3,size+8,size+8], rewritten by every backward
 
 static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int pad_left, const float* table, int S,
                            int size, int kind, float* grad_canvas, float gscale, void* stream);
@@ -1333,23 +1322,16 @@ static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int
     const float* gsrc = grad_out;
     float pre[3] = {1.f, 1.f, 1.f};
     if (kind == APH_TF_FAST) {
-      const size_t need = (size_t)S * 3 * size * size * sizeof(float);
-      if (need > g_gA_bytes) {
-        APH_CUDA_OK(cudaStreamSynchronize(st));
-        if (g_gA) cudaFree(g_gA);
-        g_gA = nullptr; g_gA_bytes = 0;
-        APH_CUDA_OK(cudaMalloc(&g_gA, need));
-        g_gA_bytes = need;
-      }
+      if (int e = g_gA.grow((size_t)S * 3 * size * size * sizeof(float), st)) return e;
       const size_t smem1 = (size_t)size * size * sizeof(float);
       static size_t configured1 = 0;
       if (smem1 > configured1) {
         APH_CUDA_OK(cudaFuncSetAttribute(k_sample_bwd_stage1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
         configured1 = smem1;
       }
-      k_sample_bwd_stage1<<<S * 3, 1024, smem1, st>>>(grad_out, table, size, g_gA);
+      k_sample_bwd_stage1<<<S * 3, 1024, smem1, st>>>(grad_out, table, size, g_gA.p);
       APH_LAUNCH_OK();
-      gsrc = g_gA;
+      gsrc = g_gA.p;
     } else if (kind == APH_TF_NORMALIZE) {
       const float sd[3] = {0.26862954f, 0.26130258f, 0.27577711f};
       for (int c = 0; c < 3; ++c) pre[c] = 1.f / sd[c];
@@ -1385,21 +1367,14 @@ static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int
     if (kornia) {
       // adjoints of normalise, jitter and the elastic stretch into gR (fully overwritten), then the rest in k_bwd_bicubic3 (mode 4)
       const int s = size + 2 * KPAD;
-      const size_t need = (size_t)S * 3 * s * s * sizeof(float);
-      if (need > g_gR_bytes) {
-        APH_CUDA_OK(cudaStreamSynchronize(st));
-        if (g_gR) cudaFree(g_gR);
-        g_gR = nullptr; g_gR_bytes = 0;
-        APH_CUDA_OK(cudaMalloc(&g_gR, need));
-        g_gR_bytes = need;
-      }
+      if (int e = g_gR.grow((size_t)S * 3 * s * s * sizeof(float), st)) return e;
       const dim3 gk((s * s + 1023) / 1024, S);
-      if (kind == APH_TF_ELASTIC) k_bwd_kornia_stage<true><<<gk, 256, 0, st>>>(grad_out, table, size, gscale, g_gR);
-      else k_bwd_kornia_stage<false><<<gk, 256, 0, st>>>(grad_out, table, size, gscale, g_gR);
+      if (kind == APH_TF_ELASTIC) k_bwd_kornia_stage<true><<<gk, 256, 0, st>>>(grad_out, table, size, gscale, g_gR.p);
+      else k_bwd_kornia_stage<false><<<gk, 256, 0, st>>>(grad_out, table, size, gscale, g_gR.p);
       APH_LAUNCH_OK();
-      bb_src = g_gR;
+      bb_src = g_gR.p;
     }
-#define APH_BB(V, F, STREAM) k_bwd_bicubic3<V, F><<<g3, 256, smem3, STREAM>>>(bb_src, g_gW, H, W, pad_top, pad_left, table, size, kind, gscale, grad_canvas)
+#define APH_BB(V, F, STREAM) k_bwd_bicubic3<V, F><<<g3, 256, smem3, STREAM>>>(bb_src, g_gW.p, H, W, pad_top, pad_left, table, size, kind, gscale, grad_canvas)
 #define APH_BB_ANY(STREAM)                                                                           \
     do {                                                                                             \
       if (vec) { if (fp32_strips) APH_BB(true, false, STREAM); else APH_BB(true, true, STREAM); }    \
@@ -1408,17 +1383,13 @@ static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int
     } while (0)
     if (kind != APH_TF_FAST) { APH_BB_ANY(st); return 0; }
     const size_t need = (size_t)S * 3 * size * size * sizeof(float);
-    if (need > g_gW_bytes) {
-      APH_CUDA_OK(cudaStreamSynchronize(st));
-      if (g_gW) cudaFree(g_gW);
-      g_gW = nullptr; g_gW_bytes = 0;
-      APH_CUDA_OK(cudaMalloc(&g_gW, need));
-      g_gW_bytes = need;
-      APH_CUDA_OK(cudaMemsetAsync(g_gW, 0, need, st));          // invariant: all-zero between calls (k_bwd_bicubic3 clears what it consumes)
+    if (need > g_gW.bytes) {
+      if (int e = g_gW.grow(need, st)) return e;
+      APH_CUDA_OK(cudaMemsetAsync(g_gW.p, 0, need, st));        // invariant: all-zero between calls (k_bwd_bicubic3 clears what it consumes)
     }
     const dim3 g1((size + WA_ROWS - 1) / WA_ROWS, S);
     // (running this chain on a side stream beside the other crops' bicubic adjoint was measured: no gain, 0.335 vs 0.333 ms -- removed)
-    k_bwd_warp_adjoint<<<g1, 256, 0, st>>>(grad_out, table, size, gscale, g_gW);
+    k_bwd_warp_adjoint<<<g1, 256, 0, st>>>(grad_out, table, size, gscale, g_gW.p);
     APH_LAUNCH_OK();
     APH_BB_ANY(st);
 #undef APH_BB_ANY

@@ -6,39 +6,19 @@
 //   -> ln_final(x[s, argmax(ids[s])]) @ text_projection
 // It runs a handful of times per script run (once per prompt, before the optimisation loop): no CUDA graph, nothing is
 // saved for a backward pass, and each layer overwrites the previous one's activations.
-#include "vit_ops.cuh"
+#include "encoder.cuh"
 #include "vit_attn_tc.cuh"
-#include <stdlib.h>
-#include <string.h>
-#include <map>
-#include <string>
-#include <vector>
 
 namespace aph {
-
-int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st);   // vit.cu
-int copy_f32(const float* src, float* dst, size_t n, cudaStream_t st);                      // vit.cu
-
 namespace {
 
-struct TextLayer {
-  float *ln1_w = nullptr, *ln1_b = nullptr, *ln2_w = nullptr, *ln2_b = nullptr;
-  float *b_qkv = nullptr, *b_o = nullptr, *b_fc = nullptr, *b_proj = nullptr;
-  bf16 *w_qkv = nullptr, *w_o = nullptr, *w_fc = nullptr, *w_proj = nullptr;   // forward B operands [N, K]
-};
-
-struct TextImpl {
+struct TextImpl : Encoder {
   aph_text_config cfg;
-  int64_t bytes = 0;
-  std::vector<void*> allocs;
-  // weights
+  // weights besides the blocks'
   float* tok_emb = nullptr;      // [vocab, D] fp32: a gather reads n*ctx rows of it once per call
   float* pos = nullptr;          // [ctx, D]
   float *lnf_w = nullptr, *lnf_b = nullptr;
   bf16* w_out = nullptr;         // text_projection^T [out, D]
-  std::vector<TextLayer> L;
-  std::map<std::string, bool> loaded;
-  bool finalized = false;
   // activations, sized for max_batch * ctx rows
   float *x = nullptr, *x_mid = nullptr;   // residual stream fp32 [M, D], ping-pong within a layer
   bf16* ln_out = nullptr;        // [M, D]
@@ -50,18 +30,6 @@ struct TextImpl {
   int* eot = nullptr;            // [max_batch] pooling position per sequence
   bf16* pooled = nullptr;        // [max_batch, D] ln_final of the pooled rows
 };
-
-template <typename Tp>
-int dev_alloc(TextImpl* t, Tp** p, size_t count) {
-  void* q = nullptr;
-  APH_CUDA_OK(cudaMalloc(&q, count * sizeof(Tp)));
-  t->allocs.push_back(q);
-  t->bytes += (int64_t)(count * sizeof(Tp));
-  *p = reinterpret_cast<Tp*>(q);
-  return 0;
-}
-
-inline int rows_grid(int rows) { return (rows * 32 + 255) / 256; }
 
 // x[row] = token_embedding[ids[row]] + positional_embedding[row % ctx]; one warp per token row.
 // An id outside [0, vocab) contributes a zero row instead of reading out of bounds.
@@ -170,13 +138,7 @@ extern "C" int aph_text_create(aph_text** out, const aph_text_config* cfg) {
   int e = 0;
   e |= dev_alloc(t, &t->tok_emb, (size_t)cfg->vocab * D); e |= dev_alloc(t, &t->pos, (size_t)cfg->context * D);
   e |= dev_alloc(t, &t->lnf_w, D); e |= dev_alloc(t, &t->lnf_b, D); e |= dev_alloc(t, &t->w_out, (size_t)O * D);
-  t->L.resize(cfg->layers);
-  for (auto& l : t->L) {
-    e |= dev_alloc(t, &l.ln1_w, D); e |= dev_alloc(t, &l.ln1_b, D); e |= dev_alloc(t, &l.ln2_w, D); e |= dev_alloc(t, &l.ln2_b, D);
-    e |= dev_alloc(t, &l.b_qkv, 3 * D); e |= dev_alloc(t, &l.b_o, D); e |= dev_alloc(t, &l.b_fc, 4 * D); e |= dev_alloc(t, &l.b_proj, D);
-    e |= dev_alloc(t, &l.w_qkv, (size_t)3 * D * D); e |= dev_alloc(t, &l.w_o, (size_t)D * D);
-    e |= dev_alloc(t, &l.w_fc, (size_t)4 * D * D); e |= dev_alloc(t, &l.w_proj, (size_t)4 * D * D);
-  }
+  e |= alloc_blocks(t, cfg->layers, D, false);
   e |= dev_alloc(t, &t->x, M * D); e |= dev_alloc(t, &t->x_mid, M * D); e |= dev_alloc(t, &t->ln_out, M * D);
   e |= dev_alloc(t, &t->qkv, M * 3 * D); e |= dev_alloc(t, &t->attn_out, M * D);
   e |= dev_alloc(t, &t->h_pre, M * 4 * D); e |= dev_alloc(t, &t->h_act, M * 4 * D);
@@ -189,9 +151,7 @@ extern "C" int aph_text_create(aph_text** out, const aph_text_config* cfg) {
 
 extern "C" int aph_text_destroy(aph_text* text) {
   if (!text) return 0;
-  TextImpl* t = reinterpret_cast<TextImpl*>(text);
-  for (void* p : t->allocs) cudaFree(p);
-  delete t;
+  delete reinterpret_cast<TextImpl*>(text);
   return 0;
 }
 
@@ -210,27 +170,8 @@ extern "C" int aph_text_load_tensor(aph_text* text, const char* key, const float
   else if (k == "ln_final.weight") { if ((e = need(D))) return e; e = copy_f32(data, t->lnf_w, D, st); }
   else if (k == "ln_final.bias") { if ((e = need(D))) return e; e = copy_f32(data, t->lnf_b, D, st); }
   else if (k == "text_projection") { if ((e = need((int64_t)D * O))) return e; e = pack(data, t->w_out, D, O, 1, st); }   // [D, out] -> [out, D]
-  else if (k.rfind("transformer.resblocks.", 0) == 0) {
-    const char* rest = k.c_str() + strlen("transformer.resblocks.");
-    char* endp = nullptr;
-    const long li = strtol(rest, &endp, 10);
-    APH_REQUIRE(endp && *endp == '.' && li >= 0 && li < t->cfg.layers, "aph_text_load_tensor: bad layer index in %s", key);
-    TextLayer& l = t->L[li];
-    const std::string f(endp + 1);
-    if (f == "ln_1.weight") { if ((e = need(D))) return e; e = copy_f32(data, l.ln1_w, D, st); }
-    else if (f == "ln_1.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.ln1_b, D, st); }
-    else if (f == "ln_2.weight") { if ((e = need(D))) return e; e = copy_f32(data, l.ln2_w, D, st); }
-    else if (f == "ln_2.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.ln2_b, D, st); }
-    else if (f == "attn.in_proj_weight") { if ((e = need((int64_t)3 * D * D))) return e; e = pack(data, l.w_qkv, 3 * D, D, 0, st); }
-    else if (f == "attn.in_proj_bias") { if ((e = need(3 * D))) return e; e = copy_f32(data, l.b_qkv, 3 * D, st); }
-    else if (f == "attn.out_proj.weight") { if ((e = need((int64_t)D * D))) return e; e = pack(data, l.w_o, D, D, 0, st); }
-    else if (f == "attn.out_proj.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.b_o, D, st); }
-    else if (f == "mlp.c_fc.weight") { if ((e = need((int64_t)4 * D * D))) return e; e = pack(data, l.w_fc, 4 * D, D, 0, st); }
-    else if (f == "mlp.c_fc.bias") { if ((e = need(4 * D))) return e; e = copy_f32(data, l.b_fc, 4 * D, st); }
-    else if (f == "mlp.c_proj.weight") { if ((e = need((int64_t)4 * D * D))) return e; e = pack(data, l.w_proj, D, 4 * D, 0, st); }
-    else if (f == "mlp.c_proj.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.b_proj, D, st); }
-    else { set_error("aph_text_load_tensor: unknown tensor %s", key); return 2; }
-  } else { set_error("aph_text_load_tensor: unknown tensor %s", key); return 2; }
+  else if (k.rfind("transformer.resblocks.", 0) == 0) e = load_block_tensor(t, k, key, data, numel, D, st, "aph_text_load_tensor");
+  else { set_error("aph_text_load_tensor: unknown tensor %s", key); return 2; }
   if (e) return e;
   t->loaded[k] = true;
   return 0;
@@ -239,12 +180,9 @@ extern "C" int aph_text_load_tensor(aph_text* text, const char* key, const float
 extern "C" int aph_text_finalize(aph_text* text) {
   APH_REQUIRE(text, "aph_text_finalize: null handle");
   TextImpl* t = reinterpret_cast<TextImpl*>(text);
-  std::vector<std::string> want = {"token_embedding.weight", "positional_embedding", "ln_final.weight", "ln_final.bias", "text_projection"};
-  const char* per[] = {"ln_1.weight", "ln_1.bias", "ln_2.weight", "ln_2.bias", "attn.in_proj_weight", "attn.in_proj_bias",
-                       "attn.out_proj.weight", "attn.out_proj.bias", "mlp.c_fc.weight", "mlp.c_fc.bias", "mlp.c_proj.weight", "mlp.c_proj.bias"};
-  for (int i = 0; i < t->cfg.layers; ++i)
-    for (const char* p : per) want.push_back("transformer.resblocks." + std::to_string(i) + "." + p);
-  for (const auto& w : want) APH_REQUIRE(t->loaded.count(w), "aph_text_finalize: tensor %s was never loaded", w.c_str());
+  if (int e = check_loaded(t, {"token_embedding.weight", "positional_embedding", "ln_final.weight", "ln_final.bias", "text_projection"},
+                           "aph_text_finalize", ""))
+    return e;
   t->finalized = true;
   return 0;
 }
@@ -262,21 +200,9 @@ extern "C" int aph_text_fwd(aph_text* text, const int64_t* tokens, int n, float*
   APH_LAUNCH_OK();
   APH_CUDA_OK(launch_k(k_text_eot, dim3(rows_grid(n)), dim3(256), (size_t)0, st, 1, tokens, t->eot, n, C));
   APH_LAUNCH_OK();
-  for (const TextLayer& w : t->L) {
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, t->x, (size_t)D, w.ln1_w, w.ln1_b, t->ln_out, t->mean, t->rstd, M, D)));
-    APH_LAUNCH_OK();
-    { GemmEpi ep; ep.bias = w.b_qkv; ep.out_bf16 = t->qkv;
-      if ((e = launch_gemm(t->ln_out, w.w_qkv, GemmShape{M, 3 * D, D}, ep, st))) return e; }
-    if ((e = attn_causal(t->qkv, t->attn_out, n, C, D, H, st))) return e;
-    { GemmEpi ep; ep.bias = w.b_o; ep.resid = t->x; ep.out_f32 = t->x_mid;
-      if ((e = launch_gemm(t->attn_out, w.w_o, GemmShape{M, D, D}, ep, st))) return e; }
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, t->x_mid, (size_t)D, w.ln2_w, w.ln2_b, t->ln_out, t->mean, t->rstd, M, D)));
-    APH_LAUNCH_OK();
-    { GemmEpi ep; ep.bias = w.b_fc; ep.out_pre = t->h_pre; ep.act = 1; ep.out_bf16 = t->h_act;
-      if ((e = launch_gemm(t->ln_out, w.w_fc, GemmShape{M, 4 * D, D}, ep, st))) return e; }
-    { GemmEpi ep; ep.bias = w.b_proj; ep.resid = t->x_mid; ep.out_f32 = t->x;
-      if ((e = launch_gemm(t->h_act, w.w_proj, GemmShape{M, D, 4 * D}, ep, st))) return e; }
-  }
+  const BlockIO io{t->x, t->x_mid, t->x, t->ln_out, t->qkv, t->attn_out, t->h_pre, t->h_act, t->mean, t->rstd, t->mean, t->rstd};
+  for (const BlockW& w : t->L)
+    if ((e = block_fwd(w, io, n, C, M, 0, D, H, attn_causal, st))) return e;
   NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_text_pool_ln<NCH>, dim3(rows_grid(n)), dim3(256), (size_t)0, st, 1, t->x, t->eot, t->lnf_w, t->lnf_b, t->pooled, n, C, D)));
   APH_LAUNCH_OK();
   GemmEpi ep; ep.out_f32 = emb;

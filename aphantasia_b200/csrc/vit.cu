@@ -6,37 +6,20 @@
 //   -> ln_post(x[:,0]) @ proj
 // The residual stream is fp32; GEMM operands are bf16; every x_l is kept (out-of-place residual) so the
 // LayerNorm backward can recompute x-hat. No weight gradients (the reference computes and discards them).
-#include "vit_ops.cuh"
+#include "encoder.cuh"
 #include "vit_attn_tc.cuh"
 #include <stdlib.h>
-#include <string>
-#include <vector>
-#include <map>
 #include <string.h>
 
 namespace aph {
 
-struct LayerW {
-  float *ln1_w = nullptr, *ln1_b = nullptr, *ln2_w = nullptr, *ln2_b = nullptr;
-  float *b_qkv = nullptr, *b_o = nullptr, *b_fc = nullptr, *b_proj = nullptr;
-  bf16 *w_qkv = nullptr, *w_qkv_t = nullptr;     // [3D, D], [D, 3D]
-  bf16 *w_o = nullptr, *w_o_t = nullptr;         // [D, D]
-  bf16 *w_fc = nullptr, *w_fc_t = nullptr;       // [4D, D], [D, 4D]
-  bf16 *w_proj = nullptr, *w_proj_t = nullptr;   // [D, 4D], [4D, D]
-};
-
-struct VitImpl {
+struct VitImpl : Encoder {
   aph_vit_config cfg;
   int g, T, D, Kp;
-  int64_t bytes = 0;
-  std::vector<void*> allocs;
-  // weights
+  // weights besides the blocks'
   bf16 *w_conv = nullptr, *w_conv_t = nullptr;   // [D, Kp], [Kp, D]
   float *cls = nullptr, *pos = nullptr, *lnpre_w = nullptr, *lnpre_b = nullptr, *lnpost_w = nullptr, *lnpost_b = nullptr;
   bf16 *w_out = nullptr, *w_out_t = nullptr;     // proj^T [out, D] (forward B operand), proj [D, out] (dgrad B operand)
-  std::vector<LayerW> L;
-  std::map<std::string, bool> loaded;
-  bool finalized = false;
   // activations (sized for max_batch)
   bf16* patches = nullptr;       // [S*g*g, Kp]
   float* tok = nullptr;          // [S*g*g, D]
@@ -145,17 +128,6 @@ static int run_cached(std::vector<VitImpl::GraphEntry>& cache, std::map<int, int
   return 0;
 }
 
-template <typename Tp>
-static int dev_alloc(VitImpl* v, Tp** p, size_t count) {
-  void* q = nullptr;
-  APH_CUDA_OK(cudaMalloc(&q, count * sizeof(Tp)));
-  v->allocs.push_back(q);
-  v->bytes += (int64_t)(count * sizeof(Tp));
-  *p = reinterpret_cast<Tp*>(q);
-  return 0;
-}
-
-// fp32 [rows, cols] -> bf16 [rows, cols] (transpose = 0) or bf16 [cols, rows] (transpose = 1)
 __global__ void __launch_bounds__(256) k_pack_weight(const float* __restrict__ in, bf16* __restrict__ out, int rows, int cols, int transpose) {
   const size_t n = (size_t)rows * cols;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -165,7 +137,6 @@ __global__ void __launch_bounds__(256) k_pack_weight(const float* __restrict__ i
   }
 }
 
-// (also used by text.cu)
 int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st) {
   const size_t n = (size_t)rows * cols;
   const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16);
@@ -179,7 +150,92 @@ int copy_f32(const float* src, float* dst, size_t n, cudaStream_t st) {
   return 0;
 }
 
-static inline int rows_grid(int rows) { return (rows * 32 + 255) / 256; }
+// The tensors of a residual block, state-dict key transformer.resblocks.<i>.<key>. An fp32 entry is a vector of rows*D elements,
+// copied as it is; a bf16 entry is a [rows*D, cols*D] matrix packed as the forward GEMM's B operand and, where the block has
+// them (w_t allocated), transposed into the data gradient's.
+using F32Slot = float* BlockW::*;
+using Bf16Slot = bf16* BlockW::*;
+struct BlockTensor {
+  const char* key;
+  int rows, cols;
+  F32Slot f32;
+  Bf16Slot w, w_t;
+};
+static const BlockTensor kBlockTensors[] = {
+    {"ln_1.weight", 1, 0, &BlockW::ln1_w, nullptr, nullptr},
+    {"ln_1.bias", 1, 0, &BlockW::ln1_b, nullptr, nullptr},
+    {"ln_2.weight", 1, 0, &BlockW::ln2_w, nullptr, nullptr},
+    {"ln_2.bias", 1, 0, &BlockW::ln2_b, nullptr, nullptr},
+    {"attn.in_proj_weight", 3, 1, nullptr, &BlockW::w_qkv, &BlockW::w_qkv_t},
+    {"attn.in_proj_bias", 3, 0, &BlockW::b_qkv, nullptr, nullptr},
+    {"attn.out_proj.weight", 1, 1, nullptr, &BlockW::w_o, &BlockW::w_o_t},
+    {"attn.out_proj.bias", 1, 0, &BlockW::b_o, nullptr, nullptr},
+    {"mlp.c_fc.weight", 4, 1, nullptr, &BlockW::w_fc, &BlockW::w_fc_t},
+    {"mlp.c_fc.bias", 4, 0, &BlockW::b_fc, nullptr, nullptr},
+    {"mlp.c_proj.weight", 1, 4, nullptr, &BlockW::w_proj, &BlockW::w_proj_t},
+    {"mlp.c_proj.bias", 1, 0, &BlockW::b_proj, nullptr, nullptr},
+};
+
+static size_t numel_of(const BlockTensor& t, int D) { return (size_t)t.rows * D * (t.w ? (size_t)t.cols * D : 1); }
+
+int alloc_blocks(Encoder* h, int layers, int D, bool dgrad) {
+  h->L.resize(layers);
+  int e = 0;
+  for (BlockW& l : h->L)
+    for (const BlockTensor& t : kBlockTensors) {
+      if (t.f32) { e |= dev_alloc(h, &(l.*t.f32), numel_of(t, D)); continue; }
+      e |= dev_alloc(h, &(l.*t.w), numel_of(t, D));
+      if (dgrad) e |= dev_alloc(h, &(l.*t.w_t), numel_of(t, D));
+    }
+  return e;
+}
+
+int load_block_tensor(Encoder* h, const std::string& k, const char* key, const float* data, int64_t numel, int D, cudaStream_t st,
+                      const char* who) {
+  const char* rest = k.c_str() + strlen("transformer.resblocks.");
+  char* endp = nullptr;
+  const long li = strtol(rest, &endp, 10);
+  APH_REQUIRE(endp && *endp == '.' && li >= 0 && li < (long)h->L.size(), "%s: bad layer index in %s", who, key);
+  BlockW& l = h->L[li];
+  for (const BlockTensor& t : kBlockTensors) {
+    if (strcmp(endp + 1, t.key) != 0) continue;
+    const size_t n = numel_of(t, D);
+    APH_REQUIRE(numel == (int64_t)n, "%s(%s): expected %lld elements, got %lld", who, key, (long long)n, (long long)numel);
+    if (t.f32) return copy_f32(data, l.*t.f32, n, st);
+    if (int e = pack(data, l.*t.w, t.rows * D, t.cols * D, 0, st)) return e;
+    return l.*t.w_t ? pack(data, l.*t.w_t, t.rows * D, t.cols * D, 1, st) : 0;
+  }
+  set_error("%s: unknown tensor %s", who, key);
+  return 2;
+}
+
+int check_loaded(const Encoder* h, std::vector<std::string> want, const char* who, const char* prefix) {
+  for (size_t i = 0; i < h->L.size(); ++i)
+    for (const BlockTensor& t : kBlockTensors) want.push_back("transformer.resblocks." + std::to_string(i) + "." + t.key);
+  for (const auto& w : want) APH_REQUIRE(h->loaded.count(w), "%s: tensor %s%s was never loaded", who, prefix, w.c_str());
+  return 0;
+}
+
+int block_fwd(const BlockW& w, const BlockIO& io, int S, int T, int Mr, int ld_tok, int D, int heads, AttnFwd attn, cudaStream_t st) {
+  const int M = S * T;
+  int e;
+  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, io.x_in, w.ln1_w, w.ln1_b, io.ln_out, io.mean1,
+                                       io.rstd1, M, D)));
+  APH_LAUNCH_OK();
+  { GemmEpi ep; ep.bias = w.b_qkv; ep.out_bf16 = io.qkv;
+    if ((e = launch_gemm(io.ln_out, w.w_qkv, GemmShape{M, 3 * D, D}, ep, st))) return e; }
+  if ((e = attn(io.qkv, io.attn_out, S, T, D, heads, st))) return e;
+  { GemmEpi ep; ep.bias = w.b_o; ep.resid = io.x_in; ep.ld_resid = ld_tok; ep.out_f32 = io.x_mid;
+    if ((e = launch_gemm(io.attn_out, w.w_o, GemmShape{Mr, D, D}, ep, st, ld_tok))) return e; }
+  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(Mr)), dim3(256), (size_t)0, st, 1, io.x_mid, w.ln2_w, w.ln2_b, io.ln_out, io.mean2,
+                                       io.rstd2, Mr, D)));
+  APH_LAUNCH_OK();
+  { GemmEpi ep; ep.bias = w.b_fc; ep.out_pre = io.h_pre; ep.act = 1; ep.out_bf16 = io.h_act;
+    if ((e = launch_gemm(io.ln_out, w.w_fc, GemmShape{Mr, 4 * D, D}, ep, st))) return e; }
+  { GemmEpi ep; ep.bias = w.b_proj; ep.resid = io.x_mid; ep.out_f32 = io.x_out;
+    if ((e = launch_gemm(io.h_act, w.w_proj, GemmShape{Mr, D, 4 * D}, ep, st))) return e; }
+  return 0;
+}
 
 // APH_ATTN_SIMT=1 selects the fp32 SIMT attention kernels (debug / comparison); default = tensor-core kernels.
 static bool attn_simt() {
@@ -187,6 +243,15 @@ static bool attn_simt() {
   if (v < 0) { const char* e = getenv("APH_ATTN_SIMT"); v = (e && e[0] == '1') ? 1 : 0; }
   return v == 1;
 }
+
+static int vit_attn_fwd(const bf16* qkv, bf16* out, int S, int T, int D, int heads, cudaStream_t st) {
+  if (!attn_simt()) return attn_dispatch(true, qkv, nullptr, out, S, T, D, heads, st);
+  k_attn_fwd<<<S * heads, 256, attn_fwd_smem(T), st>>>(qkv, out, T, D, heads);
+  APH_LAUNCH_OK();
+  return 0;
+}
+
+static Scratch g_win;   // aph_vit_bwd_sized: the R x R window gradient before k_window_expand
 
 }  // namespace aph
 
@@ -211,15 +276,7 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
   e |= dev_alloc(v, &v->cls, D); e |= dev_alloc(v, &v->pos, (size_t)T * D);
   e |= dev_alloc(v, &v->lnpre_w, D); e |= dev_alloc(v, &v->lnpre_b, D); e |= dev_alloc(v, &v->lnpost_w, D); e |= dev_alloc(v, &v->lnpost_b, D);
   e |= dev_alloc(v, &v->w_out, (size_t)D * O); e |= dev_alloc(v, &v->w_out_t, (size_t)D * O);
-  v->L.resize(Ly);
-  for (auto& l : v->L) {
-    e |= dev_alloc(v, &l.ln1_w, D); e |= dev_alloc(v, &l.ln1_b, D); e |= dev_alloc(v, &l.ln2_w, D); e |= dev_alloc(v, &l.ln2_b, D);
-    e |= dev_alloc(v, &l.b_qkv, 3 * D); e |= dev_alloc(v, &l.b_o, D); e |= dev_alloc(v, &l.b_fc, 4 * D); e |= dev_alloc(v, &l.b_proj, D);
-    e |= dev_alloc(v, &l.w_qkv, (size_t)3 * D * D); e |= dev_alloc(v, &l.w_qkv_t, (size_t)3 * D * D);
-    e |= dev_alloc(v, &l.w_o, (size_t)D * D); e |= dev_alloc(v, &l.w_o_t, (size_t)D * D);
-    e |= dev_alloc(v, &l.w_fc, (size_t)4 * D * D); e |= dev_alloc(v, &l.w_fc_t, (size_t)4 * D * D);
-    e |= dev_alloc(v, &l.w_proj, (size_t)4 * D * D); e |= dev_alloc(v, &l.w_proj_t, (size_t)4 * D * D);
-  }
+  e |= alloc_blocks(v, Ly, D, true);
   // activations
   e |= dev_alloc(v, &v->patches, Mp * v->Kp); e |= dev_alloc(v, &v->tok, Mp * D); e |= dev_alloc(v, &v->e, M * D);
   v->xs.resize(2 * Ly + 1);
@@ -248,7 +305,6 @@ extern "C" int aph_vit_destroy(aph_vit* vit) {
   VitImpl* v = reinterpret_cast<VitImpl*>(vit);
   for (auto& g : v->fwd_graphs) cudaGraphExecDestroy(g.exec);
   for (auto& g : v->bwd_graphs) cudaGraphExecDestroy(g.exec);
-  for (void* p : v->allocs) cudaFree(p);
   delete v;
   return 0;
 }
@@ -274,27 +330,8 @@ extern "C" int aph_vit_load_tensor(aph_vit* vit, const char* key, const float* d
   else if (k == "proj") {   // [D, out]: forward B operand is proj^T [out, D]; dgrad B operand is proj [D, out]
     if ((e = need((int64_t)D * O))) return e;
     e = pack(data, v->w_out, D, O, 1, st) | pack(data, v->w_out_t, D, O, 0, st);
-  } else if (k.rfind("transformer.resblocks.", 0) == 0) {
-    const char* rest = k.c_str() + strlen("transformer.resblocks.");
-    char* endp = nullptr;
-    const long li = strtol(rest, &endp, 10);
-    APH_REQUIRE(endp && *endp == '.' && li >= 0 && li < v->cfg.layers, "aph_vit_load_tensor: bad layer index in %s", key);
-    LayerW& l = v->L[li];
-    const std::string f(endp + 1);
-    if (f == "ln_1.weight") { if ((e = need(D))) return e; e = copy_f32(data, l.ln1_w, D, st); }
-    else if (f == "ln_1.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.ln1_b, D, st); }
-    else if (f == "ln_2.weight") { if ((e = need(D))) return e; e = copy_f32(data, l.ln2_w, D, st); }
-    else if (f == "ln_2.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.ln2_b, D, st); }
-    else if (f == "attn.in_proj_weight") { if ((e = need((int64_t)3 * D * D))) return e; e = pack(data, l.w_qkv, 3 * D, D, 0, st) | pack(data, l.w_qkv_t, 3 * D, D, 1, st); }
-    else if (f == "attn.in_proj_bias") { if ((e = need(3 * D))) return e; e = copy_f32(data, l.b_qkv, 3 * D, st); }
-    else if (f == "attn.out_proj.weight") { if ((e = need((int64_t)D * D))) return e; e = pack(data, l.w_o, D, D, 0, st) | pack(data, l.w_o_t, D, D, 1, st); }
-    else if (f == "attn.out_proj.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.b_o, D, st); }
-    else if (f == "mlp.c_fc.weight") { if ((e = need((int64_t)4 * D * D))) return e; e = pack(data, l.w_fc, 4 * D, D, 0, st) | pack(data, l.w_fc_t, 4 * D, D, 1, st); }
-    else if (f == "mlp.c_fc.bias") { if ((e = need(4 * D))) return e; e = copy_f32(data, l.b_fc, 4 * D, st); }
-    else if (f == "mlp.c_proj.weight") { if ((e = need((int64_t)4 * D * D))) return e; e = pack(data, l.w_proj, D, 4 * D, 0, st) | pack(data, l.w_proj_t, D, 4 * D, 1, st); }
-    else if (f == "mlp.c_proj.bias") { if ((e = need(D))) return e; e = copy_f32(data, l.b_proj, D, st); }
-    else { set_error("aph_vit_load_tensor: unknown tensor %s", key); return 2; }
-  } else { set_error("aph_vit_load_tensor: unknown tensor %s", key); return 2; }
+  } else if (k.rfind("transformer.resblocks.", 0) == 0) e = load_block_tensor(v, k, key, data, numel, D, st, "aph_vit_load_tensor");
+  else { set_error("aph_vit_load_tensor: unknown tensor %s", key); return 2; }
   if (e) return e;
   v->loaded[k] = true;
   return 0;
@@ -303,20 +340,14 @@ extern "C" int aph_vit_load_tensor(aph_vit* vit, const char* key, const float* d
 extern "C" int aph_vit_finalize(aph_vit* vit) {
   APH_REQUIRE(vit, "aph_vit_finalize: null handle");
   VitImpl* v = reinterpret_cast<VitImpl*>(vit);
-  std::vector<std::string> want = {"conv1.weight", "class_embedding", "positional_embedding", "ln_pre.weight", "ln_pre.bias",
-                                   "ln_post.weight", "ln_post.bias", "proj"};
-  const char* per[] = {"ln_1.weight", "ln_1.bias", "ln_2.weight", "ln_2.bias", "attn.in_proj_weight", "attn.in_proj_bias",
-                       "attn.out_proj.weight", "attn.out_proj.bias", "mlp.c_fc.weight", "mlp.c_fc.bias", "mlp.c_proj.weight", "mlp.c_proj.bias"};
-  for (int i = 0; i < v->cfg.layers; ++i)
-    for (const char* p : per) want.push_back("transformer.resblocks." + std::to_string(i) + "." + p);
-  for (const auto& w : want) APH_REQUIRE(v->loaded.count(w), "aph_vit_finalize: tensor visual.%s was never loaded", w.c_str());
+  if (int e = check_loaded(v, {"conv1.weight", "class_embedding", "positional_embedding", "ln_pre.weight", "ln_pre.bias", "ln_post.weight",
+                               "ln_post.bias", "proj"}, "aph_vit_finalize", "visual."))
+    return e;
   v->finalized = true;
   return 0;
 }
 
 static int vit_fwd_impl(aph_vit* vit, const float* images, int S, int side, float* emb, int save_for_bwd, void* stream);
-static float* g_win = nullptr;         // aph_vit_bwd_sized: the R x R window gradient before k_window_expand (grown on demand)
-static size_t g_win_bytes = 0;
 static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, float* grad_images, void* stream);
 
 extern "C" int aph_vit_fwd(aph_vit* vit, const float* images, int S, float* emb, int save_for_bwd, void* stream) {
@@ -386,31 +417,16 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, int side, floa
     APH_LAUNCH_OK();
   }
   for (int l = 0; l < Ly; ++l) {
-    const LayerW& w = v->L[l];
     // the last block runs on the cls rows after attention: out_proj reads rows s*T of attn_out and x_in (stride T*D)
     const bool last = l == Ly - 1;
-    const int Mr = last ? S : M, ld_tok = last ? T * D : 0;
-    float* x_in = v->xs[2 * l]; float* x_mid = v->xs[2 * l + 1]; float* x_out = v->xs[2 * l + 2];
-    float* mean1 = v->st_mean + stat_off(v, 1 + 2 * l); float* rstd1 = v->st_rstd + stat_off(v, 1 + 2 * l);
-    float* mean2 = v->st_mean + stat_off(v, 2 + 2 * l); float* rstd2 = v->st_rstd + stat_off(v, 2 + 2 * l);
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, x_in, (size_t)D, w.ln1_w, w.ln1_b, v->ln_out, mean1, rstd1, M, D)));
-    APH_LAUNCH_OK();
-    { GemmEpi ep; ep.bias = w.b_qkv; ep.out_bf16 = v->qkv[l];
-      if ((e = launch_gemm(v->ln_out, w.w_qkv, GemmShape{M, 3 * D, D}, ep, st))) return e; }
-    if (attn_simt()) { k_attn_fwd<<<S * H, 256, attn_fwd_smem(T), st>>>(v->qkv[l], v->attn_out, T, D, H); APH_LAUNCH_OK(); }
-    else if ((e = attn_dispatch(true, v->qkv[l], nullptr, v->attn_out, S, T, D, H, st))) return e;
-    { GemmEpi ep; ep.bias = w.b_o; ep.resid = x_in; ep.ld_resid = ld_tok; ep.out_f32 = x_mid;
-      if ((e = launch_gemm(v->attn_out, w.w_o, GemmShape{Mr, D, D}, ep, st, ld_tok))) return e; }
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(Mr)), dim3(256), (size_t)0, st, 1, x_mid, (size_t)D, w.ln2_w, w.ln2_b, v->ln_out, mean2, rstd2, Mr, D)));
-    APH_LAUNCH_OK();
-    { GemmEpi ep; ep.bias = w.b_fc; ep.out_pre = v->h_pre[l]; ep.act = 1; ep.out_bf16 = v->h_act;
-      if ((e = launch_gemm(v->ln_out, w.w_fc, GemmShape{Mr, 4 * D, D}, ep, st))) return e; }
-    { GemmEpi ep; ep.bias = w.b_proj; ep.resid = x_mid; ep.out_f32 = x_out;
-      if ((e = launch_gemm(v->h_act, w.w_proj, GemmShape{Mr, D, 4 * D}, ep, st))) return e; }
+    const BlockIO io{v->xs[2 * l], v->xs[2 * l + 1], v->xs[2 * l + 2], v->ln_out, v->qkv[l], v->attn_out, v->h_pre[l], v->h_act,
+                     v->st_mean + stat_off(v, 1 + 2 * l), v->st_rstd + stat_off(v, 1 + 2 * l),
+                     v->st_mean + stat_off(v, 2 + 2 * l), v->st_rstd + stat_off(v, 2 + 2 * l)};
+    if ((e = block_fwd(v->L[l], io, S, T, last ? S : M, last ? T * D : 0, D, H, vit_attn_fwd, st))) return e;
   }
   {
     float* meanp = v->st_mean + stat_off(v, 2 * Ly + 1); float* rstdp = v->st_rstd + stat_off(v, 2 * Ly + 1);
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(S)), dim3(256), (size_t)0, st, 1, v->xs[2 * Ly], (size_t)D, v->lnpost_w, v->lnpost_b, v->cls_ln,
+    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(S)), dim3(256), (size_t)0, st, 1, v->xs[2 * Ly], v->lnpost_w, v->lnpost_b, v->cls_ln,
                                                                  meanp, rstdp, S, D)));
     APH_LAUNCH_OK();
     GemmEpi ep; ep.out_f32 = v->emb_int;
@@ -452,7 +468,7 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
     APH_LAUNCH_OK();
   }
   for (int l = Ly - 1; l >= 0; --l) {
-    const LayerW& w = v->L[l];
+    const BlockW& w = v->L[l];
     // the last block's MLP and out_proj run on its S cls rows: their gradient is dxc; d out_proj lands on rows s*T of d_attn_last
     const bool last = l == Ly - 1;
     const int Mr = last ? S : M;
@@ -492,22 +508,14 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
     // a larger image (aph_vit_bwd_sized): the epilogue writes the R x R window into a scratch image, k_window_expand places it
     // and zeroes the margin, which conv1 never reads
     const bool sized = side != R;
-    if (sized) {
-      const size_t need = (size_t)S * 3 * R * R * sizeof(float);
-      if (need > g_win_bytes) {
-        APH_CUDA_OK(cudaStreamSynchronize(st));
-        if (g_win) cudaFree(g_win);
-        g_win = nullptr; g_win_bytes = 0;
-        APH_CUDA_OK(cudaMalloc(&g_win, need));
-        g_win_bytes = need;
-      }
-    }
-    GemmEpi ep; ep.out_f32 = sized ? g_win : grad_images; ep.unpatch_p = v->cfg.patch; ep.unpatch_g = g;
+    if (sized)
+      if (int e = g_win.grow((size_t)S * 3 * R * R * sizeof(float), st)) return e;
+    GemmEpi ep; ep.out_f32 = sized ? g_win.p : grad_images; ep.unpatch_p = v->cfg.patch; ep.unpatch_g = g;
     if (int e = launch_gemm(v->d_tok, v->w_conv_t, GemmShape{Mp, v->Kp, v->D}, ep, st)) return e;
     if (sized) {
       const size_t n = (size_t)S * 3 * side * side;
       APH_CUDA_OK(launch_k(k_window_expand, dim3((unsigned)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1,
-                           (const float*)g_win, grad_images, S * 3, R, side));
+                           (const float*)g_win.p, grad_images, S * 3, R, side));
       APH_LAUNCH_OK();
     }
   }
@@ -533,8 +541,8 @@ extern "C" int aph_attn_test(int fwd, int causal, const void* qkv, const void* d
 extern "C" int aph_ln_fwd_test(const float* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows, int D,
                                void* stream) {
   APH_REQUIRE(x && gamma && beta && y && mean && rstd && rows > 0 && D % 128 == 0, "aph_ln_fwd_test: null argument or rows=%d D=%d", rows, D);
-  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(rows)), dim3(256), (size_t)0, (cudaStream_t)stream, 1, x, (size_t)D, gamma,
-                                       beta, reinterpret_cast<bf16*>(y), mean, rstd, rows, D)));
+  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(rows)), dim3(256), (size_t)0, (cudaStream_t)stream, 1, x, gamma, beta,
+                                       reinterpret_cast<bf16*>(y), mean, rstd, rows, D)));
   APH_LAUNCH_OK();
   return 0;
 }

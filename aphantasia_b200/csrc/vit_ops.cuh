@@ -146,9 +146,9 @@ __global__ void __launch_bounds__(256) k_embed_lnpre(const float* __restrict__ t
   if (lane == 0) { mean_out[row] = st.mean; rstd_out[row] = st.rstd; }
 }
 
-// y = LN(x) as bf16. Input row r lives at x + r*in_stride (in_stride = D for all tokens, T*D for the cls rows).
+// y = LN(x) as bf16, x and y [rows, D].
 template <int NCH>
-__global__ void __launch_bounds__(256) k_ln_fwd(const float* __restrict__ x, size_t in_stride, const float* __restrict__ gamma,
+__global__ void __launch_bounds__(256) k_ln_fwd(const float* __restrict__ x, const float* __restrict__ gamma,
                                                 const float* __restrict__ beta, bf16* __restrict__ y, float* __restrict__ mean_out,
                                                 float* __restrict__ rstd_out, int rows, int D) {
   pdl_trigger(); pdl_wait();
@@ -156,7 +156,7 @@ __global__ void __launch_bounds__(256) k_ln_fwd(const float* __restrict__ x, siz
   if (row >= rows) return;
   constexpr int N = 4 * NCH;
   float v[N], gm[N], bt[N];
-  load_row(x + (size_t)row * in_stride, v, lane);
+  load_row(x + (size_t)row * D, v, lane);
   const RowStats st = row_stats(v, D);
   load_row(gamma, gm, lane); load_row(beta, bt, lane);
   #pragma unroll
