@@ -13,17 +13,15 @@
 // The stages are SEQUENTIAL resamplings of intermediate size x size images; stages 2-5 are evaluated by exact tap composition
 // (rotate tap -> erase test -> perspective taps) on top of the resized crop, so every intermediate is the reference's intermediate.
 //
-// Default kernels (round 2):
+// Kernels:
 //   forward : k_resize (stage 1, separable, into a library scratch image) + k_compose (stages 2-5, three channels per thread; optionally
-//             also the encoder's bf16 patch operand, aph_sample_fwd_patches);
+//             also the encoder's bf16 patch operand, aph_sample_fwd_patches). Frames whose short side is too long for k_resize's
+//             per-warp crop rows (above ~6170 px at size 224) take k_sample_fwd instead: one CTA per (crop, channel), the channel's
+//             resized crop in 196 KB of shared memory;
 //   backward: k_bwd_warp_adjoint (perspective crops: rotation adjoint as a gather, perspective adjoint by global reductions into a
 //             scratch image) + k_bwd_bicubic3 (every crop: rotation adjoint gathered inline, bicubic adjoint through per-warp strips
 //             and 16-byte vector reductions into the canvas gradient).
-// The round-1 one-kernel forms (one CTA per (crop, channel), the crop's resized image / gradient image in 196 KB of shared memory:
-// k_sample_fwd, k_sample_bwd_cas, k_sample_bwd) and the atomic-free tile gather stay selectable (APH_SAMPLE_FWD_OLD, APH_SAMPLE_BWD_OLD,
-// APH_SAMPLE_BWD_FIXED, APH_SAMPLE_BWD_GATHER) and are what tests/test_gpu_parity.py::test_sampler_backward_variants_agree compares.
 #include "aph_common.cuh"
-#include <stdlib.h>
 #include <stdint.h>
 #include <type_traits>
 
@@ -194,6 +192,8 @@ __device__ __forceinline__ void fwd_compose(const float* __restrict__ A, const C
   }
 }
 
+// Forward in one kernel, the path for frames too large for k_resize (sample_fwd_impl): one CTA per (crop, channel), the canvas read
+// through the per-CTA tap tables, the channel's resized crop in shared memory.
 __global__ void __launch_bounds__(1024, 1)
 k_sample_fwd(const float* __restrict__ canvas, int H, int W, int pad_top, int pad_left, const float* __restrict__ table,
              int size, int kind, float* __restrict__ out) {
@@ -507,358 +507,9 @@ k_compose_kornia(const float* __restrict__ Ag, const float* __restrict__ table, 
   }
 }
 
-// Shared-memory accumulation cell. fp32 atomicAdd on shared memory is a compare-and-swap loop on this architecture
-// (SASS: ATOMS.CAST.SPIN, ~6 instructions and two dependent shared round trips per add; ncu: 31 % of the backward kernel's
-// instructions, 44 % of its stall samples). The opt-in FIXED form (k_sample_bwd, APH_SAMPLE_BWD_FIXED=1) accumulates round(v * scale) with the native integer ATOMS.ADD instead; the
-// scale is chosen per (crop, channel) from the block maximum so the sum cannot overflow, and the result is order-independent.
-template <bool FIXED>
-__device__ __forceinline__ void acc_add(float* __restrict__ cell, float v) {
-  if (FIXED) atomicAdd(reinterpret_cast<int*>(cell), __float2int_rn(v));
-  else atomicAdd(cell, v);
-}
-
-template <bool PERSP, bool FIXED, bool ERASE = true>
-__device__ __forceinline__ void scatterB(float* __restrict__ gA, const CropParams& p, int y, int x, int size, float g) {
-  if (ERASE && erased(p, y, x)) return;
-  if (PERSP) {
-    const Bilin b = persp_taps(p, y, x, size);
-    const float gm = g * (b.w00 + b.w01 + b.w10 + b.w11);
-    if (b.w00 != 0.f) acc_add<FIXED>(&gA[b.y0 * size + b.x0], gm * b.w00);
-    if (b.w01 != 0.f) acc_add<FIXED>(&gA[b.y0 * size + b.x0 + 1], gm * b.w01);
-    if (b.w10 != 0.f) acc_add<FIXED>(&gA[(b.y0 + 1) * size + b.x0], gm * b.w10);
-    if (b.w11 != 0.f) acc_add<FIXED>(&gA[(b.y0 + 1) * size + b.x0 + 1], gm * b.w11);
-  } else {
-    acc_add<FIXED>(&gA[y * size + x], g);
-  }
-}
-
-// adjoint of normalise -> rotate -> erase -> perspective: scatters grad_out of one (crop, channel) into the shared gradient
-// image. `gscale` = 1/std (fp32 cells) or fixed_scale/std (integer cells).
-template <bool PERSP, bool FIXED, bool ERASE = true>
-__device__ __forceinline__ void bwd_compose(float* __restrict__ gA, const float* __restrict__ go, const CropParams& p, int size,
-                                            int warp, int lane, int nwarps, float gscale) {
-  for (int i = warp; i < size; i += nwarps) {
-    float gnext = (lane < size) ? go[i * size + lane] : 0.f;
-    for (int j = lane; j < size; j += 32) {
-      const float graw = gnext;
-      if (j + 32 < size) gnext = go[i * size + j + 32];            // next chunk's load overlaps this chunk's scatter
-      const Bilin b = rot_taps(p, i, j, size);
-      const float g = graw * gscale * (b.w00 + b.w01 + b.w10 + b.w11);
-      if (g == 0.f) continue;
-      if (b.w00 != 0.f) scatterB<PERSP, FIXED, ERASE>(gA, p, b.y0, b.x0, size, g * b.w00);
-      if (b.w01 != 0.f) scatterB<PERSP, FIXED, ERASE>(gA, p, b.y0, b.x0 + 1, size, g * b.w01);
-      if (b.w10 != 0.f) scatterB<PERSP, FIXED, ERASE>(gA, p, b.y0 + 1, b.x0, size, g * b.w10);
-      if (b.w11 != 0.f) scatterB<PERSP, FIXED, ERASE>(gA, p, b.y0 + 1, b.x0 + 1, size, g * b.w11);
-    }
-  }
-}
-
-// block-wide maximum (all threads get it); `red` = 32 floats of shared scratch
-__device__ __forceinline__ float block_max(float v, float* red) {
-  v = warp_max(v);
-  __syncthreads();
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  float m = (threadIdx.x & 31) < (blockDim.x >> 5) ? red[threadIdx.x & 31] : 0.f;
-  return warp_max(m);
-}
-
-// bicubic adjoint of the shared gradient image gA into the canvas gradient. Per 32-pixel chunk of a gradient row the horizontal
-// taps are first accumulated into a per-warp strip (the lanes' 4-tap windows overlap), then the strip is scattered to the 4
-// source rows with COALESCED global red.add (4 x span instead of 16 x 32 scattered atomics per chunk).
-template <bool FIXED>
-__device__ __forceinline__ void bwd_bicubic(const float* __restrict__ gA, float* __restrict__ strip, const TapTables& tt, float* __restrict__ gc,
-                                            int size, int warp, int lane, int nwarps, bool can_strip, float sscale, float inv_sscale) {
-  for (int i = warp; i < size; i += nwarps) {
-    const int4 yo = *reinterpret_cast<const int4*>(tt.yo + 4 * i);
-    const float4 wy = *reinterpret_cast<const float4*>(tt.yw + 4 * i);
-    const int yoff[4] = {yo.x, yo.y, yo.z, yo.w};
-    const float wya[4] = {wy.x, wy.y, wy.z, wy.w};
-    for (int j0 = 0; j0 < size; j0 += 32) {
-      const int j = j0 + lane;
-      const float g = (j < size) ? gA[i * size + j] : 0.f;
-      const int jc = min(j, size - 1);
-      const int4 xo = *reinterpret_cast<const int4*>(tt.xo + 4 * jc);
-      const float4 wx = *reinterpret_cast<const float4*>(tt.xw + 4 * jc);
-      const int xfirst = tt.xo[4 * j0], xlast = tt.xo[4 * min(j0 + 31, size - 1) + 3];
-      const int span = xlast - xfirst + 1;
-      if (can_strip && span <= STRIP) {
-        if (g != 0.f) {
-          const float gs = FIXED ? g * sscale : g;
-          acc_add<FIXED>(&strip[xo.x - xfirst], gs * wx.x); acc_add<FIXED>(&strip[xo.y - xfirst], gs * wx.y);
-          acc_add<FIXED>(&strip[xo.z - xfirst], gs * wx.z); acc_add<FIXED>(&strip[xo.w - xfirst], gs * wx.w);
-        }
-        __syncwarp();
-        for (int x = lane; x < span; x += 32) {
-          const float raw = strip[x];                                // all-zero bits in either representation = nothing landed here
-          if (__float_as_int(raw) != 0) {
-            strip[x] = 0.f;
-            const float h = FIXED ? (float)__float_as_int(raw) * inv_sscale : raw;
-#pragma unroll
-            for (int a = 0; a < 4; ++a) atomicAdd(gc + yoff[a] + xfirst + x, wya[a] * h);
-          }
-        }
-        __syncwarp();
-      } else if (g != 0.f) {
-#pragma unroll
-        for (int a = 0; a < 4; ++a) {
-          float* r = gc + yoff[a];
-          const float gy = g * wya[a];
-          atomicAdd(r + xo.x, gy * wx.x); atomicAdd(r + xo.y, gy * wx.y); atomicAdd(r + xo.z, gy * wx.z); atomicAdd(r + xo.w, gy * wx.w);
-        }
-      }
-    }
-  }
-}
-
-__global__ void __launch_bounds__(1024, 1)
-k_sample_bwd(const float* __restrict__ grad_out, int H, int W, int pad_top, int pad_left, const float* __restrict__ table,
-             int size, int kind, float* __restrict__ grad_canvas) {
-  extern __shared__ float gA[];
-  __shared__ float red[32];
-  const int crop = blockIdx.x / 3, ch = blockIdx.x - crop * 3;
-  CropParams p = load_params(table + (size_t)crop * APH_CROP_PARAM_FLOATS);
-  prescale(p, size);
-  const int n = size * size;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  const float* go = grad_out + ((size_t)crop * 3 + ch) * n;
-  const float inv_sd = (kind != APH_TF_NONE) ? 1.f / c_std[ch] : 1.f;
-  const float scale = (size > 1) ? (float)(p.cs - 1) / (float)(size - 1) : 0.f;
-  const TapTables tt = build_taps(gA + ((n + 3) & ~3), p, size, H, W, pad_top, pad_left, scale);
-  float* strip = gA + ((n + 3) & ~3) + 16 * size + warp * STRIP;
-  for (int x = lane; x < STRIP; x += 32) strip[x] = 0.f;           // the strip is re-zeroed as it is drained
-  // block maximum of |grad_out| sizes the fixed-point scale (NaN / Inf -> INFINITY: fmaxf alone would drop a NaN); the same pass
-  // clears (or, without transforms, fills) gA
-  float amax = 0.f;
-  if (kind == APH_TF_FAST) {
-    for (int idx = threadIdx.x; idx < n; idx += blockDim.x) { const float a = fabsf(go[idx]); amax = (a <= 3e38f) ? fmaxf(amax, a) : INFINITY; gA[idx] = 0.f; }
-  } else {
-    for (int idx = threadIdx.x; idx < n; idx += blockDim.x) { const float v = go[idx] * inv_sd, a = fabsf(v); amax = (a <= 3e38f) ? fmaxf(amax, a) : INFINITY; gA[idx] = v; }
-  }
-  amax = block_max(amax, red);                                      // (contains the block barriers)
-  if (amax == 0.f) return;                                          // nothing to add (block-uniform)
-  float* gc = grad_canvas + (size_t)ch * H * W;
-  const bool can_strip = (pad_top == 0 && pad_left == 0);
-  if (!(amax < 1e30f)) {                                            // Inf / NaN upstream: poison this crop's footprint, as fp32 would
-    for (int idx = threadIdx.x; idx < n; idx += blockDim.x) gA[idx] = __int_as_float(0x7fc00000);
-    __syncthreads();
-    bwd_bicubic<true>(gA, strip, tt, gc, size, warp, lane, nwarps, false, 1.f, 1.f);
-    return;
-  }
-  float gmax = amax;                                                // bound on |gA| for the strip scale
-  if (kind == APH_TF_FAST) {
-    amax *= inv_sd;
-    const bool persp = (p.flags & APH_FLAG_PERSP) != 0;
-    // fan-in bound of one gradient cell: a rotation (area preserving) lands <= 8 weighted samples on a pixel, a perspective
-    // warp of distortion <= 0.5 compresses area by far less than the extra 32x allowed here
-    const float s1 = 2147483648.f / ((persp ? 512.f : 16.f) * amax);
-    if (persp) bwd_compose<true, true>(gA, go, p, size, warp, lane, nwarps, inv_sd * s1);
-    else bwd_compose<false, true>(gA, go, p, size, warp, lane, nwarps, inv_sd * s1);
-    __syncthreads();
-    const float inv_s1 = 1.f / s1;
-    float m = 0.f;
-    for (int idx = threadIdx.x; idx < n; idx += blockDim.x) {       // integer cells -> fp32 in place, and their maximum
-      const float v = (float)__float_as_int(gA[idx]) * inv_s1;
-      gA[idx] = v; m = fmaxf(m, fabsf(v));
-    }
-    gmax = block_max(m, red);
-    if (gmax == 0.f) return;
-  }
-  // a strip cell sums <= 4 / min(scale, 1) horizontal taps of |weight| <= 1.2: 64x headroom covers crops down to size / 12
-  const float s2 = 1073741824.f / (64.f * gmax);
-  bwd_bicubic<true>(gA, strip, tt, gc, size, warp, lane, nwarps, can_strip && scale >= 0.08f, s2, 1.f / s2);
-}
-
-// Default backward: fp32 shared accumulation (compare-and-swap loops in SASS).
-__global__ void __launch_bounds__(1024, 1)
-k_sample_bwd_cas(const float* __restrict__ grad_out, int H, int W, int pad_top, int pad_left, const float* __restrict__ table,
-             int size, int kind, float* __restrict__ grad_canvas, float gscale) {
-  extern __shared__ float gA[];
-  const int crop = blockIdx.x / 3, ch = blockIdx.x - crop * 3;
-  CropParams p = load_params(table + (size_t)crop * APH_CROP_PARAM_FLOATS);
-  prescale(p, size);
-  const int n = size * size;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  const float* go = grad_out + ((size_t)crop * 3 + ch) * n;
-  // gscale: weight of this rank's shard in the all-reduced gradient (S_local / S under torchrun, 1 otherwise), folded in here
-  const float inv_sd = ((kind != APH_TF_NONE) ? 1.f / c_std[ch] : 1.f) * gscale;
-  const float scale = (size > 1) ? (float)(p.cs - 1) / (float)(size - 1) : 0.f;
-  const TapTables tt = build_taps(gA + ((n + 3) & ~3), p, size, H, W, pad_top, pad_left, scale);
-  float* strip = gA + ((n + 3) & ~3) + 16 * size + warp * STRIP;
-  for (int x = lane; x < STRIP; x += 32) strip[x] = 0.f;           // the strip is re-zeroed as it is drained below
-  if (kind == APH_TF_FAST && !(p.flags & APH_FLAG_PERSP) && identity_rot(p)) {
-    // adjoint of the angle-0 fast path of the forward: erase mask + 1/std, no scatter
-    for (int idx = threadIdx.x; idx < n; idx += blockDim.x) {
-      const int y = idx / size, x = idx - y * size;
-      gA[idx] = erased(p, y, x) ? 0.f : go[idx] * inv_sd;
-    }
-  } else if (kind == APH_TF_FAST) {
-    for (int idx = threadIdx.x; idx < n; idx += blockDim.x) gA[idx] = 0.f;
-    __syncthreads();
-    const bool er = (p.flags & APH_FLAG_ERASE) != 0;
-    if (p.flags & APH_FLAG_PERSP) { if (er) bwd_compose<true, false, true>(gA, go, p, size, warp, lane, nwarps, inv_sd); else bwd_compose<true, false, false>(gA, go, p, size, warp, lane, nwarps, inv_sd); }
-    else if (er) bwd_compose<false, false, true>(gA, go, p, size, warp, lane, nwarps, inv_sd);
-    else bwd_compose<false, false, false>(gA, go, p, size, warp, lane, nwarps, inv_sd);
-  } else {
-    for (int idx = threadIdx.x; idx < n; idx += blockDim.x) gA[idx] = go[idx] * inv_sd;
-  }
-  __syncthreads();
-  // ---- bicubic adjoint. Per 32-pixel chunk of a gradient row the horizontal taps are first accumulated into a per-warp
-  // strip (shared atomics, the lanes' 4-tap windows overlap), then the strip is scattered to the 4 source rows with
-  // COALESCED global red.add (4 x span instead of 16 x 32 scattered atomics per chunk).
-  float* gc = grad_canvas + (size_t)ch * H * W;
-  const bool can_strip = (pad_top == 0 && pad_left == 0);
-  for (int i = warp; i < size; i += nwarps) {
-    const int4 yo = *reinterpret_cast<const int4*>(tt.yo + 4 * i);
-    const float4 wy = *reinterpret_cast<const float4*>(tt.yw + 4 * i);
-    const int yoff[4] = {yo.x, yo.y, yo.z, yo.w};
-    const float wya[4] = {wy.x, wy.y, wy.z, wy.w};
-    for (int j0 = 0; j0 < size; j0 += 32) {
-      const int j = j0 + lane;
-      const float g = (j < size) ? gA[i * size + j] : 0.f;
-      const int jc = min(j, size - 1);
-      const int4 xo = *reinterpret_cast<const int4*>(tt.xo + 4 * jc);
-      const float4 wx = *reinterpret_cast<const float4*>(tt.xw + 4 * jc);
-      const int xfirst = tt.xo[4 * j0], xlast = tt.xo[4 * min(j0 + 31, size - 1) + 3];
-      const int span = xlast - xfirst + 1;
-      if (can_strip && span <= STRIP) {
-        if (g != 0.f) {
-          atomicAdd(&strip[xo.x - xfirst], g * wx.x); atomicAdd(&strip[xo.y - xfirst], g * wx.y);
-          atomicAdd(&strip[xo.z - xfirst], g * wx.z); atomicAdd(&strip[xo.w - xfirst], g * wx.w);
-        }
-        __syncwarp();
-        for (int x = lane; x < span; x += 32) {
-          const float h = strip[x];
-          if (h != 0.f) {
-            strip[x] = 0.f;
-#pragma unroll
-            for (int a = 0; a < 4; ++a) atomicAdd(gc + yoff[a] + xfirst + x, wya[a] * h);
-          }
-        }
-        __syncwarp();
-      } else if (g != 0.f) {
-#pragma unroll
-        for (int a = 0; a < 4; ++a) {
-          float* r = gc + yoff[a];
-          const float gy = g * wya[a];
-          atomicAdd(r + xo.x, gy * wx.x); atomicAdd(r + xo.y, gy * wx.y); atomicAdd(r + xo.z, gy * wx.z); atomicAdd(r + xo.w, gy * wx.w);
-        }
-      }
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------
-// Atomic-free backward for un-wrapped frames (the script's default 'uniform' / 'central' aligns).
-//   stage 1 (k_sample_bwd_stage1, transforms_fast only): rotate / erase / perspective adjoints per (crop, channel) in shared
-//            memory, result gA [S,3,size,size] written to a library scratch buffer (L2-resident at these sizes);
-//   stage 2 (k_sample_bwd_gather): one CTA owns a 16x64 canvas tile of one channel and walks the crops that cover it.
-//            The bicubic adjoint is separable: per (tile, crop) the <= 5 contributing output rows / columns and their
-//            weights (clamped border taps merged) are listed once, T = Wy^T gA is formed for the touched column range in
-//            shared memory, then each pixel reduces Wx^T T. Every canvas pixel is written exactly once: deterministic,
-//            no 457 M global atomics.
-__global__ void __launch_bounds__(1024, 1)
-k_sample_bwd_stage1(const float* __restrict__ grad_out, const float* __restrict__ table, int size, float* __restrict__ gA_out) {
-  extern __shared__ float gA[];
-  const int crop = blockIdx.x / 3, ch = blockIdx.x - crop * 3;
-  CropParams p = load_params(table + (size_t)crop * APH_CROP_PARAM_FLOATS);
-  prescale(p, size);
-  const int n = size * size;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  const float* go = grad_out + ((size_t)crop * 3 + ch) * n;
-  for (int idx = threadIdx.x; idx < n; idx += blockDim.x) gA[idx] = 0.f;
-  __syncthreads();
-  const float inv_sd = 1.f / c_std[ch];
-  if (p.flags & APH_FLAG_PERSP) bwd_compose<true, false>(gA, go, p, size, warp, lane, nwarps, inv_sd);
-  else bwd_compose<false, false>(gA, go, p, size, warp, lane, nwarps, inv_sd);
-  __syncthreads();
-  float* o = gA_out + ((size_t)crop * 3 + ch) * n;
-  for (int idx = threadIdx.x; idx < n; idx += blockDim.x) o[idx] = gA[idx];
-}
-
-constexpr int GT_H = 16, GT_W = 64, GT_CAP = 8, GT_TW = 80;
-
-// lists the output indices whose (clamped) bicubic taps hit source index `rel`, with the summed weight
-__device__ __forceinline__ int adjoint_taps(int rel, float scale, int cs, int size, int* idx_out, float* w_out) {
-  int n = 0;
-  const int lo = max(0, (int)ceilf((float)(rel - 2) / scale) - 1);
-  const int hi = min(size - 1, (int)floorf((float)(rel + 2) / scale) + 1);
-  for (int i = lo; i <= hi; ++i) {
-    int idx[4]; float w[4];
-    cubic_taps(i, scale, cs, idx, w);
-    float ws = 0.f; bool hit = false;
-#pragma unroll
-    for (int a = 0; a < 4; ++a) if (idx[a] == rel) { ws += w[a]; hit = true; }
-    if (hit && n < GT_CAP) { idx_out[n] = i; w_out[n] = ws; ++n; }
-  }
-  return n;
-}
-
-__global__ void __launch_bounds__(256)
-k_sample_bwd_gather(const float* __restrict__ gsrc, float pre_scale_r, float pre_scale_g, float pre_scale_b, const float* __restrict__ table,
-                    int S, int size, int H, int W, float* __restrict__ grad_canvas) {
-  __shared__ int rowcnt[GT_H], rowi[GT_H][GT_CAP], colcnt[GT_W], colj[GT_W][GT_CAP];
-  __shared__ float roww[GT_H][GT_CAP], colw[GT_W][GT_CAP], Tt[GT_H][GT_TW];
-  const int tiles_x = (W + GT_W - 1) / GT_W;
-  const int ch = blockIdx.y, y0 = (blockIdx.x / tiles_x) * GT_H, x0 = (blockIdx.x % tiles_x) * GT_W;
-  const int t = threadIdx.x, tx = t & (GT_W - 1), tyg = t >> 6;          // thread owns column tx, rows tyg + 4 r
-  const float pre = ch == 0 ? pre_scale_r : (ch == 1 ? pre_scale_g : pre_scale_b);
-  const int n = size * size;
-  float acc[4] = {0.f, 0.f, 0.f, 0.f};
-  for (int crop = 0; crop < S; ++crop) {
-    const float* row = table + (size_t)crop * APH_CROP_PARAM_FLOATS;
-    const int oy = (int)row[APH_F_OFFY], ox = (int)row[APH_F_OFFX], cs = (int)row[APH_F_CSIZE];
-    if (oy >= y0 + GT_H || oy + cs <= y0 || ox >= x0 + GT_W || ox + cs <= x0) continue;      // CTA-uniform
-    const float scale = (size > 1) ? (float)(cs - 1) / (float)(size - 1) : 0.f;
-    __syncthreads();
-    if (t < GT_H) {
-      const int rel = y0 + t - oy;
-      rowcnt[t] = (rel >= 0 && rel < cs && y0 + t < H) ? adjoint_taps(rel, scale, cs, size, rowi[t], roww[t]) : 0;
-    } else if (t >= 64 && t < 64 + GT_W) {
-      const int c = t - 64, rel = x0 + c - ox;
-      colcnt[c] = (rel >= 0 && rel < cs && x0 + c < W) ? adjoint_taps(rel, scale, cs, size, colj[c], colw[c]) : 0;
-    }
-    const int rx_lo = max(0, x0 - ox), rx_hi = min(cs - 1, x0 + GT_W - 1 - ox);
-    const int jlo = max(0, (int)ceilf((float)(rx_lo - 2) / scale) - 1);
-    const int jhi = min(size - 1, (int)floorf((float)(rx_hi + 2) / scale) + 1);
-    const int nj = min(jhi - jlo + 1, GT_TW);
-    __syncthreads();
-    const float* g = gsrc + ((size_t)crop * 3 + ch) * n + jlo;
-    for (int e = t; e < GT_H * nj; e += 256) {
-      const int ty = e / nj, jj = e - ty * nj;
-      float v = 0.f;
-      const int cnt = rowcnt[ty];
-      for (int a = 0; a < cnt; ++a) v += roww[ty][a] * __ldg(g + rowi[ty][a] * size + jj);
-      Tt[ty][jj] = v;
-    }
-    __syncthreads();
-    const int ccnt = colcnt[tx];
-    if (ccnt > 0) {
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const int ty = tyg + 4 * r;
-        if (rowcnt[ty] > 0) {
-          float v = 0.f;
-          for (int b = 0; b < ccnt; ++b) v += colw[tx][b] * Tt[ty][colj[tx][b] - jlo];
-          acc[r] += v;
-        }
-      }
-    }
-  }
-  if (x0 + tx < W) {
-#pragma unroll
-    for (int r = 0; r < 4; ++r) {
-      const int y = y0 + tyg + 4 * r;
-      if (y < H) grad_canvas[((size_t)ch * H + y) * W + x0 + tx] = acc[r] * pre;
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------
-// Backward, two-kernel form (round 2, default). The one-kernel form above (k_sample_bwd_cas) holds the gradient image of ONE
-// channel in 196 KB of shared memory (one CTA per SM), re-derives the rotate / perspective geometry per channel and accumulates
-// with fp32 shared atomics (compare-and-swap loops): ~420 thread instructions per pixel and channel, issue bound. Here
-//   the adjoint of normalise -> rotate -> erase is a GATHER, 3 channels per thread: the rotate stage is a rigid rotation, so the
+// Backward in two kernels.
+//   The adjoint of normalise -> rotate -> erase is a GATHER, 3 channels per thread: the rotate stage is a rigid rotation, so the
 //   output pixels whose bilinear footprint covers source pixel (y, x) lie in the 3 x 3 block around R^T (y, x) (footprint
 //   half-extent |cos| + |sin| <= sqrt 2 < 1.5). No atomics, no shared image;
 //   k_bwd_warp_adjoint : perspective crops only (20 % of the draws): that gather, then the adjoint of the perspective resampling as
@@ -1042,10 +693,12 @@ __device__ __forceinline__ void red_add_v4(float* addr, float a, float b, float 
 }
 
 // VEC: canvas rows are 16-byte aligned (W % 4 == 0, aligned base, no wrap): strips are anchored at a multiple of 4 canvas columns
-// FIXED: the strips accumulate round(v * 2^k) with the native integer shared atomic instead of the fp32 compare-and-swap loop; k is
-// chosen per 32-pixel chunk from the warp maximum of |g| so that the 24 leading bits of the largest term survive and the sum of the
-// <= 32 x 4 terms of a cell cannot overflow (cells sum <= 48 |g|max: taps have |w| <= 1.2, a clamped border pixel lands <= 1.5).
-template <bool VEC, bool FIXED>
+// The strips accumulate in integer fixed point, round(v * 2^k), with the native integer shared atomic add: fp32 atomicAdd on shared
+// memory is a compare-and-swap loop on this architecture (SASS: ATOMS.CAST.SPIN, ~6 instructions and two dependent shared round trips
+// per add). k is chosen per 32-pixel chunk from the warp maximum of |g| so that the 24 leading bits of the largest term survive and the
+// sum of the <= 32 x 4 terms of a cell cannot overflow (cells sum <= 48 |g|max: taps have |w| <= 1.2, a clamped border pixel lands
+// <= 1.5). The scale follows the chunk's largest term, not an absolute bound, so small gradients keep their relative precision.
+template <bool VEC>
 __global__ void __launch_bounds__(256, 4)
 k_bwd_bicubic3(const float* __restrict__ grad_out, float* __restrict__ gA_all, int H, int W, int pad_top, int pad_left,
                const float* __restrict__ table, int size, int kind, float gscale, float* __restrict__ grad_canvas) {
@@ -1119,7 +772,7 @@ k_bwd_bicubic3(const float* __restrict__ grad_out, float* __restrict__ gA_all, i
       const int span = xlast - xbase + 1;
       float fs_up = 1.f, fs_dn = 1.f;
       bool strip_ok = can_strip && span <= STRIP;
-      if (FIXED && strip_ok) {
+      if (strip_ok) {
         const unsigned mbits = __reduce_max_sync(0xffffffffu, __float_as_uint(fmaxf(fmaxf(fabsf(g[0]), fabsf(g[1])), fabsf(g[2]))));
         if (mbits == 0u) continue;                                 // nothing in this chunk (warp-uniform)
         const int E = min(max((int)(mbits >> 23), 25), 254);       // |g| < 2^(E - 126)
@@ -1131,15 +784,10 @@ k_bwd_bicubic3(const float* __restrict__ grad_out, float* __restrict__ gA_all, i
 #pragma unroll
         for (int c = 0; c < 3; ++c) {
           if (g[c] != 0.f) {
-            if (FIXED) {
-              int* s = reinterpret_cast<int*>(strip) + c * STRIP - xbase;
-              const float gs = g[c] * fs_up;
-              atomicAdd(s + xo.x, __float2int_rn(gs * wx.x)); atomicAdd(s + xo.y, __float2int_rn(gs * wx.y));
-              atomicAdd(s + xo.z, __float2int_rn(gs * wx.z)); atomicAdd(s + xo.w, __float2int_rn(gs * wx.w));
-            } else {
-              float* s = strip + c * STRIP - xbase;
-              atomicAdd(s + xo.x, g[c] * wx.x); atomicAdd(s + xo.y, g[c] * wx.y); atomicAdd(s + xo.z, g[c] * wx.z); atomicAdd(s + xo.w, g[c] * wx.w);
-            }
+            int* s = reinterpret_cast<int*>(strip) + c * STRIP - xbase;
+            const float gs = g[c] * fs_up;
+            atomicAdd(s + xo.x, __float2int_rn(gs * wx.x)); atomicAdd(s + xo.y, __float2int_rn(gs * wx.y));
+            atomicAdd(s + xo.z, __float2int_rn(gs * wx.z)); atomicAdd(s + xo.w, __float2int_rn(gs * wx.w));
           }
         }
         __syncwarp();
@@ -1148,10 +796,10 @@ k_bwd_bicubic3(const float* __restrict__ grad_out, float* __restrict__ gA_all, i
 #pragma unroll
             for (int c = 0; c < 3; ++c) {
               float4* sp4 = reinterpret_cast<float4*>(strip + c * STRIP) + lane;
-              float4 h = *sp4;                                     // (all-zero bits = nothing landed here, in either representation)
+              float4 h = *sp4;                                     // (all-zero bits = nothing landed here)
               if (__float_as_uint(h.x) | __float_as_uint(h.y) | __float_as_uint(h.z) | __float_as_uint(h.w)) {
                 *sp4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (FIXED) { h.x = (float)__float_as_int(h.x) * fs_dn; h.y = (float)__float_as_int(h.y) * fs_dn; h.z = (float)__float_as_int(h.z) * fs_dn; h.w = (float)__float_as_int(h.w) * fs_dn; }
+                h.x = (float)__float_as_int(h.x) * fs_dn; h.y = (float)__float_as_int(h.y) * fs_dn; h.z = (float)__float_as_int(h.z) * fs_dn; h.w = (float)__float_as_int(h.w) * fs_dn;
                 float* gc = grad_canvas + c * plane + xbase + 4 * lane;
 #pragma unroll
                 for (int a = 0; a < 4; ++a) red_add_v4(gc + yoff[a], wya[a] * h.x, wya[a] * h.y, wya[a] * h.z, wya[a] * h.w);
@@ -1165,7 +813,7 @@ k_bwd_bicubic3(const float* __restrict__ grad_out, float* __restrict__ gA_all, i
               float h = strip[c * STRIP + x];
               if (__float_as_uint(h) != 0u) {
                 strip[c * STRIP + x] = 0.f;
-                if (FIXED) h = (float)__float_as_int(h) * fs_dn;
+                h = (float)__float_as_int(h) * fs_dn;
                 float* gc = grad_canvas + c * plane + xbase + x;
 #pragma unroll
                 for (int a = 0; a < 4; ++a) atomicAdd(gc + yoff[a], wya[a] * h);
@@ -1194,9 +842,14 @@ k_bwd_bicubic3(const float* __restrict__ grad_out, float* __restrict__ gA_all, i
 
 using namespace aph;
 
+// Largest output side of the sampler. k_sample_fwd, the only forward for frames too large for k_resize, holds one channel's resized
+// crop and its tap tables in one CTA's shared memory: 210 KB of the 227 KB at this size.
+constexpr int kMaxSampleSize = 224;
+static_assert(((size_t)kMaxSampleSize * kMaxSampleSize + 4 + 16 * kMaxSampleSize) * sizeof(float) <= 227 * 1024, "k_sample_fwd at the largest size");
+
 static int check_sample_args(const char* who, int H, int W, int S, int size, int kind) {
   APH_REQUIRE(H > 0 && W > 0 && S >= 0 && size > 0, "%s: bad shape H=%d W=%d S=%d size=%d", who, H, W, S, size);
-  APH_REQUIRE(((size_t)size * size + 4 + 16 * (size_t)size + 32 * STRIP) * sizeof(float) <= 227 * 1024, "%s: size=%d does not fit one CTA's shared memory (max 224)", who, size);
+  APH_REQUIRE(size <= kMaxSampleSize, "%s: size=%d does not fit one CTA's shared memory (max %d)", who, size, kMaxSampleSize);
   APH_REQUIRE(kind >= APH_TF_NONE && kind <= APH_TF_ELASTIC, "%s: unknown transform kind %d", who, kind);
   return 0;
 }
@@ -1228,67 +881,55 @@ static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int p
   if (int e = check_sample_args("aph_sample_fwd", H, W, S, size, kind)) return e;
   if (S == 0) return 0;
   APH_REQUIRE(canvas && table && out, "aph_sample_fwd: null pointer");
-  {
-    // default: the two-kernel form (k_resize + k_compose); APH_SAMPLE_FWD_OLD=1 keeps the one-kernel form (also used when the crop
-    // strips would not fit: canvases beyond ~6000 px on the short side)
-    static int old_path = -1;
-    if (old_path < 0) { const char* e = getenv("APH_SAMPLE_FWD_OLD"); old_path = (e && e[0] == '1') ? 1 : 0; }
-    const int cap = ((H + 2 * pad_top < W + 2 * pad_left ? H + 2 * pad_top : W + 2 * pad_left) + 1 + 3) & ~3;     // crops never exceed the short side of the frame
-    const size_t smem2 = ((size_t)8 * size + (size_t)8 * cap) * sizeof(float);
-    // the kornia kinds exist in this form only (APH_SAMPLE_FWD_OLD does not apply to them)
-    const bool kornia = kind >= APH_TF_CUSTOM;
-    APH_REQUIRE(!kornia || smem2 <= 200 * 1024, "aph_sample_fwd: a %dx%d frame is too large for transform kind %d", H + 2 * pad_top, W + 2 * pad_left, kind);
-    if ((!old_path || kornia) && smem2 <= 200 * 1024) {
-      cudaStream_t st = (cudaStream_t)stream;
-      float* dst = out;
-      if (kind >= APH_TF_FAST) {
-        if (int e = g_A.grow((size_t)S * 3 * size * size * sizeof(float), st)) return e;
-        dst = g_A.p;
-      }
-      static size_t conf = 0;
-      if (smem2 > conf) {
-        APH_CUDA_OK(cudaFuncSetAttribute(k_resize<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-        APH_CUDA_OK(cudaFuncSetAttribute(k_resize<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-        conf = smem2;
-      }
-      const int rows_per_cta = 32;
-      const dim3 g1(S * 3, (size + rows_per_cta - 1) / rows_per_cta);
-      if (pad_top || pad_left) k_resize<true><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
-      else k_resize<false><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
-      APH_LAUNCH_OK();
-      if (kind == APH_TF_FAST) {
-        const int tiles = ((size + 15) / 16) * ((size + 15) / 16);
-        k_compose<<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
-        APH_LAUNCH_OK();
-      } else if (kornia) {
-        const int s = size + 2 * KPAD, tiles = ((s + 15) / 16) * ((s + 15) / 16);
-        if (kind == APH_TF_ELASTIC) k_compose_kornia<true><<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
-        else k_compose_kornia<false><<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
-        APH_LAUNCH_OK();
-      }
-      if (patches_written) *patches_written = 1;
-      return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int cap = ((H + 2 * pad_top < W + 2 * pad_left ? H + 2 * pad_top : W + 2 * pad_left) + 1 + 3) & ~3;     // crops never exceed the short side of the frame
+  const size_t smem2 = ((size_t)8 * size + (size_t)8 * cap) * sizeof(float);
+  const bool kornia = kind >= APH_TF_CUSTOM;
+  APH_REQUIRE(!kornia || smem2 <= 200 * 1024, "aph_sample_fwd: a %dx%d frame is too large for transform kind %d", H + 2 * pad_top, W + 2 * pad_left, kind);
+  if (smem2 > 200 * 1024) {
+    // k_resize holds one crop row per warp in shared memory, sized by the frame's short side; above ~6170 px (at size 224) that does not
+    // fit, and the one-kernel form, which reads the canvas through its tap tables, is the forward there (it writes no patch operand)
+    const size_t smem = ((size_t)size * size + 4 + 16 * (size_t)size) * sizeof(float);
+    static size_t configured = 0;
+    if (smem > configured) {
+      APH_CUDA_OK(cudaFuncSetAttribute(k_sample_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      configured = smem;
     }
+    k_sample_fwd<<<S * 3, 1024, smem, st>>>(canvas, H, W, pad_top, pad_left, table, size, kind, out);
+    APH_LAUNCH_OK();
+    return 0;
   }
-  const size_t smem = ((size_t)size * size + 4 + 16 * (size_t)size) * sizeof(float);   // no strips in the forward: the rest stays L1
-  static size_t configured = 0;
-  if (smem > configured) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_sample_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
+  float* dst = out;
+  if (kind >= APH_TF_FAST) {
+    if (int e = g_A.grow((size_t)S * 3 * size * size * sizeof(float), st)) return e;
+    dst = g_A.p;
   }
-  k_sample_fwd<<<S * 3, 1024, smem, (cudaStream_t)stream>>>(canvas, H, W, pad_top, pad_left, table, size, kind, out);
+  static size_t conf = 0;
+  if (smem2 > conf) {
+    APH_CUDA_OK(cudaFuncSetAttribute(k_resize<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+    APH_CUDA_OK(cudaFuncSetAttribute(k_resize<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+    conf = smem2;
+  }
+  const int rows_per_cta = 32;
+  const dim3 g1(S * 3, (size + rows_per_cta - 1) / rows_per_cta);
+  if (pad_top || pad_left) k_resize<true><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
+  else k_resize<false><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
   APH_LAUNCH_OK();
+  if (kind == APH_TF_FAST) {
+    const int tiles = ((size + 15) / 16) * ((size + 15) / 16);
+    k_compose<<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
+    APH_LAUNCH_OK();
+  } else if (kornia) {
+    const int s = size + 2 * KPAD, tiles = ((s + 15) / 16) * ((s + 15) / 16);
+    if (kind == APH_TF_ELASTIC) k_compose_kornia<true><<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
+    else k_compose_kornia<false><<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
+    APH_LAUNCH_OK();
+  }
+  if (patches_written) *patches_written = 1;
   return 0;
 }
 
-namespace aph {
-__global__ void __launch_bounds__(256) k_scale_inplace(float* __restrict__ p, size_t n, float a) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) p[i] *= a;
-}
-}  // namespace aph
-
 static Scratch g_gW;                   // warp-stage adjoint scratch [S,3,size,size] of the default backward (all-zero between calls)
-static Scratch g_gA;                   // stage-1 scratch [S,3,size,size]
 static Scratch g_gR;                   // kornia kinds: d loss / d rotated image [S,3,size+8,size+8], rewritten by every backward
 
 static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int pad_left, const float* table, int S,
@@ -1308,80 +949,28 @@ static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int
                            int size, int kind, float* grad_canvas, float gscale, void* stream) {
   if (int e = check_sample_args("aph_sample_bwd", H, W, S, size, kind)) return e;
   APH_REQUIRE(grad_canvas, "aph_sample_bwd: null grad_canvas");
-  // The atomic scatter is faster than this gather (per-(tile, crop) list building + 3 barriers dominate the gather),
-  // so the gather is opt-in: APH_SAMPLE_BWD_GATHER=1 gives a bit-reproducible gradient.
-  static int force_scatter = -1;
-  if (force_scatter < 0) { const char* e = getenv("APH_SAMPLE_BWD_GATHER"); force_scatter = (e && e[0] == '1') ? 0 : 1; }
-  // (crops never upsample by more than 1/0.9 when min(H, W) >= size, which bounds the adjoint tap lists of the gather kernel)
-  // The kornia kinds run the default kernels only: APH_SAMPLE_BWD_GATHER / _OLD / _FIXED do not apply to them.
-  const bool kornia = kind >= APH_TF_CUSTOM;
-  if (S > 0 && pad_top == 0 && pad_left == 0 && !force_scatter && !kornia && (H < W ? H : W) >= size) {
-    // ---- atomic-free path: (stage 1) + tile gather
-    APH_REQUIRE(grad_out && table, "aph_sample_bwd: null pointer");
-    cudaStream_t st = (cudaStream_t)stream;
-    const float* gsrc = grad_out;
-    float pre[3] = {1.f, 1.f, 1.f};
-    if (kind == APH_TF_FAST) {
-      if (int e = g_gA.grow((size_t)S * 3 * size * size * sizeof(float), st)) return e;
-      const size_t smem1 = (size_t)size * size * sizeof(float);
-      static size_t configured1 = 0;
-      if (smem1 > configured1) {
-        APH_CUDA_OK(cudaFuncSetAttribute(k_sample_bwd_stage1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem1));
-        configured1 = smem1;
-      }
-      k_sample_bwd_stage1<<<S * 3, 1024, smem1, st>>>(grad_out, table, size, g_gA.p);
-      APH_LAUNCH_OK();
-      gsrc = g_gA.p;
-    } else if (kind == APH_TF_NORMALIZE) {
-      const float sd[3] = {0.26862954f, 0.26130258f, 0.27577711f};
-      for (int c = 0; c < 3; ++c) pre[c] = 1.f / sd[c];
-    }
-    dim3 grid(((W + GT_W - 1) / GT_W) * ((H + GT_H - 1) / GT_H), 3);
-    k_sample_bwd_gather<<<grid, 256, 0, st>>>(gsrc, pre[0] * gscale, pre[1] * gscale, pre[2] * gscale, table, S, size, H, W, grad_canvas);
-    APH_LAUNCH_OK();
-    return 0;
-  }
-  APH_CUDA_OK(cudaMemsetAsync(grad_canvas, 0, (size_t)3 * H * W * sizeof(float), (cudaStream_t)stream));
+  cudaStream_t st = (cudaStream_t)stream;
+  APH_CUDA_OK(cudaMemsetAsync(grad_canvas, 0, (size_t)3 * H * W * sizeof(float), st));
   if (S == 0) return 0;
   APH_REQUIRE(grad_out && table, "aph_sample_bwd: null pointer");
-  // default: the two-kernel form (k_bwd_warp_adjoint + k_bwd_bicubic3); APH_SAMPLE_BWD_OLD=1 keeps the one-kernel form
-  static int old_bwd = -1;
-  if (old_bwd < 0) { const char* e = getenv("APH_SAMPLE_BWD_OLD"); const char* f = getenv("APH_SAMPLE_BWD_FIXED"); old_bwd = ((e && e[0] == '1') || (f && f[0] == '1')) ? 1 : 0; }
-  if (!old_bwd || kornia) {
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t smem3 = ((size_t)8 * size + 8 * 3 * STRIP) * sizeof(float);
-    static size_t configured3 = 48 * 1024;
-    if (smem3 > configured3) {
-      APH_CUDA_OK((cudaFuncSetAttribute(k_bwd_bicubic3<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3)));
-      APH_CUDA_OK((cudaFuncSetAttribute(k_bwd_bicubic3<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3)));
-      APH_CUDA_OK((cudaFuncSetAttribute(k_bwd_bicubic3<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3)));
-      APH_CUDA_OK((cudaFuncSetAttribute(k_bwd_bicubic3<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3)));
-      configured3 = smem3;
-    }
-    const bool vec = pad_top == 0 && pad_left == 0 && W % 4 == 0 && ((uintptr_t)grad_canvas & 15) == 0;
-    const dim3 g3((size + BB_ROWS - 1) / BB_ROWS, S);
-    // strips in integer fixed point (native shared atomic add) by default; APH_SAMPLE_STRIP_FP32=1: fp32 strips (compare-and-swap loops)
-    static int fp32_strips = -1;
-    if (fp32_strips < 0) { const char* e = getenv("APH_SAMPLE_STRIP_FP32"); fp32_strips = (e && e[0] == '1') ? 1 : 0; }
-    const float* bb_src = grad_out;
-    if (kornia) {
-      // adjoints of normalise, jitter and the elastic stretch into gR (fully overwritten), then the rest in k_bwd_bicubic3 (mode 4)
-      const int s = size + 2 * KPAD;
-      if (int e = g_gR.grow((size_t)S * 3 * s * s * sizeof(float), st)) return e;
-      const dim3 gk((s * s + 1023) / 1024, S);
-      if (kind == APH_TF_ELASTIC) k_bwd_kornia_stage<true><<<gk, 256, 0, st>>>(grad_out, table, size, gscale, g_gR.p);
-      else k_bwd_kornia_stage<false><<<gk, 256, 0, st>>>(grad_out, table, size, gscale, g_gR.p);
-      APH_LAUNCH_OK();
-      bb_src = g_gR.p;
-    }
-#define APH_BB(V, F, STREAM) k_bwd_bicubic3<V, F><<<g3, 256, smem3, STREAM>>>(bb_src, g_gW.p, H, W, pad_top, pad_left, table, size, kind, gscale, grad_canvas)
-#define APH_BB_ANY(STREAM)                                                                           \
-    do {                                                                                             \
-      if (vec) { if (fp32_strips) APH_BB(true, false, STREAM); else APH_BB(true, true, STREAM); }    \
-      else { if (fp32_strips) APH_BB(false, false, STREAM); else APH_BB(false, true, STREAM); }      \
-      APH_LAUNCH_OK();                                                                               \
-    } while (0)
-    if (kind != APH_TF_FAST) { APH_BB_ANY(st); return 0; }
+  const size_t smem3 = ((size_t)8 * size + 8 * 3 * STRIP) * sizeof(float);
+  static size_t configured3 = 48 * 1024;
+  if (smem3 > configured3) {
+    APH_CUDA_OK(cudaFuncSetAttribute(k_bwd_bicubic3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
+    APH_CUDA_OK(cudaFuncSetAttribute(k_bwd_bicubic3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
+    configured3 = smem3;
+  }
+  const float* bb_src = grad_out;
+  if (kind >= APH_TF_CUSTOM) {
+    // adjoints of normalise, jitter and the elastic stretch into gR (fully overwritten), then the rest in k_bwd_bicubic3 (mode 4)
+    const int s = size + 2 * KPAD;
+    if (int e = g_gR.grow((size_t)S * 3 * s * s * sizeof(float), st)) return e;
+    const dim3 gk((s * s + 1023) / 1024, S);
+    if (kind == APH_TF_ELASTIC) k_bwd_kornia_stage<true><<<gk, 256, 0, st>>>(grad_out, table, size, gscale, g_gR.p);
+    else k_bwd_kornia_stage<false><<<gk, 256, 0, st>>>(grad_out, table, size, gscale, g_gR.p);
+    APH_LAUNCH_OK();
+    bb_src = g_gR.p;
+  } else if (kind == APH_TF_FAST) {
     const size_t need = (size_t)S * 3 * size * size * sizeof(float);
     if (need > g_gW.bytes) {
       if (int e = g_gW.grow(need, st)) return e;
@@ -1391,30 +980,11 @@ static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int
     // (running this chain on a side stream beside the other crops' bicubic adjoint was measured: no gain, 0.335 vs 0.333 ms -- removed)
     k_bwd_warp_adjoint<<<g1, 256, 0, st>>>(grad_out, table, size, gscale, g_gW.p);
     APH_LAUNCH_OK();
-    APH_BB_ANY(st);
-#undef APH_BB_ANY
-#undef APH_BB
-    APH_LAUNCH_OK();
-    return 0;
   }
-  const size_t smem = ((size_t)size * size + 4 + 16 * (size_t)size + 32 * STRIP) * sizeof(float);
-  static size_t configured = 0;
-  if (smem > configured) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_sample_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_sample_bwd_cas, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured = smem;
-  }
-  // APH_SAMPLE_BWD_FIXED=1: integer fixed-point shared accumulation (order-independent shared stage). Measured equal to the
-  // fp32 compare-and-swap kernel (0.581 vs 0.578 ms at C2, profiles/README.md), so the plain fp32 kernel stays the default.
-  static int fixed = -1;
-  if (fixed < 0) { const char* e = getenv("APH_SAMPLE_BWD_FIXED"); fixed = (e && e[0] == '1') ? 1 : 0; }
-  if (fixed) {
-    k_sample_bwd<<<S * 3, 1024, smem, (cudaStream_t)stream>>>(grad_out, H, W, pad_top, pad_left, table, size, kind, grad_canvas);
-    APH_LAUNCH_OK();
-    if (gscale != 1.f) { k_scale_inplace<<<num_sms() * 4, 256, 0, (cudaStream_t)stream>>>(grad_canvas, (size_t)3 * H * W, gscale); APH_LAUNCH_OK(); }
-    return 0;
-  }
-  k_sample_bwd_cas<<<S * 3, 1024, smem, (cudaStream_t)stream>>>(grad_out, H, W, pad_top, pad_left, table, size, kind, grad_canvas, gscale);
+  const bool vec = pad_top == 0 && pad_left == 0 && W % 4 == 0 && ((uintptr_t)grad_canvas & 15) == 0;
+  const dim3 g3((size + BB_ROWS - 1) / BB_ROWS, S);
+  if (vec) k_bwd_bicubic3<true><<<g3, 256, smem3, st>>>(bb_src, g_gW.p, H, W, pad_top, pad_left, table, size, kind, gscale, grad_canvas);
+  else k_bwd_bicubic3<false><<<g3, 256, smem3, st>>>(bb_src, g_gW.p, H, W, pad_top, pad_left, table, size, kind, gscale, grad_canvas);
   APH_LAUNCH_OK();
   return 0;
 }

@@ -122,36 +122,6 @@ def test_sampler_vs_reference_golden(L, golden, name):
     assert _rel(canvas.grad[:, :, ::st, ::st], golden['smp_%s_gcanvas' % name]) < 1e-4
 
 
-def test_sampler_backward_variants_agree(L):
-    """Backward variants (each in its own process): default = three-kernel form (rotation adjoint as a gather, 3 channels per thread);
-    APH_SAMPLE_BWD_OLD=1 = one-kernel form, fp32 compare-and-swap shared accumulation; APH_SAMPLE_BWD_FIXED=1 = one-kernel form, integer
-    fixed-point shared accumulation; APH_SAMPLE_BWD_GATHER=1 = atomic-free tile gather. All must agree to fp32 round-off, also
-    for gradients 1e-6 in magnitude (the fixed-point scale is per crop, not absolute)."""
-    import os, subprocess, sys
-    code = """
-import torch, numpy as np, sys
-sys.path.insert(0, %r)
-from aphantasia_b200 import transforms
-from aphantasia_b200.utils import slice_imgs
-torch.manual_seed(11); np.random.seed(11)
-c = torch.rand(1, 3, 360, 640).cuda().requires_grad_(True)
-torch.manual_seed(5); np.random.seed(5)
-out = slice_imgs([c], 24, 224, transforms.transforms_fast, 'uniform', 0.4)[0]
-torch.manual_seed(6)
-(out * (torch.randn(out.shape) * float(sys.argv[2])).cuda()).sum().backward()
-torch.save(c.grad.cpu(), sys.argv[1])
-""" % os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    for mag in ('1.0', '1e-6'):
-        outs = []
-        for k, env_add in enumerate((dict(APH_SAMPLE_BWD_FIXED='1'), dict(), dict(APH_SAMPLE_BWD_GATHER='1'), dict(APH_SAMPLE_BWD_OLD='1'))):
-            path = '/tmp/aph_bwd_variant_%d.pt' % k
-            subprocess.check_call([sys.executable, '-c', code, path, mag], env=dict(os.environ, **env_add))
-            outs.append(torch.load(path))
-        # the one-kernel variants share the forward's tap arithmetic; the default evaluates the rotation adjoint's weights from the
-        # inverse map (|sample - pixel| hat function): same values to a few ulp of the 224-pixel coordinate
-        assert _rel(outs[0], outs[3]) < 1e-5 and _rel(outs[2], outs[3]) < 1e-5 and _rel(outs[1], outs[3]) < 3e-5
-
-
 def test_sampler_abi_non_rotation_matrix(L):
     """The C ABI takes any 2x2 inverse affine matrix per crop; the reference's sampler only draws rotations. Rows with a sheared /
     scaled matrix (with and without a perspective hit) must take the general scatter adjoint, rows with a rotation the gather:
@@ -196,8 +166,11 @@ def test_sampler_abi_non_rotation_matrix(L):
     assert _rel(g3, co2.grad) < 1e-4
 
 
-@pytest.mark.parametrize('kind', [0, 1, 2])
-def test_sampler_vs_oracle_720p(L, kind):
+@pytest.mark.parametrize('kind,cot_scale', [(0, 1.), (1, 1.), (2, 1.), (0, 1e-6), (1, 1e-6), (2, 1e-6)],
+                         ids=['0', '1', '2', '0-cot1e-6', '1-cot1e-6', '2-cot1e-6'])
+def test_sampler_vs_oracle_720p(L, kind, cot_scale):
+    """cot_scale 1e-6: the backward's fixed-point strips take their scale from each 32-pixel chunk, not from an absolute bound, so a
+    gradient 1e-6 in magnitude meets the same relative bar."""
     from aphantasia_b200 import _rng, transforms
     from aphantasia_b200.utils import slice_imgs
     tf = [None, transforms.normalize(), transforms.transforms_fast][kind]
@@ -212,11 +185,54 @@ def test_sampler_vs_oracle_720p(L, kind):
     co = canvas.clone().requires_grad_(True)
     ref = R.sample_crops(co, tabs[0], 224, kind)
     _seed(6)
-    cot = torch.randn(ref.shape)
+    cot = torch.randn(ref.shape) * cot_scale
     (out * cot.cuda()).sum().backward()
     (ref * cot).sum().backward()
     assert _rel(out, ref) < 1e-5
     assert _rel(cc.grad, co.grad) < 1e-4
+
+
+@pytest.mark.parametrize('kind', [0, 1, 2])
+def test_sampler_large_frame_vs_oracle(L, kind):
+    """A frame whose short side is too long for k_resize's per-warp crop rows (above ~6170 px at size 224) takes the one-kernel
+    forward, which writes no patch operand. A small canvas wrap-padded by a wide overscan makes such a frame cheaply on the device;
+    one crop is nearly as large as the frame. Forward and backward vs the oracle."""
+    from aphantasia_b200 import _rng
+    from aphantasia_b200._lib import check, lib, stream_ptr
+    H, W, size, pad_top, pad_left = 300, 420, 224, 3000, 2950
+    fh, fw = H + 2 * pad_top, W + 2 * pad_left
+    assert 8 * (size + ((min(fh, fw) + 4) & ~3)) * 4 > 200 * 1024        # k_resize's shared memory at this frame: over its limit
+    _seed(13)
+    tab = np.zeros((4, _rng.CROP_PARAM_FLOATS), np.float32)
+    for row, (oy, ox, cs) in zip(tab, [(40, 70, 6200), (3000, 2950, 300), (5100, 400, 1100), (10, 6000, 260)]):
+        row[_rng.F_OFFY], row[_rng.F_OFFX], row[_rng.F_CSIZE] = oy, ox, cs
+        row[_rng.F_ROT:_rng.F_ROT + 4] = (1., 0., 0., 1.)
+        if kind == 2:
+            row[_rng.F_FLAGS] = _rng.draw_fast(row, size)
+    if kind == 2:
+        assert int(tab[0, _rng.F_FLAGS]) & 1 and tab[0, _rng.F_ANGLE] != 0, 'the largest crop should have a perspective hit and a rotation'
+    S = len(tab)
+    canvas = torch.rand(1, 3, H, W)
+    co = canvas.clone().requires_grad_(True)
+    ref = R.sample_crops(co, tab, size, kind, frame=(pad_top, pad_left, fh, fw))
+    _seed(6)
+    cot = torch.randn(ref.shape)
+    (ref * cot).sum().backward()
+    x = canvas.cuda().contiguous(); t = torch.tensor(tab).cuda(); cg = cot.cuda().contiguous()
+    out = torch.empty(S, 3, size, size, device='cuda'); g = torch.empty(1, 3, H, W, device='cuda')
+    patches = torch.empty(S * 7 * 7, 3 * 32 * 32, dtype=torch.bfloat16, device='cuda')
+    wrote = C.c_int(-1)
+    check(lib().aph_sample_fwd_patches(x.data_ptr(), H, W, pad_top, pad_left, t.data_ptr(), S, size, kind, out.data_ptr(), patches.data_ptr(),
+                                       32, C.byref(wrote), stream_ptr()), 'fwd')
+    check(lib().aph_sample_bwd(cg.data_ptr(), H, W, pad_top, pad_left, t.data_ptr(), S, size, kind, g.data_ptr(), stream_ptr()), 'bwd')
+    torch.cuda.synchronize()
+    assert wrote.value == 0
+    assert _rel(out, ref) < 1e-5
+    assert _rel(g, co.grad) < 1e-4
+    out_k = torch.empty(S, 3, size + 8, size + 8, device='cuda')
+    for k in (3, 4):                                                    # the kornia kinds have no one-kernel form: they refuse the frame
+        assert lib().aph_sample_fwd(x.data_ptr(), H, W, pad_top, pad_left, t.data_ptr(), S, size, k, out_k.data_ptr(), stream_ptr()) != 0
+        assert b'too large' in lib().aph_last_error()
 
 
 # ---------------------------------------------------------------------------------------------- loss / adam

@@ -121,29 +121,6 @@ def test_gscale_scales_the_gradient_only_and_scratch_stays_clean(kind):
     assert _rel(bwd(y), g1) < 1e-6
 
 
-def test_legacy_sampler_switches_do_not_change_the_new_kinds():
-    """APH_SAMPLE_*_OLD / _FIXED / _GATHER select retired forms for the other kinds; the new kinds must give the same result."""
-    code = r'''
-import sys, torch, numpy as np
-sys.path.insert(0, "%s"); sys.path.insert(0, "%s")
-from test_transforms_kornia_gpu import _abi
-res = []
-for kind in (3, 4):
-    fwd, bwd, (S, side, H, W) = _abi(kind)
-    x = torch.rand(1, 3, H, W, device='cuda', generator=torch.Generator('cuda').manual_seed(1))
-    y = torch.randn(S, 3, side, side, device='cuda', generator=torch.Generator('cuda').manual_seed(2))
-    res += [fwd(x).double().sum().item(), bwd(y).double().abs().sum().item()]
-print(" ".join("%%.10e" %% v for v in res))
-''' % (ROOT, os.path.join(ROOT, 'tests'))
-    outs = []
-    for env_add in ({}, {'APH_SAMPLE_FWD_OLD': '1', 'APH_SAMPLE_BWD_OLD': '1'}, {'APH_SAMPLE_BWD_FIXED': '1'}, {'APH_SAMPLE_BWD_GATHER': '1'}):
-        r = subprocess.run([sys.executable, '-c', code], capture_output=True, text=True, timeout=600, env=dict(os.environ, **env_add))
-        assert r.returncode == 0, r.stderr[-2000:]
-        outs.append(np.array([float(v) for v in r.stdout.split()]))
-    for o in outs[1:]:
-        np.testing.assert_allclose(o, outs[0], rtol=1e-6)
-
-
 # ---------------------------------------------------------------------------------------------- encoder on the size + 8 batch
 def _model(name):
     from aphantasia_b200.clip import CLIP, synthetic_visual_state_dict
