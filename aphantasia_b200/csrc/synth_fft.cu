@@ -418,15 +418,23 @@ extern "C" int aph_fft_plan_create(aph_fft_plan** plan_out, int H, int W) {
   APH_CUDA_OK(cudaMemcpy(p->twW, tw.data(), W * sizeof(float2), cudaMemcpyHostToDevice));
   APH_CUDA_OK(cudaMalloc(&p->T, (size_t)3 * H * p->Wh * sizeof(float2)));
   APH_CUDA_OK(cudaMalloc(&p->gimg, (size_t)3 * H * W * sizeof(float)));
+  // The shared-memory limit is an attribute of the kernel, not of the plan: only ever raise it, so that creating a plan with
+  // shorter lines does not break the launches of a larger plan that is still alive.
+  auto raise_smem = [](const void* fn, size_t bytes) -> cudaError_t {
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, fn);
+    if (e != cudaSuccess || (int)bytes <= fa.maxDynamicSharedSizeBytes) return e;
+    return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+  };
   if (p->colSingle) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_col_fft<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_col));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_col_fft<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_col));
+    APH_CUDA_OK(raise_smem((const void*)k_col_fft<true, true>, p->smem_col));
+    APH_CUDA_OK(raise_smem((const void*)k_col_fft<false, true>, p->smem_col));
   } else {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_col_fft<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_col));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_col_fft<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_col));
+    APH_CUDA_OK(raise_smem((const void*)k_col_fft<true>, p->smem_col));
+    APH_CUDA_OK(raise_smem((const void*)k_col_fft<false>, p->smem_col));
   }
-  APH_CUDA_OK(cudaFuncSetAttribute(k_row_c2r, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_row));
-  APH_CUDA_OK(cudaFuncSetAttribute(k_row_r2c, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)p->smem_row));
+  APH_CUDA_OK(raise_smem((const void*)k_row_c2r, p->smem_row));
+  APH_CUDA_OK(raise_smem((const void*)k_row_r2c, p->smem_row));
   *plan_out = reinterpret_cast<aph_fft_plan*>(p);
   return 0;
 }
