@@ -21,6 +21,9 @@ _SIGS = {
                                     c_f32p, C.c_void_p, c_f32p, C.c_void_p]),
     'aph_synth_fft_bwd': (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, C.c_void_p, c_f32p, C.c_float, C.c_void_p, C.c_int,
                                     c_f32p, C.c_void_p]),
+    'aph_un_rgb': (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_float, c_f32p, C.c_void_p]),
+    'aph_fft_analyze': (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, C.c_void_p]),
+    'aph_dwt_analyze': (C.c_int, [C.c_void_p, c_f32p, C.c_void_p, C.c_void_p, C.c_void_p]),
     'aph_dwt_plan_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int]),
     'aph_dwt_plan_destroy': (C.c_int, [C.c_void_p]),
     'aph_dwt_plan_levels': (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_void_p, C.c_void_p]),

@@ -9,6 +9,8 @@
 // numerators inside the band, where (g_r, g_c) = (g0,g0) for ll, (g1,g0) for lh, (g0,g1) for hl, (g1,g1) for hh.
 // One launch per level: k_dwt_level_fwd (thread = output pixel, (L/2)^2 taps x 4 bands from L1/L2) and its exact adjoint
 // k_dwt_level_bwd (thread = coefficient position, L^2 taps of the output gradient, all 4 band gradients at once).
+// The analysis of an image file (DWTForward, image.py:82-94) is separable: per level, finest first, k_dwt_afb_w filters along
+// W (stride 2, L taps, symmetric extension) and k_dwt_afb_h along H into LL and the three bands.
 #include "synth_common.cuh"
 #include <vector>
 #include <algorithm>
@@ -28,6 +30,60 @@ struct DwtPlanImpl {
   float* dll[kMaxLevels];                  // gradient w.r.t. ll[i]
   float* gimg = nullptr; float* gx = nullptr;
 };
+
+// Half-sample symmetric extension of index j onto [0, n) (pytorch_wavelets mypad 'symmetric'): period 2n, so it also wraps
+// lines shorter than the filter more than once.
+__device__ __forceinline__ int sym_index(int j, int n) {
+  const int per = 2 * n;
+  j %= per;
+  if (j < 0) j += per;
+  return j < n ? j : per - 1 - j;
+}
+
+// Analysis along W (pytorch_wavelets afb1d, dim 3, mode 'symmetric'): x [3][h][w] -> rows [3][2][h][ow] = (lo, hi), with
+// lo[k] = sum_t g0[t] x[sym(2k + t - pad)], hi with g1 (dec_lo[L-1-t] = rec_lo[t]), pad = (2 (ow - 1) - w + L) / 2.
+__global__ void __launch_bounds__(256) k_dwt_afb_w(const float* __restrict__ x, int h, int w, float* __restrict__ rows, int ow, Filt f) {
+  const int pad = (2 * (ow - 1) - w + f.L) / 2;
+  const size_t total = (size_t)3 * h * ow;
+  for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(idx / ((size_t)h * ow));
+    const int r = (int)(idx - (size_t)c * h * ow);
+    const int y = r / ow, k = r - y * ow;
+    const float* line = x + ((size_t)c * h + y) * w;
+    float lo = 0.f, hi = 0.f;
+    for (int t = 0; t < f.L; ++t) {
+      const float v = __ldg(line + sym_index(2 * k + t - pad, w));
+      lo += f.g0[t] * v; hi += f.g1[t] * v;
+    }
+    rows[(((size_t)c * 2 + 0) * h + y) * ow + k] = lo;
+    rows[(((size_t)c * 2 + 1) * h + y) * ow + k] = hi;
+  }
+}
+
+// Analysis along H of both halves: ll [3][oh][ow] and bands [3][3][oh][ow] * s in pytorch_wavelets' order (LH = H-high of the
+// W-low half, HL = H-low of the W-high half, HH).
+__global__ void __launch_bounds__(256) k_dwt_afb_h(const float* __restrict__ rows, int h, int ow, float* __restrict__ ll,
+                                                   float* __restrict__ bands, float s, int oh, Filt f) {
+  const int pad = (2 * (oh - 1) - h + f.L) / 2;
+  const size_t total = (size_t)3 * oh * ow;
+  for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
+    const int c = (int)(idx / ((size_t)oh * ow));
+    const int r = (int)(idx - (size_t)c * oh * ow);
+    const int k = r / ow, l = r - k * ow;
+    const float* lo = rows + (size_t)c * 2 * h * ow + l;
+    const float* hi = lo + (size_t)h * ow;
+    float a_ll = 0.f, a_lh = 0.f, a_hl = 0.f, a_hh = 0.f;
+    for (int t = 0; t < f.L; ++t) {
+      const size_t o = (size_t)sym_index(2 * k + t - pad, h) * ow;
+      const float vl = __ldg(lo + o), vh = __ldg(hi + o);
+      a_ll += f.g0[t] * vl; a_lh += f.g1[t] * vl; a_hl += f.g0[t] * vh; a_hh += f.g1[t] * vh;
+    }
+    ll[idx] = a_ll;
+    bands[((size_t)(c * 3 + 0) * oh + k) * ow + l] = s * a_lh;
+    bands[((size_t)(c * 3 + 1) * oh + k) * ow + l] = s * a_hl;
+    bands[((size_t)(c * 3 + 2) * oh + k) * ow + l] = s * a_hh;
+  }
+}
 
 // out [3][oh][ow] = SFB2D(ll [3][*][llw] (logical h x w), bands [3][3][h][w] * s)
 __global__ void __launch_bounds__(256) k_dwt_level_fwd(const float* __restrict__ ll, int llh_alloc, int llw, const float* __restrict__ bands, float s,
@@ -232,6 +288,37 @@ extern "C" int aph_synth_dwt_bwd(aph_dwt_plan* plan, const float* grad_out, cons
     const size_t n = (size_t)3 * llh * llw;
     k_dwt_level_bwd<<<grid_for(n), 256, 0, st>>>(dout, p->oh[i], p->ow[i], dll, llh, llw, grad_Ys[i + 1], scales_host[i], p->lh[i], p->lw[i], p->f);
     APH_LAUNCH_OK();
+  }
+  return 0;
+}
+
+// Analysis (image-file resume, aphantasia/image.py:82-94): DWTForward(J, mode 'symmetric') of img [3,H,W], finest level first;
+// Ys as in aph_synth_dwt_fwd (written here), Yh_i multiplied by inv_scales_host[i]. Level i's LL lands in ll[i + 1], which
+// holds the oh[i + 1] x ow[i + 1] >= lh[i] x lw[i] synthesis output of that level, and the last one in Yl.
+// The row-filtered halves [3][2][h][ow] of each level go to a stream-ordered allocation of exactly that level's size, freed
+// behind the level's two launches: the long-lived plan keeps nothing for the analysis, and no size formula can fall short
+// when lines shorter than the filter make the levels grow (h -> (h + L - 1) / 2 > h for h < L - 1).
+extern "C" int aph_dwt_analyze(aph_dwt_plan* plan, const float* img, const float* inv_scales_host, float* const* Ys, void* stream) {
+  APH_REQUIRE(plan && img && inv_scales_host && Ys, "aph_dwt_analyze: null pointer");
+  DwtPlanImpl* p = reinterpret_cast<DwtPlanImpl*>(plan);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int J = p->J;
+  const float* x = img;
+  int h = p->H, w = p->W;
+  for (int i = 0; i < J; ++i) {
+    const int oh = p->lh[i], ow = p->lw[i];
+    float* rows = nullptr;
+    APH_CUDA_OK(cudaMallocAsync((void**)&rows, (size_t)3 * 2 * h * ow * sizeof(float), st));
+    float* ll = (i == J - 1) ? Ys[0] : p->ll[i + 1];
+    k_dwt_afb_w<<<grid_for((size_t)3 * h * ow), 256, 0, st>>>(x, h, w, rows, ow, p->f);
+    const cudaError_t e1 = cudaGetLastError();
+    if (e1 == cudaSuccess)
+      k_dwt_afb_h<<<grid_for((size_t)3 * oh * ow), 256, 0, st>>>(rows, h, ow, ll, Ys[i + 1], inv_scales_host[i], oh, p->f);
+    const cudaError_t e2 = e1 == cudaSuccess ? cudaGetLastError() : e1;
+    APH_CUDA_OK(cudaFreeAsync(rows, st));
+    APH_CUDA_OK(e2);
+    count_launch(2);
+    x = ll; h = oh; w = ow;
   }
   return 0;
 }

@@ -17,6 +17,9 @@
 //   k_finish_bwd: g_img = Mn^T . (g*out*(1-out)); accumulates sum g_img.x      (pointwise)
 //   k_row_r2c   : g_x = (c/sigma)(g_img - (x-mu) * dot/((N-1) sigma^2)) formed on load; two real rows
 //                 per complex forward DFT; interior columns x2; writes dT.
+//   k_row_rfft  : analysis row pass (image-file resume): plain load of the image, two real rows per complex forward DFT,
+//                 writes T; k_col_fft<false> then finishes rfftn and multiplies by the analysis scale.
+//   k_un_rgb    : uint8 HWC picture -> planar fp32 through the inverse colour matrix (un_rgb).
 #include "synth_common.cuh"
 #include <vector>
 #include <algorithm>
@@ -371,6 +374,52 @@ __global__ void __launch_bounds__(256) k_row_r2c(const float* __restrict__ gimg,
   }
 }
 
+// Row pass of the analysis rfftn(img, 'ortho'): the same two-rows-per-complex-DFT split as k_row_r2c, on a plain load of img
+// [3][H][W] and without the adjoint's doubling of the interior columns: every column is A = (Z[k] + conj(Z[W-k])) / 2.
+__global__ void __launch_bounds__(256) k_row_rfft(const float* __restrict__ img, float2* __restrict__ T, const float2* __restrict__ twg,
+                                                  int H, int W, int Wh, int P, float norm, Radices rad) {
+  extern __shared__ float2 smem[];
+  const int LS = W + 1;
+  float2* tw = smem;
+  float2* bufA = tw + W;
+  float2* bufB = bufA + P * LS;
+  const int pairs_per_ch = (H + 1) / 2;
+  const int groups = (pairs_per_ch + P - 1) / P;
+  const int ch = blockIdx.x / groups, pbase = (blockIdx.x % groups) * P;
+  const int np = min(P, pairs_per_ch - pbase);
+  for (int i = threadIdx.x; i < W; i += blockDim.x) tw[i] = twg[i];
+  for (int idx = threadIdx.x; idx < np * W; idx += blockDim.x) {
+    const int p = idx / W, n = idx - p * W;
+    const int r0 = 2 * (pbase + p), r1 = r0 + 1;
+    const size_t i0 = ((size_t)ch * H + r0) * W + n;
+    bufA[p * LS + n] = make_float2(img[i0], r1 < H ? img[i0 + W] : 0.f);
+  }
+  __syncthreads();
+  float2* res = fft_lines<true>(bufA, bufB, tw, W, rad, np, LS);
+  const float f = 0.5f * norm;
+  for (int idx = threadIdx.x; idx < np * Wh; idx += blockDim.x) {
+    const int p = idx / Wh, k = idx - p * Wh;
+    const int r0 = 2 * (pbase + p), r1 = r0 + 1;
+    const float2 z = res[p * LS + k];
+    const float2 zc = res[p * LS + ((W - k) % W)];
+    T[((size_t)ch * H + r0) * Wh + k] = make_float2((z.x + zc.x) * f, (z.y - zc.y) * f);
+    if (r1 < H) T[((size_t)ch * H + r1) * Wh + k] = make_float2((z.y + zc.y) * f, (zc.x - z.x) * f);
+  }
+}
+
+// un_rgb (aphantasia/image.py:185-197): uint8 HWC -> planar [3][H][W] = gain * Minv . ((x / 255 - mean) / std), in the
+// reference's order of operations (divide, subtract, divide, 3x3 mix, gain).
+__global__ void __launch_bounds__(256) k_un_rgb(const uint8_t* __restrict__ hwc, size_t hw, ColMat mi, float gain, float* __restrict__ out) {
+  const float mean[3] = {0.48145466f, 0.4578275f, 0.40821073f}, std_[3] = {0.26862954f, 0.26130258f, 0.27577711f};
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < hw; i += (size_t)gridDim.x * blockDim.x) {
+    float v[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) v[c] = ((float)hwc[3 * i + c] / 255.f - mean[c]) / std_[c];
+#pragma unroll
+    for (int d = 0; d < 3; ++d) out[d * hw + i] = gain * (mi.m[3 * d] * v[0] + mi.m[3 * d + 1] * v[1] + mi.m[3 * d + 2] * v[2]);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 }  // namespace aph
 
@@ -435,6 +484,7 @@ extern "C" int aph_fft_plan_create(aph_fft_plan** plan_out, int H, int W) {
   }
   APH_CUDA_OK(raise_smem((const void*)k_row_c2r, p->smem_row));
   APH_CUDA_OK(raise_smem((const void*)k_row_r2c, p->smem_row));
+  APH_CUDA_OK(raise_smem((const void*)k_row_rfft, p->smem_row));
   *plan_out = reinterpret_cast<aph_fft_plan*>(p);
   return 0;
 }
@@ -515,6 +565,35 @@ extern "C" int aph_synth_fft_bwd_adam(aph_fft_plan* plan, const float* grad_out,
   a.p = reinterpret_cast<float2*>(params); a.m = reinterpret_cast<float2*>(m); a.v = reinterpret_cast<float2*>(v);
   a.step_size = (float)(lr / bc1); a.b1 = b1; a.b2 = b2; a.eps = eps; a.inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2)); a.on = 1;
   return synth_fft_bwd_impl(plan, grad_out, out, x_raw, stats, scale, contrast, colmat_host, apply_sigmoid, grad_params, a, stream);
+}
+
+// Analysis (image-file resume, aphantasia/image.py:208-220): spectrum [3,H,Wh,2] = ascale * rfftn(img [3,H,W], 'ortho'). The row
+// pass writes the plan's T; the column pass is the synthesis backward's forward DFT, which already multiplies by a per-bin scale.
+extern "C" int aph_fft_analyze(aph_fft_plan* plan, const float* img, const float* ascale, float* spectrum, void* stream) {
+  APH_REQUIRE(plan && img && ascale && spectrum, "aph_fft_analyze: null pointer");
+  FftPlanImpl* p = reinterpret_cast<FftPlanImpl*>(plan);
+  cudaStream_t st = (cudaStream_t)stream;
+  const int H = p->H, W = p->W, Wh = p->Wh;
+  const int groups = ((H + 1) / 2 + p->rowP - 1) / p->rowP;
+  const float norm = (float)(1.0 / sqrt((double)H * W));
+  k_row_rfft<<<3 * groups, 256, p->smem_row, st>>>(img, p->T, p->twW, H, W, Wh, p->rowP, norm, p->rw);
+  APH_LAUNCH_OK();
+  const int col_tiles = (Wh + p->colC - 1) / p->colC;
+  if (p->colSingle) k_col_fft<false, true><<<3 * col_tiles, 512, p->smem_col, st>>>(p->T, reinterpret_cast<float2*>(spectrum), ascale, nullptr, 0,
+                                                                                     p->twH, H, Wh, p->colC, p->rh, AdamArgs{});
+  else k_col_fft<false><<<3 * col_tiles, 256, p->smem_col, st>>>(p->T, reinterpret_cast<float2*>(spectrum), ascale, nullptr, 0,
+                                                                p->twH, H, Wh, p->colC, p->rh, AdamArgs{});
+  APH_LAUNCH_OK();
+  return 0;
+}
+
+extern "C" int aph_un_rgb(const uint8_t* hwc, int H, int W, const float* inv_colmat_host, float gain, float* out, void* stream) {
+  APH_REQUIRE(hwc && inv_colmat_host && out && H > 0 && W > 0, "aph_un_rgb: bad arguments");
+  const size_t hw = (size_t)H * W;
+  const int blocks = (int)std::min<size_t>((hw + 255) / 256, (size_t)num_sms() * 8);
+  k_un_rgb<<<blocks, 256, 0, (cudaStream_t)stream>>>(hwc, hw, make_colmat(inv_colmat_host), gain, out);
+  APH_LAUNCH_OK();
+  return 0;
 }
 
 namespace aph {

@@ -14,13 +14,106 @@ from . import _dist, _pool
 from ._lib import check, lib, require_cuda, stream_ptr
 
 
-def _color_matrix_host(colors):
-    """Mn[d][c] such that out_d = sum_c Mn[d][c] * img_c  (image.py:15-22: einsum('nchw,cd->ndhw', img, M.T))."""
+def _color_correlation(colors):
+    """The normalised colour matrix m (fp32) of to_valid_rgb / un_rgb; colcorr_t = m.T  (image.py:15-19, 186-190)."""
     m = torch.tensor([[0.26, 0.09, 0.02], [0.27, 0.00, -0.05], [0.27, -0.09, 0.03]])
     m = m / torch.tensor([colors, 1., 1.])
-    m = m / m.norm(dim=0).max()
+    return m / m.norm(dim=0).max()
+
+
+def _color_matrix_host(colors):
+    """Mn[d][c] such that out_d = sum_c Mn[d][c] * img_c  (image.py:15-22: einsum('nchw,cd->ndhw', img, M.T))."""
+    m = _color_correlation(colors)
     # colcorr_t = m.T ; out[d] = sum_c img[c] * colcorr_t[c, d] = sum_c m[d, c] * img[c]
     return (C.c_float * 9)(*[float(v) for v in m.reshape(-1)])
+
+
+# ---- starting from an image file (image.py:82-107, 130-150, 185-220) ---------------------------------------------------------
+def _is_image_file(path):
+    """resume_fft's / init_dwt's test (image.py:45, 138): .jpeg and .tiff are not in the list and go to torch.load."""
+    return os.path.splitext(path)[1].lower()[1:] in ['jpg', 'png', 'tif', 'bmp']
+
+
+def _rgb_u8(img):
+    """A decoded picture as contiguous uint8 [H,W,3] under utils.img_read's channel rules (grey -> 3 channels, RGBA -> RGB)."""
+    img = np.asarray(img)
+    if img.dtype != np.uint8:
+        raise ValueError('aphantasia_b200: starting from an image needs 8-bit colour (a uint8 array); this one is %s' % img.dtype)
+    if img.ndim == 2 or (img.ndim == 3 and img.shape[2] == 1):
+        img = np.dstack((img, img, img))
+    if img.ndim == 3 and img.shape[2] == 4:
+        img = img[:, :, :3]
+    if img.ndim != 3 or img.shape[2] != 3:
+        raise ValueError('aphantasia_b200: expected a grey, RGB or RGBA picture, got an array of shape %s' % (img.shape,))
+    return np.require(img, requirements=['C', 'W'])          # a decoder's read-only buffer is copied: torch shares writable memory only
+
+
+def _un_rgb(img, colors, gain):
+    """gain * un_rgb(img, colors) as a CUDA tensor [1,3,H,W] (aph_un_rgb: one upload of 3 bytes per pixel)."""
+    img = _rgb_u8(img)
+    h, w = img.shape[:2]
+    inv = torch.linalg.inv(_color_correlation(colors).T)           # inv(colcorr_t) in fp32, as image.py:191
+    # einsum('nchw,cd->ndhw', x, inv): out_d = sum_c inv[c, d] x_c, so Minv[d][c] = inv[c][d]
+    minv = (C.c_float * 9)(*[float(v) for v in inv.T.reshape(-1)])
+    src = torch.from_numpy(img).cuda()
+    out = torch.empty(1, 3, h, w, device=src.device)
+    check(lib().aph_un_rgb(src.data_ptr(), h, w, minv, float(gain), out.data_ptr(), stream_ptr()), 'aph_un_rgb')
+    return out
+
+
+def un_rgb(image, colors=1.):
+    """Drop-in for image.py:185-197 on a uint8 HWC picture: CUDA tensor [1,3,H,W]."""
+    return _un_rgb(image, colors, 1.)
+
+
+def _prime_factors(n):
+    out, p = [], 2
+    while p * p <= n:
+        while n % p == 0:
+            out.append(p); n //= p
+        p += 1
+    return out + ([n] if n > 1 else [])
+
+
+def _check_fft_size(h, w):
+    """The FFT generator's lengths are products of primes <= 13: refuse any other picture size before any GPU work."""
+    for n in (w, h):
+        f = _prime_factors(n)
+        if f and f[-1] > 13:
+            raise ValueError('%d×%d: %d = %s; the FFT generator needs prime factors ≤ 13; crop or resize the image, or use --dwt'
+                             % (w, h, n, '·'.join(str(v) for v in f)))
+
+
+def _analysis_scale(h, wh, decay, sd):
+    """sd * 500000 / un_spectrum's scale, float64 on the host, cast once (image.py:199-206, 218-219, 147). un_spectrum
+    recovers w from the half-spectrum width, (wh - 1) * 2: for an odd image width that is W - 1, and so are its frequencies."""
+    w = (wh - 1) * 2
+    scale = 1. / np.maximum(rfft2d_freqs(h, w), 1. / max(w, h)) ** decay
+    scale *= np.sqrt(w * h)
+    return torch.tensor(sd * 500000. / scale).float()
+
+
+def _img2fft(img, decay, colors, sd):
+    """sd * img2fft(img, decay, colors): [1,3,H,W//2+1,2] on the GPU (aph_un_rgb, then aph_fft_analyze)."""
+    img = _rgb_u8(img)
+    h, w = img.shape[:2]
+    _check_fft_size(h, w)
+    plan = C.c_void_p()
+    check(lib().aph_fft_plan_create(C.byref(plan), h, w), 'aph_fft_plan_create')
+    try:
+        x = _un_rgb(img, colors, 1.)
+        ascale = _analysis_scale(h, w // 2 + 1, decay, sd).cuda()
+        spectrum = torch.empty(1, 3, h, w // 2 + 1, 2, device=x.device)
+        check(lib().aph_fft_analyze(plan, x.data_ptr(), ascale.data_ptr(), spectrum.data_ptr(), stream_ptr()), 'aph_fft_analyze')
+        torch.cuda.current_stream().synchronize()          # the plan's scratch is in use until then
+    finally:
+        lib().aph_fft_plan_destroy(plan)
+    return spectrum
+
+
+def img2fft(img_in, decay=1., colors=1.):
+    """Drop-in for image.py:208-220: the spectrum parameters [1,3,H,W//2+1,2] (CUDA) of the picture img_in."""
+    return _img2fft(img_in, decay, colors, 1.)
 
 
 def rfft2d_freqs(h, w):
@@ -111,7 +204,8 @@ class FFTImage:
 
 
 def resume_fft(resume=None, shape=None, decay=None, colors=1.6, sd=0.01):
-    """image.py:130-150. Image-file resume (img2fft) is init-time and out of scope; .pt / tensor resume is kept."""
+    """image.py:130-150. An image file is analysed on the GPU with resume_fft's own colors (fft_image passes none) and returns
+    its (H, W); every rank computes the same bits from the same file."""
     size = None
     if resume is None:
         params_shape = [*shape[:3], shape[3] // 2 + 1, 2]
@@ -121,12 +215,16 @@ def resume_fft(resume=None, shape=None, decay=None, colors=1.6, sd=0.01):
         params = params.cuda()
     elif isinstance(resume, str):
         if os.path.isfile(resume):
-            if os.path.splitext(resume)[1].lower()[1:] in ['jpg', 'png', 'tif', 'bmp']:
-                raise NotImplementedError('aphantasia_b200: resuming from an image file (img2fft) is not on the CUDA hot path')
-            params = torch.load(resume)
-            if isinstance(params, list): params = params[0]
-            params = params.detach().cuda()
-            params *= sd
+            if _is_image_file(resume):
+                from .utils import img_read
+                img_in = img_read(resume)
+                params = _img2fft(img_in, decay, colors, sd)          # `params *= sd` is folded into the analysis scale
+                size = img_in.shape[:2]
+            else:
+                params = torch.load(resume)
+                if isinstance(params, list): params = params[0]
+                params = params.detach().cuda()
+                params *= sd
         else:
             print(' Snapshot not found:', resume); exit()
     else:
@@ -191,7 +289,13 @@ def pixel_image(shape, resume=None, sd=1., *noargs, **nokwargs):
     if resume is None:
         image_t = torch.randn(*shape) * sd
     elif isinstance(resume, str):
-        raise NotImplementedError('aphantasia_b200: pixel_image resume from an image file (un_rgb) is init-time, out of the hot path')
+        if not os.path.isfile(resume):
+            print(' Image not found:', resume); exit()
+        from .utils import img_read
+        img_in = img_read(resume)
+        image_t = _un_rgb(img_in, 2., 3.3)
+        size = img_in.shape[:2]
+        print(resume, size)
     else:
         if isinstance(resume, list): resume = resume[0]
         image_t = resume
@@ -296,8 +400,7 @@ class DWTImage:
         self.J = J.value
         self.level_hw = [(dims[2 * i], dims[2 * i + 1]) for i in range(self.J)]
         self.out_hw = (ohw[0], ohw[1])
-        h0, w0 = self.level_hw[0]
-        self.scales = [((h0 * w0) / (hh * ww)) ** (1. - sharp) for (hh, ww) in self.level_hw]      # image.py:73-80
+        self.scales = _dwt_scales(self.level_hw, sharp)
         self.scales_c = (C.c_float * self.J)(*[float(v) for v in self.scales])
         self.Ys = None
 
@@ -319,10 +422,49 @@ class DWTImage:
         return self.fused(shift, contrast, None, False)
 
 
-def dwt_image(shape, wave='coif2', sharp=0.3, colors=1., resume=None):
-    """Drop-in for image.py:61-71 / init_dwt :33-59: returns (Ys, image_f, size) with Ys = [Yl, Yh_1 (finest) .. Yh_J]
-    ~ N(0,1) leaves. Resume from a .pt list / tensors is kept; image-file resume (img2dwt) is init-time, out of scope."""
-    _dist.init()
+def _dwt_scales(level_hw, sharp):
+    """image.py:73-80 from the band sizes, finest first."""
+    h0, w0 = level_hw[0]
+    return [((h0 * w0) / (hh * ww)) ** (1. - sharp) for (hh, ww) in level_hw]
+
+
+def dwt_scale(Ys, sharp):
+    """Drop-in for image.py:73-80."""
+    return _dwt_scales([tuple(y.shape[3:5]) for y in Ys[1:]], sharp)
+
+
+def _img2dwt(img, gen, colors, sharp=0.3):
+    """img2dwt (image.py:82-94) on the plan of `gen`, which has the picture's size: [Yl, Yh_1 .. Yh_J] CUDA tensors, each
+    Yh_i divided by its scale at `sharp`."""
+    x = _un_rgb(img, colors, 1.)
+    Ys = [torch.empty(sh, device=x.device) for sh in gen.param_shapes()]
+    inv = (C.c_float * gen.J)(*[1. / s for s in _dwt_scales(gen.level_hw, sharp)])
+    ptrs = (C.c_void_p * len(Ys))(*[y.data_ptr() for y in Ys])
+    check(lib().aph_dwt_analyze(gen.plan, x.data_ptr(), inv, ptrs, stream_ptr()), 'aph_dwt_analyze')
+    return Ys
+
+
+def img2dwt(img_in, wave='coif2', sharp=0.3, colors=1.):
+    """Drop-in for image.py:82-94: the wavelet parameters [Yl, Yh_1 (finest) .. Yh_J] (CUDA) of the picture img_in."""
+    img = _rgb_u8(img_in)
+    gen = DWTImage([1, 3, *img.shape[:2]], wave, sharp)
+    Ys = _img2dwt(img, gen, colors, sharp)
+    torch.cuda.current_stream().synchronize()              # the plan's scratch is in use until then
+    return Ys
+
+
+def _init_dwt(resume, shape, wave, sharp, colors):
+    """init_dwt (image.py:33-59) with the generator built for the size it settles on, the picture's for an image file:
+    (gen, Ys, size). The picture's bands are divided by the scales at init_dwt's sharp = 0.3 whatever `sharp` is."""
+    size, img_in = None, None
+    if isinstance(resume, str):
+        if not os.path.isfile(resume):
+            print(' Snapshot not found:', resume); exit()
+        if _is_image_file(resume):
+            from .utils import img_read
+            img_in = _rgb_u8(img_read(resume))
+            size = img_in.shape[:2]
+            shape = [1, 3, *size]
     gen = DWTImage(shape, wave, sharp)
     if resume is None:
         Ys = [torch.randn(*sh) for sh in gen.param_shapes()]          # same draw order as init_dwt (image.py:42)
@@ -330,15 +472,29 @@ def dwt_image(shape, wave='coif2', sharp=0.3, colors=1., resume=None):
             Ys = [y.cuda() for y in Ys]
             for y in Ys: torch.distributed.broadcast(y, 0)
         Ys = [y.cuda() for y in Ys]
+    elif img_in is not None:
+        Ys = _img2dwt(img_in, gen, colors)
+        print(' loaded image', resume, img_in.shape, 'level', len(Ys) - 1)
     elif isinstance(resume, str):
-        if not os.path.isfile(resume):
-            print(' Snapshot not found:', resume); exit()
-        if os.path.splitext(resume)[1].lower()[1:] in ['jpg', 'png', 'tif', 'bmp']:
-            raise NotImplementedError('aphantasia_b200: resuming from an image file (img2dwt) is not on the CUDA hot path')
         Ys = [y.detach().cuda() for y in torch.load(resume)]
     else:
         Ys = [y.cuda() for y in resume]
+    return gen, Ys, size
+
+
+def init_dwt(resume=None, shape=None, wave=None, colors=None):
+    """Drop-in for image.py:33-59: (Ys, None, None, size); the pytorch_wavelets transforms it also returns do not exist here."""
+    _, Ys, size = _init_dwt(resume, shape, wave, 0.3, colors)
+    torch.cuda.current_stream().synchronize()              # the analysis plan goes with `gen`
+    return Ys, None, None, size
+
+
+def dwt_image(shape, wave='coif2', sharp=0.3, colors=1., resume=None):
+    """Drop-in for image.py:61-71 / init_dwt :33-59: returns (Ys, image_f, size) with Ys = [Yl, Yh_1 (finest) .. Yh_J]
+    ~ N(0,1) leaves, or the analysis of an image file at that file's size (returned as `size`), or a .pt list / tensors."""
+    _dist.init()
+    gen, Ys, size = _init_dwt(resume, shape, wave, sharp, colors)
     assert [tuple(y.shape) for y in Ys] == gen.param_shapes(), 'dwt_image: parameter shapes do not match this size / wavelet'
     Ys = [y.requires_grad_(True) for y in Ys]
     gen.Ys = Ys
-    return Ys, gen, None
+    return Ys, gen, size

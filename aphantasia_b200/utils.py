@@ -346,8 +346,20 @@ def img_list(path, subdir=None):
     return sorted([f for f in files if os.path.isfile(f)])
 
 
+def _pil_imread(path):
+    """imageio.imread's decoding through PIL (what dropin/imageio uses): palette images come back as RGB(A) colours."""
+    from PIL import Image
+    with Image.open(path) as im:
+        if im.mode == 'P':
+            im = im.convert('RGBA' if 'transparency' in im.info else 'RGB')
+        return np.asarray(im)
+
+
 def img_read(path):
-    from imageio import imread
+    try:
+        from imageio import imread
+    except ImportError:
+        imread = _pil_imread
     img = imread(path)
     if (img.ndim == 2) or (img.shape[2] == 1):
         img = np.dstack((img, img, img))

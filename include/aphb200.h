@@ -85,6 +85,17 @@ int aph_synth_fft_bwd(aph_fft_plan* plan, const float* grad_out, const float* ou
                       const float* colmat_host, int apply_sigmoid,
                       float* grad_params, void* stream);
 
+/* ---- starting from an image file (resume_fft / img2fft / img2dwt / pixel_image, aphantasia/image.py:82-107,130-150,185-220).
+ * aph_un_rgb: un_rgb (image.py:185-197). hwc: DEVICE uint8 [H,W,3] (grey / RGBA are made 3-channel on the host, as
+ * utils.img_read does); out [3,H,W] = gain * Minv . ((x/255 - mean) / std) with the CLIP normalisation of transforms.py:106;
+ * inv_colmat_host: 9 floats, HOST, row-major Minv[d][c] = inverse(colcorr_t)[c][d] (the inverse of to_valid_rgb's mix).
+ * gain is 1 (img2fft / img2dwt) or 3.3 (pixel_image).                                                               */
+int aph_un_rgb(const uint8_t* hwc, int H, int W, const float* inv_colmat_host, float gain, float* out, void* stream);
+/* aph_fft_analyze: spectrum [3,H,Wh,2] = ascale [H,Wh] * rfftn(img [3,H,W], norm='ortho') on a plan of the image's size.
+ * img2fft's division by un_spectrum's scale, its factor 500000 and resume_fft's sd are all folded into ascale. Uses the
+ * plan's scratch: do not interleave with a synthesis on the same plan and stream order.                              */
+int aph_fft_analyze(aph_fft_plan* plan, const float* img, const float* ascale, float* spectrum, void* stream);
+
 /* Wavelet parameterisation (BASELINE config 3). Replaces dwt_image.inner (aphantasia/image.py:66-69):
  *   img = DWTInverse((Yl, [Yh_i * scale_i])) * contrast / std, fused with to_valid_rgb like the FFT path.
  * DWTInverse is pytorch_wavelets' (third-party, mode 'symmetric'); rec_lo / rec_hi (HOST, L taps) are the
@@ -103,6 +114,11 @@ int aph_synth_dwt_fwd(aph_dwt_plan* plan, const float* const* Ys, const float* s
 int aph_synth_dwt_bwd(aph_dwt_plan* plan, const float* grad_out, const float* out, const float* x_raw,
                       double* stats, const float* scales_host, float contrast, const float* colmat_host,
                       int apply_sigmoid, float* const* grad_Ys, void* stream);
+/* Analysis of an image (img2dwt, aphantasia/image.py:82-94): DWTForward(J, wave, mode='symmetric') of img [3,H,W] (H, W of
+ * the plan), rows filtered before columns, bands (LH, HL, HH). Ys: HOST array of J+1 DEVICE pointers shaped as for
+ * aph_synth_dwt_fwd, overwritten; Yh_i is multiplied by inv_scales_host[i] (HOST [J]). Uses the plan's LL scratch; the
+ * row-filtered halves of each level live in a stream-ordered allocation (cudaMallocAsync) freed behind that level.        */
+int aph_dwt_analyze(aph_dwt_plan* plan, const float* img, const float* inv_scales_host, float* const* Ys, void* stream);
 
 /* Direct RGB parameterisation: pixel_image.inner (aphantasia/image.py:112-118): img = x*contrast/std(x) (or /3.3 with
  * fixcontrast), fused with to_valid_rgb. x / out / grad_x are [3,H,W]; stats as above.                             */
