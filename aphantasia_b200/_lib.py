@@ -64,6 +64,7 @@ _SIGS = {
                                             C.c_int, c_f32p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]),
     'aph_gemm_variant_launches': (C.c_int64, [C.c_int, C.c_int]),
     'aph_attn_test': (C.c_int, [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    'aph_attn_long_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     'aph_ln_fwd_test': (C.c_int, [c_f32p, c_f32p, c_f32p, C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_int, C.c_void_p]),
     'aph_ln_bwd_test': (C.c_int, [C.c_void_p, C.c_int, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                   C.c_int, c_f32p, C.c_void_p]),

@@ -2,7 +2,7 @@
 `clip.load(name, jit=False) -> (model, preprocess)`, `clip.tokenize`, `model.encode_image`, `model.encode_text`,
 `model.visual.input_resolution`.
 
-The image encoder (ViT-B/32, ViT-B/16) runs forward and data-gradient in libaphb200.so (csrc/vit.cu: wgmma
+The image encoder (ViT-B/32, ViT-B/16, ViT-L/14) runs forward and data-gradient in libaphb200.so (csrc/vit.cu: wgmma
 GEMMs + fused kernels). Weights: an OpenAI state dict if `APH_CLIP_WEIGHTS=<file.pt>` is set (a TorchScript archive as
 OpenAI ships them, or a plain state dict), else seeded synthetic weights of the same architecture.
 The text encoder (csrc/text.cu, forward only) runs once per prompt before the optimisation loop when the weights hold
@@ -23,7 +23,8 @@ from .._lib import TextConfig, VitConfig, check, lib, require_cuda, stream_ptr
 from ._bpe import SimpleTokenizer
 
 _MODELS = {'ViT-B/32': dict(patch=32, width=768, layers=12, heads=12, out_dim=512, res=224),
-           'ViT-B/16': dict(patch=16, width=768, layers=12, heads=12, out_dim=512, res=224)}
+           'ViT-B/16': dict(patch=16, width=768, layers=12, heads=12, out_dim=512, res=224),
+           'ViT-L/14': dict(patch=14, width=1024, layers=24, heads=16, out_dim=768, res=224)}
 
 
 def available_models():

@@ -110,4 +110,9 @@ __device__ __forceinline__ float warp_max(float v) {
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + __expf(-x)); }
 
+// Row length of the encoder's patch-embedding operand (conv1 as a GEMM): the 3 p^2 pixels of a patch, zero-padded to a
+// multiple of 128 (the K step of the forward GEMM, and the N tile of the data-gradient GEMM, whose N is this length).
+// 3072 for p = 32 and 768 for p = 16 (no padding), 640 for p = 14 (52 zero columns).
+__host__ __device__ constexpr int patch_k(int p) { return (3 * p * p + 127) / 128 * 128; }
+
 }  // namespace aph

@@ -48,8 +48,8 @@ int load_block_tensor(Encoder* h, const std::string& k, const char* key, const f
 // every key of `want` and of the blocks was loaded; a missing one is named as prefix + key
 int check_loaded(const Encoder* h, std::vector<std::string> want, const char* who, const char* prefix);
 
-// fp32 [rows, cols] -> bf16 [rows, cols] (transpose = 0) or bf16 [cols, rows] (transpose = 1)
-int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st);
+// fp32 [rows, cols] -> bf16 [rows, cols] (transpose = 0, row stride ld, 0 = cols) or bf16 [cols, rows] (transpose = 1)
+int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st, int ld = 0);
 int copy_f32(const float* src, float* dst, size_t n, cudaStream_t st);
 
 // grid of the one-warp-per-row kernels

@@ -262,13 +262,14 @@ k_sample_fwd(const float* __restrict__ canvas, int H, int W, int pad_top, int pa
 //              without a warp stage.
 //   k_compose: stages 2-5 for ALL THREE channels of a pixel per thread: one evaluation of the rotate (and perspective) taps,
 //              4 (16) gathers per channel from the scratch image through L1.
-// The encoder's patch-embedding GEMM reads its A operand patch-major in bf16: [S*g*g, 3*p*p], row = s*g*g + gy*g + gx,
-// col = c*p*p + py*p + px (conv1 weight layout, vit_ops.cuh k_patchify). With `patches` set the sampler's last stage writes that
-// operand beside the fp32 batch (SURVEY 2.4 k10-k12), so the encoder does not re-read 4 bytes per pixel to produce it.
+// The encoder's patch-embedding GEMM reads its A operand patch-major in bf16: [S*g*g, patch_k(p)], row = s*g*g + gy*g + gx,
+// col = c*p*p + py*p + px (conv1 weight layout, vit_ops.cuh k_patchify; the columns >= 3 p^2 are zero padding, never written).
+// With `patches` set the sampler's last stage writes that operand beside the fp32 batch (SURVEY 2.4 k10-k12), so the encoder
+// does not re-read 4 bytes per pixel to produce it.
 struct PatchOut { __nv_bfloat16* base; int p, g; };
 __device__ __forceinline__ size_t patch_index(const PatchOut& po, int s, int c, int i, int j) {
   const int gy = i / po.p, py = i - gy * po.p, gx = j / po.p, px = j - gx * po.p;
-  return ((size_t)(s * po.g + gy) * po.g + gx) * (size_t)(3 * po.p * po.p) + (size_t)(c * po.p + py) * po.p + px;
+  return ((size_t)(s * po.g + gy) * po.g + gx) * (size_t)patch_k(po.p) + (size_t)(c * po.p + py) * po.p + px;
 }
 
 template <bool WRAP>

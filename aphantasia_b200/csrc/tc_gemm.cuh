@@ -33,7 +33,7 @@ struct GemmEpi {
   bf16* out_bf16 = nullptr;        // bf16 [M, N]
   bf16* out_pre = nullptr;         // bf16 [M, N] pre-activation (acc + bias), saved for backward
   int act = 0;                     // 1 = QuickGELU x*sigmoid(1.702x)
-  int unpatch_p = 0;               // >0: out_f32 is [S,3,R,R]; row = s*g*g + gy*g + gx, col = c*p*p + py*p + px
+  int unpatch_p = 0;               // >0: out_f32 is [S,3,R,R]; row = s*g*g + gy*g + gx, col = c*p*p + py*p + px (cols >= 3p^2 dropped)
   int unpatch_g = 0;
   // row strides in elements, 0 = N (dense). ld_out covers out_f32 / out_bf16 / out_pre and gelu_in, which has the output's rows.
   // A strided output leaves the rows between its rows untouched (the encoder's last block writes only the class-token rows).
@@ -205,6 +205,7 @@ __device__ __forceinline__ void epi_store2(const GemmEpi& epi, size_t out_row, s
     *reinterpret_cast<float2*>(epi.out_f32 + off) = make_float2(v0 + bb.x + r.x, v1 + bb.y + r.y);
   } else {   // EPI_UNPATCH: col = c*p*p + py*p + px with p even, so (col, col + 1) are adjacent pixels of one image row
     const int p = epi.unpatch_p, g = epi.unpatch_g, R = p * g;
+    if (col >= 3 * p * p) return;    // the operand's zero padding up to patch_k(p) (p = 14): no pixel of this patch
     const int ch = col / (p * p), rem = col - ch * p * p, py = rem / p, px = rem - py * p;
     const int s = row / (g * g), pr = row - s * g * g, gy = pr / g, gx = pr - gy * g;
     *reinterpret_cast<float2*>(epi.out_f32 + (((size_t)s * 3 + ch) * R + gy * p + py) * R + gx * p + px) = make_float2(v0, v1);

@@ -1,4 +1,4 @@
-// vit.cu -- CLIP ViT-B image encoder handle: packed bf16 weights, activation arena, forward and
+// vit.cu -- CLIP ViT image encoder handle (B/32, B/16, L/14): packed bf16 weights, activation arena, forward and
 // data-gradient backward built from the wgmma GEMM (tc_gemm.cuh) and the kernels of vit_ops.cuh.
 //
 // Restates OpenAI clip/model.py VisionTransformer.forward (third-party, SURVEY.md A5):
@@ -8,6 +8,7 @@
 // LayerNorm backward can recompute x-hat. No weight gradients (the reference computes and discards them).
 #include "encoder.cuh"
 #include "vit_attn_tc.cuh"
+#include "vit_attn_stream.cuh"
 #include <stdlib.h>
 #include <string.h>
 
@@ -15,13 +16,13 @@ namespace aph {
 
 struct VitImpl : Encoder {
   aph_vit_config cfg;
-  int g, T, D, Kp;
+  int g, T, D, Kp;                // Kp = patch_k(patch): the patch operand's row length, 3 p^2 zero-padded to a multiple of 128
   // weights besides the blocks'
-  bf16 *w_conv = nullptr, *w_conv_t = nullptr;   // [D, Kp], [Kp, D]
+  bf16 *w_conv = nullptr, *w_conv_t = nullptr;   // [D, Kp], [Kp, D]; the pad columns / rows are zero
   float *cls = nullptr, *pos = nullptr, *lnpre_w = nullptr, *lnpre_b = nullptr, *lnpost_w = nullptr, *lnpost_b = nullptr;
   bf16 *w_out = nullptr, *w_out_t = nullptr;     // proj^T [out, D] (forward B operand), proj [D, out] (dgrad B operand)
   // activations (sized for max_batch)
-  bf16* patches = nullptr;       // [S*g*g, Kp]
+  bf16* patches = nullptr;       // [S*g*g, Kp]; columns >= 3 p^2 zeroed at creation and never written
   float* tok = nullptr;          // [S*g*g, D]
   float* e = nullptr;            // [M, D] pre-ln_pre
   // Everything the caller gets comes from the cls rows s*T of the last block's output (ln_post reads x[:, 0]). So past its
@@ -50,6 +51,7 @@ struct VitImpl : Encoder {
                                  // written, so every other row stays exactly zero (layers below overwrite all rows of d_attn)
   bf16* d_qkv = nullptr;         // [M, 3D]
   bf16* d_tok = nullptr;         // [S*g*g, D]
+  float2* attn_stats = nullptr;  // [S*heads*T] (lse, delta) of the streaming attention backward (T > 256 only), reused by every layer
   int last_S = -1;
   // CUDA-graph cache: the ~90 launches of a forward (or backward) are replayed as one graph when the call repeats with the
   // same batch size and the same input/output pointers (the optimisation loop does); keyed, small LRU
@@ -128,19 +130,20 @@ static int run_cached(std::vector<VitImpl::GraphEntry>& cache, std::map<int, int
   return 0;
 }
 
-__global__ void __launch_bounds__(256) k_pack_weight(const float* __restrict__ in, bf16* __restrict__ out, int rows, int cols, int transpose) {
+// ld: row stride of the untransposed output (>= cols; the columns past cols are not written)
+__global__ void __launch_bounds__(256) k_pack_weight(const float* __restrict__ in, bf16* __restrict__ out, int rows, int cols, int transpose, int ld) {
   const size_t n = (size_t)rows * cols;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
     const int r = (int)(i / cols), c = (int)(i - (size_t)r * cols);
     const bf16 v = __float2bfloat16_rn(in[i]);
-    if (transpose) out[(size_t)c * rows + r] = v; else out[i] = v;
+    if (transpose) out[(size_t)c * rows + r] = v; else out[(size_t)r * ld + c] = v;
   }
 }
 
-int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st) {
+int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st, int ld) {
   const size_t n = (size_t)rows * cols;
   const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16);
-  k_pack_weight<<<blocks, 256, 0, st>>>(src, dst, rows, cols, transpose);
+  k_pack_weight<<<blocks, 256, 0, st>>>(src, dst, rows, cols, transpose, ld > 0 ? ld : cols);
   APH_LAUNCH_OK();
   return 0;
 }
@@ -244,7 +247,15 @@ static bool attn_simt() {
   return v == 1;
 }
 
+// The resident kernels (attn_dispatch, and the SIMT ones) keep a head's keys in shared memory and serve T <= 256; longer
+// sequences (ViT-L/14: T = 257) take the streaming kernels of vit_attn_stream.cuh.
+constexpr int kAttnResidentMaxT = 256;
+
 static int vit_attn_fwd(const bf16* qkv, bf16* out, int S, int T, int D, int heads, cudaStream_t st) {
+  if (T > kAttnResidentMaxT) {
+    APH_REQUIRE(!attn_simt(), "attention: APH_ATTN_SIMT=1 selects the SIMT kernels, which serve T <= %d (T=%d); unset it", kAttnResidentMaxT, T);
+    return attn_stream(true, qkv, nullptr, out, nullptr, S, T, D, heads, st);
+  }
   if (!attn_simt()) return attn_dispatch(true, qkv, nullptr, out, S, T, D, heads, st);
   k_attn_fwd<<<S * heads, 256, attn_fwd_smem(T), st>>>(qkv, out, T, D, heads);
   APH_LAUNCH_OK();
@@ -262,12 +273,12 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
   APH_REQUIRE(cfg->width % 128 == 0 && (cfg->width / 128 == 1 || cfg->width / 128 == 2 || cfg->width / 128 == 6 || cfg->width / 128 == 8),
               "aph_vit_create: width %d unsupported (128, 256, 768, 1024)", cfg->width);
   APH_REQUIRE(cfg->heads * 64 == cfg->width, "aph_vit_create: head dim must be 64 (width %d, heads %d)", cfg->width, cfg->heads);
-  APH_REQUIRE(cfg->res % cfg->patch == 0 && cfg->patch % 8 == 0, "aph_vit_create: res %d / patch %d", cfg->res, cfg->patch);
+  APH_REQUIRE(cfg->patch >= 2 && cfg->patch % 2 == 0 && cfg->res % cfg->patch == 0, "aph_vit_create: res %d / patch %d (the patch must be even)",
+              cfg->res, cfg->patch);
   APH_REQUIRE(cfg->out_dim % 128 == 0 && cfg->max_batch > 0 && cfg->layers > 0, "aph_vit_create: out_dim %d must be a multiple of 128", cfg->out_dim);
   VitImpl* v = new VitImpl();
   v->cfg = *cfg;
-  v->g = cfg->res / cfg->patch; v->T = v->g * v->g + 1; v->D = cfg->width; v->Kp = 3 * cfg->patch * cfg->patch;
-  APH_REQUIRE(v->T <= 256 && v->Kp % 128 == 0, "aph_vit_create: T=%d (max 256) Kp=%d", v->T, v->Kp);
+  v->g = cfg->res / cfg->patch; v->T = v->g * v->g + 1; v->D = cfg->width; v->Kp = patch_k(cfg->patch);
   const int D = v->D, T = v->T, S = cfg->max_batch, Ly = cfg->layers, O = cfg->out_dim;
   const size_t M = (size_t)S * T, Mp = (size_t)S * v->g * v->g;
   int e = 0;
@@ -291,11 +302,19 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
   e |= dev_alloc(v, &v->dx, M * D); e |= dev_alloc(v, &v->dx_bf, M * D); e |= dev_alloc(v, &v->dh, M * 4 * D);
   e |= dev_alloc(v, &v->d_ln, M * D); e |= dev_alloc(v, &v->d_attn, M * D); e |= dev_alloc(v, &v->d_attn_last, M * D);
   e |= dev_alloc(v, &v->d_qkv, M * 3 * D); e |= dev_alloc(v, &v->d_tok, Mp * D);
+  if (T > kAttnResidentMaxT) e |= dev_alloc(v, &v->attn_stats, M * cfg->heads);
   if (e) { aph_vit_destroy(reinterpret_cast<aph_vit*>(v)); return 1; }
   APH_CUDA_OK(cudaMemset(v->d_attn_last, 0, M * D * sizeof(bf16)));
+  if (v->Kp != 3 * cfg->patch * cfg->patch) {   // the zero padding of the patch operand and of conv1's packed weights
+    APH_CUDA_OK(cudaMemset(v->patches, 0, Mp * v->Kp * sizeof(bf16)));
+    APH_CUDA_OK(cudaMemset(v->w_conv, 0, (size_t)D * v->Kp * sizeof(bf16)));
+    APH_CUDA_OK(cudaMemset(v->w_conv_t, 0, (size_t)D * v->Kp * sizeof(bf16)));
+  }
   APH_CUDA_OK(cudaDeviceSynchronize());     // the zeros are in place before any caller stream (blocking or not) can read them
-  APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_fwd_smem(T)));
-  APH_CUDA_OK(cudaFuncSetAttribute(k_attn_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_bwd_smem(T)));
+  if (T <= kAttnResidentMaxT) {             // above that the SIMT kernels' shared memory does not fit (and they are not run)
+    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_fwd_smem(T)));
+    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_bwd_smem(T)));
+  }
   *out = reinterpret_cast<aph_vit*>(v);
   return 0;
 }
@@ -320,7 +339,11 @@ extern "C" int aph_vit_load_tensor(aph_vit* vit, const char* key, const float* d
   if (k.rfind("visual.", 0) == 0) k = k.substr(7);
   auto need = [&](int64_t n) -> int { APH_REQUIRE(numel == n, "aph_vit_load_tensor(%s): expected %lld elements, got %lld", key, (long long)n, (long long)numel); return 0; };
   int e = 0;
-  if (k == "conv1.weight") { if ((e = need((int64_t)D * v->Kp))) return e; e = pack(data, v->w_conv, D, v->Kp, 0, st) | pack(data, v->w_conv_t, D, v->Kp, 1, st); }
+  if (k == "conv1.weight") {   // [D, 3, p, p] = [D, 3 p^2] into the first 3 p^2 columns (rows of the transpose) of [D, Kp] / [Kp, D]
+    const int P3 = 3 * v->cfg.patch * v->cfg.patch;
+    if ((e = need((int64_t)D * P3))) return e;
+    e = pack(data, v->w_conv, D, P3, 0, st, v->Kp) | pack(data, v->w_conv_t, D, P3, 1, st);
+  }
   else if (k == "class_embedding") { if ((e = need(D))) return e; e = copy_f32(data, v->cls, D, st); }
   else if (k == "positional_embedding") { if ((e = need((int64_t)v->T * D))) return e; e = copy_f32(data, v->pos, (size_t)v->T * D, st); }
   else if (k == "ln_pre.weight") { if ((e = need(D))) return e; e = copy_f32(data, v->lnpre_w, D, st); }
@@ -400,8 +423,14 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, int side, floa
   // torch.cuda.empty_cache() per step) still replays it.
   if (images) {
     const int g = v->g, Mp = S * g * g;
-    const size_t n8 = (size_t)Mp * v->Kp / 8;
-    APH_CUDA_OK(launch_k(k_patchify, dim3((unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1, images, v->patches, S, v->cfg.patch, g, side));
+    const int p = v->cfg.patch;
+    if (v->Kp == 3 * p * p) {                // rows without padding (p = 16, 32): 8 columns per thread
+      const size_t n8 = (size_t)Mp * v->Kp / 8;
+      APH_CUDA_OK(launch_k(k_patchify<false>, dim3((unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1, images, v->patches, S, p, g, side));
+    } else {                                 // padded rows (p = 14): pixel pairs
+      const size_t n2 = (size_t)Mp * 3 * p * p / 2;
+      APH_CUDA_OK(launch_k(k_patchify<true>, dim3((unsigned)std::min<size_t>((n2 + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1, images, v->patches, S, p, g, side));
+    }
     APH_LAUNCH_OK();
   }
   const int rc = run_cached(v->fwd_graphs, v->warm_fwd, v->stamp, v->graph_misses, nullptr, nullptr, S, save_for_bwd, st, [&]() -> int {
@@ -487,7 +516,10 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
     // attention branch: d_attn = dx . W_o; (dq,dk,dv) = attn'(...); d_ln1 = d_qkv . W_qkv
     { GemmEpi ep; ep.out_bf16 = d_attn; ep.ld_out = last ? T * D : 0;
       if ((e = launch_gemm(gx_bf, w.w_o_t, GemmShape{Mr, D, D}, ep, st))) return e; }
-    if (attn_simt()) { k_attn_bwd<<<S * H, 256, attn_bwd_smem(T), st>>>(v->qkv[l], d_attn, v->d_qkv, T, D, H); APH_LAUNCH_OK(); }
+    if (T > kAttnResidentMaxT) {
+      APH_REQUIRE(!attn_simt(), "attention: APH_ATTN_SIMT=1 selects the SIMT kernels, which serve T <= %d (T=%d); unset it", kAttnResidentMaxT, T);
+      if ((e = attn_stream(false, v->qkv[l], d_attn, v->d_qkv, v->attn_stats, S, T, D, H, st))) return e;
+    } else if (attn_simt()) { k_attn_bwd<<<S * H, 256, attn_bwd_smem(T), st>>>(v->qkv[l], d_attn, v->d_qkv, T, D, H); APH_LAUNCH_OK(); }
     else if ((e = attn_dispatch(false, v->qkv[l], d_attn, v->d_qkv, S, T, D, H, st))) return e;
     { GemmEpi ep; ep.out_bf16 = v->d_ln;
       if ((e = launch_gemm(v->d_qkv, w.w_qkv_t, GemmShape{M, D, 3 * D}, ep, st))) return e; }
@@ -525,7 +557,9 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
 namespace aph { int attn_causal_test(const bf16* qkv, bf16* out, int S, int T, int D, int heads, cudaStream_t st); }   // text.cu
 
 // Test entries (tests/test_encoder_kernels_gpu.py): the encoder's attention and LayerNorm kernels on caller-supplied operands,
-// dispatched exactly as the encoder (and, for causal attention, the text tower) dispatches them.
+// dispatched exactly as the encoder (and, for causal attention, the text tower) dispatches them. aph_attn_test covers the
+// resident kernels (T <= 256, the image tower's dispatch below the streaming kernels); aph_attn_long_test covers the streaming
+// kernels the encoder runs for T > 256, at any T >= 1.
 extern "C" int aph_attn_test(int fwd, int causal, const void* qkv, const void* dout, void* out, int S, int T, int D, int heads, void* stream) {
   APH_REQUIRE(qkv && out && (fwd || dout), "aph_attn_test: null argument");
   APH_REQUIRE(S > 0 && T > 0 && heads > 0 && D == 64 * heads, "aph_attn_test: S=%d T=%d D=%d heads=%d (head dim must be 64)", S, T, D, heads);
@@ -536,6 +570,19 @@ extern "C" int aph_attn_test(int fwd, int causal, const void* qkv, const void* d
     return attn_causal_test(q, reinterpret_cast<bf16*>(out), S, T, D, heads, st);
   }
   return attn_dispatch(fwd != 0, q, reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(out), S, T, D, heads, st);
+}
+
+extern "C" int aph_attn_long_test(int fwd, const void* qkv, const void* dout, void* out, int S, int T, int D, int heads, void* stream) {
+  APH_REQUIRE(qkv && out && (fwd || dout), "aph_attn_long_test: null argument");
+  APH_REQUIRE(S > 0 && T > 0 && heads > 0 && D == 64 * heads, "aph_attn_long_test: S=%d T=%d D=%d heads=%d (head dim must be 64)", S, T, D, heads);
+  cudaStream_t st = (cudaStream_t)stream;
+  const bf16* q = reinterpret_cast<const bf16*>(qkv);
+  if (fwd) return attn_stream(true, q, nullptr, reinterpret_cast<bf16*>(out), nullptr, S, T, D, heads, st);
+  float2* stats = nullptr;                   // stream-ordered scratch: freed behind the two backward launches
+  APH_CUDA_OK(cudaMallocAsync(&stats, (size_t)S * heads * T * sizeof(float2), st));
+  const int rc = attn_stream(false, q, reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(out), stats, S, T, D, heads, st);
+  APH_CUDA_OK(cudaFreeAsync(stats, st));
+  return rc;
 }
 
 extern "C" int aph_ln_fwd_test(const float* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows, int D,

@@ -22,10 +22,28 @@ namespace aph {
   }
 
 // ---------------------------------------------------------------------------------------------
-// images fp32 [S,3,side,side] -> patches bf16 [S*g*g, 3*p*p], col = c*p*p + py*p + px  (conv1 weight layout); side >= R = p*g:
-// conv1 reads the top-left R x R window
+// images fp32 [S,3,side,side] -> patches bf16 [S*g*g, patch_k(p)], col = c*p*p + py*p + px  (conv1 weight layout); side >= R = p*g:
+// conv1 reads the top-left R x R window. The columns >= 3 p^2 of a row are padding (zeroed at create) and never written here.
+// PAIRS = false (p % 16 == 0, rows without padding): 8 columns per thread. PAIRS = true (any even p, e.g. 14): 2 columns per
+// thread, so that neither a patch-row boundary nor the end of the 3 p^2 columns falls inside one thread's vector.
+template <bool PAIRS>
 static __global__ void __launch_bounds__(256) k_patchify(const float* __restrict__ img, bf16* __restrict__ out, int S, int p, int g, int side) {
   pdl_trigger(); pdl_wait();
+  if (PAIRS) {
+    const int R = side, P3 = 3 * p * p, Kp = patch_k(p);
+    const size_t total = (size_t)S * g * g * P3 / 2;
+    for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
+      const size_t e = idx * 2;
+      const int row = (int)(e / P3), col = (int)(e - (size_t)row * P3);
+      const int s = row / (g * g), pr = row - s * g * g, gy = pr / g, gx = pr - gy * g;
+      const int c = col / (p * p), rem = col - c * p * p, py = rem / p, px = rem - py * p;
+      const float* src = img + (((size_t)s * 3 + c) * R + gy * p + py) * R + gx * p + px;
+      // px and p are even: with an even side the pair is 8-byte aligned
+      const float2 a = (R & 1) == 0 ? __ldg(reinterpret_cast<const float2*>(src)) : make_float2(__ldg(src), __ldg(src + 1));
+      *reinterpret_cast<__nv_bfloat162*>(out + (size_t)row * Kp + col) = __floats2bfloat162_rn(a.x, a.y);
+    }
+    return;
+  }
   const int R = side, Kp = 3 * p * p;
   const size_t total = (size_t)S * g * g * Kp / 8;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {

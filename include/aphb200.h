@@ -169,17 +169,17 @@ int aph_rng_crop_tables(uint8_t* torch_state, int64_t torch_state_bytes, uint32_
                         int H, int W, int frame_h, int frame_w, int size, int kind, float macro, int n_imgs,
                         float* tables);
 
-/* ================= L1: CLIP ViT-B image encoder ===============================================
+/* ================= L1: CLIP ViT image encoder (B/32, B/16, L/14) ==================================
  * Replaces clip.model.CLIP.encode_image / VisionTransformer.forward (third-party OpenAI clip; call
  * sites clip_fft.py:216,254,276) and its autograd data-gradient. Weights are frozen: no weight
  * gradients are computed (the reference computes and discards them, clip_fft.py:293-295).           */
 typedef struct aph_vit aph_vit;
 typedef struct {
-  int32_t patch;      /* 32 or 16                                   */
-  int32_t width;      /* 768                                        */
-  int32_t layers;     /* 12                                         */
-  int32_t heads;      /* 12 (head dim must be 64)                   */
-  int32_t out_dim;    /* 512                                        */
+  int32_t patch;      /* 32, 16 or 14 (any even patch)              */
+  int32_t width;      /* 768 (1024 for ViT-L/14; also 128, 256)     */
+  int32_t layers;     /* 12 (24)                                    */
+  int32_t heads;      /* 12 (16) (head dim must be 64)              */
+  int32_t out_dim;    /* 512 (768)                                  */
   int32_t res;        /* input resolution, 224                      */
   int32_t max_batch;  /* largest S a call will pass                 */
   int32_t reserved;
@@ -195,8 +195,10 @@ int aph_vit_finalize(aph_vit* vit);
 int aph_vit_fwd(aph_vit* vit, const float* images, int S, float* emb, int save_for_bwd, void* stream);
 /* Patch operand hand-over (SURVEY 2.4 k10-k12: the sampler emits the patch-major bf16 A operand of conv1, replacing the
  * fp32 round trip x.type(dtype) -> conv1's im2col of the reference's clip/model.py VisionTransformer.forward):
- * aph_vit_patch_operand returns the handle's operand buffer [S*grid*grid, 3*patch*patch] bf16 (row = s*grid*grid + gy*grid + gx,
- * col = c*patch*patch + py*patch + px) for aph_sample_fwd_patches to fill; aph_vit_fwd_prepatched then runs the forward on it.  */
+ * aph_vit_patch_operand returns the handle's operand buffer [S*grid*grid, patch_k(patch)] bf16 (row = s*grid*grid + gy*grid + gx,
+ * col = c*patch*patch + py*patch + px) for aph_sample_fwd_patches to fill; aph_vit_fwd_prepatched then runs the forward on it.
+ * The row stride patch_k(p) is 3*p*p rounded up to a multiple of 128 (3072 for p = 32, 768 for p = 16, 640 for p = 14); the
+ * columns from 3*p*p on are zero, set once at create and written by no one.                                                   */
 int aph_vit_patch_operand(aph_vit* vit, int S, void** patches_bf16, int* patch, int* grid);
 int aph_vit_fwd_prepatched(aph_vit* vit, int S, float* emb, int save_for_bwd, void* stream);
 /* grad_emb [S,out_dim] -> grad_images [S,3,res,res] (overwritten). Uses activations of the last
@@ -264,11 +266,14 @@ int64_t aph_gemm_variant_launches(int variant, int epi);
  * fwd = 1: out bf16 [S*T, D]; fwd = 0: dout bf16 [S*T, D] in, out = dqkv bf16 [S*T, 3*D]. causal = 0 runs the image
  * tower's dispatch (T <= 256), causal = 1 the text tower's causal forward (T <= 112; there is no causal backward).
  * Unsupported shapes return an error and launch nothing.
+ * aph_attn_long_test: the streaming attention kernels the image tower runs for T > 256 (ViT-L/14: T = 257), on the same
+ * operands as aph_attn_test with causal = 0, for any T >= 1.
  * aph_ln_fwd_test: k_ln_fwd on x fp32 [rows, D] (row stride D) -> y bf16 [rows, D], mean / rstd fp32 [rows].
  * aph_ln_bwd_test: k_ln_bwd with dy fp32 (dy_bf16 = 0) or bf16 (dy_bf16 = 1) [rows, D]; mode 0: dx (+)= LN'(dy) (fp32 dx and
  * bf16 dx_bf16, accumulate = 1 adds to dx); mode 1: dx = LN'(dy) + dcls[s] on rows s*T (dcls fp32 [rows/T, D]); mode 2:
  * the non-class rows into dx_bf16 = dtok bf16 [rows/T*(T-1), D], dx unused. D in {128, 256, 512, 768, 1024}.            */
 int aph_attn_test(int fwd, int causal, const void* qkv, const void* dout, void* out, int S, int T, int D, int heads, void* stream);
+int aph_attn_long_test(int fwd, const void* qkv, const void* dout, void* out, int S, int T, int D, int heads, void* stream);
 int aph_ln_fwd_test(const float* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows, int D,
                     void* stream);
 int aph_ln_bwd_test(const void* dy, int dy_bf16, const float* x, const float* mean, const float* rstd, const float* gamma, float* dx,
