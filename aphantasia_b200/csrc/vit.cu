@@ -240,26 +240,18 @@ int block_fwd(const BlockW& w, const BlockIO& io, int S, int T, int Mr, int ld_t
   return 0;
 }
 
-// APH_ATTN_SIMT=1 selects the fp32 SIMT attention kernels (debug / comparison); default = tensor-core kernels.
-static bool attn_simt() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("APH_ATTN_SIMT"); v = (e && e[0] == '1') ? 1 : 0; }
-  return v == 1;
-}
-
-// The resident kernels (attn_dispatch, and the SIMT ones) keep a head's keys in shared memory and serve T <= 256; longer
-// sequences (ViT-L/14: T = 257) take the streaming kernels of vit_attn_stream.cuh.
+// The resident kernels (attn_dispatch) keep a head's keys in shared memory and serve T <= 256; longer sequences
+// (ViT-L/14: T = 257) take the streaming kernels of vit_attn_stream.cuh, whose backward needs `stats` (attn_stats).
 constexpr int kAttnResidentMaxT = 256;
 
+static int vit_attn(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_or_dqkv, float2* stats, int S, int T, int D, int heads,
+                    cudaStream_t st) {
+  if (T > kAttnResidentMaxT) return attn_stream(fwd, qkv, dout, out_or_dqkv, stats, S, T, D, heads, st);
+  return attn_dispatch(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
+}
+
 static int vit_attn_fwd(const bf16* qkv, bf16* out, int S, int T, int D, int heads, cudaStream_t st) {
-  if (T > kAttnResidentMaxT) {
-    APH_REQUIRE(!attn_simt(), "attention: APH_ATTN_SIMT=1 selects the SIMT kernels, which serve T <= %d (T=%d); unset it", kAttnResidentMaxT, T);
-    return attn_stream(true, qkv, nullptr, out, nullptr, S, T, D, heads, st);
-  }
-  if (!attn_simt()) return attn_dispatch(true, qkv, nullptr, out, S, T, D, heads, st);
-  k_attn_fwd<<<S * heads, 256, attn_fwd_smem(T), st>>>(qkv, out, T, D, heads);
-  APH_LAUNCH_OK();
-  return 0;
+  return vit_attn(true, qkv, nullptr, out, nullptr, S, T, D, heads, st);
 }
 
 static Scratch g_win;   // aph_vit_bwd_sized: the R x R window gradient before k_window_expand
@@ -311,10 +303,6 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
     APH_CUDA_OK(cudaMemset(v->w_conv_t, 0, (size_t)D * v->Kp * sizeof(bf16)));
   }
   APH_CUDA_OK(cudaDeviceSynchronize());     // the zeros are in place before any caller stream (blocking or not) can read them
-  if (T <= kAttnResidentMaxT) {             // above that the SIMT kernels' shared memory does not fit (and they are not run)
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_fwd_smem(T)));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_bwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_bwd_smem(T)));
-  }
   *out = reinterpret_cast<aph_vit*>(v);
   return 0;
 }
@@ -516,11 +504,7 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
     // attention branch: d_attn = dx . W_o; (dq,dk,dv) = attn'(...); d_ln1 = d_qkv . W_qkv
     { GemmEpi ep; ep.out_bf16 = d_attn; ep.ld_out = last ? T * D : 0;
       if ((e = launch_gemm(gx_bf, w.w_o_t, GemmShape{Mr, D, D}, ep, st))) return e; }
-    if (T > kAttnResidentMaxT) {
-      APH_REQUIRE(!attn_simt(), "attention: APH_ATTN_SIMT=1 selects the SIMT kernels, which serve T <= %d (T=%d); unset it", kAttnResidentMaxT, T);
-      if ((e = attn_stream(false, v->qkv[l], d_attn, v->d_qkv, v->attn_stats, S, T, D, H, st))) return e;
-    } else if (attn_simt()) { k_attn_bwd<<<S * H, 256, attn_bwd_smem(T), st>>>(v->qkv[l], d_attn, v->d_qkv, T, D, H); APH_LAUNCH_OK(); }
-    else if ((e = attn_dispatch(false, v->qkv[l], d_attn, v->d_qkv, S, T, D, H, st))) return e;
+    if ((e = vit_attn(false, v->qkv[l], d_attn, v->d_qkv, v->attn_stats, S, T, D, H, st))) return e;
     { GemmEpi ep; ep.out_bf16 = v->d_ln;
       if ((e = launch_gemm(v->d_qkv, w.w_qkv_t, GemmShape{M, D, 3 * D}, ep, st))) return e; }
     // ln_1: back to all M rows; in the last block dx is written here for the first time (+ dxc on the cls rows)

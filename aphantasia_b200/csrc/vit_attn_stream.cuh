@@ -26,19 +26,6 @@ constexpr size_t kStreamFwdSmem = (size_t)3 * kStreamRows * 128;  // Q, K, V til
 constexpr size_t kStreamBwdSmem = (size_t)4 * kStreamRows * 128 + kStreamRows * sizeof(float2);   // 2 own + 2 streamed tiles, stats
 static_assert(kStreamFwdSmem <= 48 * 1024 && kStreamBwdSmem <= 48 * 1024, "streaming attention: static shared memory above 48 KB");
 
-// masks and scales the 16 x 16 logit tile (c0: keys key0 + 2t, +1; c1: key0 + 8 + 2t, +1) of one warp; returns nothing, updates
-// the row maxima mx0 (row g) and mx1 (row g + 8)
-__device__ __forceinline__ void stream_mask_scale(float (&c0)[4], float (&c1)[4], int key0, int T, int t, float& mx0, float& mx1) {
-#pragma unroll
-  for (int u = 0; u < 2; ++u) {
-    float* cc = u ? c1 : c0;
-    const int col = key0 + u * 8 + 2 * t;
-    cc[0] = (col < T) ? cc[0] * kAttnScaleLog2 : -INFINITY; cc[1] = (col + 1 < T) ? cc[1] * kAttnScaleLog2 : -INFINITY;
-    cc[2] = (col < T) ? cc[2] * kAttnScaleLog2 : -INFINITY; cc[3] = (col + 1 < T) ? cc[3] * kAttnScaleLog2 : -INFINITY;
-    mx0 = fmaxf(mx0, fmaxf(cc[0], cc[1])); mx1 = fmaxf(mx1, fmaxf(cc[2], cc[3]));
-  }
-}
-
 __global__ void __launch_bounds__(128) k_attn_fwd_stream(const bf16* __restrict__ qkv, bf16* __restrict__ out, int T, int D, int heads) {
   pdl_trigger(); pdl_wait();
   __shared__ __align__(128) uint8_t sm[kStreamFwdSmem];
@@ -55,8 +42,7 @@ __global__ void __launch_bounds__(128) k_attn_fwd_stream(const bf16* __restrict_
   load_tile64(Qs, base + (size_t)q0 * ld, ld, kStreamRows, T - q0, 128);
   uint32_t qa[4][4];
   float o[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) { o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f; }
+  zero_acc(o);
   float m0 = -INFINITY, m1 = -INFINITY, l0 = 0.f, l1 = 0.f;       // l: this lane's share of the row sums
   for (int k0 = 0; k0 < T; k0 += kStreamRows) {
     if (k0 > 0) __syncthreads();                                   // the previous K / V tile is consumed
@@ -70,7 +56,7 @@ __global__ void __launch_bounds__(128) k_attn_fwd_stream(const bf16* __restrict_
 #pragma unroll
     for (int n2 = 0; n2 < 4; ++n2) {
       qk_tile(c[2 * n2], c[2 * n2 + 1], qa, ks_a, n2 * 16, lane);
-      stream_mask_scale(c[2 * n2], c[2 * n2 + 1], k0 + n2 * 16, T, t, mx0, mx1);
+      mask_scale(c[2 * n2], c[2 * n2 + 1], k0 + n2 * 16, T, t, mx0, mx1);
     }
     // key k0 < T is in every tile, so the new maxima are finite; on the first tile m = -inf and the rescale factor is 0
     const float mn0 = fmaxf(m0, quad_max(mx0)), mn1 = fmaxf(m1, quad_max(mx1));
@@ -79,27 +65,12 @@ __global__ void __launch_bounds__(128) k_attn_fwd_stream(const bf16* __restrict_
     l0 *= a0; l1 *= a1;
 #pragma unroll
     for (int i = 0; i < 8; ++i) { o[i][0] *= a0; o[i][1] *= a0; o[i][2] *= a1; o[i][3] *= a1; }
-#pragma unroll
-    for (int n = 0; n < 8; ++n) {
-      c[n][0] = exp2f(c[n][0] - m0); c[n][1] = exp2f(c[n][1] - m0); c[n][2] = exp2f(c[n][2] - m1); c[n][3] = exp2f(c[n][3] - m1);
-      l0 += c[n][0] + c[n][1]; l1 += c[n][2] + c[n][3];
-    }
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) {
-      const uint32_t pa[4] = {pack2(c[2 * kk][0], c[2 * kk][1]), pack2(c[2 * kk][2], c[2 * kk][3]),
-                              pack2(c[2 * kk + 1][0], c[2 * kk + 1][1]), pack2(c[2 * kk + 1][2], c[2 * kk + 1][3])};
-      av_step(o, pa, vs_a, kk * 16, lane);
-    }
+    exp_rowsum(c, m0, m1, l0, l1);
+    pv_acc<4>(o, c, vs_a, lane);
   }
   if (!live) return;
   const float i0 = 1.f / quad_sum(l0), i1 = 1.f / quad_sum(l1);
-  const int row0 = q0 + r0 + g, row1 = row0 + 8;
-#pragma unroll
-  for (int dt = 0; dt < 8; ++dt) {
-    const int col = h * 64 + dt * 8 + 2 * t;
-    if (row0 < T) *reinterpret_cast<__nv_bfloat162*>(out + ((size_t)s * T + row0) * D + col) = __floats2bfloat162_rn(o[dt][0] * i0, o[dt][1] * i0);
-    if (row1 < T) *reinterpret_cast<__nv_bfloat162*>(out + ((size_t)s * T + row1) * D + col) = __floats2bfloat162_rn(o[dt][2] * i1, o[dt][3] * i1);
-  }
+  store_frag(out, (size_t)s * T, D, h * 64, o, q0 + r0 + g, T, t, i0, i1);
 }
 
 // dQ and the row statistics of one query block. stats: float2 [S*heads, T] = (lse, delta) per query row (log2 domain).
@@ -135,7 +106,7 @@ __global__ void __launch_bounds__(128) k_attn_bwd_stream_q(const bf16* __restric
     for (int n2 = 0; n2 < 4; ++n2) {
       qk_tile(c[2 * n2], c[2 * n2 + 1], qa, ks_a, n2 * 16, lane);
       qk_tile(e[2 * n2], e[2 * n2 + 1], ga, vs_a, n2 * 16, lane);
-      stream_mask_scale(c[2 * n2], c[2 * n2 + 1], k0 + n2 * 16, T, t, mx0, mx1);
+      mask_scale(c[2 * n2], c[2 * n2 + 1], k0 + n2 * 16, T, t, mx0, mx1);
     }
     const float mn0 = fmaxf(m0, quad_max(mx0)), mn1 = fmaxf(m1, quad_max(mx1));
     const float a0 = exp2f(m0 - mn0), a1 = exp2f(m1 - mn1);
@@ -159,8 +130,7 @@ __global__ void __launch_bounds__(128) k_attn_bwd_stream_q(const bf16* __restric
   }
   // ---- pass 2: P, dS (scaled by 1/8) and dQ = dS K
   float dq[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) { dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f; }
+  zero_acc(dq);
   for (int k0 = 0; k0 < T; k0 += kStreamRows) {
     __syncthreads();
     load_tile64(Ks, base + D + (size_t)k0 * ld, ld, kStreamRows, T - k0, 128);
@@ -186,13 +156,7 @@ __global__ void __launch_bounds__(128) k_attn_bwd_stream_q(const bf16* __restric
     }
   }
   if (!live) return;
-  bf16* obase = dqkv + (size_t)s * T * ld + h * 64;
-#pragma unroll
-  for (int dt = 0; dt < 8; ++dt) {
-    const int col = dt * 8 + 2 * t;
-    if (row0 < T) *reinterpret_cast<__nv_bfloat162*>(obase + (size_t)row0 * ld + col) = __floats2bfloat162_rn(dq[dt][0], dq[dt][1]);
-    if (row1 < T) *reinterpret_cast<__nv_bfloat162*>(obase + (size_t)row1 * ld + col) = __floats2bfloat162_rn(dq[dt][2], dq[dt][3]);
-  }
+  store_frag(dqkv + (size_t)s * T * ld + h * 64, 0, ld, 0, dq, row0, T, t);
 }
 
 // dK and dV of one key block, from the statistics k_attn_bwd_stream_q saved. Each warp owns 16 keys as the rows of its MMAs:
@@ -218,8 +182,7 @@ __global__ void __launch_bounds__(128) k_attn_bwd_stream_kv(const bf16* __restri
   load_tile64(Vs, base + 2 * D + (size_t)k0 * ld, ld, kStreamRows, T - k0, 128);
   uint32_t ka[4][4], va[4][4];
   float dk[8][4], dv[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) { dk[i][0] = dk[i][1] = dk[i][2] = dk[i][3] = 0.f; dv[i][0] = dv[i][1] = dv[i][2] = dv[i][3] = 0.f; }
+  zero_acc(dk); zero_acc(dv);
   for (int q0 = 0; q0 < T; q0 += kStreamRows) {
     if (q0 > 0) __syncthreads();
     load_tile64(Qs, base + (size_t)q0 * ld, ld, kStreamRows, T - q0, 128);

@@ -1,8 +1,12 @@
 // vit_attn_tc.cuh -- tensor-core attention core of the CLIP ViT (head dim 64, T <= 256), forward and backward.
 //
-// softmax(Q K^T / 8) V per (sample, head); one CTA per (sample, head). The sequence is tiny (T = 50 for
-// ViT-B/32, 197 for ViT-B/16), so K and V of a head stay resident in shared memory and the whole problem is a
-// handful of 16x8x16 bf16 MMAs per warp (mma.sync, fp32 accumulate); softmax statistics live in registers.
+// softmax(Q K^T / 8) V per (sample, head). One kernel family per sequence length, chosen from T:
+//   T <= 32, <= 64    k_attn_fwd_tc1<2/4>, k_attn_bwd_tc1<2/4>        persistent CTAs, TMA double buffer (this file)
+//   T <= 112, 208, 256 k_attn_fwd_tc<8, 7/13/16>, k_attn_bwd_tc<8, ..> one CTA per (sample, head) (this file)
+//   T > 256           k_attn_fwd_stream, k_attn_bwd_stream_q + _kv     K / V streamed in 64-key tiles (vit_attn_stream.cuh)
+// The text tower runs k_attn_fwd_tc<4/8, 2/4/7, CAUSAL = true> (text.cu). The sequence is tiny (T = 50 for ViT-B/32, 197
+// for ViT-B/16), so here K and V of a head stay resident in shared memory and the whole problem is a handful of 16x8x16
+// bf16 MMAs per warp (mma.sync, fp32 accumulate); softmax statistics live in registers.
 //   forward : S = Q K^T -> softmax (exp2, fp32) -> O = P V                       (P never leaves registers)
 //   backward: 3 register-light passes per query block recompute S / P / dP = dO V^T tile by tile
 //             (row max+sum, then delta = rowsum(P o dP), then dS = P o (dP - delta)): dQ = dS K from registers;
@@ -12,7 +16,6 @@
 // bank-conflict free. qkv is bf16 [S*T, 3*D] (q | k | v), out / dout bf16 [S*T, D], dqkv bf16 [S*T, 3*D].
 #pragma once
 #include "tc_gemm.cuh"
-#include <stdlib.h>
 
 namespace aph {
 
@@ -79,6 +82,79 @@ __device__ __forceinline__ void av_step(float (&acc)[8][4], const uint32_t (&a)[
   }
 }
 
+__device__ __forceinline__ void zero_acc(float (&acc)[8][4]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) { acc[i][0] = acc[i][1] = acc[i][2] = acc[i][3] = 0.f; }
+}
+
+// masks and scales the 16 x 16 logit tile (c0: keys key0 + 2t, +1; c1: key0 + 8 + 2t, +1) of one warp and updates the row
+// maxima mx0 (row g) and mx1 (row g + 8). Keys >= T become -inf; so do, under CAUSAL, keys after the lane's query rows qrow
+// (cc[0], cc[1]) and qrow + 8 (cc[2], cc[3]), where key 0 always survives.
+template <bool CAUSAL = false>
+__device__ __forceinline__ void mask_scale(float (&c0)[4], float (&c1)[4], int key0, int T, int t, float& mx0, float& mx1, int qrow = 0) {
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    float* cc = u ? c1 : c0;
+    const int col = key0 + u * 8 + 2 * t;
+    const int qa0 = qrow, qa1 = qa0 + 8;
+    cc[0] = (col < T && (!CAUSAL || col <= qa0)) ? cc[0] * kAttnScaleLog2 : -INFINITY;
+    cc[1] = (col + 1 < T && (!CAUSAL || col + 1 <= qa0)) ? cc[1] * kAttnScaleLog2 : -INFINITY;
+    cc[2] = (col < T && (!CAUSAL || col <= qa1)) ? cc[2] * kAttnScaleLog2 : -INFINITY;
+    cc[3] = (col + 1 < T && (!CAUSAL || col + 1 <= qa1)) ? cc[3] * kAttnScaleLog2 : -INFINITY;
+    mx0 = fmaxf(mx0, fmaxf(cc[0], cc[1])); mx1 = fmaxf(mx1, fmaxf(cc[2], cc[3]));
+  }
+}
+
+// c = exp2(c - m) in place (m0 for row g, m1 for row g + 8); adds this lane's share of the row sums to l0, l1
+template <int N>
+__device__ __forceinline__ void exp_rowsum(float (&c)[N][4], float m0, float m1, float& l0, float& l1) {
+#pragma unroll
+  for (int n = 0; n < N; ++n) {
+    c[n][0] = exp2f(c[n][0] - m0); c[n][1] = exp2f(c[n][1] - m0); c[n][2] = exp2f(c[n][2] - m1); c[n][3] = exp2f(c[n][3] - m1);
+    l0 += c[n][0] + c[n][1]; l1 += c[n][2] + c[n][3];
+  }
+}
+
+// o += P V for the NT2 16-key tiles of P (fp32 registers, packed to bf16 here) and the V tile at vs_a
+template <int NT2>
+__device__ __forceinline__ void pv_acc(float (&o)[8][4], const float (&c)[2 * NT2][4], uint32_t vs_a, int lane) {
+#pragma unroll
+  for (int kk = 0; kk < NT2; ++kk) {
+    const uint32_t pa[4] = {pack2(c[2 * kk][0], c[2 * kk][1]), pack2(c[2 * kk][2], c[2 * kk][3]),
+                            pack2(c[2 * kk + 1][0], c[2 * kk + 1][1]), pack2(c[2 * kk + 1][2], c[2 * kk + 1][3])};
+    av_step(o, pa, vs_a, kk * 16, lane);
+  }
+}
+
+// Phase B of the resident backwards, key tile kt: dV += P^T dO and dK += dS^T Q over the QB query rows of the parked P / dS
+// tiles (pitch PB), read transposed
+template <int QB>
+__device__ __forceinline__ void key_tile_acc(float (&dv)[8][4], float (&dk)[8][4], uint32_t ps_a, uint32_t ds_a, uint32_t gs_a, uint32_t qs_a,
+                                             int kt, int PB, int lane) {
+#pragma unroll
+  for (int ks = 0; ks < QB / 16; ++ks) {
+    uint32_t pa[4], da[4];
+    const int srow = ks * 16 + (lane & 7) + ((lane >> 4) << 3), chunk = kt * 2 + ((lane >> 3) & 1);
+    ldsm4t(pa, ps_a + swz(srow, chunk, PB));
+    ldsm4t(da, ds_a + swz(srow, chunk, PB));
+    av_step(dv, pa, gs_a, ks * 16, lane);
+    av_step(dk, da, qs_a, ks * 16, lane);
+  }
+}
+
+// Stores one warp's 16 x 64 fp32 fragment as bf16: fragment row g, scaled by s0, to row `row` and row g + 8, scaled by s1, to
+// row + 8, at dst + (rb + row) * ld + c0 + column; rows >= T are skipped
+__device__ __forceinline__ void store_frag(bf16* dst, size_t rb, size_t ld, int c0, const float (&a)[8][4], int row, int T, int t,
+                                           float s0 = 1.f, float s1 = 1.f) {
+  const int row0 = row, row1 = row0 + 8;
+#pragma unroll
+  for (int dt = 0; dt < 8; ++dt) {
+    const int col = c0 + dt * 8 + 2 * t;
+    if (row0 < T) *reinterpret_cast<__nv_bfloat162*>(dst + (rb + row0) * ld + col) = __floats2bfloat162_rn(a[dt][0] * s0, a[dt][1] * s0);
+    if (row1 < T) *reinterpret_cast<__nv_bfloat162*>(dst + (rb + row1) * ld + col) = __floats2bfloat162_rn(a[dt][2] * s1, a[dt][3] * s1);
+  }
+}
+
 // ---------------------------------------------------------------------------------------------
 // CAUSAL (the CLIP text tower): query row i attends to keys j <= i only; forward only.
 template <int NW, int NT2, bool CAUSAL = false>
@@ -110,51 +186,25 @@ __global__ void __launch_bounds__(NW * 32) k_attn_fwd_tc(const bf16* __restrict_
 #pragma unroll
     for (int n2 = 0; n2 < NT2; ++n2) {
       qk_tile(c[2 * n2], c[2 * n2 + 1], qa, ks_a, n2 * 16, lane);
-#pragma unroll
-      for (int u = 0; u < 2; ++u) {
-        const int col = n2 * 16 + u * 8 + 2 * t;
-        float* cc = c[2 * n2 + u];
-        // causal: this lane's query rows are q0 + r0 + g (cc[0], cc[1]) and that + 8 (cc[2], cc[3]); key 0 always survives
-        const int qa0 = q0 + r0 + g, qa1 = qa0 + 8;
-        cc[0] = (col < T && (!CAUSAL || col <= qa0)) ? cc[0] * kAttnScaleLog2 : -INFINITY;
-        cc[1] = (col + 1 < T && (!CAUSAL || col + 1 <= qa0)) ? cc[1] * kAttnScaleLog2 : -INFINITY;
-        cc[2] = (col < T && (!CAUSAL || col <= qa1)) ? cc[2] * kAttnScaleLog2 : -INFINITY;
-        cc[3] = (col + 1 < T && (!CAUSAL || col + 1 <= qa1)) ? cc[3] * kAttnScaleLog2 : -INFINITY;
-        m0 = fmaxf(m0, fmaxf(cc[0], cc[1])); m1 = fmaxf(m1, fmaxf(cc[2], cc[3]));
-      }
+      mask_scale<CAUSAL>(c[2 * n2], c[2 * n2 + 1], n2 * 16, T, t, m0, m1, q0 + r0 + g);
     }
     m0 = quad_max(m0); m1 = quad_max(m1);
     float l0 = 0.f, l1 = 0.f;
-#pragma unroll
-    for (int n = 0; n < 2 * NT2; ++n) {
-      c[n][0] = exp2f(c[n][0] - m0); c[n][1] = exp2f(c[n][1] - m0); c[n][2] = exp2f(c[n][2] - m1); c[n][3] = exp2f(c[n][3] - m1);
-      l0 += c[n][0] + c[n][1]; l1 += c[n][2] + c[n][3];
-    }
+    exp_rowsum(c, m0, m1, l0, l1);
     l0 = quad_sum(l0); l1 = quad_sum(l1);
     float o[8][4];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) { o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f; }
-#pragma unroll
-    for (int kk = 0; kk < NT2; ++kk) {
-      uint32_t pa[4] = {pack2(c[2 * kk][0], c[2 * kk][1]), pack2(c[2 * kk][2], c[2 * kk][3]),
-                        pack2(c[2 * kk + 1][0], c[2 * kk + 1][1]), pack2(c[2 * kk + 1][2], c[2 * kk + 1][3])};
-      av_step(o, pa, vs_a, kk * 16, lane);
-    }
+    zero_acc(o);
+    pv_acc<NT2>(o, c, vs_a, lane);
     const float i0 = 1.f / l0, i1 = 1.f / l1;
-    const int row0 = q0 + r0 + g, row1 = row0 + 8;
-#pragma unroll
-    for (int dt = 0; dt < 8; ++dt) {
-      const int col = h * 64 + dt * 8 + 2 * t;
-      if (row0 < T) *reinterpret_cast<__nv_bfloat162*>(out + ((size_t)s * T + row0) * D + col) = __floats2bfloat162_rn(o[dt][0] * i0, o[dt][1] * i0);
-      if (row1 < T) *reinterpret_cast<__nv_bfloat162*>(out + ((size_t)s * T + row1) * D + col) = __floats2bfloat162_rn(o[dt][2] * i1, o[dt][3] * i1);
-    }
+    store_frag(out, (size_t)s * T, D, h * 64, o, q0 + r0 + g, T, t, i0, i1);
   }
 }
 
 // ---------------------------------------------------------------------------------------------
 template <int NW, int NT2>
-__global__ void __launch_bounds__(NW * 32, NW == 4 ? 3 : 1) k_attn_bwd_tc(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, bf16* __restrict__ dqkv,
+__global__ void __launch_bounds__(NW * 32, 1) k_attn_bwd_tc(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, bf16* __restrict__ dqkv,
                                                          int T, int D, int heads) {
+  static_assert(NT2 > 4, "k_attn_bwd_tc serves T > 64; k_attn_bwd_tc1 serves T <= 64");
   pdl_trigger(); pdl_wait();
   extern __shared__ __align__(128) uint8_t sm[];
   constexpr int TK = NT2 * 16, QB = NW * 16, KT = (NT2 + NW - 1) / NW, PB = ((TK + 63) / 64) * 128;
@@ -173,9 +223,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 4 ? 3 : 1) k_attn_bwd_tc(const 
   float dv[KT][8][4], dk[KT][8][4];
   if (!ONE_BLOCK) {
 #pragma unroll
-    for (int i = 0; i < KT; ++i)
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { dv[i][j][0] = dv[i][j][1] = dv[i][j][2] = dv[i][j][3] = 0.f; dk[i][j][0] = dk[i][j][1] = dk[i][j][2] = dk[i][j][3] = 0.f; }
+    for (int i = 0; i < KT; ++i) { zero_acc(dv[i]); zero_acc(dk[i]); }
   }
 
   load_tile64(Qs, base, ld, QB, T, NW * 32);                 // first query block rides along with K / V
@@ -194,55 +242,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 4 ? 3 : 1) k_attn_bwd_tc(const 
       load_a_frags(qa, qs_a, r0, lane);
       load_a_frags(ga, gs_a, r0, lane);
       float dq[8][4];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) { dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f; }
-      if (NT2 <= 4) {
-        // ---- register-resident variant: S and dP are computed once
-        float c[2 * NT2][4], e[2 * NT2][4];
-        float m0 = -INFINITY, m1 = -INFINITY;
-#pragma unroll
-        for (int n2 = 0; n2 < NT2; ++n2) {
-          qk_tile(c[2 * n2], c[2 * n2 + 1], qa, ks_a, n2 * 16, lane);
-          qk_tile(e[2 * n2], e[2 * n2 + 1], ga, vs_a, n2 * 16, lane);
-#pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            const int cl = n2 * 16 + u * 8 + 2 * t;
-            float* cc = c[2 * n2 + u];
-            cc[0] = (cl < T) ? cc[0] * kAttnScaleLog2 : -INFINITY; cc[1] = (cl + 1 < T) ? cc[1] * kAttnScaleLog2 : -INFINITY;
-            cc[2] = (cl < T) ? cc[2] * kAttnScaleLog2 : -INFINITY; cc[3] = (cl + 1 < T) ? cc[3] * kAttnScaleLog2 : -INFINITY;
-            m0 = fmaxf(m0, fmaxf(cc[0], cc[1])); m1 = fmaxf(m1, fmaxf(cc[2], cc[3]));
-          }
-        }
-        m0 = quad_max(m0); m1 = quad_max(m1);
-        float l0 = 0.f, l1 = 0.f, d0 = 0.f, d1 = 0.f;
-#pragma unroll
-        for (int n = 0; n < 2 * NT2; ++n) {
-          c[n][0] = exp2f(c[n][0] - m0); c[n][1] = exp2f(c[n][1] - m0); c[n][2] = exp2f(c[n][2] - m1); c[n][3] = exp2f(c[n][3] - m1);
-          l0 += c[n][0] + c[n][1]; l1 += c[n][2] + c[n][3];
-          d0 += c[n][0] * e[n][0] + c[n][1] * e[n][1]; d1 += c[n][2] * e[n][2] + c[n][3] * e[n][3];
-        }
-        l0 = quad_sum(l0); l1 = quad_sum(l1); d0 = quad_sum(d0); d1 = quad_sum(d1);
-        const float i0 = 1.f / l0, i1 = 1.f / l1;
-        d0 *= i0; d1 *= i1;
-#pragma unroll
-        for (int n2 = 0; n2 < NT2; ++n2) {
-          uint32_t pa[4], da[4];
-#pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            const float* cc = c[2 * n2 + u]; const float* ee = e[2 * n2 + u];
-            const float p0 = cc[0] * i0, p1 = cc[1] * i0, p2 = cc[2] * i1, p3 = cc[3] * i1;
-            pa[2 * u] = pack2(p0, p1); pa[2 * u + 1] = pack2(p2, p3);
-            da[2 * u] = pack2(p0 * (ee[0] - d0) * 0.125f, p1 * (ee[1] - d0) * 0.125f);
-            da[2 * u + 1] = pack2(p2 * (ee[2] - d1) * 0.125f, p3 * (ee[3] - d1) * 0.125f);
-            const int chunk = n2 * 2 + u;
-            *reinterpret_cast<uint32_t*>(Ps + swz(r0 + g, chunk, PB) + 4 * t) = pa[2 * u];
-            *reinterpret_cast<uint32_t*>(Ps + swz(r0 + g + 8, chunk, PB) + 4 * t) = pa[2 * u + 1];
-            *reinterpret_cast<uint32_t*>(Ds + swz(r0 + g, chunk, PB) + 4 * t) = da[2 * u];
-            *reinterpret_cast<uint32_t*>(Ds + swz(r0 + g + 8, chunk, PB) + 4 * t) = da[2 * u + 1];
-          }
-          av_step(dq, da, ks_a, n2 * 16, lane);
-        }
-      } else {
+      zero_acc(dq);
       // pass 1: row max and sum
       float m0 = -INFINITY, m1 = -INFINITY;
 #pragma unroll 1
@@ -302,37 +302,18 @@ __global__ void __launch_bounds__(NW * 32, NW == 4 ? 3 : 1) k_attn_bwd_tc(const 
         }
         av_step(dq, da, ks_a, n2 * 16, lane);
       }
-      }
-      const int row0 = q0 + r0 + g, row1 = row0 + 8;
-#pragma unroll
-      for (int dt = 0; dt < 8; ++dt) {
-        const int col = dt * 8 + 2 * t;
-        if (row0 < T) *reinterpret_cast<__nv_bfloat162*>(obase + (size_t)row0 * ld + col) = __floats2bfloat162_rn(dq[dt][0], dq[dt][1]);
-        if (row1 < T) *reinterpret_cast<__nv_bfloat162*>(obase + (size_t)row1 * ld + col) = __floats2bfloat162_rn(dq[dt][2], dq[dt][3]);
-      }
+      store_frag(obase, 0, ld, 0, dq, q0 + r0 + g, T, t);
     }
     __syncthreads();
     // ---------------- phase B: key tiles owned by this warp, reduced over the block's query rows
     if (ONE_BLOCK) {
 #pragma unroll
-      for (int i = 0; i < KT; ++i)
-#pragma unroll
-        for (int j = 0; j < 8; ++j) { dv[i][j][0] = dv[i][j][1] = dv[i][j][2] = dv[i][j][3] = 0.f; dk[i][j][0] = dk[i][j][1] = dk[i][j][2] = dk[i][j][3] = 0.f; }
+      for (int i = 0; i < KT; ++i) { zero_acc(dv[i]); zero_acc(dk[i]); }
     }
 #pragma unroll
     for (int i = 0; i < KT; ++i) {
       const int kt = warp + i * NW;
-      if (kt < NT2) {
-#pragma unroll
-        for (int ks = 0; ks < QB / 16; ++ks) {
-          uint32_t pa[4], da[4];
-          const int srow = ks * 16 + (lane & 7) + ((lane >> 4) << 3), chunk = kt * 2 + ((lane >> 3) & 1);
-          ldsm4t(pa, ps_a + swz(srow, chunk, PB));
-          ldsm4t(da, ds_a + swz(srow, chunk, PB));
-          av_step(dv[i], pa, gs_a, ks * 16, lane);
-          av_step(dk[i], da, qs_a, ks * 16, lane);
-        }
-      }
+      if (kt < NT2) key_tile_acc<QB>(dv[i], dk[i], ps_a, ds_a, gs_a, qs_a, kt, PB, lane);
     }
   }
 #pragma unroll
@@ -363,6 +344,8 @@ __global__ void __launch_bounds__(NW * 32, NW == 4 ? 3 : 1) k_attn_bwd_tc(const 
 // computes the current one. The tiles are fetched by TMA (one thread, 3-4 cp.async.bulk.tensor.3d per item, completion on an
 // mbarrier) from a [S][T][cols] view of the token matrix whose out-of-range token rows arrive zero-filled; the per-thread
 // cp.async loop this replaced was 20 % of the backward kernel's instructions (measured in an earlier version).
+// k_attn_fwd_tc1's tile code, both backwards' P / dS packing and every dK / dV store stay written out: routing any of them
+// through the shared routines above changes the compiled instructions (register allocation and address arithmetic).
 template <int NT2>
 __global__ void __launch_bounds__(128) k_attn_fwd_tc1(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_q,
                                                       bf16* __restrict__ out, int T, int D, int heads, int items) {
@@ -484,22 +467,14 @@ __global__ void __launch_bounds__(128, 2) k_attn_bwd_tc1(const __grid_constant__
       load_a_frags(qa, qs_a, r0, lane);
       load_a_frags(ga, gs_a, r0, lane);
       float dq[8][4];
-#pragma unroll
-      for (int i = 0; i < 8; ++i) { dq[i][0] = dq[i][1] = dq[i][2] = dq[i][3] = 0.f; }
+      zero_acc(dq);
       float c[2 * NT2][4], e[2 * NT2][4];
       float m0 = -INFINITY, m1 = -INFINITY;
 #pragma unroll
       for (int n2 = 0; n2 < NT2; ++n2) {
         qk_tile(c[2 * n2], c[2 * n2 + 1], qa, ks_a, n2 * 16, lane);
         qk_tile(e[2 * n2], e[2 * n2 + 1], ga, vs_a, n2 * 16, lane);
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int cl = n2 * 16 + u * 8 + 2 * t;
-          float* cc = c[2 * n2 + u];
-          cc[0] = (cl < T) ? cc[0] * kAttnScaleLog2 : -INFINITY; cc[1] = (cl + 1 < T) ? cc[1] * kAttnScaleLog2 : -INFINITY;
-          cc[2] = (cl < T) ? cc[2] * kAttnScaleLog2 : -INFINITY; cc[3] = (cl + 1 < T) ? cc[3] * kAttnScaleLog2 : -INFINITY;
-          m0 = fmaxf(m0, fmaxf(cc[0], cc[1])); m1 = fmaxf(m1, fmaxf(cc[2], cc[3]));
-        }
+        mask_scale(c[2 * n2], c[2 * n2 + 1], n2 * 16, T, t, m0, m1);
       }
       m0 = quad_max(m0); m1 = quad_max(m1);
       float l0 = 0.f, l1 = 0.f, d0 = 0.f, d1 = 0.f;
@@ -530,28 +505,13 @@ __global__ void __launch_bounds__(128, 2) k_attn_bwd_tc1(const __grid_constant__
         }
         av_step(dq, da, ks_a, n2 * 16, lane);
       }
-      const int row0 = r0 + g, row1 = row0 + 8;
-#pragma unroll
-      for (int dt = 0; dt < 8; ++dt) {
-        const int col = dt * 8 + 2 * t;
-        if (row0 < T) *reinterpret_cast<__nv_bfloat162*>(obase + (size_t)row0 * ld + col) = __floats2bfloat162_rn(dq[dt][0], dq[dt][1]);
-        if (row1 < T) *reinterpret_cast<__nv_bfloat162*>(obase + (size_t)row1 * ld + col) = __floats2bfloat162_rn(dq[dt][2], dq[dt][3]);
-      }
+      store_frag(obase, 0, ld, 0, dq, r0 + g, T, t);
     }
     __syncthreads();
     if (warp < NT2) {          // key tile kt = warp
       float dv[8][4], dk[8][4];
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { dv[j][0] = dv[j][1] = dv[j][2] = dv[j][3] = 0.f; dk[j][0] = dk[j][1] = dk[j][2] = dk[j][3] = 0.f; }
-#pragma unroll
-      for (int ks = 0; ks < QB / 16; ++ks) {
-        uint32_t pa[4], da[4];
-        const int srow = ks * 16 + (lane & 7) + ((lane >> 4) << 3), chunk = warp * 2 + ((lane >> 3) & 1);
-        ldsm4t(pa, ps_a + swz(srow, chunk, PB));
-        ldsm4t(da, ds_a + swz(srow, chunk, PB));
-        av_step(dv, pa, gs_a, ks * 16, lane);
-        av_step(dk, da, qs_a, ks * 16, lane);
-      }
+      zero_acc(dv); zero_acc(dk);
+      key_tile_acc<QB>(dv, dk, ps_a, ds_a, gs_a, qs_a, warp, PB, lane);
       const int key0 = warp * 16 + g, key1 = key0 + 8;
 #pragma unroll
       for (int dt = 0; dt < 8; ++dt) {
@@ -605,7 +565,7 @@ template <int NW, int NT2> constexpr size_t attn_tc_bwd_smem() {
   return (size_t)(2 * NT2 * 16 + 2 * NW * 16) * 128 + (size_t)2 * NW * 16 * (((NT2 * 16 + 63) / 64) * 128);
 }
 
-// Host dispatch over the supported (warps, key-tile) shapes: T <= 32, 64, 112, 208, 256.
+// Host launch of one (warps, key-tile) shape of the one-CTA-per-(sample, head) kernels; attn_dispatch picks it from T.
 template <int NW, int NT2>
 static int attn_launch(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_or_dqkv, int S, int T, int D, int heads, cudaStream_t st) {
   static bool cfg = false;
@@ -623,12 +583,8 @@ static int attn_launch(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_or
 }
 
 static int attn_dispatch(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_or_dqkv, int S, int T, int D, int heads, cudaStream_t st) {
-  static int nopipe = -1;
-  if (nopipe < 0) { const char* e = getenv("APH_ATTN_NOPIPE"); nopipe = (e && e[0] == '1') ? 1 : 0; }
-  if (!nopipe && T <= 32) return attn_launch1<2>(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
-  if (!nopipe && T <= 64) return attn_launch1<4>(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
-  if (T <= 32) return attn_launch<4, 2>(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
-  if (T <= 64) return attn_launch<4, 4>(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
+  if (T <= 32) return attn_launch1<2>(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
+  if (T <= 64) return attn_launch1<4>(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
   if (T <= 112) return attn_launch<8, 7>(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
   if (T <= 208) return attn_launch<8, 13>(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
   if (T <= 256) return attn_launch<8, 16>(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
