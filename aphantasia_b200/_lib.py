@@ -76,6 +76,17 @@ _SIGS = {
     'aph_head_bwd': (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     'aph_synth_fft_bwd_adam': (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, C.c_void_p, c_f32p, C.c_float, C.c_void_p, C.c_int,
                                          c_f32p, c_f32p, c_f32p, c_f32p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p]),
+    'aph_lpips_create': (C.c_int, [C.POINTER(C.c_void_p)]),
+    'aph_lpips_destroy': (C.c_int, [C.c_void_p]),
+    'aph_lpips_load_tensor': (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.c_int64, C.c_void_p]),
+    'aph_lpips_finalize': (C.c_int, [C.c_void_p]),
+    'aph_lpips_fwd': (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_uint64, C.c_int, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int,
+                                C.POINTER(C.c_int64), C.c_void_p]),
+    'aph_lpips_bwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int64, c_f32p, C.c_void_p]),
+    'aph_lpips_conv_test': (C.c_int, [C.c_int, C.c_void_p, c_f32p, c_f32p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_int, C.c_void_p]),
+    'aph_lpips_conv0_test': (C.c_int, [C.c_int, C.c_void_p, c_f32p, c_f32p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    'aph_lpips_pool_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     'aph_allreduce_sym': (C.c_int, [C.c_uint64, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_void_p]),
     'aph_adam_step': (C.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p]),
 }

@@ -97,6 +97,12 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst_saddr, const CUtensorMa
   asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                ::"r"(dst_saddr), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z) : "memory");
 }
+// 4-D tile load (x = channel, y = column, z = row, w = image) of an NHWC activation; coordinates may be negative or past the
+// edge: those elements arrive zero-filled (the 3x3 convolution's padding, conv_tc.cuh)
+__device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int x, int y, int z, int w) {
+  asm volatile("cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+               ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(x), "r"(y), "r"(z), "r"(w) : "memory");
+}
 // same with an L2 eviction-priority hint (weights are re-read by every M tile: evict_last)
 __device__ __forceinline__ void tma_load_2d_hint(void* dst, const CUtensorMap* m, uint64_t* bar, int x, int y, uint64_t policy) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
@@ -126,6 +132,17 @@ template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile
 // D[64 x BN] (+)= A[64 x 16] . B[BN x 16]^T, fp32 accumulators d[BN/2] in the m64nNk16 fragment layout
 template <int BN> struct Wgmma;
 #define APH_WG_REGS8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
+template <> struct Wgmma<64> {      // the 64-channel layers of the LPIPS VGG (conv_tc.cuh)
+  static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db, int acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+        : APH_WG_REGS8(0), APH_WG_REGS8(8), APH_WG_REGS8(16), APH_WG_REGS8(24)
+        : "l"(da), "l"(db), "r"(acc));
+  }
+};
 template <> struct Wgmma<128> {
   static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, int acc) {
     asm volatile(
@@ -399,6 +416,8 @@ k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 // 2-D bf16 tensor map: tensor [rows, K] with rows `row_stride` elements apart (K when 0), box [box_rows, 64] with 128B swizzle.
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int K, int box_rows, int64_t row_stride = 0);
 int make_tmap_bf16_tokens(CUtensorMap* out, const void* base, int cols, int T, int S, int box_rows);
+// 4-D view {C, W, H, N} of a bf16 NHWC activation, box {64 channels, box_w columns, box_h rows, 1 image}, 128B swizzle
+int make_tmap_bf16_nhwc(CUtensorMap* out, const void* base, int N, int H, int W, int C, int box_h, int box_w);
 // Launches the GEMM on `st`. A: [M,K] with rows `lda` elements apart (K when 0), B: [N,K] device bf16. Requires K % 64 == 0,
 // N % 128 == 0, and row strides that are multiples of 16 bytes.
 int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st, int lda = 0);

@@ -57,6 +57,23 @@ int make_tmap_bf16_tokens(CUtensorMap* out, const void* base, int cols, int T, i
   return 0;
 }
 
+// 4-D view of an NHWC activation for the 3x3 convolution (conv_tc.cuh): the producer loads the box at coordinates shifted by the
+// tap's (dy, dx), and the rows / columns outside the image arrive zero-filled, which is the convolution's padding 1.
+int make_tmap_bf16_nhwc(CUtensorMap* out, const void* base, int N, int H, int W, int C, int box_h, int box_w) {
+  EncodeTiledFn enc = get_encode();
+  APH_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
+  APH_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && C % 64 == 0, "tensor map (NHWC): base not 16-byte aligned or C=%d not a multiple of 64", C);
+  const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  const cuuint64_t gstride[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+  const cuuint32_t box[4] = {64u, (cuuint32_t)box_w, (cuuint32_t)box_h, 1u};
+  const cuuint32_t estr[4] = {1, 1, 1, 1};
+  const CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), gdim, gstride, box, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  APH_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (NHWC) failed: CUresult %d (N=%d H=%d W=%d C=%d)", (int)r, N, H, W, C);
+  return 0;
+}
+
 // ---- optional per-launch event timing (bench.py's roofline: the GEMM kernel's real time inside a step)
 static bool g_prof = false;
 bool gemm_profiling_on() { return g_prof; }

@@ -1,6 +1,4 @@
-"""lpips stand-in: clip_fft.py:22 imports it at top level but only uses it with --sync (off by default)."""
-
-
-class LPIPS:
-    def __init__(self, *a, **k):
-        raise NotImplementedError('lpips is not installed in this environment (only needed for --sync)')
+"""Drop-in for the lpips package -> aphantasia_b200.lpips (clip_fft.py --sync: lpips.LPIPS(net='vgg'))."""
+from aphantasia_b200.lpips import *  # noqa: F401,F403
+import aphantasia_b200.lpips as _m
+globals().update({k: v for k, v in vars(_m).items() if not k.startswith("__")})

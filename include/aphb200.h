@@ -302,6 +302,39 @@ int aph_derivat_bwd(const float* img, int C, int H, int W, const float* upstream
 int aph_head_fwd(const float* emb, int S, int D, const float* w, const float* b, float* out, void* stream);
 int aph_head_bwd(const float* grad_out, const float* w, int S, int D, float* grad_emb, void* stream);
 
+/* ---- LPIPS image-composition loss (clip_fft.py --sync: lpips.LPIPS(net='vgg'), clip_fft.py:220,270) --------------------
+ * lpips v0.1, net='vgg', lpips=True, spatial=False: scaling layer, VGG16 features[0:30] (13 conv3x3 + ReLU, 4 max-pools), per-tap
+ * unit-normalised features, squared difference weighted by the tap's lin weights, spatial mean, sum over the 5 taps.
+ * Keys of aph_lpips_load_tensor (fp32 DEVICE data): torchvision's "features.{i}.weight" [Co,Ci,3,3] / "features.{i}.bias" for
+ * i in {0,2,5,7,10,12,14,17,19,21,24,26,28}, and lpips' "lin{t}.model.1.weight" [1,C,1,1], t = 0..4. The 3x3 weights are packed
+ * once, to bf16 [Co, 9 Ci] for the forward and [Ci, 9 Co] (flipped) for the data gradient.                                   */
+typedef struct aph_lpips aph_lpips;
+int aph_lpips_create(aph_lpips** h);
+int aph_lpips_destroy(aph_lpips* h);
+int aph_lpips_load_tensor(aph_lpips* h, const char* key, const float* data, int64_t numel, void* stream);
+int aph_lpips_finalize(aph_lpips* h);
+/* in0, in1 [N,3,H,W] (H, W >= 16) -> out [N] = LPIPS(in0[n], in1[n]); normalize = 1 maps inputs from [0,1] to [-1,1].
+ * The features of in1 are cached under ref_key (non-zero; 0 = do not reuse): in1 may be NULL when ref_key matches the cached
+ * features of the same N, H, W, and then no reference pass runs. save_for_bwd = 1 keeps the activations of in0;
+ * *generation (may be NULL) receives this forward's stamp. Every forward voids the activations saved by earlier ones.      */
+int aph_lpips_fwd(aph_lpips* h, const float* in0, const float* in1, uint64_t ref_key, int N, int H, int W, int normalize,
+                  float* out, int save_for_bwd, int64_t* generation, void* stream);
+/* grad_out [N] DEVICE -> grad_in0 [N,3,H,W] (overwritten). Fails, launching nothing, if `generation` is not the last forward's
+ * or that forward did not save.                                                                                            */
+int aph_lpips_bwd(aph_lpips* h, const float* grad_out, int64_t generation, float* grad_in0, void* stream);
+/* Test entries on caller buffers (bf16 NHWC activations):
+ * aph_lpips_conv_test: one 3x3 layer, weight fp32 [Cout,Cin,3,3] packed as the loader does. fwd = 1: x [N,H,W,Cin] ->
+ *   out = relu(conv(x) + bias) [N,H,W,Cout]; fwd = 0: x = dy [N,H,W,Cout] -> out = dx [N,H,W,Cin], with mask (NULL = none)
+ *   [N,H,W,Cin]: out = mask > 0 ? dx : 0. Cin, Cout multiples of 64.
+ * aph_lpips_conv0_test: conv1_1 (3 -> 64, fp32). fwd = 1: in = image fp32 [N,3,H,W] -> out bf16 [N,H,W,64] (ReLU output,
+ *   after the scaling layer); fwd = 0: in = dz bf16 [N,H,W,64] -> out fp32 [N,3,H,W].
+ * aph_lpips_pool_test: 2x2 max-pool, C % 8 == 0. fwd = 1: out = pool(x); fwd = 0: out [N,H,W,C] = adjoint of dy [N,H/2,W/2,C]. */
+int aph_lpips_conv_test(int fwd, const void* x, const float* weight, const float* bias, const void* mask, void* out, int N, int H,
+                        int W, int Cin, int Cout, void* stream);
+int aph_lpips_conv0_test(int fwd, const void* in, const float* weight, const float* bias, void* out, int N, int H, int W,
+                         int normalize, void* stream);
+int aph_lpips_pool_test(int fwd, const void* x, const void* dy, void* out, int N, int H, int W, int C, void* stream);
+
 /* ================= step glue ==================================================================
  * torch.optim.Adam(betas=(b1,b2)) single-tensor update (clip_fft.py:108-115,295), bias-corrected. */
 int aph_adam_step(float* p, const float* g, float* m, float* v, int64_t n,
