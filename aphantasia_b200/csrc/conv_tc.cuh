@@ -6,9 +6,9 @@
 // spatial block of 8 rows x 16 columns of one image. Its A operand for one (tap, 64-channel chunk) is ONE 4-D TMA load of the NHWC
 // tensor at coordinates shifted by the tap's (dy, dx): the box lands in shared memory as 128 rows of 128 B, swizzled exactly as the
 // GEMM's 2-D A tile, and the rows / columns outside the image arrive zero-filled, which is the padding. No im2col buffer exists.
-// The schedule is the encoder GEMM's cooperative one (tc_gemm.cuh: TMA producer warpgroup, two consumer warpgroups on rows
-// 0-63 / 64-127, the same stage ring, barriers and wgmma wrappers); tiles are persistent over (image, tile row, tile column, N
-// block). Pixels of a partial tile (45 x 80, 22 x 40, ...) are computed on zeros and not stored.
+// The kernel runs the encoder GEMM's kernel body (gemm_body in tc_gemm.cuh) on its cooperative schedule; this file supplies the
+// pixel-tile decode, the tap-shifted A load and the epilogue. Tiles are persistent over (image, tile row, tile column, N block).
+// Pixels of a partial tile (45 x 80, 22 x 40, ...) are computed on zeros and not stored.
 //
 // The data gradient of the same layer is the same kernel: dx = conv3x3(dy, W flipped and transposed), packed [C_in, 9 C_out].
 // Epilogues (bf16 NHWC out, 16 B per lane after the quad transpose of tc_gemm.cuh):
@@ -60,94 +60,60 @@ __device__ __forceinline__ void conv_store_bf16x32(const ConvEpi& epi, size_t pi
   if (valid) st_global_16(epi.out + off, w);
 }
 
+// The convolution as a gemm_body problem (tc_gemm.cuh). Tile = (image, tile row, tile column, N block), in row-major order;
+// K block kb is (tap, 64-channel chunk) = (kb / cchunks, kb % cchunks).
+template <int BN, int EPI>
+struct ConvProblem {
+  static constexpr bool PDL = false;
+  const ConvShape& cs;
+  const ConvEpi& epi;
+
+  __device__ __forceinline__ int tiles_img() const { return cs.tiles_y * cs.tiles_x; }
+  __device__ __forceinline__ int cchunks() const { return cs.Cin / GEMM_BK; }
+  __device__ __forceinline__ int n_tiles() const { return cs.Cout / BN; }
+  __device__ __forceinline__ int num_tiles() const { return cs.N * tiles_img() * n_tiles(); }
+  __device__ __forceinline__ int k_blocks() const { return 9 * cchunks(); }
+  __device__ __forceinline__ bool has_tile(int tile) const { return tile < num_tiles(); }
+
+  struct Tile { int img, ty, tx, n_blk; };
+  __device__ __forceinline__ Tile tile(int tile) const {
+    const int m_blk = tile / n_tiles(), n_blk = tile - m_blk * n_tiles();
+    const int img = m_blk / tiles_img(), r = m_blk - img * tiles_img(), ty = r / cs.tiles_x;
+    return {img, ty, r - ty * cs.tiles_x, n_blk};
+  }
+
+  // the 8 x 16 x 64 box of x at the tile's pixels shifted by the tap's (dy, dx)
+  __device__ __forceinline__ void load_a(void* dst, const CUtensorMap* map_x, uint64_t* bar, Tile t, int kb) const {
+    const int tap = kb / cchunks(), ch = kb - tap * cchunks();
+    tma_load_4d(dst, map_x, bar, ch * GEMM_BK, t.tx * CONV_TW + tap % 3 - 1, t.ty * CONV_TH + tap / 3 - 1, t.img);
+  }
+
+  __device__ __forceinline__ void epilogue(const float (&d)[1][BN / 2], Tile t, int row_in_tile, int col_in_tile, int lane) const {
+    // rows row_in_tile and row_in_tile + 8 are columns x0, x0 + 8 of tile row y
+    const int y = t.ty * CONV_TH + row_in_tile / CONV_TW, x0 = t.tx * CONV_TW + row_in_tile % CONV_TW, x1 = x0 + 8;
+    const bool v0ok = y < cs.H && x0 < cs.W, v1ok = y < cs.H && x1 < cs.W;
+    const size_t pix0 = ((size_t)t.img * cs.H + y) * cs.W + x0, pix1 = pix0 + 8;
+#pragma unroll
+    for (int j0 = 0; j0 < BN / 8; j0 += 4) {            // 32-column chunks
+      const int col0 = t.n_blk * BN + 8 * j0;
+      float2 bb[4];
+      float v0[8], v1[8];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        bb[i] = (EPI == CONV_BIAS_RELU) ? __ldg(reinterpret_cast<const float2*>(epi.bias + col0 + 8 * i + col_in_tile)) : make_float2(0.f, 0.f);
+        v0[2 * i] = d[0][4 * (j0 + i)]; v0[2 * i + 1] = d[0][4 * (j0 + i) + 1];
+        v1[2 * i] = d[0][4 * (j0 + i) + 2]; v1[2 * i + 1] = d[0][4 * (j0 + i) + 3];
+      }
+      conv_store_bf16x32<EPI>(epi, pix0, v0ok, cs.Cout, col0, lane & 3, v0, bb);
+      conv_store_bf16x32<EPI>(epi, pix1, v1ok, cs.Cout, col0, lane & 3, v1, bb);
+    }
+  }
+};
+
 template <int BN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 k_conv3x3_tc(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ CUtensorMap map_w, ConvShape cs, ConvEpi epi) {
-  using L = GemmCfg<BN>;
-  constexpr int STAGES = L::STAGES;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
-  uint64_t* empty_bar = full_bar + STAGES;
-
-  const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
-  const int n_tiles = cs.Cout / BN, tiles_img = cs.tiles_y * cs.tiles_x;
-  const int num_tiles = cs.N * tiles_img * n_tiles, cchunks = cs.Cin / GEMM_BK, k_blocks = 9 * cchunks;
-
-  if (threadIdx.x == 0) {
-    tma_prefetch_desc(&map_x); tma_prefetch_desc(&map_w);
-    for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 2); }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (wg == 0) {
-    setmaxnreg_dec<40>();
-    if (tid == 0) {
-      // ===== TMA producer: per k block one shifted 8 x 16 x 64 box of x and one BN x 64 box of the packed weights
-      const uint64_t pol_b = l2_policy_evict_last();
-      uint32_t it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
-        const int img = m_blk / tiles_img, r = m_blk - img * tiles_img, ty = r / cs.tiles_x, tx = r - ty * cs.tiles_x;
-        for (int kb = 0; kb < k_blocks; ++kb, ++it) {
-          const int tap = kb / cchunks, ch = kb - tap * cchunks;
-          const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
-          mbar_wait(&empty_bar[s], ph ^ 1);
-          uint8_t* sa = smem + s * L::STAGE_BYTES;
-          mbar_expect_tx(&full_bar[s], L::STAGE_BYTES);
-          tma_load_4d(sa, &map_x, &full_bar[s], ch * GEMM_BK, tx * CONV_TW + tap % 3 - 1, ty * CONV_TH + tap / 3 - 1, img);
-          tma_load_2d_hint(sa + L::A_BYTES, &map_w, &full_bar[s], kb * GEMM_BK, n_blk * BN, pol_b);
-        }
-      }
-    }
-  } else {
-    setmaxnreg_inc<232>();
-    // ===== consumer warpgroup c: rows 64 c .. 64 c + 63 of every tile
-    const int c = wg - 1, warp = tid >> 5, lane = tid & 31;
-    const int row_in_tile = 64 * c + 16 * warp + (lane >> 2), col_in_tile = 2 * (lane & 3);
-    // rows row_in_tile and row_in_tile + 8 are columns px, px + 8 of tile row py
-    const int py = row_in_tile / CONV_TW, px = row_in_tile % CONV_TW;
-    uint32_t it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      float d[BN / 2];
-#pragma unroll
-      for (int r = 0; r < BN / 2; ++r) d[r] = 0.f;
-      for (int kb = 0; kb < k_blocks; ++kb, ++it) {
-        const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        const uint64_t ds = make_smem_desc(smem_u32(smem + s * L::STAGE_BYTES));
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GEMM_BK / GEMM_UK; ++k)
-          Wgmma<BN>::mma(d, ds + (uint64_t)(c * 512 + 2 * k), ds + (uint64_t)(L::A_BYTES / 16 + 2 * k), (kb | k) != 0);
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (kb > 0 && tid == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
-      }
-      wgmma_wait<0>();
-      if (tid == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
-      const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
-      const int img = m_blk / tiles_img, r = m_blk - img * tiles_img, ty = r / cs.tiles_x, tx = r - ty * cs.tiles_x;
-      const int y = ty * CONV_TH + py, x0 = tx * CONV_TW + px, x1 = x0 + 8;
-      const bool v0ok = y < cs.H && x0 < cs.W, v1ok = y < cs.H && x1 < cs.W;
-      const size_t pix0 = ((size_t)img * cs.H + y) * cs.W + x0, pix1 = pix0 + 8;
-#pragma unroll
-      for (int j0 = 0; j0 < BN / 8; j0 += 4) {            // 32-column chunks
-        const int col0 = n_blk * BN + 8 * j0;
-        float2 bb[4];
-        float v0[8], v1[8];
-#pragma unroll
-        for (int t = 0; t < 4; ++t) {
-          bb[t] = (EPI == CONV_BIAS_RELU) ? __ldg(reinterpret_cast<const float2*>(epi.bias + col0 + 8 * t + col_in_tile)) : make_float2(0.f, 0.f);
-          v0[2 * t] = d[4 * (j0 + t)]; v0[2 * t + 1] = d[4 * (j0 + t) + 1];
-          v1[2 * t] = d[4 * (j0 + t) + 2]; v1[2 * t + 1] = d[4 * (j0 + t) + 3];
-        }
-        conv_store_bf16x32<EPI>(epi, pix0, v0ok, cs.Cout, col0, lane & 3, v0, bb);
-        conv_store_bf16x32<EPI>(epi, pix1, v1ok, cs.Cout, col0, lane & 3, v1, bb);
-      }
-    }
-  }
+  gemm_body<BN, false>(map_x, map_w, ConvProblem<BN, EPI>{cs, epi});
 }
 
 // Launches the convolution on `st`: x bf16 NHWC [N,H,W,Cin], wpack bf16 [Cout, 9 Cin]; Cin and Cout multiples of 64.

@@ -17,6 +17,8 @@
 // for the patch-embed data gradient. bf16 outputs are stored 16 B per lane after an exchange inside each quad of lanes.
 // Rows >= M are zero-filled by TMA on load and not stored. A, the residual and the outputs may have a row stride larger than
 // their width (the encoder's last block reads and writes the class-token rows s*T of token-major matrices in place).
+// The kernel body (gemm_body: stage ring, mbarriers, producer and consumer loops) is shared with the LPIPS 3x3 convolution
+// (conv_tc.cuh), which supplies its own tile decode, A load and epilogue through a Problem type.
 #pragma once
 #include "aph_common.cuh"
 #include <cuda.h>
@@ -290,27 +292,35 @@ __device__ __forceinline__ void epi_store_bf16x32(const GemmEpi& epi, int row, b
   }
 }
 
+// The kernel body of the GEMM and of the 3x3 convolution (conv_tc.cuh): shared-memory stage ring, mbarriers, producer / consumer
+// split, main loop. A Problem supplies what differs between the two:
+//   PDL                                    whether the kernel takes part in programmatic dependent launch
+//   num_tiles(), k_blocks()                tiles; 64-wide K blocks per tile
+//   has_tile(tile)                         tile < num_tiles(), as the consumer warpgroups test it
+//   tile(tile)                             decodes a tile index into a Tile, which has the tile's N block n_blk
+//   load_a(dst, map_a, bar, t, kb)         the TMA load of the 128 x 64 A box of (Tile t, K block kb), complete_tx on bar
+//   epilogue(d, t, row, col, lane)         stores finished Tile t from the accumulator fragments d[h][BN / 2] of m64 row
+//                                          block h; this thread's first element is (row + 64 h, col) of the tile
+// The producer decodes each tile before its k-block loop: the compiler does not move a division across the mbarrier waits, so a
+// decode inside load_a would be redone for every stage.
 // PINGPONG = false ("cooperative"): both consumer warpgroups work on every tile, rows 0-63 / 64-127, one m64nBNk16 per k16.
 // PINGPONG = true: consumer warpgroup c owns the whole 128 x 128 tiles i = c, c + 2, ... of this CTA's schedule (two m64n128k16
 // per k16: rows 0-63 and 64-127). Two named barriers hand the mainloop back and forth, so one warpgroup issues the MMAs of tile
 // i while the other stores tile i - 1: the tensor pipe and the epilogue's HBM traffic overlap instead of taking turns.
-template <int BN, bool PINGPONG, int EPI>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, GemmShape shp, GemmEpi epi) {
+template <int BN, bool PINGPONG, class Problem>
+__device__ __forceinline__ void gemm_body(const CUtensorMap& map_a, const CUtensorMap& map_b, const Problem& pb) {
   static_assert(BN == 128 || !PINGPONG, "the ping-pong schedule runs 128 x 128 tiles");
   using L = GemmCfg<BN>;
   constexpr int STAGES = L::STAGES;
   constexpr int MMAS = PINGPONG ? 2 : 1;          // m64 row blocks per consumer warpgroup and tile
-  constexpr bool HAS_BIAS = (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_RESID);
-  pdl_trigger();
+  if constexpr (Problem::PDL) pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int wg = threadIdx.x >> 7, tid = threadIdx.x & 127;
-  const int m_tiles = (shp.M + GEMM_BM - 1) / GEMM_BM, n_tiles = shp.N / BN;
-  const int num_tiles = m_tiles * n_tiles, k_blocks = shp.K / GEMM_BK;
+  const int num_tiles = pb.num_tiles(), k_blocks = pb.k_blocks();
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&map_a); tma_prefetch_desc(&map_b);
@@ -318,7 +328,7 @@ k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     fence_barrier_init();
   }
   __syncthreads();
-  pdl_wait();                  // everything above overlapped the previous kernel's tail; operands are read from here on
+  if constexpr (Problem::PDL) pdl_wait();   // everything above overlapped the previous kernel's tail; operands are read from here on
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
@@ -327,14 +337,14 @@ k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
       const uint64_t pol_b = l2_policy_evict_last();      // B = weights: shared by all M tiles
       uint32_t it = 0;
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
+        const auto t = pb.tile(tile);
         for (int kb = 0; kb < k_blocks; ++kb, ++it) {
           const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
           mbar_wait(&empty_bar[s], ph ^ 1);
           uint8_t* sa = smem + s * L::STAGE_BYTES;
           mbar_expect_tx(&full_bar[s], L::STAGE_BYTES);
-          tma_load_2d(sa, &map_a, &full_bar[s], kb * GEMM_BK, m_blk * GEMM_BM);
-          tma_load_2d_hint(sa + L::A_BYTES, &map_b, &full_bar[s], kb * GEMM_BK, n_blk * BN, pol_b);
+          pb.load_a(sa, &map_a, &full_bar[s], t, kb);
+          tma_load_2d_hint(sa + L::A_BYTES, &map_b, &full_bar[s], kb * GEMM_BK, t.n_blk * BN, pol_b);
         }
       }
     }
@@ -346,8 +356,7 @@ k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     // this CTA's tiles are blockIdx.x + i * gridDim.x, i = 0, 1, ...; their stages follow each other in the ring (`it`)
     uint32_t it = PINGPONG ? c * k_blocks : 0;
     const int tile_step = (PINGPONG ? 2 : 1) * gridDim.x;
-    // (the loop bounds compare rows with shp.M, a kernel parameter, rather than keep num_tiles in a register)
-    for (int tile = blockIdx.x + (PINGPONG ? c * gridDim.x : 0); tile / n_tiles * GEMM_BM < shp.M; tile += tile_step) {
+    for (int tile = blockIdx.x + (PINGPONG ? c * gridDim.x : 0); pb.has_tile(tile); tile += tile_step) {
       // Ping-pong: wait until the other warpgroup has issued the previous tile. This also keeps every full-barrier wait below at
       // most one phase ahead of the barrier (the stage's previous use, in that tile or earlier, has already been waited for).
       if (PINGPONG && tile != (int)blockIdx.x) consumer_bar_sync(1 + c);
@@ -372,44 +381,80 @@ k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         wgmma_wait<1>();                                 // the previous stage's MMAs have retired: hand that stage back
         if (kb > 0 && tid == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
       }
-      if (PINGPONG && (tile + (int)gridDim.x) / n_tiles * GEMM_BM < shp.M) consumer_bar_arrive(1 + (c ^ 1));    // the other warpgroup may issue the next tile
+      if (PINGPONG && pb.has_tile(tile + (int)gridDim.x)) consumer_bar_arrive(1 + (c ^ 1));    // the other warpgroup may issue the next tile
       wgmma_wait<0>();
       if (tid == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
       if (PINGPONG) it += k_blocks;                    // skip the other warpgroup's tile
-      const int m_blk = tile / n_tiles, n_blk = tile - m_blk * n_tiles;
-      // ---- epilogue straight from the accumulator fragments: d[h][4j + {0,1}] = (row, col + {0,1}), d[h][4j + {2,3}] = (row + 8, ...)
+      pb.epilogue(d, pb.tile(tile), row_in_tile, col_in_tile, lane);
+    }
+  }
+}
+
+// The encoder GEMM as a gemm_body problem: A is [M, K], tile = (128-row block, BN-column block), fused epilogue of kind EPI.
+template <int BN, int EPI>
+struct GemmProblem {
+  static constexpr bool PDL = true;
+  const GemmShape& shp;
+  const GemmEpi& epi;
+
+  __device__ __forceinline__ int num_tiles() const { return (shp.M + GEMM_BM - 1) / GEMM_BM * n_tiles(); }
+  __device__ __forceinline__ int n_tiles() const { return shp.N / BN; }
+  __device__ __forceinline__ int k_blocks() const { return shp.K / GEMM_BK; }
+  // (compares rows with shp.M, a kernel parameter, rather than keep num_tiles in a consumer register)
+  __device__ __forceinline__ bool has_tile(int tile) const { return tile / n_tiles() * GEMM_BM < shp.M; }
+
+  struct Tile { int m_blk, n_blk; };
+  __device__ __forceinline__ Tile tile(int tile) const {
+    const int m_blk = tile / n_tiles();
+    return {m_blk, tile - m_blk * n_tiles()};
+  }
+
+  __device__ __forceinline__ void load_a(void* dst, const CUtensorMap* map_a, uint64_t* bar, Tile t, int kb) const {
+    tma_load_2d(dst, map_a, bar, kb * GEMM_BK, t.m_blk * GEMM_BM);
+  }
+
+  // straight from the accumulator fragments: d[h][4j + {0,1}] = (row, col + {0,1}), d[h][4j + {2,3}] = (row + 8, ...)
+  template <int MMAS>
+  __device__ __forceinline__ void epilogue(const float (&d)[MMAS][BN / 2], Tile tl, int row_in_tile, int col_in_tile, int lane) const {
+    constexpr bool HAS_BIAS = (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_RESID);
+    const int m_blk = tl.m_blk, n_blk = tl.n_blk;
 #pragma unroll
-      for (int h = 0; h < MMAS; ++h) {
-        const int row0 = m_blk * GEMM_BM + 64 * h + row_in_tile, row1 = row0 + 8;
-        if constexpr (epi_bf16_out<EPI>()) {
+    for (int h = 0; h < MMAS; ++h) {
+      const int row0 = m_blk * GEMM_BM + 64 * h + row_in_tile, row1 = row0 + 8;
+      if constexpr (epi_bf16_out<EPI>()) {
 #pragma unroll
-          for (int j0 = 0; j0 < BN / 8; j0 += 4) {        // 32-column chunks
-            const int col0 = n_blk * BN + 8 * j0;
-            float2 bb[4];
-            float v0[8], v1[8];
+        for (int j0 = 0; j0 < BN / 8; j0 += 4) {        // 32-column chunks
+          const int col0 = n_blk * BN + 8 * j0;
+          float2 bb[4];
+          float v0[8], v1[8];
 #pragma unroll
-            for (int t = 0; t < 4; ++t) {
-              bb[t] = HAS_BIAS ? __ldg(reinterpret_cast<const float2*>(epi.bias + col0 + 8 * t + col_in_tile)) : make_float2(0.f, 0.f);
-              v0[2 * t] = d[h][4 * (j0 + t)]; v0[2 * t + 1] = d[h][4 * (j0 + t) + 1];
-              v1[2 * t] = d[h][4 * (j0 + t) + 2]; v1[2 * t + 1] = d[h][4 * (j0 + t) + 3];
-            }
-            epi_store_bf16x32<EPI>(epi, row0, row0 < shp.M, col0, lane & 3, v0, bb);
-            epi_store_bf16x32<EPI>(epi, row1, row1 < shp.M, col0, lane & 3, v1, bb);
+          for (int t = 0; t < 4; ++t) {
+            bb[t] = HAS_BIAS ? __ldg(reinterpret_cast<const float2*>(epi.bias + col0 + 8 * t + col_in_tile)) : make_float2(0.f, 0.f);
+            v0[2 * t] = d[h][4 * (j0 + t)]; v0[2 * t + 1] = d[h][4 * (j0 + t) + 1];
+            v1[2 * t] = d[h][4 * (j0 + t) + 2]; v1[2 * t + 1] = d[h][4 * (j0 + t) + 3];
           }
-        } else {
-          const size_t out0 = (size_t)row0 * epi.ld_out, out1 = out0 + 8 * (size_t)epi.ld_out;
-          const size_t res0 = (EPI == EPI_BIAS_RESID) ? (size_t)row0 * epi.ld_resid : 0, res1 = res0 + 8 * (size_t)epi.ld_resid;
+          epi_store_bf16x32<EPI>(epi, row0, row0 < shp.M, col0, lane & 3, v0, bb);
+          epi_store_bf16x32<EPI>(epi, row1, row1 < shp.M, col0, lane & 3, v1, bb);
+        }
+      } else {
+        const size_t out0 = (size_t)row0 * epi.ld_out, out1 = out0 + 8 * (size_t)epi.ld_out;
+        const size_t res0 = (EPI == EPI_BIAS_RESID) ? (size_t)row0 * epi.ld_resid : 0, res1 = res0 + 8 * (size_t)epi.ld_resid;
 #pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            const int col = n_blk * BN + 8 * j + col_in_tile;
-            const float2 bb = HAS_BIAS ? __ldg(reinterpret_cast<const float2*>(epi.bias + col)) : make_float2(0.f, 0.f);
-            if (row0 < shp.M) epi_store2<EPI>(epi, out0, res0, row0, col, d[h][4 * j], d[h][4 * j + 1], bb);
-            if (row1 < shp.M) epi_store2<EPI>(epi, out1, res1, row1, col, d[h][4 * j + 2], d[h][4 * j + 3], bb);
-          }
+        for (int j = 0; j < BN / 8; ++j) {
+          const int col = n_blk * BN + 8 * j + col_in_tile;
+          const float2 bb = HAS_BIAS ? __ldg(reinterpret_cast<const float2*>(epi.bias + col)) : make_float2(0.f, 0.f);
+          if (row0 < shp.M) epi_store2<EPI>(epi, out0, res0, row0, col, d[h][4 * j], d[h][4 * j + 1], bb);
+          if (row1 < shp.M) epi_store2<EPI>(epi, out1, res1, row1, col, d[h][4 * j + 2], d[h][4 * j + 3], bb);
         }
       }
     }
   }
+};
+
+template <int BN, bool PINGPONG, int EPI>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+k_gemm_bf16_tn(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, GemmShape shp, GemmEpi epi) {
+  gemm_body<BN, PINGPONG>(map_a, map_b, GemmProblem<BN, EPI>{shp, epi});
 }
 
 // ---- host side ---------------------------------------------------------------------------------
