@@ -134,11 +134,8 @@ def draw_fast(row, size):
 
 
 def draw_crop_table(count, canvas_hw, size=224, kind=TF_FAST, align='uniform', macro=0., n_imgs=1):
-    """Crop tables for one slice_imgs call: native replay (libaphb200.so: aph_rng_crop_tables) unless APH_RNG_PY=1;
-    draw_crop_table_py below is the executable specification both are tested against."""
-    import os
-    if os.environ.get('APH_RNG_PY', '0') == '1':
-        return draw_crop_table_py(count, canvas_hw, size, kind, align, macro, n_imgs)
+    """Crop tables for one slice_imgs call, from the native replay (libaphb200.so: aph_rng_crop_tables);
+    draw_crop_table_py below is the executable specification it is tested against."""
     return draw_crop_table_native(count, canvas_hw, size, kind, align, macro, n_imgs)
 
 

@@ -71,27 +71,6 @@ struct Scratch {
   }
 };
 
-// Programmatic dependent launch: a kernel calls pdl_trigger() first thing (its dependents may start being scheduled as SMs
-// drain) and pdl_wait() before its first global-memory access (blocks until the preceding grid has completed and flushed).
-// The prologue in between (barrier init, descriptor prefetch, index setup) overlaps the predecessor's tail.
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-
-bool pdl_enabled();            // api.cu: APH_PDL=1 enables (off by default: no measured gain on top of the graph cache)
-
-// cudaLaunchKernelEx wrapper: optional cluster width and the programmatic-serialization attribute
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, int cluster, Args... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute at[2];
-  int n = 0;
-  if (cluster > 1) { at[n].id = cudaLaunchAttributeClusterDimension; at[n].val.clusterDim.x = cluster; at[n].val.clusterDim.y = 1; at[n].val.clusterDim.z = 1; ++n; }
-  if (pdl_enabled()) { at[n].id = cudaLaunchAttributeProgrammaticStreamSerialization; at[n].val.programmaticStreamSerializationAllowed = 1; ++n; }
-  cfg.attrs = at; cfg.numAttrs = n;
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -1,7 +1,6 @@
 // api.cu -- library-wide state of libaphb200.so: error string, version, launch counter.
 #include "aph_common.cuh"
 #include <string.h>
-#include <stdlib.h>
 
 namespace aph {
 static thread_local char tls_error[512] = "";
@@ -12,12 +11,6 @@ void set_error(const char* fmt, ...) {
   va_start(ap, fmt);
   vsnprintf(tls_error, sizeof(tls_error), fmt, ap);
   va_end(ap);
-}
-bool pdl_enabled() {
-  static int v = -1;
-  // opt-in (APH_PDL=1): with the CUDA-graph cache already removing launch gaps it measured 151.2 vs 152.7 steps/s at C2
-  if (v < 0) { const char* e = getenv("APH_PDL"); v = (e && e[0] == '1') ? 1 : 0; }
-  return v == 1;
 }
 }  // namespace aph
 

@@ -64,7 +64,6 @@ __device__ __forceinline__ void conv_store_bf16x32(const ConvEpi& epi, size_t pi
 // K block kb is (tap, 64-channel chunk) = (kb / cchunks, kb % cchunks).
 template <int BN, int EPI>
 struct ConvProblem {
-  static constexpr bool PDL = false;
   const ConvShape& cs;
   const ConvEpi& epi;
 

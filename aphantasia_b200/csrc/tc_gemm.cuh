@@ -294,7 +294,6 @@ __device__ __forceinline__ void epi_store_bf16x32(const GemmEpi& epi, int row, b
 
 // The kernel body of the GEMM and of the 3x3 convolution (conv_tc.cuh): shared-memory stage ring, mbarriers, producer / consumer
 // split, main loop. A Problem supplies what differs between the two:
-//   PDL                                    whether the kernel takes part in programmatic dependent launch
 //   num_tiles(), k_blocks()                tiles; 64-wide K blocks per tile
 //   has_tile(tile)                         tile < num_tiles(), as the consumer warpgroups test it
 //   tile(tile)                             decodes a tile index into a Tile, which has the tile's N block n_blk
@@ -313,7 +312,6 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a, const CUtens
   using L = GemmCfg<BN>;
   constexpr int STAGES = L::STAGES;
   constexpr int MMAS = PINGPONG ? 2 : 1;          // m64 row blocks per consumer warpgroup and tile
-  if constexpr (Problem::PDL) pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + L::BAR_OFFSET);
@@ -328,7 +326,6 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a, const CUtens
     fence_barrier_init();
   }
   __syncthreads();
-  if constexpr (Problem::PDL) pdl_wait();   // everything above overlapped the previous kernel's tail; operands are read from here on
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
@@ -393,7 +390,6 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a, const CUtens
 // The encoder GEMM as a gemm_body problem: A is [M, K], tile = (128-row block, BN-column block), fused epilogue of kind EPI.
 template <int BN, int EPI>
 struct GemmProblem {
-  static constexpr bool PDL = true;
   const GemmShape& shp;
   const GemmEpi& epi;
 

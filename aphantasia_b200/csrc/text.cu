@@ -36,7 +36,6 @@ struct TextImpl : Encoder {
 template <int NCH>
 __global__ void __launch_bounds__(256) k_text_embed(const int64_t* __restrict__ ids, const float* __restrict__ tok_emb,
                                                     const float* __restrict__ pos, float* __restrict__ x, int rows, int ctx, int D, int vocab) {
-  pdl_trigger(); pdl_wait();
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (row >= rows) return;
   constexpr int N = 4 * NCH;
@@ -55,7 +54,6 @@ __global__ void __launch_bounds__(256) k_text_embed(const int64_t* __restrict__ 
 
 // eot[s] = first position of the largest id of sequence s (torch.argmax semantics); one warp per sequence.
 __global__ void __launch_bounds__(256) k_text_eot(const int64_t* __restrict__ ids, int* __restrict__ eot, int n, int ctx) {
-  pdl_trigger(); pdl_wait();
   const int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (s >= n) return;
   long long best = ids[(size_t)s * ctx];
@@ -77,7 +75,6 @@ __global__ void __launch_bounds__(256) k_text_eot(const int64_t* __restrict__ id
 template <int NCH>
 __global__ void __launch_bounds__(256) k_text_pool_ln(const float* __restrict__ x, const int* __restrict__ eot, const float* __restrict__ gamma,
                                                       const float* __restrict__ beta, bf16* __restrict__ y, int n, int ctx, int D) {
-  pdl_trigger(); pdl_wait();
   const int s = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (s >= n) return;
   constexpr int N = 4 * NCH;
@@ -98,7 +95,7 @@ int attn_causal_launch(const bf16* qkv, bf16* out, int S, int T, int D, int head
     APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd_tc<NW, NT2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_tc_fwd_smem<NW, NT2>()));
     cfg = true;
   }
-  APH_CUDA_OK(launch_k(k_attn_fwd_tc<NW, NT2, true>, dim3(S * heads), dim3(NW * 32), attn_tc_fwd_smem<NW, NT2>(), st, 1, qkv, out, T, D, heads));
+  k_attn_fwd_tc<NW, NT2, true><<<S * heads, NW * 32, attn_tc_fwd_smem<NW, NT2>(), st>>>(qkv, out, T, D, heads);
   APH_LAUNCH_OK();
   return 0;
 }
@@ -196,14 +193,14 @@ extern "C" int aph_text_fwd(aph_text* text, const int64_t* tokens, int n, float*
   const int D = t->cfg.width, C = t->cfg.context, H = t->cfg.heads, O = t->cfg.out_dim;
   const int M = n * C;
   int e;
-  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_text_embed<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, tokens, t->tok_emb, t->pos, t->x, M, C, D, t->cfg.vocab)));
+  NCH_DISPATCH(D, k_text_embed<NCH><<<rows_grid(M), 256, 0, st>>>(tokens, t->tok_emb, t->pos, t->x, M, C, D, t->cfg.vocab));
   APH_LAUNCH_OK();
-  APH_CUDA_OK(launch_k(k_text_eot, dim3(rows_grid(n)), dim3(256), (size_t)0, st, 1, tokens, t->eot, n, C));
+  k_text_eot<<<rows_grid(n), 256, 0, st>>>(tokens, t->eot, n, C);
   APH_LAUNCH_OK();
   const BlockIO io{t->x, t->x_mid, t->x, t->ln_out, t->qkv, t->attn_out, t->h_pre, t->h_act, t->mean, t->rstd, t->mean, t->rstd};
   for (const BlockW& w : t->L)
     if ((e = block_fwd(w, io, n, C, M, 0, D, H, attn_causal, st))) return e;
-  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_text_pool_ln<NCH>, dim3(rows_grid(n)), dim3(256), (size_t)0, st, 1, t->x, t->eot, t->lnf_w, t->lnf_b, t->pooled, n, C, D)));
+  NCH_DISPATCH(D, k_text_pool_ln<NCH><<<rows_grid(n), 256, 0, st>>>(t->x, t->eot, t->lnf_w, t->lnf_b, t->pooled, n, C, D));
   APH_LAUNCH_OK();
   GemmEpi ep; ep.out_f32 = emb;
   return launch_gemm(t->pooled, t->w_out, GemmShape{n, O, D}, ep, st);

@@ -71,20 +71,15 @@ static size_t stat_off(const VitImpl* v, int k) {
 
 bool gemm_profiling_on();      // vit_gemm.cu
 
-static bool graphs_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("APH_VIT_GRAPH"); v = (e && e[0] == '0') ? 0 : 1; }
-  return v == 1 && !gemm_profiling_on();
-}
-
 // Runs `body` through the graph cache: 1st call with a key runs eagerly (lazy one-time initialisations are not capturable),
 // 2nd call captures + instantiates, later calls replay.
 template <typename Body>
 static int run_cached(std::vector<VitImpl::GraphEntry>& cache, std::map<int, int>& warm, unsigned long long& stamp, int& misses,
                       const void* in, const void* out, int S, int flag, cudaStream_t& st, Body body) {
-  // a caller whose buffers move every step (clip_fft.py calls torch.cuda.empty_cache() per step) would re-capture forever:
-  // after 6 never-replayed captures in a row the handle stays eager
-  if (!graphs_enabled() || misses > 6) return body();
+  // GEMM profiling (aph_prof_gemm) records events around each launch, so it runs eagerly. A caller whose buffers move every
+  // step (clip_fft.py calls torch.cuda.empty_cache() per step) would re-capture forever: after 6 never-replayed captures in a
+  // row the handle stays eager
+  if (gemm_profiling_on() || misses > 6) return body();
   for (auto& g : cache)
     if (g.in == in && g.out == out && g.S == S && g.flag == flag) {
       g.stamp = ++stamp;
@@ -222,16 +217,14 @@ int check_loaded(const Encoder* h, std::vector<std::string> want, const char* wh
 int block_fwd(const BlockW& w, const BlockIO& io, int S, int T, int Mr, int ld_tok, int D, int heads, AttnFwd attn, cudaStream_t st) {
   const int M = S * T;
   int e;
-  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, io.x_in, w.ln1_w, w.ln1_b, io.ln_out, io.mean1,
-                                       io.rstd1, M, D)));
+  NCH_DISPATCH(D, k_ln_fwd<NCH><<<rows_grid(M), 256, 0, st>>>(io.x_in, w.ln1_w, w.ln1_b, io.ln_out, io.mean1, io.rstd1, M, D));
   APH_LAUNCH_OK();
   { GemmEpi ep; ep.bias = w.b_qkv; ep.out_bf16 = io.qkv;
     if ((e = launch_gemm(io.ln_out, w.w_qkv, GemmShape{M, 3 * D, D}, ep, st))) return e; }
   if ((e = attn(io.qkv, io.attn_out, S, T, D, heads, st))) return e;
   { GemmEpi ep; ep.bias = w.b_o; ep.resid = io.x_in; ep.ld_resid = ld_tok; ep.out_f32 = io.x_mid;
     if ((e = launch_gemm(io.attn_out, w.w_o, GemmShape{Mr, D, D}, ep, st, ld_tok))) return e; }
-  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(Mr)), dim3(256), (size_t)0, st, 1, io.x_mid, w.ln2_w, w.ln2_b, io.ln_out, io.mean2,
-                                       io.rstd2, Mr, D)));
+  NCH_DISPATCH(D, k_ln_fwd<NCH><<<rows_grid(Mr), 256, 0, st>>>(io.x_mid, w.ln2_w, w.ln2_b, io.ln_out, io.mean2, io.rstd2, Mr, D));
   APH_LAUNCH_OK();
   { GemmEpi ep; ep.bias = w.b_fc; ep.out_pre = io.h_pre; ep.act = 1; ep.out_bf16 = io.h_act;
     if ((e = launch_gemm(io.ln_out, w.w_fc, GemmShape{Mr, 4 * D, D}, ep, st))) return e; }
@@ -414,10 +407,10 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, int side, floa
     const int p = v->cfg.patch;
     if (v->Kp == 3 * p * p) {                // rows without padding (p = 16, 32): 8 columns per thread
       const size_t n8 = (size_t)Mp * v->Kp / 8;
-      APH_CUDA_OK(launch_k(k_patchify<false>, dim3((unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1, images, v->patches, S, p, g, side));
+      k_patchify<false><<<(unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)num_sms() * 16), 256, 0, st>>>(images, v->patches, S, p, g, side);
     } else {                                 // padded rows (p = 14): pixel pairs
       const size_t n2 = (size_t)Mp * 3 * p * p / 2;
-      APH_CUDA_OK(launch_k(k_patchify<true>, dim3((unsigned)std::min<size_t>((n2 + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1, images, v->patches, S, p, g, side));
+      k_patchify<true><<<(unsigned)std::min<size_t>((n2 + 255) / 256, (size_t)num_sms() * 16), 256, 0, st>>>(images, v->patches, S, p, g, side);
     }
     APH_LAUNCH_OK();
   }
@@ -429,8 +422,8 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, int side, floa
   {
     GemmEpi ep; ep.out_f32 = v->tok;
     if ((e = launch_gemm(v->patches, v->w_conv, GemmShape{Mp, D, v->Kp}, ep, st))) return e;
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_embed_lnpre<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, v->tok, v->cls, v->pos, v->lnpre_w, v->lnpre_b, v->e, v->xs[0],
-                                                                      v->st_mean, v->st_rstd, S, T, D)));
+    NCH_DISPATCH(D, k_embed_lnpre<NCH><<<rows_grid(M), 256, 0, st>>>(v->tok, v->cls, v->pos, v->lnpre_w, v->lnpre_b, v->e, v->xs[0],
+                                                                       v->st_mean, v->st_rstd, S, T, D));
     APH_LAUNCH_OK();
   }
   for (int l = 0; l < Ly; ++l) {
@@ -443,8 +436,7 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, int side, floa
   }
   {
     float* meanp = v->st_mean + stat_off(v, 2 * Ly + 1); float* rstdp = v->st_rstd + stat_off(v, 2 * Ly + 1);
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(S)), dim3(256), (size_t)0, st, 1, v->xs[2 * Ly], v->lnpost_w, v->lnpost_b, v->cls_ln,
-                                                                 meanp, rstdp, S, D)));
+    NCH_DISPATCH(D, k_ln_fwd<NCH><<<rows_grid(S), 256, 0, st>>>(v->xs[2 * Ly], v->lnpost_w, v->lnpost_b, v->cls_ln, meanp, rstdp, S, D));
     APH_LAUNCH_OK();
     GemmEpi ep; ep.out_f32 = v->emb_int;
     if ((e = launch_gemm(v->cls_ln, v->w_out, GemmShape{S, O, D}, ep, st))) return e;
@@ -468,7 +460,7 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
   cudaStream_t st = (cudaStream_t)stream;
   {   // caller-owned input: converted outside the cached graph (see aph_vit_fwd)
     const size_t n = (size_t)S * v->cfg.out_dim;
-    APH_CUDA_OK(launch_k(k_f32_to_bf16, dim3((int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8)), dim3(256), (size_t)0, st, 1, grad_emb, v->d_emb, n));
+    k_f32_to_bf16<<<(int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8), 256, 0, st>>>(grad_emb, v->d_emb, n);
     APH_LAUNCH_OK();
   }
   const int rc = run_cached(v->bwd_graphs, v->warm_bwd, v->stamp, v->graph_misses, nullptr, nullptr, S, 0, st, [&]() -> int {
@@ -480,8 +472,8 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
     if ((e = launch_gemm(v->d_emb, v->w_out_t, GemmShape{S, D, O}, ep, st))) return e;
     // ln_post: the gradient reaching the last block is non-zero on its cls rows only; it is kept compact in dxc / dxc_bf
     float* meanp = v->st_mean + stat_off(v, 2 * Ly + 1); float* rstdp = v->st_rstd + stat_off(v, 2 * Ly + 1);
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH>, dim3(rows_grid(S)), dim3(256), (size_t)0, st, 1, v->d_cls, v->xs[2 * Ly], meanp, rstdp, v->lnpost_w, v->dxc, v->dxc_bf,
-                                                                 S, T, D, 0, 0, (const float*)nullptr)));
+    NCH_DISPATCH(D, k_ln_bwd<NCH><<<rows_grid(S), 256, 0, st>>>(v->d_cls, v->xs[2 * Ly], meanp, rstdp, v->lnpost_w, v->dxc, v->dxc_bf,
+                                                                S, T, D, 0, 0, (const float*)nullptr));
     APH_LAUNCH_OK();
   }
   for (int l = Ly - 1; l >= 0; --l) {
@@ -498,8 +490,8 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
       if ((e = launch_gemm(gx_bf, w.w_proj_t, GemmShape{Mr, 4 * D, D}, ep, st))) return e; }
     { GemmEpi ep; ep.out_bf16 = v->d_ln;
       if ((e = launch_gemm(v->dh, w.w_fc_t, GemmShape{Mr, D, 4 * D}, ep, st))) return e; }
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH, bf16>, dim3(rows_grid(Mr)), dim3(256), (size_t)0, st, 1, v->d_ln, x_mid, mean2, rstd2, w.ln2_w, gx, gx_bf, Mr, T, D, 0, 1,
-                                         (const float*)nullptr)));
+    NCH_DISPATCH(D, k_ln_bwd<NCH, bf16><<<rows_grid(Mr), 256, 0, st>>>(v->d_ln, x_mid, mean2, rstd2, w.ln2_w, gx, gx_bf, Mr, T, D, 0, 1,
+                                                                       (const float*)nullptr));
     APH_LAUNCH_OK();
     // attention branch: d_attn = dx . W_o; (dq,dk,dv) = attn'(...); d_ln1 = d_qkv . W_qkv
     { GemmEpi ep; ep.out_bf16 = d_attn; ep.ld_out = last ? T * D : 0;
@@ -508,13 +500,13 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
     { GemmEpi ep; ep.out_bf16 = v->d_ln;
       if ((e = launch_gemm(v->d_qkv, w.w_qkv_t, GemmShape{M, D, 3 * D}, ep, st))) return e; }
     // ln_1: back to all M rows; in the last block dx is written here for the first time (+ dxc on the cls rows)
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH, bf16>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, v->d_ln, x_in, mean1, rstd1, w.ln1_w, v->dx, v->dx_bf, M, T, D,
-                                         last ? 1 : 0, 1, (const float*)(last ? v->dxc : nullptr))));
+    NCH_DISPATCH(D, k_ln_bwd<NCH, bf16><<<rows_grid(M), 256, 0, st>>>(v->d_ln, x_in, mean1, rstd1, w.ln1_w, v->dx, v->dx_bf, M, T, D,
+                                                                      last ? 1 : 0, 1, (const float*)(last ? v->dxc : nullptr)));
     APH_LAUNCH_OK();
   }
   // ln_pre backward (cls rows dropped) and patch-embed data gradient scattered back to NCHW
-  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH>, dim3(rows_grid(M)), dim3(256), (size_t)0, st, 1, v->dx, v->e, v->st_mean, v->st_rstd, v->lnpre_w, nullptr, v->d_tok, M, T, D, 2, 0,
-                                       (const float*)nullptr)));
+  NCH_DISPATCH(D, k_ln_bwd<NCH><<<rows_grid(M), 256, 0, st>>>(v->dx, v->e, v->st_mean, v->st_rstd, v->lnpre_w, nullptr, v->d_tok, M, T, D, 2, 0,
+                                                              (const float*)nullptr));
   APH_LAUNCH_OK();
   return 0;
   });
@@ -530,8 +522,8 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
     if (int e = launch_gemm(v->d_tok, v->w_conv_t, GemmShape{Mp, v->Kp, v->D}, ep, st)) return e;
     if (sized) {
       const size_t n = (size_t)S * 3 * side * side;
-      APH_CUDA_OK(launch_k(k_window_expand, dim3((unsigned)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16)), dim3(256), (size_t)0, st, 1,
-                           (const float*)g_win.p, grad_images, S * 3, R, side));
+      k_window_expand<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16), 256, 0, st>>>((const float*)g_win.p, grad_images,
+                                                                                                            S * 3, R, side);
       APH_LAUNCH_OK();
     }
   }
@@ -572,8 +564,7 @@ extern "C" int aph_attn_long_test(int fwd, const void* qkv, const void* dout, vo
 extern "C" int aph_ln_fwd_test(const float* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows, int D,
                                void* stream) {
   APH_REQUIRE(x && gamma && beta && y && mean && rstd && rows > 0 && D % 128 == 0, "aph_ln_fwd_test: null argument or rows=%d D=%d", rows, D);
-  NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_fwd<NCH>, dim3(rows_grid(rows)), dim3(256), (size_t)0, (cudaStream_t)stream, 1, x, gamma, beta,
-                                       reinterpret_cast<bf16*>(y), mean, rstd, rows, D)));
+  NCH_DISPATCH(D, k_ln_fwd<NCH><<<rows_grid(rows), 256, 0, (cudaStream_t)stream>>>(x, gamma, beta, reinterpret_cast<bf16*>(y), mean, rstd, rows, D));
   APH_LAUNCH_OK();
   return 0;
 }
@@ -587,11 +578,11 @@ extern "C" int aph_ln_bwd_test(const void* dy, int dy_bf16, const float* x, cons
   cudaStream_t st = (cudaStream_t)stream;
   bf16* dxb = reinterpret_cast<bf16*>(dx_bf16);
   if (dy_bf16)
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH, bf16>, dim3(rows_grid(rows)), dim3(256), (size_t)0, st, 1, reinterpret_cast<const bf16*>(dy), x,
-                                         mean, rstd, gamma, dx, dxb, rows, T, D, mode, accumulate, dcls)))
+    NCH_DISPATCH(D, k_ln_bwd<NCH, bf16><<<rows_grid(rows), 256, 0, st>>>(reinterpret_cast<const bf16*>(dy), x, mean, rstd, gamma, dx, dxb,
+                                                                         rows, T, D, mode, accumulate, dcls))
   else
-    NCH_DISPATCH(D, APH_CUDA_OK(launch_k(k_ln_bwd<NCH>, dim3(rows_grid(rows)), dim3(256), (size_t)0, st, 1, reinterpret_cast<const float*>(dy), x,
-                                         mean, rstd, gamma, dx, dxb, rows, T, D, mode, accumulate, dcls)))
+    NCH_DISPATCH(D, k_ln_bwd<NCH><<<rows_grid(rows), 256, 0, st>>>(reinterpret_cast<const float*>(dy), x, mean, rstd, gamma, dx, dxb,
+                                                                   rows, T, D, mode, accumulate, dcls))
   APH_LAUNCH_OK();
   return 0;
 }

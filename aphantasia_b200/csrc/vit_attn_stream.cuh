@@ -27,7 +27,6 @@ constexpr size_t kStreamBwdSmem = (size_t)4 * kStreamRows * 128 + kStreamRows * 
 static_assert(kStreamFwdSmem <= 48 * 1024 && kStreamBwdSmem <= 48 * 1024, "streaming attention: static shared memory above 48 KB");
 
 __global__ void __launch_bounds__(128) k_attn_fwd_stream(const bf16* __restrict__ qkv, bf16* __restrict__ out, int T, int D, int heads) {
-  pdl_trigger(); pdl_wait();
   __shared__ __align__(128) uint8_t sm[kStreamFwdSmem];
   uint8_t* Qs = sm; uint8_t* Ks = Qs + kStreamRows * 128; uint8_t* Vs = Ks + kStreamRows * 128;
   const int nb = (T + kStreamRows - 1) / kStreamRows;
@@ -76,7 +75,6 @@ __global__ void __launch_bounds__(128) k_attn_fwd_stream(const bf16* __restrict_
 // dQ and the row statistics of one query block. stats: float2 [S*heads, T] = (lse, delta) per query row (log2 domain).
 __global__ void __launch_bounds__(128) k_attn_bwd_stream_q(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, bf16* __restrict__ dqkv,
                                                            float2* __restrict__ stats, int T, int D, int heads) {
-  pdl_trigger(); pdl_wait();
   __shared__ __align__(128) uint8_t sm[kStreamBwdSmem];
   uint8_t* Qs = sm; uint8_t* Gs = Qs + kStreamRows * 128; uint8_t* Ks = Gs + kStreamRows * 128; uint8_t* Vs = Ks + kStreamRows * 128;
   const int nb = (T + kStreamRows - 1) / kStreamRows;
@@ -163,7 +161,6 @@ __global__ void __launch_bounds__(128) k_attn_bwd_stream_q(const bf16* __restric
 // S^T = K Q^T and dP^T = V dO^T per streamed query tile, then dV += P^T dO and dK += dS^T Q straight from registers.
 __global__ void __launch_bounds__(128) k_attn_bwd_stream_kv(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, bf16* __restrict__ dqkv,
                                                             const float2* __restrict__ stats, int T, int D, int heads) {
-  pdl_trigger(); pdl_wait();
   __shared__ __align__(128) uint8_t sm[kStreamBwdSmem];
   uint8_t* Ks = sm; uint8_t* Vs = Ks + kStreamRows * 128; uint8_t* Qs = Vs + kStreamRows * 128; uint8_t* Gs = Qs + kStreamRows * 128;
   float2* Ls = reinterpret_cast<float2*>(Gs + kStreamRows * 128);
@@ -236,14 +233,13 @@ static int attn_stream(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_or
   const size_t blocks = (size_t)S * heads * ((T + kStreamRows - 1) / kStreamRows);
   APH_REQUIRE(blocks < (1u << 31), "attention: S=%d T=%d heads=%d is too many blocks", S, T, heads);
   if (fwd) {
-    APH_CUDA_OK(launch_k(k_attn_fwd_stream, dim3((unsigned)blocks), dim3(128), (size_t)0, st, 1, qkv, out_or_dqkv, T, D, heads));
+    k_attn_fwd_stream<<<(unsigned)blocks, 128, 0, st>>>(qkv, out_or_dqkv, T, D, heads);
     APH_LAUNCH_OK();
     return 0;
   }
-  APH_CUDA_OK(launch_k(k_attn_bwd_stream_q, dim3((unsigned)blocks), dim3(128), (size_t)0, st, 1, qkv, dout, out_or_dqkv, stats, T, D, heads));
+  k_attn_bwd_stream_q<<<(unsigned)blocks, 128, 0, st>>>(qkv, dout, out_or_dqkv, stats, T, D, heads);
   APH_LAUNCH_OK();
-  APH_CUDA_OK(launch_k(k_attn_bwd_stream_kv, dim3((unsigned)blocks), dim3(128), (size_t)0, st, 1, qkv, dout, out_or_dqkv, (const float2*)stats, T, D,
-                       heads));
+  k_attn_bwd_stream_kv<<<(unsigned)blocks, 128, 0, st>>>(qkv, dout, out_or_dqkv, (const float2*)stats, T, D, heads);
   APH_LAUNCH_OK();
   return 0;
 }

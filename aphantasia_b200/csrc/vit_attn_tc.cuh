@@ -159,7 +159,6 @@ __device__ __forceinline__ void store_frag(bf16* dst, size_t rb, size_t ld, int 
 // CAUSAL (the CLIP text tower): query row i attends to keys j <= i only; forward only.
 template <int NW, int NT2, bool CAUSAL = false>
 __global__ void __launch_bounds__(NW * 32) k_attn_fwd_tc(const bf16* __restrict__ qkv, bf16* __restrict__ out, int T, int D, int heads) {
-  pdl_trigger(); pdl_wait();
   extern __shared__ __align__(128) uint8_t sm[];
   constexpr int TK = NT2 * 16, QB = NW * 16;
   uint8_t* Ks = sm; uint8_t* Vs = Ks + TK * 128; uint8_t* Qs = Vs + TK * 128;
@@ -205,7 +204,6 @@ template <int NW, int NT2>
 __global__ void __launch_bounds__(NW * 32, 1) k_attn_bwd_tc(const bf16* __restrict__ qkv, const bf16* __restrict__ dout, bf16* __restrict__ dqkv,
                                                          int T, int D, int heads) {
   static_assert(NT2 > 4, "k_attn_bwd_tc serves T > 64; k_attn_bwd_tc1 serves T <= 64");
-  pdl_trigger(); pdl_wait();
   extern __shared__ __align__(128) uint8_t sm[];
   constexpr int TK = NT2 * 16, QB = NW * 16, KT = (NT2 + NW - 1) / NW, PB = ((TK + 63) / 64) * 128;
   uint8_t* Ks = sm; uint8_t* Vs = Ks + TK * 128; uint8_t* Qs = Vs + TK * 128; uint8_t* Gs = Qs + QB * 128;
@@ -349,7 +347,6 @@ __global__ void __launch_bounds__(NW * 32, 1) k_attn_bwd_tc(const bf16* __restri
 template <int NT2>
 __global__ void __launch_bounds__(128) k_attn_fwd_tc1(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_q,
                                                       bf16* __restrict__ out, int T, int D, int heads, int items) {
-  pdl_trigger(); pdl_wait();
   extern __shared__ __align__(1024) uint8_t sm_raw[];
   __shared__ __align__(8) uint64_t full[2];
   constexpr int TK = NT2 * 16, QB = 64, BUF = (2 * TK + QB) * 128;
@@ -427,7 +424,6 @@ template <int NT2>
 __global__ void __launch_bounds__(128, 2) k_attn_bwd_tc1(const __grid_constant__ CUtensorMap tm_kv, const __grid_constant__ CUtensorMap tm_q,
                                                          const __grid_constant__ CUtensorMap tm_do, bf16* __restrict__ dqkv,
                                                          int T, int D, int heads, int items) {
-  pdl_trigger(); pdl_wait();
   extern __shared__ __align__(1024) uint8_t sm_raw[];
   __shared__ __align__(8) uint64_t full[2];
   constexpr int TK = NT2 * 16, QB = 64, PB = 128, BUF = (2 * TK + 2 * QB) * 128;
@@ -549,12 +545,12 @@ static int attn_launch1(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_o
   if (fwd) {
     const int per_sm = (int)(220 * 1024 / smem_f) < 6 ? (int)(220 * 1024 / smem_f) : 6;
     const int grid = items < num_sms() * per_sm ? items : num_sms() * per_sm;
-    APH_CUDA_OK(launch_k(k_attn_fwd_tc1<NT2>, dim3(grid), dim3(128), smem_f, st, 1, tm_kv, tm_q, out_or_dqkv, T, D, heads, items));
+    k_attn_fwd_tc1<NT2><<<grid, 128, smem_f, st>>>(tm_kv, tm_q, out_or_dqkv, T, D, heads, items);
   } else {
     if (int e = make_tmap_bf16_tokens(&tm_do, dout, D, T, S, 64)) return e;
     const int per_sm = (int)(220 * 1024 / smem_b) < 3 ? (int)(220 * 1024 / smem_b) : 3;
     const int grid = items < num_sms() * per_sm ? items : num_sms() * per_sm;
-    APH_CUDA_OK(launch_k(k_attn_bwd_tc1<NT2>, dim3(grid), dim3(128), smem_b, st, 1, tm_kv, tm_q, tm_do, out_or_dqkv, T, D, heads, items));
+    k_attn_bwd_tc1<NT2><<<grid, 128, smem_b, st>>>(tm_kv, tm_q, tm_do, out_or_dqkv, T, D, heads, items);
   }
   APH_LAUNCH_OK();
   return 0;
@@ -576,8 +572,8 @@ static int attn_launch(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_or
     APH_CUDA_OK(cudaFuncSetAttribute(k_attn_bwd_tc<NW, NT2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     cfg = true;
   }
-  if (fwd) APH_CUDA_OK(launch_k(k_attn_fwd_tc<NW, NT2>, dim3(S * heads), dim3(NW * 32), attn_tc_fwd_smem<NW, NT2>(), st, 1, qkv, out_or_dqkv, T, D, heads));
-  else APH_CUDA_OK(launch_k(k_attn_bwd_tc<NW, NT2>, dim3(S * heads), dim3(NW * 32), attn_tc_bwd_smem<NW, NT2>(), st, 1, qkv, dout, out_or_dqkv, T, D, heads));
+  if (fwd) k_attn_fwd_tc<NW, NT2><<<S * heads, NW * 32, attn_tc_fwd_smem<NW, NT2>(), st>>>(qkv, out_or_dqkv, T, D, heads);
+  else k_attn_bwd_tc<NW, NT2><<<S * heads, NW * 32, attn_tc_bwd_smem<NW, NT2>(), st>>>(qkv, dout, out_or_dqkv, T, D, heads);
   APH_LAUNCH_OK();
   return 0;
 }

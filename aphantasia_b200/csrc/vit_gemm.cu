@@ -102,7 +102,7 @@ static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi
   const int grid = tiles < num_sms() ? tiles : num_sms();
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   if (g_prof) { cudaEventCreate(&e0); cudaEventCreate(&e1); cudaEventRecord(e0, st); }
-  APH_CUDA_OK(launch_k(k_gemm_bf16_tn<BN, PINGPONG, EPI>, dim3(grid), dim3(GEMM_THREADS), (size_t)L::SMEM, st, 1, ma, mb, shp, epi));
+  k_gemm_bf16_tn<BN, PINGPONG, EPI><<<grid, GEMM_THREADS, (size_t)L::SMEM, st>>>(ma, mb, shp, epi);
   APH_LAUNCH_OK();
   if (g_prof) { cudaEventRecord(e1, st); g_prof_ev.emplace_back(e0, e1); g_prof_flops.push_back(2.0 * shp.M * shp.N * shp.K); }
   return 0;

@@ -28,7 +28,6 @@ namespace aph {
 // thread, so that neither a patch-row boundary nor the end of the 3 p^2 columns falls inside one thread's vector.
 template <bool PAIRS>
 static __global__ void __launch_bounds__(256) k_patchify(const float* __restrict__ img, bf16* __restrict__ out, int S, int p, int g, int side) {
-  pdl_trigger(); pdl_wait();
   if (PAIRS) {
     const int R = side, P3 = 3 * p * p, Kp = patch_k(p);
     const size_t total = (size_t)S * g * g * P3 / 2;
@@ -68,7 +67,6 @@ static __global__ void __launch_bounds__(256) k_patchify(const float* __restrict
 
 // planes [n,R,R] -> [n,side,side] (side >= R): the window at the top left, zeros in the margin
 static __global__ void __launch_bounds__(256) k_window_expand(const float* __restrict__ src, float* __restrict__ dst, int n, int R, int side) {
-  pdl_trigger(); pdl_wait();
   const size_t total = (size_t)n * side * side;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
     const size_t plane = idx / ((size_t)side * side);
@@ -78,7 +76,6 @@ static __global__ void __launch_bounds__(256) k_window_expand(const float* __res
 }
 
 static __global__ void __launch_bounds__(256) k_f32_to_bf16(const float* __restrict__ in, bf16* __restrict__ out, size_t n) {
-  pdl_trigger(); pdl_wait();
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     out[i] = __float2bfloat16_rn(in[i]);
 }
@@ -143,7 +140,6 @@ __global__ void __launch_bounds__(256) k_embed_lnpre(const float* __restrict__ t
                                                      const float* __restrict__ beta, float* __restrict__ e_out,
                                                      float* __restrict__ x0, float* __restrict__ mean_out, float* __restrict__ rstd_out,
                                                      int S, int T, int D) {
-  pdl_trigger(); pdl_wait();
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (row >= S * T) return;
   const int s = row / T, t = row - s * T;
@@ -169,7 +165,6 @@ template <int NCH>
 __global__ void __launch_bounds__(256) k_ln_fwd(const float* __restrict__ x, const float* __restrict__ gamma,
                                                 const float* __restrict__ beta, bf16* __restrict__ y, float* __restrict__ mean_out,
                                                 float* __restrict__ rstd_out, int rows, int D) {
-  pdl_trigger(); pdl_wait();
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (row >= rows) return;
   constexpr int N = 4 * NCH;
@@ -209,7 +204,6 @@ __global__ void __launch_bounds__(256) k_ln_bwd(const DY* __restrict__ dy, const
                                                 const float* __restrict__ rstd, const float* __restrict__ gamma,
                                                 float* __restrict__ dx, bf16* __restrict__ dx_bf16, int rows, int T, int D,
                                                 int mode, int accumulate, const float* __restrict__ dcls) {
-  pdl_trigger(); pdl_wait();
   const int r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (r >= rows) return;
   constexpr int N = 4 * NCH;
