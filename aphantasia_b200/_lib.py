@@ -33,6 +33,7 @@ _SIGS = {
     'aph_pixel_bwd': (C.c_int, [c_f32p, c_f32p, c_f32p, C.c_void_p, C.c_int64, C.c_float, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_void_p]),
     'aph_valid_rgb_fwd': (C.c_int, [c_f32p, C.c_int64, C.c_void_p, c_f32p, C.c_void_p]),
     'aph_valid_rgb_bwd': (C.c_int, [c_f32p, c_f32p, C.c_int64, C.c_void_p, c_f32p, C.c_void_p]),
+    'aph_affine_fwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p, c_f32p, C.c_void_p]),
     'aph_sample_fwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     'aph_sample_fwd_patches': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_void_p, C.c_int,
                                          C.POINTER(C.c_int), C.c_void_p]),

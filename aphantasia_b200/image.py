@@ -171,28 +171,50 @@ class _SynthFFT(torch.autograd.Function):
         return gp, None, None, None, None, None
 
 
+# ---- one FFT plan per (H, W) and one radial scale per (H, W, decay) for the life of the process. illustrip.py builds a new
+# fft_image every frame (illustrip.py:409); a plan of its own would cost four cudaMalloc on creation and four device-synchronising
+# cudaFree when the previous frame's generator is dropped, plus an upload of the scale.
+# Sharing a plan is safe because no plan buffer carries data from one API call to the next (csrc/synth_fft.cu): the twiddles are
+# written once at creation and only read; T and gimg are scratch that every call (aph_synth_fft_fwd / _bwd / _bwd_adam,
+# aph_fft_analyze) writes before it reads them within that same call. Calls issued on one stream therefore never see each other's
+# scratch, whichever generator issues them; generators sharing a plan must not run their calls concurrently on different streams.
+_fft_plans = {}
+_fft_scales = {}
+fft_plans_created = 0          # plans this process has created for fft_image generators
+
+
+def _shared_fft_plan(h, w):
+    global fft_plans_created
+    plan = _fft_plans.get((h, w))
+    if plan is None:
+        plan = C.c_void_p()
+        check(lib().aph_fft_plan_create(C.byref(plan), h, w), 'aph_fft_plan_create')
+        _fft_plans[(h, w)] = plan
+        fft_plans_created += 1
+    return plan
+
+
+def _shared_fft_scale(h, w, decay_power):
+    key = (h, w, float(decay_power))
+    scale = _fft_scales.get(key)
+    if scale is None:
+        freqs = rfft2d_freqs(h, w)
+        s = 1. / np.maximum(freqs, 4. / max(h, w)) ** decay_power      # image.py:159-161 (float64 on the host)
+        s *= np.sqrt(h * w)
+        scale = _fft_scales[key] = torch.tensor(s).float().contiguous().cuda()
+    return scale
+
+
 class FFTImage:
     """The `image_f` closure of fft_image (image.py:164-175) as a callable object, so to_valid_rgb can fuse into it."""
 
     def __init__(self, params, h, w, decay_power):
         self.params, self.h, self.w, self.wh = params, h, w, w // 2 + 1
-        freqs = rfft2d_freqs(h, w)
-        scale = 1. / np.maximum(freqs, 4. / max(h, w)) ** decay_power      # image.py:159-161 (float64 on the host)
-        scale *= np.sqrt(h * w)
-        self.scale = torch.tensor(scale).float().contiguous().cuda()
-        plan = C.c_void_p()
-        check(lib().aph_fft_plan_create(C.byref(plan), h, w), 'aph_fft_plan_create')
-        self.plan = plan
+        self.scale = _shared_fft_scale(h, w, decay_power)
+        self.plan = _shared_fft_plan(h, w)
         self.fused_opt, self.pending_fwd = None, 0          # aphantasia_b200.optim.Adam hooks in here (row f2)
         from .optim import register_generator
         register_generator(params, self)
-
-    def __del__(self):
-        try:
-            if getattr(self, 'plan', None):
-                lib().aph_fft_plan_destroy(self.plan)
-        except Exception:
-            pass
 
     def fused(self, shift, contrast, colmat, sigmoid):
         if torch.is_grad_enabled() and self.params.requires_grad:

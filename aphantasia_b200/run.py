@@ -7,8 +7,11 @@
 Why a launcher: `python /path/clip_fft.py` puts the SCRIPT's directory at sys.path[0], ahead of PYTHONPATH, so
 `from aphantasia.image import ...` (clip_fft.py:24-25) would resolve to the reference's own package sitting next to the
 script, not to dropin/aphantasia. Here dropin/ is inserted ahead of the script directory, the reference's module names
-(`aphantasia`, `clip`, `imageio`, `lpips`) are imported FIRST and checked to come from dropin/, and only then the script
-runs as __main__ (runpy). Equivalent without this module: `PYTHONSAFEPATH=1 PYTHONPATH=<repo>/dropin:<repo> python clip_fft.py`.
+(`aphantasia`, `clip`, `imageio`, `lpips`, `depth`) are imported FIRST and checked to come from dropin/, and only then the
+script runs as __main__ (runpy). Before it runs, torchvision.transforms.functional.affine is routed through
+aphantasia_b200.motion (illustrip.py's per-frame camera motion; clip_fft.py never calls it). Equivalent without this module:
+`PYTHONSAFEPATH=1 PYTHONPATH=<repo>/dropin:<repo> python clip_fft.py`. For illustrip.py that runs the drop-in too, but its
+per-frame motion stays on torchvision's own path unless `aphantasia_b200.motion.install()` is called before the script runs.
 """
 import atexit
 import os
@@ -19,7 +22,7 @@ import time
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG_DIR)
 DROPIN = os.path.join(ROOT, 'dropin')
-SHADOWED = ('aphantasia', 'clip', 'imageio', 'lpips')
+SHADOWED = ('aphantasia', 'clip', 'imageio', 'lpips', 'depth')
 
 
 def install_dropin(script_dir=None):
@@ -45,7 +48,7 @@ def install_dropin(script_dir=None):
             raise
         f = os.path.abspath(getattr(m, '__file__', '') or '')
         origins[name] = f
-        if name in ('aphantasia', 'clip') and not f.startswith(DROPIN + os.sep):
+        if name in ('aphantasia', 'clip', 'depth') and not f.startswith(DROPIN + os.sep):
             raise RuntimeError('aphantasia_b200.run: `%s` resolved to %s, not to %s -- the script would run the reference '
                                'PyTorch path, not libaphb200.so' % (name, f, DROPIN))
     return origins
@@ -70,6 +73,8 @@ def main(argv=None):
         sys.stderr.write('aphantasia_b200.run: no such script: %s\n' % script)
         return 2
     origins = install_dropin(os.path.dirname(script))
+    from . import motion
+    motion.install()
     if os.environ.get('APH_FUSED_ADAM', '0') == '1':          # row f2: torch.optim.Adam over our spectrum -> fused into the synth backward
         from . import optim
         optim.install()

@@ -4,6 +4,8 @@ slice_imgs (utils.py:218-254) and sim_func (utils.py:276-295) are the hot-path e
 replays the reference's RNG order into a parameter table (_rng.py) and two fused CUDA launches each way do the rest
 (csrc/sample.cu; csrc/loss.cu for the loss). The remaining names are the thin IO helpers clip_fft.py imports.
 """
+import collections.abc
+import math
 import os
 
 import numpy as np
@@ -469,3 +471,213 @@ def aesthetic_model(clip_model='ViT-B/32'):
 
 def plot_text(txt, size=224):
     raise NotImplementedError('aphantasia_b200: plot_text needs matplotlib; never called by clip_fft.py')
+
+
+# ---------------------------------------------------------------------------------------------- helpers illustrip.py / illustra.py import
+# (illustrip.py:28, illustra.py:19). Host-side list, path and timeline helpers; the values they return are the original's
+# (utils.py:32-38, 47-59, 102-126, 149-216, 299-396), bit for bit where NumPy / SciPy compute them.
+def intrl(a, b, step=2):
+    """Replaces every `step`-th entry of list `a` (from index `step` on) by the entry of `b` at that index, in place."""
+    assert len(a) == len(b), ' diff lengths: %d %d' % (len(a), len(b))
+    assert step > 1
+    for k in range(step, len(a), step):
+        a[k] = b[k]
+    return a
+
+
+def file_list(path, ext=None, subdir=None):
+    """Sorted paths of the files in `path` (recursively with subdir=True); ext: a suffix string, or a list of extensions."""
+    if subdir is True:
+        found = [os.path.join(d, f) for d, _, names in os.walk(path) for f in names]
+    else:
+        found = [os.path.join(path, f) for f in os.listdir(path)]
+    if isinstance(ext, list):
+        found = [f for f in found if os.path.splitext(f.lower())[1][1:] in ext]
+    elif isinstance(ext, str):
+        found = [f for f in found if f.endswith(ext)]
+    elif ext is not None:
+        print(' Unknown extension/type for file list!')
+    return sorted(f for f in found if os.path.isfile(f))
+
+
+def cvshow(img):
+    """The original opens an OpenCV preview window; there is no display to show it on, so this does nothing."""
+
+
+def _write_dict(d, out, indent=''):
+    for k in sorted(d.keys()):
+        v = d[k]
+        if isinstance(v, collections.abc.Mapping):
+            out(indent + str(k), ' \n')
+            _write_dict(v, out, indent + '   ')
+        else:
+            out('%s%s: %s' % (indent, str(k), str(v)), ' \n')
+
+
+def save_cfg(args, dir='./', file='config.txt'):
+    """Writes the arguments (a Namespace or a dict), sorted by name, one `name: value ` line each, to dir/file; prints
+    them when file is None."""
+    if dir != '':
+        os.makedirs(dir, exist_ok=True)
+    try:
+        args = vars(args)
+    except TypeError:
+        pass
+    if file is None:
+        _write_dict(args, lambda line, end: print(line))
+    else:
+        with open(os.path.join(dir, file), 'w') as f:
+            _write_dict(args, lambda line, end: f.write(line + end))
+
+
+def tile_pad(xt, padding, symm=False):
+    """Pads the last two axes by (left, right, top, bottom) by repeating the image (symm=True: mirroring it), for any pad
+    length: every padded index maps back into the image through a periodic index map."""
+    h, w = xt.shape[-2:]
+    left, right, top, bottom = padding
+
+    def wrap(idx, lo, hi):
+        period = hi - lo
+        if symm is True:
+            m = np.fmod(idx - lo, 2 * period)
+            m = np.where(m < 0, m + 2 * period, m)
+            m = np.where(m >= period, 2 * period - m, m) + lo
+        else:
+            m = np.remainder(idx - lo, period) + lo
+        return np.array(m, dtype=idx.dtype)
+
+    cols = wrap(np.arange(-left, w + right), -0.5, w - 0.5)
+    rows = wrap(np.arange(-top, h + bottom), -0.5, h - 0.5)
+    xx, yy = np.meshgrid(cols, rows)
+    return xt[..., yy, xx]
+
+
+def pad_up_to(x, size, type='centr'):
+    """Pads [..., H, W] up to size = (H', W') with tile_pad: centred by default, at the far side with 'side' in type,
+    mirrored with 'symm' in type."""
+    if list(x.shape[2:]) == list(size):
+        return x
+    padding = []
+    for have, want in zip(list(x.shape[2:])[::-1], list(size)[::-1]):     # width first, then height
+        extra = want - have
+        first = 0 if 'side' in type.lower() else extra // 2
+        padding += [first, extra - first]
+    return tile_pad(x, padding, symm=('symm' in type.lower()))
+
+
+def smoothstep(x, NN=1., xmin=0., xmax=1.):
+    """The order-N smoothstep polynomial of x clipped to [xmin, xmax], N = ceil(NN); a fractional NN averages it with x."""
+    import scipy.special
+    N = math.ceil(NN)
+    x = np.clip((x - xmin) / (xmax - xmin), 0, 1)
+    poly = 0
+    for n in range(N + 1):
+        poly += scipy.special.comb(N + n, n) * scipy.special.comb(2 * N + 1, N - n) * (-x) ** n
+    poly *= x ** (N + 1)
+    return (x + poly) / 2 if NN != N else poly
+
+
+def _steps01(num_steps, smooth):
+    xs = [k / (num_steps - 1) for k in range(num_steps)]
+    return [smoothstep(x, smooth) for x in xs] if smooth > 0 else xs
+
+
+def slerp(z1, z2, num_steps=None, x=None, smooth=0.5):
+    """Torch tensors z1 -> z2: the straight line between them, rescaled at each point to |z1| over the norm of the line
+    from z1 to z2 rescaled to |z1|. num_steps points from 0 to 1, or the single point x; concatenated along axis 0."""
+    n1 = z1.norm()
+    z2_on_sphere = z2 * (n1 / z2.norm())
+    xs = _steps01(num_steps, 0) if num_steps is not None else [x]
+    if smooth > 0:
+        xs = [smoothstep(t, smooth) for t in xs]
+    out = []
+    for t in xs:
+        plain = z1 + (z2 - z1) * t
+        norm = (z1 + (z2_on_sphere - z1) * t).norm()
+        if norm != 0:
+            point = plain * (n1 / norm)
+        out.append(point)          # a zero norm repeats the previous point, as the original does
+    return torch.cat(out)
+
+
+def get_z(shape, rnd, uniform=False):
+    return rnd.uniform(0., 1., shape) if uniform else rnd.randn(*shape)
+
+
+def lerp(z1, z2, num_steps, smooth=0.):
+    return np.array([z1 + (z2 - z1) * t for t in _steps01(num_steps, smooth)])
+
+
+def slerp_np(z1, z2, num_steps, smooth=0.):
+    """NumPy slerp (see slerp) with num_steps points from z1 to z2."""
+    n1 = np.linalg.norm(z1)
+    z2_on_sphere = z2 * (n1 / np.linalg.norm(z2))
+    out = []
+    for t in _steps01(num_steps, smooth):
+        plain = z1 + (z2 - z1) * t
+        out.append(plain * (n1 / np.linalg.norm(z1 + (z2_on_sphere - z1) * t)))
+    return np.array(out)
+
+
+def cublerp(points, steps, fstep, looped=True):
+    """Cubic spline through `steps` key points placed fstep frames apart, closed by the first point (looped) or the last:
+    steps * fstep + 1 frames."""
+    from scipy.interpolate import CubicSpline
+    keys = np.array([k * fstep for k in range(steps + 1)])
+    closing = points[0] if looped is True else points[-1]
+    spline = CubicSpline(keys, np.concatenate((points, np.expand_dims(closing, 0))))
+    return spline(np.arange(steps * fstep + 1))
+
+
+def _clock_seed():
+    """What the original's latent_anima does without a seed: reseed NumPy's global stream from the clock
+    (np.random.seed(int((time.time() % 1) * 9999)), whose None return becomes the seed) and draw the key latents from a
+    RandomState seeded by the OS. Returns that RandomState's seed, drawn here so it can be shared: under torchrun rank 0's
+    clock value and seed are broadcast, so that every rank moves its replicated canvas the same way and continues the same
+    NumPy stream (the crop replay reads it)."""
+    import time
+    vals = np.array([int((time.time() % 1) * 9999)] + list(np.frombuffer(os.urandom(16), np.uint32)), np.int64)
+    if _dist.world() > 1:
+        t = torch.from_numpy(vals).to('cuda' if _dist.backend_is_nccl() else 'cpu')
+        torch.distributed.broadcast(t, 0)
+        vals = t.cpu().numpy()
+    np.random.seed(int(vals[0]))
+    return vals[1:].astype(np.uint32)
+
+
+def latent_anima(shape, frames, transit, key_latents=None, smooth=0.5, uniform=False, cubic=False, gauss=False, start_lat=None,
+                 seed=None, looped=True, verbose=False):
+    """A timeline of `frames` latents of `shape`: key latents drawn (or given) every `transit` frames, joined by a cubic
+    spline (cubic=True) or by lerp (uniform=True) / slerp segments, optionally smoothed by a wrapped Gaussian."""
+    if key_latents is None:
+        transit = int(max(1, min(frames // 2, transit)))
+    steps = max(1, math.ceil(frames / transit))
+    log = ' timeline: %d steps by %d' % (steps, transit)
+    rnd = np.random.RandomState(_clock_seed() if seed is None else seed)
+    if key_latents is None:
+        key_latents = np.array([get_z(shape, rnd, uniform) for _ in range(steps)])
+    if start_lat is not None:
+        key_latents[0] = start_lat
+
+    if transit == 1:
+        latents = key_latents
+    elif cubic:
+        latents = cublerp(key_latents, steps, transit, looped)
+        log += ', cubic'
+    else:
+        parts = [np.expand_dims(key_latents[0], 0)]
+        for k in range(steps):
+            nxt = (k + 1) % steps if looped is True else min(k + 1, steps - 1)
+            join = lerp if uniform is True else slerp_np
+            parts.append(join(key_latents[k], key_latents[nxt], transit, smooth=smooth))
+        latents = np.concatenate(parts)
+    latents = np.array(latents)
+
+    if gauss:
+        from scipy.ndimage import gaussian_filter
+        blurred = gaussian_filter(latents, [transit, 0, 0], mode='wrap')
+        latents = blurred / np.linalg.norm(blurred, axis=-1, keepdims=True) * math.sqrt(np.prod(shape))
+        log += ', gauss'
+    if verbose:
+        print(log)
+    return latents[1:] if latents.shape[0] > frames else latents

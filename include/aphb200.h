@@ -132,6 +132,14 @@ int aph_valid_rgb_fwd(const float* img, int64_t hw, const float* colmat_host, fl
 int aph_valid_rgb_bwd(const float* grad_out, const float* out, int64_t hw, const float* colmat_host,
                       float* grad_img, void* stream);
 
+/* ================= per-frame camera motion (illustrip.py) =====================================
+ * Replaces frame_transform's T.functional.affine(img, angle, shift, scale, shear, fill=0, interpolation=BILINEAR)
+ * (illustrip.py:130-138) on a CUDA tensor: torchvision's _gen_affine_grid (pixel-centre grid, align_corners=False),
+ * grid_sample bilinear with zero padding, and the fill-0 blend out = sample(img) * sample(ones). Forward only.
+ * in / out [planes,H,W] (must not alias); inv_matrix_host: 6 doubles, HOST, the inverse matrix of torchvision's
+ * _get_inverse_affine_matrix (centre (0, 0) = the image centre). One launch.                                      */
+int aph_affine_fwd(const float* in, int planes, int H, int W, const double* inv_matrix_host, float* out, void* stream);
+
 /* ================= L2: multi-crop sampler =====================================================
  * Replaces the per-crop Python loop of slice_imgs (aphantasia/utils.py:243-253) + transforms_fast
  * (aphantasia/transforms.py:165-170): bicubic(A=-0.75, align_corners, crop-clamped) -> perspective
