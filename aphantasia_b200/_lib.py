@@ -73,7 +73,14 @@ _SIGS = {
     'aph_sim_fwd': (C.c_int, [c_f32p, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, c_f32p, C.c_void_p]),
     'aph_derivat_fwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p, c_f32p, C.c_void_p]),
     'aph_derivat_bwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, C.c_void_p]),
-    'aph_head_fwd': (C.c_int, [c_f32p, C.c_int, C.c_int, c_f32p, c_f32p, c_f32p, C.c_void_p]),
+    'aph_derivat_sobel_fwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p, c_f32p, C.c_void_p]),
+    'aph_derivat_sobel_bwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, C.c_void_p]),
+    'aph_cppn_create': (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
+    'aph_cppn_destroy': (C.c_int, [C.c_void_p]),
+    'aph_cppn_fwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), c_f32p, C.c_void_p]),
+    'aph_cppn_bwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), c_f32p, C.POINTER(C.c_void_p),
+                               C.c_void_p]),
+    'aph_head_fwd':(C.c_int, [c_f32p, C.c_int, C.c_int, c_f32p, c_f32p, c_f32p, C.c_void_p]),
     'aph_head_bwd': (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     'aph_synth_fft_bwd_adam': (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, C.c_void_p, c_f32p, C.c_float, C.c_void_p, C.c_int,
                                          c_f32p, c_f32p, c_f32p, c_f32p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p]),

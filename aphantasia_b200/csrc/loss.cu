@@ -108,6 +108,71 @@ __global__ void __launch_bounds__(256) k_derivat_bwd(const float* __restrict__ i
   }
 }
 
+// derivat(img, mode='sobel') (/root/reference/aphantasia/utils.py:262-264; cppn.py:291-292 --sharp):
+//   mean |kornia.filters.spatial_gradient(img)|: the 3x3 Sobel pair normalised by 1/8, replicate padding, both directions,
+//   the mean over the N C 2 H W outputs. sums[0] accumulates |gx| + |gy| in fp64; k_derivat_sobel_fin divides.
+// gx (y, x) = (sum over the rows y-1, y, y+1 with weights 1, 2, 1 of p(., x+1) - p(., x-1)) / 8, indices clamped to the frame;
+// gy is the same with the axes swapped.
+__device__ __forceinline__ void sobel_at(const float* __restrict__ pl, int H, int W, int y, int x, float& gx, float& gy) {
+  const int ym = max(y - 1, 0), yp = min(y + 1, H - 1), xm = max(x - 1, 0), xp = min(x + 1, W - 1);
+  const float* rm = pl + (size_t)ym * W;
+  const float* r0 = pl + (size_t)y * W;
+  const float* rp = pl + (size_t)yp * W;
+  gx = ((rm[xp] - rm[xm]) + 2.f * (r0[xp] - r0[xm]) + (rp[xp] - rp[xm])) * 0.125f;
+  gy = ((rp[xm] - rm[xm]) + 2.f * (rp[x] - rm[x]) + (rp[xp] - rm[xp])) * 0.125f;
+}
+__global__ void __launch_bounds__(256) k_derivat_sobel_fwd(const float* __restrict__ img, int C, int H, int W, double* __restrict__ sums) {
+  const size_t hw = (size_t)H * W, n = (size_t)C * hw;
+  double s = 0.;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t c = i / hw, q = i - c * hw;
+    const int y = (int)(q / W), x = (int)(q - (size_t)y * W);
+    float gx, gy;
+    sobel_at(img + c * hw, H, W, y, x, gx, gy);
+    s += fabsf(gx) + fabsf(gy);
+  }
+  s = warp_sum_d(s);
+  __shared__ double red[8];
+  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) red[wid] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double a = 0.;
+    for (int i = 0; i < 8; ++i) a += red[i];
+    atomicAdd(&sums[0], a);
+  }
+}
+__global__ void k_derivat_sobel_fin(const double* __restrict__ sums, double n, float* __restrict__ value) { *value = (float)(sums[0] / n); }
+// Adjoint: pixel (yy, xx) gathers sign(g) k from every output (y, x) within one pixel whose clamped tap lands on it (several
+// taps of an edge output land on the same edge pixel), times upstream / (8 N C 2 H W). sign(0) = 0, as torch.abs's gradient.
+__global__ void __launch_bounds__(256) k_derivat_sobel_bwd(const float* __restrict__ img, int C, int H, int W, const float* __restrict__ up,
+                                                           float scale, float* __restrict__ grad) {
+  const size_t hw = (size_t)H * W, n = (size_t)C * hw;
+  const float g = up[0] * scale;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t c = i / hw, q = i - c * hw;
+    const int yy = (int)(q / W), xx = (int)(q - (size_t)yy * W);
+    const float* pl = img + c * hw;
+    float acc = 0.f;                       // integer-valued: exact
+    for (int y = max(yy - 1, 0); y <= min(yy + 1, H - 1); ++y)
+      for (int x = max(xx - 1, 0); x <= min(xx + 1, W - 1); ++x) {
+        float gx, gy;
+        sobel_at(pl, H, W, y, x, gx, gy);
+        const float sx = sgnf(gx), sy = sgnf(gy);
+        if (sx == 0.f && sy == 0.f) continue;
+        for (int a = 0; a < 3; ++a) {
+          if (min(max(y + a - 1, 0), H - 1) != yy) continue;
+          for (int b = 0; b < 3; ++b) {
+            if (min(max(x + b - 1, 0), W - 1) != xx) continue;
+            // Sobel taps (row a, column b): x kernel (b - 1) (2 - |a - 1|), y kernel (a - 1) (2 - |b - 1|)
+            acc += sx * (float)((b - 1) * (2 - abs(a - 1))) + sy * (float)((a - 1) * (2 - abs(b - 1)));
+          }
+        }
+      }
+    grad[i] = g * acc;
+  }
+}
+
 // Linear head on the embeddings (the LAION aesthetic predictor of --aest is nn.Linear(512, 1), utils.py:402-413; clip_fft.py:255-256):
 // out[s] = <emb_s, w> + b; one warp per sample.
 __global__ void __launch_bounds__(256) k_head_fwd(const float* __restrict__ emb, int S, int D, const float* __restrict__ w,
@@ -149,6 +214,28 @@ extern "C" int aph_derivat_bwd(const float* img, int C, int H, int W, const floa
   const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8);
   k_derivat_bwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(img, C, H, W, upstream, (float)(1.0 / ((double)C * H * (W - 1))),
                                                          (float)(1.0 / ((double)C * (H - 1) * W)), grad_img);
+  APH_LAUNCH_OK();
+  return 0;
+}
+
+extern "C" int aph_derivat_sobel_fwd(const float* img, int C, int H, int W, double* sums, float* value, void* stream) {
+  APH_REQUIRE(img && sums && value && C > 0 && H > 0 && W > 0, "aph_derivat_sobel_fwd: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  APH_CUDA_OK(cudaMemsetAsync(sums, 0, sizeof(double), st));
+  const size_t n = (size_t)C * H * W;
+  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8);
+  k_derivat_sobel_fwd<<<blocks, 256, 0, st>>>(img, C, H, W, sums);
+  APH_LAUNCH_OK();
+  k_derivat_sobel_fin<<<1, 1, 0, st>>>(sums, 2.0 * (double)n, value);
+  APH_LAUNCH_OK();
+  return 0;
+}
+
+extern "C" int aph_derivat_sobel_bwd(const float* img, int C, int H, int W, const float* upstream, float* grad_img, void* stream) {
+  APH_REQUIRE(img && upstream && grad_img && C > 0 && H > 0 && W > 0, "aph_derivat_sobel_bwd: bad arguments");
+  const size_t n = (size_t)C * H * W;
+  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8);
+  k_derivat_sobel_bwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(img, C, H, W, upstream, (float)(1.0 / (16.0 * (double)n)), grad_img);
   APH_LAUNCH_OK();
   return 0;
 }

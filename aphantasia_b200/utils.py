@@ -400,12 +400,36 @@ class _Derivat(torch.autograd.Function):
         return grad
 
 
+class _DerivatSobel(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, img):
+        x = img.detach().contiguous().float()
+        C, H, W = x.shape[0] * x.shape[1], x.shape[2], x.shape[3]
+        sums = torch.empty(1, device=x.device, dtype=torch.float64)
+        val = torch.empty((), device=x.device, dtype=torch.float32)
+        check(lib().aph_derivat_sobel_fwd(x.data_ptr(), C, H, W, sums.data_ptr(), val.data_ptr(), stream_ptr()), 'aph_derivat_sobel_fwd')
+        ctx.save_for_backward(x)
+        return val
+
+    @staticmethod
+    def backward(ctx, g):
+        x, = ctx.saved_tensors
+        up = g.detach().float().reshape(1).contiguous()
+        grad = torch.empty_like(x)
+        check(lib().aph_derivat_sobel_bwd(x.data_ptr(), x.shape[0] * x.shape[1], x.shape[2], x.shape[3], up.data_ptr(), grad.data_ptr(),
+                                          stream_ptr()), 'aph_derivat_sobel_bwd')
+        return grad
+
+
 def derivat(img, mode='sobel'):
-    """utils.py:256-268. clip_fft.py:272 only ever passes mode='naiv' (the finite-difference branch): one fused reduction
-    kernel + its adjoint (csrc/loss.cu). The kornia / conv2d modes are not provided."""
-    if mode in ('scharr', 'sobel'):
-        raise NotImplementedError('aphantasia_b200.derivat: only the finite-difference mode used by clip_fft.py is provided')
+    """utils.py:256-268. clip_fft.py:272 passes mode='naiv' (the finite-difference branch), cppn.py:292 mode='sobel'
+    (mean |kornia spatial_gradient|): each is one fused reduction kernel + its adjoint (csrc/loss.cu). 'scharr' is not provided."""
+    if mode == 'scharr':
+        raise NotImplementedError("aphantasia_b200.derivat: mode='scharr' is not provided; 'sobel' and the finite-difference mode are")
     require_cuda(img, 'derivat input')
+    if mode == 'sobel':
+        assert img.dim() == 4, 'derivat expects [N,C,H,W]'
+        return _DerivatSobel.apply(img)
     assert img.dim() == 4 and img.shape[2] > 1 and img.shape[3] > 1, 'derivat expects [N,C,H,W]'
     return _Derivat.apply(img)
 

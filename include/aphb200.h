@@ -140,6 +140,26 @@ int aph_valid_rgb_bwd(const float* grad_out, const float* out, int64_t hw, const
  * _get_inverse_affine_matrix (centre (0, 0) = the image centre). One launch.                                      */
 int aph_affine_fwd(const float* in, int planes, int H, int W, const double* inv_matrix_host, float* out, void* stream);
 
+/* ================= CPPN generator (cppn.py) ===================================================
+ * Replaces CPPN.forward (cppn.py:71-116): a per-pixel MLP from the coordinate to RGB, written as 1x1 convolutions.
+ * Layer 0: 2 -> nf; layers 1 .. layers-1: kh -> nf; output: kh -> 3, sigmoid. kh = 2 nf for act 0 `unbias`
+ * (t = atan z, cat(t / 0.67, (t^2 - 0.45) / 0.396)) and act 1 `comp` (cat(t / 0.67, t^2 / 0.6)), kh = nf for act 2 `relu`
+ * ((relu z - 0.4) / 0.58). The hidden layers' products run in TF32 (operands rounded by cvt.rna), everything else in fp32.
+ * aph_cppn_create accepts nf a multiple of 8 in [8, 64] and layers in [1, 32] and refuses anything else (host only, no GPU
+ * work). The handle owns the backward's scratch.
+ * params / dparams: HOST arrays of 2 (layers + 1) DEVICE pointers {W0, b0, W1, b1, ..., W_layers, b_layers}, W_l the
+ * nn.Conv2d weight [out, in, 1, 1] (8-byte aligned), read in place by every call.
+ * coords [N,2,H,W] -> out [N,3,H,W]; pixel p = n H W + h W + w. One launch.                                        */
+typedef struct aph_cppn aph_cppn;
+int aph_cppn_create(int nf, int layers, int act, aph_cppn** handle);
+int aph_cppn_destroy(aph_cppn* handle);
+int aph_cppn_fwd(aph_cppn* handle, const float* coords, int N, int H, int W, const float* const* params, float* out,
+                 void* stream);
+/* grad_out [N,3,H,W] -> every dparams tensor (overwritten); no coordinate gradient. Recomputes the forward. Two launches;
+ * the weight gradient is reduced in a fixed order, so repeated calls give bit-identical results.                        */
+int aph_cppn_bwd(aph_cppn* handle, const float* coords, int N, int H, int W, const float* const* params,
+                 const float* grad_out, float* const* dparams, void* stream);
+
 /* ================= L2: multi-crop sampler =====================================================
  * Replaces the per-crop Python loop of slice_imgs (aphantasia/utils.py:243-253) + transforms_fast
  * (aphantasia/transforms.py:165-170): bicubic(A=-0.75, align_corners, crop-clamped) -> perspective
@@ -305,6 +325,11 @@ int aph_sim_fwd(const float* v1, int n1, const float* v2, int S, int D, int kind
  * upstream gradient read from a DEVICE scalar.                                                      */
 int aph_derivat_fwd(const float* img, int C, int H, int W, double* sums, float* value, void* stream);
 int aph_derivat_bwd(const float* img, int C, int H, int W, const float* upstream, float* grad_img, void* stream);
+/* derivat(img, mode='sobel') (aphantasia/utils.py:262-264; cppn.py:291-292 --sharp): mean |kornia spatial_gradient(img)|, the
+ * Sobel pair normalised by 1/8 with replicate padding, over the 2*C*H*W outputs. img [C,H,W] (C = N*channels); sums = double[1]
+ * device scratch. The backward multiplies by the upstream gradient read from a DEVICE scalar; sign(0) = 0.            */
+int aph_derivat_sobel_fwd(const float* img, int C, int H, int W, double* sums, float* value, void* stream);
+int aph_derivat_sobel_bwd(const float* img, int C, int H, int W, const float* upstream, float* grad_img, void* stream);
 /* Linear head on the embeddings: the LAION aesthetic predictor of --aest is nn.Linear(D, 1)
  * (aphantasia/utils.py:402-413; clip_fft.py:255-256). out[s] = <emb_s, w> + b[0] (b may be NULL).   */
 int aph_head_fwd(const float* emb, int S, int D, const float* w, const float* b, float* out, void* stream);
