@@ -75,7 +75,7 @@ _SIGS = {
     'aph_derivat_bwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, C.c_void_p]),
     'aph_derivat_sobel_fwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p, c_f32p, C.c_void_p]),
     'aph_derivat_sobel_bwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, C.c_void_p]),
-    'aph_cppn_create': (C.c_int, [C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
+    'aph_cppn_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int]),
     'aph_cppn_destroy': (C.c_int, [C.c_void_p]),
     'aph_cppn_fwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), c_f32p, C.c_void_p]),
     'aph_cppn_bwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), c_f32p, C.POINTER(C.c_void_p),
@@ -124,9 +124,48 @@ def lib():
     return _lib
 
 
-def check(rc, what):
+def check(rc, what, error=RuntimeError):
     if rc != 0:
-        raise RuntimeError('%s failed (rc=%d): %s' % (what, rc, lib().aph_last_error().decode('utf-8', 'replace')))
+        raise error('%s failed (rc=%d): %s' % (what, rc, lib().aph_last_error().decode('utf-8', 'replace')))
+
+
+class Handle:
+    """One library object `<api>`, made by `<api>_create(&handle, *args)` and owned from then on: close() (or garbage
+    collection) destroys it once, after the device's pending work, which may still use it, has finished. ctypes takes it
+    wherever the ABI takes the handle. A create that fails raises `error`."""
+
+    def __init__(self, api, *args, error=RuntimeError):
+        self.api, self.loaded = api, False
+        h = C.c_void_p()
+        check(getattr(lib(), api + '_create')(C.byref(h), *args), api + '_create', error)
+        self._as_parameter_ = h
+
+    def load(self, state_dict, prefix=''):
+        """`<api>_load_tensor` for every fp32 tensor of `state_dict` (key = prefix + its key), then `<api>_finalize`: `loaded`
+        once that succeeds. A failed load raises RuntimeError and leaves the handle owned and not loaded."""
+        import torch
+        load, st = getattr(lib(), self.api + '_load_tensor'), stream_ptr()
+        for k, v in state_dict.items():
+            d = v.cuda()
+            check(load(self, (prefix + k).encode(), d.data_ptr(), d.numel(), st), '%s_load_tensor(%s)' % (self.api, k))
+        torch.cuda.current_stream().synchronize()      # the staging copies `d` die with this scope
+        check(getattr(lib(), self.api + '_finalize')(self), self.api + '_finalize')
+        self.loaded = True
+
+    def close(self):
+        h = self.__dict__.pop('_as_parameter_', None)
+        self.loaded = False
+        if h is not None:
+            import torch
+            if torch.cuda.is_initialized():
+                torch.cuda.synchronize()
+            getattr(lib(), self.api + '_destroy')(h)
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:          # interpreter shutdown: the modules this needs may be gone
+            pass
 
 
 def stream_ptr():

@@ -19,7 +19,7 @@ from collections import OrderedDict
 import torch
 
 from .. import _patchlink, _pool, _trace
-from .._lib import TextConfig, VitConfig, check, lib, require_cuda, stream_ptr
+from .._lib import Handle, TextConfig, VitConfig, check, lib, require_cuda, stream_ptr
 from ._bpe import SimpleTokenizer
 
 _MODELS = {'ViT-B/32': dict(patch=32, width=768, layers=12, heads=12, out_dim=512, res=224),
@@ -103,34 +103,21 @@ def has_text_tower(state_dict):
 
 
 class _Tower:
-    """A tower's device handle, built through the C ABI's `<api>_create`, `_load_tensor` and `_finalize` from `self._sd`.
-    The handle is owned from its creation on: when a load or the finalize fails, close() still frees it."""
-    _api = None
+    """A tower's device handle (a `Handle` of `_api`), loaded from `self._sd` for batches of up to max_batch samples. It is
+    owned from its creation on: when a load or the finalize fails, close() still frees it."""
+    _api, _prefix = None, ''
     handle, max_batch = None, 0
 
-    def _build(self, cfg, max_batch, prefix=''):
+    def _build(self, cfg, max_batch):
         self.close()
-        h = C.c_void_p()
-        check(getattr(lib(), self._api + '_create')(C.byref(h), C.byref(cfg)), self._api + '_create')
-        self.handle = h
-        load, st = getattr(lib(), self._api + '_load_tensor'), stream_ptr()
-        for k, v in self._sd.items():
-            d = v.cuda()
-            check(load(h, (prefix + k).encode(), d.data_ptr(), d.numel(), st), '%s_load_tensor(%s)' % (self._api, k))
-        torch.cuda.current_stream().synchronize()      # staging copies `d` die with this scope
-        check(getattr(lib(), self._api + '_finalize')(h), self._api + '_finalize')
+        self.handle = Handle(self._api, C.byref(cfg))
+        self.handle.load(self._sd, self._prefix)
         self.max_batch = int(max_batch)
 
     def close(self):
         if self.handle is not None:
-            getattr(lib(), self._api + '_destroy')(self.handle)
-            self.handle, self.max_batch = None, 0
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
+            self.handle.close()
+        self.handle, self.max_batch = None, 0
 
 
 class TextTransformer(_Tower):
@@ -220,7 +207,7 @@ class _EncodeImage(torch.autograd.Function):
 
 class VisionTransformer(_Tower):
     """Handle-owning mirror of clip.model.VisionTransformer (forward only through the C ABI)."""
-    _api = 'aph_vit'
+    _api, _prefix = 'aph_vit', 'visual.'
 
     def __init__(self, state_dict, max_batch=None):
         sd = {k[len('visual.'):]: v for k, v in state_dict.items() if k.startswith('visual.')}
@@ -242,8 +229,7 @@ class VisionTransformer(_Tower):
         """(Re)creates the device handle so that its activation arena holds S samples."""
         if self.handle is not None and S <= self.max_batch:
             return
-        self._build(VitConfig(self.patch_size, self.width, self.layers, self.heads, self.output_dim, self.input_resolution, int(S), 0),
-                    S, 'visual.')
+        self._build(VitConfig(self.patch_size, self.width, self.layers, self.heads, self.output_dim, self.input_resolution, int(S), 0), S)
         self._handle_epoch += 1
 
     def _fwd(self, xi, S, emb, save_for_bwd):

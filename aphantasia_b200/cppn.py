@@ -15,7 +15,7 @@ import torch
 import torch.nn as nn
 
 from . import _trace
-from ._lib import check, lib, require_cuda, stream_ptr
+from ._lib import Handle, check, lib, require_cuda, stream_ptr
 
 __all__ = ['ConvLayer', 'CPPN']
 
@@ -77,11 +77,7 @@ class CPPN(nn.Module):
             raise _unsupported('nf_out = %s' % nf_out)
         if act_fn not in ACTS:
             raise _unsupported("act_fn = '%s'" % act_fn)
-        h = C.c_void_p()
-        rc = lib().aph_cppn_create(int(nf_hid), int(num_layers), ACTS[act_fn], h)
-        if rc != 0:
-            raise NotImplementedError(lib().aph_last_error().decode('utf-8', 'replace'))
-        self._handle = h.value
+        self._handle = Handle('aph_cppn', int(nf_hid), int(num_layers), ACTS[act_fn], error=NotImplementedError)
         self.act_fn = act_fn
         nf_hid_in = nf_hid if act_fn == 'relu' else nf_hid * 2
         net = [ConvLayer(nf_in, nf_hid, act_fn)]
@@ -89,17 +85,6 @@ class CPPN(nn.Module):
             net.append(ConvLayer(nf_hid_in, nf_hid, act_fn))
         net.append(ConvLayer(nf_hid_in, nf_out, 'sigmoid'))
         self.net = nn.Sequential(*net)
-
-    def __del__(self):
-        h = self.__dict__.get('_handle')
-        if h is not None and lib is not None:
-            try:
-                if torch.cuda.is_initialized():
-                    torch.cuda.synchronize()
-                lib().aph_cppn_destroy(h)
-            except Exception:
-                pass
-            self._handle = None
 
     def _params(self):
         ps = []

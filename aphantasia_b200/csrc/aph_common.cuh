@@ -11,6 +11,8 @@
 
 namespace aph {
 
+typedef __nv_bfloat16 bf16;
+
 void set_error(const char* fmt, ...);          // defined in api.cu (thread-local message)
 extern std::atomic<long long> g_launches;      // kernels launched by this library
 

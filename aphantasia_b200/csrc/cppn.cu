@@ -467,7 +467,7 @@ int check_call(const aph_cppn* h, const float* coords, int N, int H, int W, cons
 
 }  // namespace
 
-extern "C" int aph_cppn_create(int nf, int layers, int act, aph_cppn** handle) {
+extern "C" int aph_cppn_create(aph_cppn** handle, int nf, int layers, int act) {
   APH_REQUIRE(handle, "aph_cppn_create: bad arguments");
   APH_REQUIRE(nf >= 8 && nf <= 64 && nf % 8 == 0, "aph_cppn_create: nf = %d is not supported: nf must be a multiple of 8 in [8, 64]", nf);
   APH_REQUIRE(layers >= 1 && layers <= CPPN_MAX_LAYERS, "aph_cppn_create: layers = %d is not supported: layers must be in [1, %d]",

@@ -1,10 +1,9 @@
-// encoder.cuh -- what the CLIP image tower (vit.cu) and text tower (text.cu) share: a handle's device allocations, the residual
-// block's weights (allocated, loaded and checked from one table of its tensors) and the block's forward. Defined in vit.cu.
+// encoder.cuh -- what the CLIP image tower (vit.cu) and text tower (text.cu) share: the residual block's weights, added to the
+// handle's weight table (weights.cuh) block by block, and the block's forward. Defined in vit.cu.
 #pragma once
 #include "vit_ops.cuh"
+#include "weights.cuh"
 #include <map>
-#include <string>
-#include <vector>
 
 namespace aph {
 
@@ -19,38 +18,13 @@ struct BlockW {
   bf16 *w_proj = nullptr, *w_proj_t = nullptr;   // [D, 4D], [4D, D]
 };
 
-// The part of a tower's handle that both towers have. Its device allocations are freed with it.
-struct Encoder {
-  int64_t bytes = 0;                      // aph_vit_bytes / aph_text_bytes
-  std::vector<void*> allocs;
+// The part of a tower's handle that both towers have
+struct Encoder : Weights {
   std::vector<BlockW> L;
-  std::map<std::string, bool> loaded;     // state-dict keys, the image tower's without "visual."
-  bool finalized = false;
-  ~Encoder() { for (void* p : allocs) cudaFree(p); }
 };
 
-template <typename Tp>
-int dev_alloc(Encoder* h, Tp** p, size_t count) {
-  void* q = nullptr;
-  APH_CUDA_OK(cudaMalloc(&q, count * sizeof(Tp)));
-  h->allocs.push_back(q);
-  h->bytes += (int64_t)(count * sizeof(Tp));
-  *p = reinterpret_cast<Tp*>(q);
-  return 0;
-}
-
-// `layers` blocks of width D; with dgrad, also the transposed operands of the data gradient
-int alloc_blocks(Encoder* h, int layers, int D, bool dgrad);
-// k = "transformer.resblocks.<i>.<field>" -> block i's slot (and its transpose when allocated). `key` is the caller's key and
-// `who` the entry point, for the error messages.
-int load_block_tensor(Encoder* h, const std::string& k, const char* key, const float* data, int64_t numel, int D, cudaStream_t st,
-                      const char* who);
-// every key of `want` and of the blocks was loaded; a missing one is named as prefix + key
-int check_loaded(const Encoder* h, std::vector<std::string> want, const char* who, const char* prefix);
-
-// fp32 [rows, cols] -> bf16 [rows, cols] (transpose = 0, row stride ld, 0 = cols) or bf16 [cols, rows] (transpose = 1)
-int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st, int ld = 0);
-int copy_f32(const float* src, float* dst, size_t n, cudaStream_t st);
+// `layers` blocks of width D under "transformer.resblocks.<i>."; with dgrad, also the transposed operands of the data gradient
+int add_blocks(Encoder* h, int layers, int D, bool dgrad);
 
 // grid of the one-warp-per-row kernels
 inline int rows_grid(int rows) { return (rows * 32 + 255) / 256; }

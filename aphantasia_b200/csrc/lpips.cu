@@ -18,9 +18,7 @@
 // under a caller-supplied key (clip_fft.py passes the same reference picture every step). Both grow to the largest shape seen and
 // survive torch.cuda.empty_cache(). Every forward bumps a generation; a backward must name the generation it belongs to.
 #include "conv_tc.cuh"
-#include <string.h>
-#include <string>
-#include <vector>
+#include "weights.cuh"
 
 namespace aph {
 
@@ -229,18 +227,6 @@ __global__ void __launch_bounds__(256) k_tap_bwd(const bf16* __restrict__ f0, co
   }
 }
 
-// ---- weight packing --------------------------------------------------------------------------------------
-// w fp32 [Co, Ci, 3, 3] -> forward operand wf [Co][tap][Ci] and data-gradient operand wb [Ci][tap][Co] = w[co][ci][8 - tap]
-__global__ void k_pack_w(const float* __restrict__ w, int Co, int Ci, bf16* __restrict__ wf, bf16* __restrict__ wb) {
-  const size_t n = (size_t)Co * Ci * 9;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int t = (int)(i % 9), ci = (int)((i / 9) % Ci), co = (int)(i / (9 * (size_t)Ci));
-    const bf16 v = __float2bfloat16(w[i]);
-    if (wf) wf[((size_t)co * 9 + t) * Ci + ci] = v;
-    if (wb) wb[((size_t)ci * 9 + (8 - t)) * Co + co] = v;
-  }
-}
-
 // ---- launchers ----------------------------------------------------------------------------------------------
 template <int BN, int EPI>
 static int conv_cfg(const void* x, const void* wpack, const ConvShape& cs, const ConvEpi& epi, cudaStream_t st) {
@@ -314,13 +300,12 @@ struct LpLayout {           // element offsets (bf16) of the 13 conv outputs and
 
 using namespace aph;
 
-struct aph_lpips {
+struct aph_lpips : Weights {
   float* w0 = nullptr;                      // conv1_1 fp32 [64][27]
   float* bias[LP_CONVS] = {};               // fp32 [Cout]
   bf16* wf[LP_CONVS] = {};                  // [Cout, 9 Cin] (l >= 1)
   bf16* wb[LP_CONVS] = {};                  // [Cin, 9 Cout] (l >= 1)
   float* lin[LP_TAPS] = {};                 // [C_t]
-  bool got_w[LP_CONVS] = {}, got_b[LP_CONVS] = {}, got_lin[LP_TAPS] = {}, finalized = false;
   Scratch main_arena, ref_arena, grads, part;
   int64_t generation = 0, saved_generation = -1;
   int sN = 0, sH = 0, sW = 0, s_norm = 0;   // shape of the saved forward
@@ -346,83 +331,37 @@ static int vgg_forward(aph_lpips* h, const float* img, int N, int H, int W, int 
   return 0;
 }
 
+// Keys: torchvision's "features.{i}.weight" [Co,Ci,3,3] / "features.{i}.bias" [Co] for the 13 convolutions, and lpips'
+// "lin{t}.model.1.weight" [1,C,1,1]. Other keys are refused (the Python loader drops the classifier and anything else).
 extern "C" int aph_lpips_create(aph_lpips** out) {
   APH_REQUIRE(out, "aph_lpips_create: null handle pointer");
   aph_lpips* h = new aph_lpips();
-  cudaError_t e = cudaMalloc(&h->w0, 64 * 27 * sizeof(float));
-  for (int l = 0; l < LP_CONVS && e == cudaSuccess; ++l) {
-    e = cudaMalloc(&h->bias[l], kCout[l] * sizeof(float));
-    if (l > 0 && e == cudaSuccess) e = cudaMalloc(&h->wf[l], (size_t)kCout[l] * 9 * kCin[l] * sizeof(bf16));
-    if (l > 0 && e == cudaSuccess) e = cudaMalloc(&h->wb[l], (size_t)kCout[l] * 9 * kCin[l] * sizeof(bf16));
+  int e = 0;
+  for (int l = 0; l < LP_CONVS; ++l) {
+    const std::string f = "features." + std::to_string(kFeatIdx[l]);
+    if (l == 0) e |= h->add_f32(f + ".weight", &h->w0, 64 * 27);
+    else e |= h->add_conv3x3(f + ".weight", kCout[l], kCin[l], &h->wf[l], &h->wb[l]);
+    e |= h->add_f32(f + ".bias", &h->bias[l], kCout[l]);
   }
-  for (int t = 0; t < LP_TAPS && e == cudaSuccess; ++t) e = cudaMalloc(&h->lin[t], kCout[kTapConv[t]] * sizeof(float));
-  if (e != cudaSuccess) { aph_lpips_destroy(h); APH_CUDA_OK(e); }
+  for (int t = 0; t < LP_TAPS; ++t) e |= h->add_f32("lin" + std::to_string(t) + ".model.1.weight", &h->lin[t], kCout[kTapConv[t]]);
+  if (e) { aph_lpips_destroy(h); return 1; }
   *out = h;
   return 0;
 }
 
 extern "C" int aph_lpips_destroy(aph_lpips* h) {
   if (!h) return 0;
-  cudaFree(h->w0);
-  for (int l = 0; l < LP_CONVS; ++l) { cudaFree(h->bias[l]); cudaFree(h->wf[l]); cudaFree(h->wb[l]); }
-  for (int t = 0; t < LP_TAPS; ++t) cudaFree(h->lin[t]);
   cudaFree(h->main_arena.p); cudaFree(h->ref_arena.p); cudaFree(h->grads.p); cudaFree(h->part.p);
   delete h;
   return 0;
 }
 
-// Keys: torchvision's "features.{i}.weight" [Co,Ci,3,3] / "features.{i}.bias" [Co] for the 13 convolutions, and lpips'
-// "lin{t}.model.1.weight" [1,C,1,1]. Other keys are refused (the Python loader drops the classifier and anything else).
 extern "C" int aph_lpips_load_tensor(aph_lpips* h, const char* key, const float* data, int64_t numel, void* stream) {
-  APH_REQUIRE(h && key && data, "aph_lpips_load_tensor: bad arguments");
-  cudaStream_t st = (cudaStream_t)stream;
-  int idx = -1;
-  char kind[16] = "";
-  if (sscanf(key, "features.%d.%15s", &idx, kind) == 2) {
-    int l = -1;
-    for (int i = 0; i < LP_CONVS; ++i) if (kFeatIdx[i] == idx) l = i;
-    APH_REQUIRE(l >= 0, "aph_lpips_load_tensor: %s is not one of VGG16's 13 convolutions", key);
-    if (!strcmp(kind, "bias")) {
-      APH_REQUIRE(numel == kCout[l], "aph_lpips_load_tensor: %s has %lld elements, expected %d", key, (long long)numel, kCout[l]);
-      APH_CUDA_OK(cudaMemcpyAsync(h->bias[l], data, numel * sizeof(float), cudaMemcpyDeviceToDevice, st));
-      h->got_b[l] = true;
-    } else if (!strcmp(kind, "weight")) {
-      const int64_t want = (int64_t)kCout[l] * kCin[l] * 9;
-      APH_REQUIRE(numel == want, "aph_lpips_load_tensor: %s has %lld elements, expected %lld", key, (long long)numel, (long long)want);
-      if (l == 0) {
-        APH_CUDA_OK(cudaMemcpyAsync(h->w0, data, numel * sizeof(float), cudaMemcpyDeviceToDevice, st));
-      } else {
-        k_pack_w<<<grid_for((size_t)want, 256), 256, 0, st>>>(data, kCout[l], kCin[l], h->wf[l], h->wb[l]);
-        APH_LAUNCH_OK();
-      }
-      h->got_w[l] = true;
-    } else {
-      set_error("aph_lpips_load_tensor: unknown key %s", key);
-      return 2;
-    }
-    h->finalized = false;
-    return 0;
-  }
-  int t = -1;
-  char rest[32] = "";
-  if (sscanf(key, "lin%d.%31s", &t, rest) == 2 && !strcmp(rest, "model.1.weight") && t >= 0 && t < LP_TAPS) {
-    APH_REQUIRE(numel == kCout[kTapConv[t]], "aph_lpips_load_tensor: %s has %lld elements, expected %d", key, (long long)numel,
-                kCout[kTapConv[t]]);
-    APH_CUDA_OK(cudaMemcpyAsync(h->lin[t], data, numel * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    h->got_lin[t] = true;
-    h->finalized = false;
-    return 0;
-  }
-  set_error("aph_lpips_load_tensor: unknown key %s", key);
-  return 2;
+  return load_tensor(h, key, data, numel, (cudaStream_t)stream, "aph_lpips_load_tensor");
 }
 
 extern "C" int aph_lpips_finalize(aph_lpips* h) {
-  APH_REQUIRE(h, "aph_lpips_finalize: null handle");
-  for (int l = 0; l < LP_CONVS; ++l)
-    APH_REQUIRE(h->got_w[l] && h->got_b[l], "aph_lpips_finalize: features.%d.weight / bias not loaded", kFeatIdx[l]);
-  for (int t = 0; t < LP_TAPS; ++t) APH_REQUIRE(h->got_lin[t], "aph_lpips_finalize: lin%d.model.1.weight not loaded", t);
-  h->finalized = true;
+  if (int e = finalize(h, "aph_lpips_finalize")) return e;
   h->ref_key = 0;           // new weights: cached reference features are void
   ++h->generation;
   return 0;
@@ -524,8 +463,7 @@ extern "C" int aph_lpips_conv_test(int fwd, const void* x, const float* weight, 
   bf16* wp = nullptr;
   const size_t n = (size_t)Cout * Cin * 9;
   APH_CUDA_OK(cudaMallocAsync(&wp, n * sizeof(bf16), st));
-  k_pack_w<<<grid_for(n, 256), 256, 0, st>>>(weight, Cout, Cin, fwd ? wp : nullptr, fwd ? nullptr : wp);
-  APH_LAUNCH_OK();
+  if (int r = pack_conv3x3(weight, Cout, Cin, fwd ? wp : nullptr, fwd ? nullptr : wp, st)) return r;
   ConvEpi e;
   e.out = reinterpret_cast<bf16*>(out);
   int r;

@@ -25,8 +25,6 @@
 
 namespace aph {
 
-typedef __nv_bfloat16 bf16;
-
 struct GemmEpi {
   const float* bias = nullptr;     // [N]
   const float* resid = nullptr;    // fp32 [M, N], added last

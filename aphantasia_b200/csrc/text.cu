@@ -133,14 +133,16 @@ extern "C" int aph_text_create(aph_text** out, const aph_text_config* cfg) {
   const int D = cfg->width, O = cfg->out_dim, B = cfg->max_batch;
   const size_t M = (size_t)B * cfg->context;
   int e = 0;
-  e |= dev_alloc(t, &t->tok_emb, (size_t)cfg->vocab * D); e |= dev_alloc(t, &t->pos, (size_t)cfg->context * D);
-  e |= dev_alloc(t, &t->lnf_w, D); e |= dev_alloc(t, &t->lnf_b, D); e |= dev_alloc(t, &t->w_out, (size_t)O * D);
-  e |= alloc_blocks(t, cfg->layers, D, false);
-  e |= dev_alloc(t, &t->x, M * D); e |= dev_alloc(t, &t->x_mid, M * D); e |= dev_alloc(t, &t->ln_out, M * D);
-  e |= dev_alloc(t, &t->qkv, M * 3 * D); e |= dev_alloc(t, &t->attn_out, M * D);
-  e |= dev_alloc(t, &t->h_pre, M * 4 * D); e |= dev_alloc(t, &t->h_act, M * 4 * D);
-  e |= dev_alloc(t, &t->mean, M); e |= dev_alloc(t, &t->rstd, M);
-  e |= dev_alloc(t, &t->eot, (size_t)B); e |= dev_alloc(t, &t->pooled, (size_t)B * D);
+  e |= t->add_f32("token_embedding.weight", &t->tok_emb, (size_t)cfg->vocab * D);
+  e |= t->add_f32("positional_embedding", &t->pos, (size_t)cfg->context * D);
+  e |= t->add_f32("ln_final.weight", &t->lnf_w, D); e |= t->add_f32("ln_final.bias", &t->lnf_b, D);
+  e |= t->add_bf16("text_projection", D, O, nullptr, &t->w_out);   // [D, out] -> [out, D]
+  e |= add_blocks(t, cfg->layers, D, false);
+  e |= t->alloc(&t->x, M * D); e |= t->alloc(&t->x_mid, M * D); e |= t->alloc(&t->ln_out, M * D);
+  e |= t->alloc(&t->qkv, M * 3 * D); e |= t->alloc(&t->attn_out, M * D);
+  e |= t->alloc(&t->h_pre, M * 4 * D); e |= t->alloc(&t->h_act, M * 4 * D);
+  e |= t->alloc(&t->mean, M); e |= t->alloc(&t->rstd, M);
+  e |= t->alloc(&t->eot, (size_t)B); e |= t->alloc(&t->pooled, (size_t)B * D);
   if (e) { aph_text_destroy(reinterpret_cast<aph_text*>(t)); return 1; }
   *out = reinterpret_cast<aph_text*>(t);
   return 0;
@@ -155,34 +157,10 @@ extern "C" int aph_text_destroy(aph_text* text) {
 extern "C" int64_t aph_text_bytes(const aph_text* text) { return text ? reinterpret_cast<const TextImpl*>(text)->bytes : 0; }
 
 extern "C" int aph_text_load_tensor(aph_text* text, const char* key, const float* data, int64_t numel, void* stream) {
-  APH_REQUIRE(text && key && data, "aph_text_load_tensor: null argument");
-  TextImpl* t = reinterpret_cast<TextImpl*>(text);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int D = t->cfg.width, O = t->cfg.out_dim, C = t->cfg.context;
-  const std::string k(key);
-  auto need = [&](int64_t n) -> int { APH_REQUIRE(numel == n, "aph_text_load_tensor(%s): expected %lld elements, got %lld", key, (long long)n, (long long)numel); return 0; };
-  int e = 0;
-  if (k == "token_embedding.weight") { if ((e = need((int64_t)t->cfg.vocab * D))) return e; e = copy_f32(data, t->tok_emb, (size_t)t->cfg.vocab * D, st); }
-  else if (k == "positional_embedding") { if ((e = need((int64_t)C * D))) return e; e = copy_f32(data, t->pos, (size_t)C * D, st); }
-  else if (k == "ln_final.weight") { if ((e = need(D))) return e; e = copy_f32(data, t->lnf_w, D, st); }
-  else if (k == "ln_final.bias") { if ((e = need(D))) return e; e = copy_f32(data, t->lnf_b, D, st); }
-  else if (k == "text_projection") { if ((e = need((int64_t)D * O))) return e; e = pack(data, t->w_out, D, O, 1, st); }   // [D, out] -> [out, D]
-  else if (k.rfind("transformer.resblocks.", 0) == 0) e = load_block_tensor(t, k, key, data, numel, D, st, "aph_text_load_tensor");
-  else { set_error("aph_text_load_tensor: unknown tensor %s", key); return 2; }
-  if (e) return e;
-  t->loaded[k] = true;
-  return 0;
+  return load_tensor(reinterpret_cast<TextImpl*>(text), key, data, numel, (cudaStream_t)stream, "aph_text_load_tensor");
 }
 
-extern "C" int aph_text_finalize(aph_text* text) {
-  APH_REQUIRE(text, "aph_text_finalize: null handle");
-  TextImpl* t = reinterpret_cast<TextImpl*>(text);
-  if (int e = check_loaded(t, {"token_embedding.weight", "positional_embedding", "ln_final.weight", "ln_final.bias", "text_projection"},
-                           "aph_text_finalize", ""))
-    return e;
-  t->finalized = true;
-  return 0;
-}
+extern "C" int aph_text_finalize(aph_text* text) { return finalize(reinterpret_cast<TextImpl*>(text), "aph_text_finalize"); }
 
 extern "C" int aph_text_fwd(aph_text* text, const int64_t* tokens, int n, float* emb, void* stream) {
   APH_REQUIRE(text && tokens && emb, "aph_text_fwd: null argument");

@@ -9,8 +9,6 @@
 #include "encoder.cuh"
 #include "vit_attn_tc.cuh"
 #include "vit_attn_stream.cuh"
-#include <stdlib.h>
-#include <string.h>
 
 namespace aph {
 
@@ -125,93 +123,21 @@ static int run_cached(std::vector<VitImpl::GraphEntry>& cache, std::map<int, int
   return 0;
 }
 
-// ld: row stride of the untransposed output (>= cols; the columns past cols are not written)
-__global__ void __launch_bounds__(256) k_pack_weight(const float* __restrict__ in, bf16* __restrict__ out, int rows, int cols, int transpose, int ld) {
-  const size_t n = (size_t)rows * cols;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const int r = (int)(i / cols), c = (int)(i - (size_t)r * cols);
-    const bf16 v = __float2bfloat16_rn(in[i]);
-    if (transpose) out[(size_t)c * rows + r] = v; else out[(size_t)r * ld + c] = v;
-  }
-}
-
-int pack(const float* src, bf16* dst, int rows, int cols, int transpose, cudaStream_t st, int ld) {
-  const size_t n = (size_t)rows * cols;
-  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16);
-  k_pack_weight<<<blocks, 256, 0, st>>>(src, dst, rows, cols, transpose, ld > 0 ? ld : cols);
-  APH_LAUNCH_OK();
-  return 0;
-}
-
-int copy_f32(const float* src, float* dst, size_t n, cudaStream_t st) {
-  APH_CUDA_OK(cudaMemcpyAsync(dst, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st));
-  return 0;
-}
-
-// The tensors of a residual block, state-dict key transformer.resblocks.<i>.<key>. An fp32 entry is a vector of rows*D elements,
-// copied as it is; a bf16 entry is a [rows*D, cols*D] matrix packed as the forward GEMM's B operand and, where the block has
-// them (w_t allocated), transposed into the data gradient's.
-using F32Slot = float* BlockW::*;
-using Bf16Slot = bf16* BlockW::*;
-struct BlockTensor {
-  const char* key;
-  int rows, cols;
-  F32Slot f32;
-  Bf16Slot w, w_t;
-};
-static const BlockTensor kBlockTensors[] = {
-    {"ln_1.weight", 1, 0, &BlockW::ln1_w, nullptr, nullptr},
-    {"ln_1.bias", 1, 0, &BlockW::ln1_b, nullptr, nullptr},
-    {"ln_2.weight", 1, 0, &BlockW::ln2_w, nullptr, nullptr},
-    {"ln_2.bias", 1, 0, &BlockW::ln2_b, nullptr, nullptr},
-    {"attn.in_proj_weight", 3, 1, nullptr, &BlockW::w_qkv, &BlockW::w_qkv_t},
-    {"attn.in_proj_bias", 3, 0, &BlockW::b_qkv, nullptr, nullptr},
-    {"attn.out_proj.weight", 1, 1, nullptr, &BlockW::w_o, &BlockW::w_o_t},
-    {"attn.out_proj.bias", 1, 0, &BlockW::b_o, nullptr, nullptr},
-    {"mlp.c_fc.weight", 4, 1, nullptr, &BlockW::w_fc, &BlockW::w_fc_t},
-    {"mlp.c_fc.bias", 4, 0, &BlockW::b_fc, nullptr, nullptr},
-    {"mlp.c_proj.weight", 1, 4, nullptr, &BlockW::w_proj, &BlockW::w_proj_t},
-    {"mlp.c_proj.bias", 1, 0, &BlockW::b_proj, nullptr, nullptr},
-};
-
-static size_t numel_of(const BlockTensor& t, int D) { return (size_t)t.rows * D * (t.w ? (size_t)t.cols * D : 1); }
-
-int alloc_blocks(Encoder* h, int layers, int D, bool dgrad) {
+int add_blocks(Encoder* h, int layers, int D, bool dgrad) {
   h->L.resize(layers);
   int e = 0;
-  for (BlockW& l : h->L)
-    for (const BlockTensor& t : kBlockTensors) {
-      if (t.f32) { e |= dev_alloc(h, &(l.*t.f32), numel_of(t, D)); continue; }
-      e |= dev_alloc(h, &(l.*t.w), numel_of(t, D));
-      if (dgrad) e |= dev_alloc(h, &(l.*t.w_t), numel_of(t, D));
-    }
-  return e;
-}
-
-int load_block_tensor(Encoder* h, const std::string& k, const char* key, const float* data, int64_t numel, int D, cudaStream_t st,
-                      const char* who) {
-  const char* rest = k.c_str() + strlen("transformer.resblocks.");
-  char* endp = nullptr;
-  const long li = strtol(rest, &endp, 10);
-  APH_REQUIRE(endp && *endp == '.' && li >= 0 && li < (long)h->L.size(), "%s: bad layer index in %s", who, key);
-  BlockW& l = h->L[li];
-  for (const BlockTensor& t : kBlockTensors) {
-    if (strcmp(endp + 1, t.key) != 0) continue;
-    const size_t n = numel_of(t, D);
-    APH_REQUIRE(numel == (int64_t)n, "%s(%s): expected %lld elements, got %lld", who, key, (long long)n, (long long)numel);
-    if (t.f32) return copy_f32(data, l.*t.f32, n, st);
-    if (int e = pack(data, l.*t.w, t.rows * D, t.cols * D, 0, st)) return e;
-    return l.*t.w_t ? pack(data, l.*t.w_t, t.rows * D, t.cols * D, 1, st) : 0;
+  for (int i = 0; i < layers; ++i) {
+    BlockW& l = h->L[i];
+    const std::string p = "transformer.resblocks." + std::to_string(i) + ".";
+    auto mat = [&](const char* key, int rows, int cols, bf16** w, bf16** w_t) { e |= h->add_bf16(p + key, rows, cols, w, dgrad ? w_t : nullptr); };
+    auto vec = [&](const char* key, int n, float** v) { e |= h->add_f32(p + key, v, n); };
+    vec("ln_1.weight", D, &l.ln1_w); vec("ln_1.bias", D, &l.ln1_b); vec("ln_2.weight", D, &l.ln2_w); vec("ln_2.bias", D, &l.ln2_b);
+    mat("attn.in_proj_weight", 3 * D, D, &l.w_qkv, &l.w_qkv_t); vec("attn.in_proj_bias", 3 * D, &l.b_qkv);
+    mat("attn.out_proj.weight", D, D, &l.w_o, &l.w_o_t); vec("attn.out_proj.bias", D, &l.b_o);
+    mat("mlp.c_fc.weight", 4 * D, D, &l.w_fc, &l.w_fc_t); vec("mlp.c_fc.bias", 4 * D, &l.b_fc);
+    mat("mlp.c_proj.weight", D, 4 * D, &l.w_proj, &l.w_proj_t); vec("mlp.c_proj.bias", D, &l.b_proj);
   }
-  set_error("%s: unknown tensor %s", who, key);
-  return 2;
-}
-
-int check_loaded(const Encoder* h, std::vector<std::string> want, const char* who, const char* prefix) {
-  for (size_t i = 0; i < h->L.size(); ++i)
-    for (const BlockTensor& t : kBlockTensors) want.push_back("transformer.resblocks." + std::to_string(i) + "." + t.key);
-  for (const auto& w : want) APH_REQUIRE(h->loaded.count(w), "%s: tensor %s%s was never loaded", who, prefix, w.c_str());
-  return 0;
+  return e;
 }
 
 int block_fwd(const BlockW& w, const BlockIO& io, int S, int T, int Mr, int ld_tok, int D, int heads, AttnFwd attn, cudaStream_t st) {
@@ -266,28 +192,31 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
   v->g = cfg->res / cfg->patch; v->T = v->g * v->g + 1; v->D = cfg->width; v->Kp = patch_k(cfg->patch);
   const int D = v->D, T = v->T, S = cfg->max_batch, Ly = cfg->layers, O = cfg->out_dim;
   const size_t M = (size_t)S * T, Mp = (size_t)S * v->g * v->g;
+  v->prefix = "visual.";
   int e = 0;
-  // weights
-  e |= dev_alloc(v, &v->w_conv, (size_t)D * v->Kp); e |= dev_alloc(v, &v->w_conv_t, (size_t)D * v->Kp);
-  e |= dev_alloc(v, &v->cls, D); e |= dev_alloc(v, &v->pos, (size_t)T * D);
-  e |= dev_alloc(v, &v->lnpre_w, D); e |= dev_alloc(v, &v->lnpre_b, D); e |= dev_alloc(v, &v->lnpost_w, D); e |= dev_alloc(v, &v->lnpost_b, D);
-  e |= dev_alloc(v, &v->w_out, (size_t)D * O); e |= dev_alloc(v, &v->w_out_t, (size_t)D * O);
-  e |= alloc_blocks(v, Ly, D, true);
+  // weights. conv1 [D, 3, p, p] = [D, 3 p^2] goes into the first 3 p^2 columns (rows of the transpose) of [D, Kp] / [Kp, D];
+  // proj [D, out] is the data gradient's B operand as it is, the forward's transposed
+  e |= v->add_bf16("conv1.weight", D, 3 * cfg->patch * cfg->patch, &v->w_conv, &v->w_conv_t, v->Kp);
+  e |= v->add_f32("class_embedding", &v->cls, D); e |= v->add_f32("positional_embedding", &v->pos, (size_t)T * D);
+  e |= v->add_f32("ln_pre.weight", &v->lnpre_w, D); e |= v->add_f32("ln_pre.bias", &v->lnpre_b, D);
+  e |= v->add_f32("ln_post.weight", &v->lnpost_w, D); e |= v->add_f32("ln_post.bias", &v->lnpost_b, D);
+  e |= v->add_bf16("proj", D, O, &v->w_out_t, &v->w_out);
+  e |= add_blocks(v, Ly, D, true);
   // activations
-  e |= dev_alloc(v, &v->patches, Mp * v->Kp); e |= dev_alloc(v, &v->tok, Mp * D); e |= dev_alloc(v, &v->e, M * D);
+  e |= v->alloc(&v->patches, Mp * v->Kp); e |= v->alloc(&v->tok, Mp * D); e |= v->alloc(&v->e, M * D);
   v->xs.resize(2 * Ly + 1);
-  for (int i = 0; i <= 2 * Ly; ++i) e |= dev_alloc(v, &v->xs[i], (i >= 2 * Ly - 1 ? (size_t)S : M) * D);
-  e |= dev_alloc(v, &v->ln_out, M * D); e |= dev_alloc(v, &v->attn_out, M * D); e |= dev_alloc(v, &v->h_act, M * 4 * D);
+  for (int i = 0; i <= 2 * Ly; ++i) e |= v->alloc(&v->xs[i], (i >= 2 * Ly - 1 ? (size_t)S : M) * D);
+  e |= v->alloc(&v->ln_out, M * D); e |= v->alloc(&v->attn_out, M * D); e |= v->alloc(&v->h_act, M * 4 * D);
   v->qkv.resize(Ly); v->h_pre.resize(Ly);
-  for (int i = 0; i < Ly; ++i) { e |= dev_alloc(v, &v->qkv[i], M * 3 * D); e |= dev_alloc(v, &v->h_pre[i], (i == Ly - 1 ? (size_t)S : M) * 4 * D); }
-  e |= dev_alloc(v, &v->st_mean, stat_off(v, 2 * Ly + 2)); e |= dev_alloc(v, &v->st_rstd, stat_off(v, 2 * Ly + 2));
-  e |= dev_alloc(v, &v->cls_ln, (size_t)S * D); e |= dev_alloc(v, &v->emb_int, (size_t)S * O);
-  e |= dev_alloc(v, &v->d_emb, (size_t)S * O); e |= dev_alloc(v, &v->d_cls, (size_t)S * D);
-  e |= dev_alloc(v, &v->dxc, (size_t)S * D); e |= dev_alloc(v, &v->dxc_bf, (size_t)S * D);
-  e |= dev_alloc(v, &v->dx, M * D); e |= dev_alloc(v, &v->dx_bf, M * D); e |= dev_alloc(v, &v->dh, M * 4 * D);
-  e |= dev_alloc(v, &v->d_ln, M * D); e |= dev_alloc(v, &v->d_attn, M * D); e |= dev_alloc(v, &v->d_attn_last, M * D);
-  e |= dev_alloc(v, &v->d_qkv, M * 3 * D); e |= dev_alloc(v, &v->d_tok, Mp * D);
-  if (T > kAttnResidentMaxT) e |= dev_alloc(v, &v->attn_stats, M * cfg->heads);
+  for (int i = 0; i < Ly; ++i) { e |= v->alloc(&v->qkv[i], M * 3 * D); e |= v->alloc(&v->h_pre[i], (i == Ly - 1 ? (size_t)S : M) * 4 * D); }
+  e |= v->alloc(&v->st_mean, stat_off(v, 2 * Ly + 2)); e |= v->alloc(&v->st_rstd, stat_off(v, 2 * Ly + 2));
+  e |= v->alloc(&v->cls_ln, (size_t)S * D); e |= v->alloc(&v->emb_int, (size_t)S * O);
+  e |= v->alloc(&v->d_emb, (size_t)S * O); e |= v->alloc(&v->d_cls, (size_t)S * D);
+  e |= v->alloc(&v->dxc, (size_t)S * D); e |= v->alloc(&v->dxc_bf, (size_t)S * D);
+  e |= v->alloc(&v->dx, M * D); e |= v->alloc(&v->dx_bf, M * D); e |= v->alloc(&v->dh, M * 4 * D);
+  e |= v->alloc(&v->d_ln, M * D); e |= v->alloc(&v->d_attn, M * D); e |= v->alloc(&v->d_attn_last, M * D);
+  e |= v->alloc(&v->d_qkv, M * 3 * D); e |= v->alloc(&v->d_tok, Mp * D);
+  if (T > kAttnResidentMaxT) e |= v->alloc(&v->attn_stats, M * cfg->heads);
   if (e) { aph_vit_destroy(reinterpret_cast<aph_vit*>(v)); return 1; }
   APH_CUDA_OK(cudaMemset(v->d_attn_last, 0, M * D * sizeof(bf16)));
   if (v->Kp != 3 * cfg->patch * cfg->patch) {   // the zero padding of the patch operand and of conv1's packed weights
@@ -312,44 +241,10 @@ extern "C" int aph_vit_destroy(aph_vit* vit) {
 extern "C" int64_t aph_vit_bytes(const aph_vit* vit) { return vit ? reinterpret_cast<const VitImpl*>(vit)->bytes : 0; }
 
 extern "C" int aph_vit_load_tensor(aph_vit* vit, const char* key, const float* data, int64_t numel, void* stream) {
-  APH_REQUIRE(vit && key && data, "aph_vit_load_tensor: null argument");
-  VitImpl* v = reinterpret_cast<VitImpl*>(vit);
-  cudaStream_t st = (cudaStream_t)stream;
-  const int D = v->D, O = v->cfg.out_dim;
-  std::string k(key);
-  if (k.rfind("visual.", 0) == 0) k = k.substr(7);
-  auto need = [&](int64_t n) -> int { APH_REQUIRE(numel == n, "aph_vit_load_tensor(%s): expected %lld elements, got %lld", key, (long long)n, (long long)numel); return 0; };
-  int e = 0;
-  if (k == "conv1.weight") {   // [D, 3, p, p] = [D, 3 p^2] into the first 3 p^2 columns (rows of the transpose) of [D, Kp] / [Kp, D]
-    const int P3 = 3 * v->cfg.patch * v->cfg.patch;
-    if ((e = need((int64_t)D * P3))) return e;
-    e = pack(data, v->w_conv, D, P3, 0, st, v->Kp) | pack(data, v->w_conv_t, D, P3, 1, st);
-  }
-  else if (k == "class_embedding") { if ((e = need(D))) return e; e = copy_f32(data, v->cls, D, st); }
-  else if (k == "positional_embedding") { if ((e = need((int64_t)v->T * D))) return e; e = copy_f32(data, v->pos, (size_t)v->T * D, st); }
-  else if (k == "ln_pre.weight") { if ((e = need(D))) return e; e = copy_f32(data, v->lnpre_w, D, st); }
-  else if (k == "ln_pre.bias") { if ((e = need(D))) return e; e = copy_f32(data, v->lnpre_b, D, st); }
-  else if (k == "ln_post.weight") { if ((e = need(D))) return e; e = copy_f32(data, v->lnpost_w, D, st); }
-  else if (k == "ln_post.bias") { if ((e = need(D))) return e; e = copy_f32(data, v->lnpost_b, D, st); }
-  else if (k == "proj") {   // [D, out]: forward B operand is proj^T [out, D]; dgrad B operand is proj [D, out]
-    if ((e = need((int64_t)D * O))) return e;
-    e = pack(data, v->w_out, D, O, 1, st) | pack(data, v->w_out_t, D, O, 0, st);
-  } else if (k.rfind("transformer.resblocks.", 0) == 0) e = load_block_tensor(v, k, key, data, numel, D, st, "aph_vit_load_tensor");
-  else { set_error("aph_vit_load_tensor: unknown tensor %s", key); return 2; }
-  if (e) return e;
-  v->loaded[k] = true;
-  return 0;
+  return load_tensor(reinterpret_cast<VitImpl*>(vit), key, data, numel, (cudaStream_t)stream, "aph_vit_load_tensor");
 }
 
-extern "C" int aph_vit_finalize(aph_vit* vit) {
-  APH_REQUIRE(vit, "aph_vit_finalize: null handle");
-  VitImpl* v = reinterpret_cast<VitImpl*>(vit);
-  if (int e = check_loaded(v, {"conv1.weight", "class_embedding", "positional_embedding", "ln_pre.weight", "ln_pre.bias", "ln_post.weight",
-                               "ln_post.bias", "proj"}, "aph_vit_finalize", "visual."))
-    return e;
-  v->finalized = true;
-  return 0;
-}
+extern "C" int aph_vit_finalize(aph_vit* vit) { return finalize(reinterpret_cast<VitImpl*>(vit), "aph_vit_finalize"); }
 
 static int vit_fwd_impl(aph_vit* vit, const float* images, int S, int side, float* emb, int save_for_bwd, void* stream);
 static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, float* grad_images, void* stream);

@@ -11,7 +11,7 @@ import numpy as np
 import torch
 
 from . import _dist, _pool
-from ._lib import check, lib, require_cuda, stream_ptr
+from ._lib import Handle, check, lib, require_cuda, stream_ptr
 
 
 def _color_correlation(colors):
@@ -98,16 +98,11 @@ def _img2fft(img, decay, colors, sd):
     img = _rgb_u8(img)
     h, w = img.shape[:2]
     _check_fft_size(h, w)
-    plan = C.c_void_p()
-    check(lib().aph_fft_plan_create(C.byref(plan), h, w), 'aph_fft_plan_create')
-    try:
-        x = _un_rgb(img, colors, 1.)
-        ascale = _analysis_scale(h, w // 2 + 1, decay, sd).cuda()
-        spectrum = torch.empty(1, 3, h, w // 2 + 1, 2, device=x.device)
-        check(lib().aph_fft_analyze(plan, x.data_ptr(), ascale.data_ptr(), spectrum.data_ptr(), stream_ptr()), 'aph_fft_analyze')
-        torch.cuda.current_stream().synchronize()          # the plan's scratch is in use until then
-    finally:
-        lib().aph_fft_plan_destroy(plan)
+    plan = Handle('aph_fft_plan', h, w)
+    x = _un_rgb(img, colors, 1.)
+    ascale = _analysis_scale(h, w // 2 + 1, decay, sd).cuda()
+    spectrum = torch.empty(1, 3, h, w // 2 + 1, 2, device=x.device)
+    check(lib().aph_fft_analyze(plan, x.data_ptr(), ascale.data_ptr(), spectrum.data_ptr(), stream_ptr()), 'aph_fft_analyze')
     return spectrum
 
 
@@ -413,12 +408,10 @@ class DWTImage:
         h, w = int(shape[2]), int(shape[3])
         rec_lo, rec_hi = reconstruction_filters(wave)
         L = len(rec_lo)
-        plan = C.c_void_p()
-        check(lib().aph_dwt_plan_create(C.byref(plan), h, w, (C.c_float * L)(*rec_lo), (C.c_float * L)(*rec_hi), L), 'aph_dwt_plan_create')
-        self.plan = plan
+        self.plan = Handle('aph_dwt_plan', h, w, (C.c_float * L)(*rec_lo), (C.c_float * L)(*rec_hi), L)
         J = C.c_int()
         dims = (C.c_int * 32)(); ohw = (C.c_int * 2)()
-        check(lib().aph_dwt_plan_levels(plan, C.byref(J), dims, ohw), 'aph_dwt_plan_levels')
+        check(lib().aph_dwt_plan_levels(self.plan, C.byref(J), dims, ohw), 'aph_dwt_plan_levels')
         self.J = J.value
         self.level_hw = [(dims[2 * i], dims[2 * i + 1]) for i in range(self.J)]
         self.out_hw = (ohw[0], ohw[1])
@@ -429,13 +422,6 @@ class DWTImage:
     def param_shapes(self):
         hJ, wJ = self.level_hw[-1]
         return [(1, 3, hJ, wJ)] + [(1, 3, 3, hh, ww) for (hh, ww) in self.level_hw]
-
-    def __del__(self):
-        try:
-            if getattr(self, 'plan', None):
-                lib().aph_dwt_plan_destroy(self.plan)
-        except Exception:
-            pass
 
     def fused(self, shift, contrast, colmat, sigmoid):
         return _SynthDWT.apply(self, contrast, colmat, sigmoid, *self.Ys)
@@ -470,9 +456,7 @@ def img2dwt(img_in, wave='coif2', sharp=0.3, colors=1.):
     """Drop-in for image.py:82-94: the wavelet parameters [Yl, Yh_1 (finest) .. Yh_J] (CUDA) of the picture img_in."""
     img = _rgb_u8(img_in)
     gen = DWTImage([1, 3, *img.shape[:2]], wave, sharp)
-    Ys = _img2dwt(img, gen, colors, sharp)
-    torch.cuda.current_stream().synchronize()              # the plan's scratch is in use until then
-    return Ys
+    return _img2dwt(img, gen, colors, sharp)
 
 
 def _init_dwt(resume, shape, wave, sharp, colors):
@@ -507,7 +491,6 @@ def _init_dwt(resume, shape, wave, sharp, colors):
 def init_dwt(resume=None, shape=None, wave=None, colors=None):
     """Drop-in for image.py:33-59: (Ys, None, None, size); the pytorch_wavelets transforms it also returns do not exist here."""
     _, Ys, size = _init_dwt(resume, shape, wave, 0.3, colors)
-    torch.cuda.current_stream().synchronize()              # the analysis plan goes with `gen`
     return Ys, None, None, size
 
 

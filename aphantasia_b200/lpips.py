@@ -10,12 +10,12 @@ Weights: torchvision's VGG16 state dict from $APH_LPIPS_VGG or torch.hub's check
 linear layers from $APH_LPIPS_LIN (lpips' weights/v0.1/vgg.pth). Without them, seeded synthetic weights are used, loudly.
 """
 import os
-from ctypes import c_int64 as C_int64, c_void_p as C_void_p
+from ctypes import c_int64 as C_int64
 
 import torch
 
 from . import _trace
-from ._lib import check, lib, require_cuda, stream_ptr
+from ._lib import Handle, check, lib, require_cuda, stream_ptr
 
 __all__ = ['LPIPS']
 
@@ -144,27 +144,18 @@ class LPIPS:
             print('Setting up [LPIPS] perceptual loss: trunk [vgg], v[%s], spatial [off]' % version)
 
     def _ensure(self):
-        if self._handle is not None:
+        """Creates and loads the device handle on first use. A handle whose load failed is freed and built again, so the load's
+        error is raised again."""
+        if self._handle is not None and self._handle.loaded:
             return
-        h = C_void_p()
-        check(lib().aph_lpips_create(h), 'aph_lpips_create')
-        self._handle = h.value
-        st = stream_ptr()
-        for k, v in self._sd.items():
-            d = v.cuda()
-            check(lib().aph_lpips_load_tensor(self._handle, k.encode(), d.data_ptr(), d.numel(), st), 'aph_lpips_load_tensor')
-            torch.cuda.current_stream().synchronize()           # `d` dies with this iteration
-        check(lib().aph_lpips_finalize(self._handle), 'aph_lpips_finalize')
+        self.close()
+        self._handle = Handle('aph_lpips')
+        self._handle.load(self._sd)
 
-    def __del__(self):
-        h = getattr(self, '_handle', None)
-        if h is not None and lib is not None:
-            try:
-                torch.cuda.synchronize()
-                lib().aph_lpips_destroy(h)
-            except Exception:
-                pass
-            self._handle = None
+    def close(self):
+        if self._handle is not None:
+            self._handle.close()
+        self._handle, self._ref = None, None
 
     # nn.Module surface used by the scripts
     def cuda(self, *a, **k): return self

@@ -151,7 +151,7 @@ int aph_affine_fwd(const float* in, int planes, int H, int W, const double* inv_
  * nn.Conv2d weight [out, in, 1, 1] (8-byte aligned), read in place by every call.
  * coords [N,2,H,W] -> out [N,3,H,W]; pixel p = n H W + h W + w. One launch.                                        */
 typedef struct aph_cppn aph_cppn;
-int aph_cppn_create(int nf, int layers, int act, aph_cppn** handle);
+int aph_cppn_create(aph_cppn** handle, int nf, int layers, int act);
 int aph_cppn_destroy(aph_cppn* handle);
 int aph_cppn_fwd(aph_cppn* handle, const float* coords, int N, int H, int W, const float* const* params, float* out,
                  void* stream);

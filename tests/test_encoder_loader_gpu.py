@@ -1,13 +1,14 @@
-"""The weight-loading contract of the image and text encoder handles (aph_vit_* / aph_text_*), at small geometries: a tensor
-with the wrong element count, an unknown key and a bad layer index are refused with a message that names them, finalize
-names a tensor that was never loaded, and the Python wrappers keep (and close() frees) a handle whose load failed."""
+"""The weight-loading contract of the handles that take a state dict: the image and text encoders (aph_vit_* / aph_text_*, at
+small geometries) and LPIPS (aph_lpips_*). A tensor with the wrong element count, an unknown key and a bad layer index are
+refused with a message that names them, finalize names a tensor that was never loaded, and the Python wrappers keep (and
+close() frees) a handle whose load failed."""
 import contextlib
 import ctypes as C
 
 import pytest
 import torch
 
-from aphantasia_b200 import _lib, clip
+from aphantasia_b200 import _lib, clip, lpips
 
 pytestmark = pytest.mark.gpu
 LAYERS, WIDTH = 2, 128
@@ -23,16 +24,22 @@ def _text_sd():
     return clip.synthetic_text_state_dict(width=WIDTH, layers=LAYERS, heads=2, out_dim=128, context=16, vocab=500, seed=0)
 
 
+def _lpips_sd():
+    return {**lpips.synthetic_vgg_state_dict(), **lpips.synthetic_lin_state_dict()}
+
+
 class Tower:
-    """One tower through the raw C ABI: its entry points, config, key prefix and a state dict on the GPU."""
+    """One handle kind through the raw C ABI: its entry points, create arguments, key prefix and a state dict on the GPU."""
 
     def __init__(self, name):
         if name == 'image':
             self.api, self.prefix, sd = 'aph_vit', 'visual.', _image_sd()
-            self.cfg = _lib.VitConfig(32, WIDTH, LAYERS, 2, 128, 64, 2, 0)
-        else:
+            self.cfg = [C.byref(_lib.VitConfig(32, WIDTH, LAYERS, 2, 128, 64, 2, 0))]
+        elif name == 'text':
             self.api, self.prefix, sd = 'aph_text', '', _text_sd()
-            self.cfg = _lib.TextConfig(WIDTH, LAYERS, 2, 128, 16, 500, 2, 0)
+            self.cfg = [C.byref(_lib.TextConfig(WIDTH, LAYERS, 2, 128, 16, 500, 2, 0))]
+        else:
+            self.api, self.prefix, sd, self.cfg = 'aph_lpips', '', _lpips_sd(), []
         self.sd = {k: v.contiguous().cuda() for k, v in sd.items()}
 
     def fn(self, what):
@@ -44,7 +51,7 @@ class Tower:
     @contextlib.contextmanager
     def handle(self):
         h = C.c_void_p()
-        assert self.fn('create')(C.byref(h), C.byref(self.cfg)) == 0, _error()
+        assert self.fn('create')(C.byref(h), *self.cfg) == 0, _error()
         try:
             yield h
         finally:
@@ -61,6 +68,11 @@ def _error():
 
 @pytest.fixture(params=['image', 'text'])
 def tower(request):
+    return Tower(request.param)
+
+
+@pytest.fixture(params=['image', 'text', 'lpips'])
+def any_handle(request):
     return Tower(request.param)
 
 
@@ -89,8 +101,35 @@ def test_unknown_keys_and_bad_layer_indices_are_refused(tower):
             assert 'bad layer index in %s' % key in _error()
 
 
-def test_finalize_names_the_missing_tensor(tower):
-    assert len(tower.sd) == (8 if tower.api == 'aph_vit' else 5) + LAYERS * len(FIELDS)
+@pytest.mark.parametrize('key', ['features.0.weight', 'features.0.bias', 'features.2.weight', 'features.28.weight',
+                                 'features.28.bias', 'lin0.model.1.weight', 'lin4.model.1.weight'])
+def test_lpips_tensor_with_wrong_size_is_refused(key):
+    """conv1_1's fp32 copy, a packed 3x3 convolution, a bias and a linear layer each check their element count."""
+    tower = Tower('lpips')
+    n = tower.sd[key].numel()
+    buf = torch.zeros(n + 64, device='cuda')
+    with tower.handle() as h:
+        for bad in (n - 1, n + 64):
+            assert tower.load(h, key, buf, bad) == 2
+            msg = _error()
+            assert key in msg and 'expected %d elements, got %d' % (n, bad) in msg, msg
+        assert tower.load(h, key, buf, n) == 0, _error()
+
+
+def test_lpips_unknown_keys_are_refused():
+    """A ReLU or max-pool index of VGG16's features, a sixth linear layer and anything else: no such tensor."""
+    tower = Tower('lpips')
+    buf = torch.zeros(64 * 27, device='cuda')
+    with tower.handle() as h:
+        for key in ('features.3.weight', 'features.1.bias', 'features.30.weight', 'lin5.model.1.weight', 'lin0.model.0.weight',
+                    'classifier.0.weight', 'features.0'):
+            assert tower.load(h, key, buf, 64) == 2
+            assert 'unknown tensor %s' % key in _error(), _error()
+
+
+def test_finalize_names_the_missing_tensor(any_handle):
+    tower = any_handle
+    assert len(tower.sd) == {'aph_vit': 8 + LAYERS * len(FIELDS), 'aph_text': 5 + LAYERS * len(FIELDS), 'aph_lpips': 2 * 13 + 5}[tower.api]
     for missing in tower.sd:
         with tower.handle() as h:
             for k, v in tower.sd.items():
@@ -105,22 +144,31 @@ def test_finalize_names_the_missing_tensor(tower):
         assert tower.fn('finalize')(h) == 0, _error()
 
 
-@pytest.mark.parametrize('name', ['image', 'text'])
+@pytest.mark.parametrize('name', ['image', 'text', 'lpips'])
 def test_wrapper_owns_the_handle_of_a_failed_load(name):
-    """A state dict with one tensor of the wrong size: _ensure raises, and the wrapper still holds the handle it created, so
-    close() frees it instead of leaking it."""
+    """A state dict with one tensor of the wrong size: building the handle raises, the wrapper still holds the handle it created
+    (not loaded), a second attempt raises the load's error again, and close() frees the handle instead of leaking it."""
     if name == 'image':
         sd = _image_sd()
-        key = 'visual.transformer.resblocks.1.mlp.c_fc.bias'
-        sd[key] = torch.zeros(4 * WIDTH - 1)
-        model, nbytes = clip.VisionTransformer(sd), _lib.lib().aph_vit_bytes
-    else:
+        sd['visual.transformer.resblocks.1.mlp.c_fc.bias'] = torch.zeros(4 * WIDTH - 1)
+        model, n = clip.VisionTransformer(sd), 4 * WIDTH
+        build, held = (lambda: model._ensure(2)), (lambda: model.handle)
+    elif name == 'text':
         sd = _text_sd()
-        key = 'transformer.resblocks.1.mlp.c_fc.bias'
-        sd[key] = torch.zeros(4 * WIDTH - 1)
-        model, nbytes = clip.TextTransformer(sd), _lib.lib().aph_text_bytes
-    with pytest.raises(RuntimeError, match='expected %d elements, got %d' % (4 * WIDTH, 4 * WIDTH - 1)):
-        model._ensure(2)
-    assert model.handle is not None and nbytes(model.handle) > 0
+        sd['transformer.resblocks.1.mlp.c_fc.bias'] = torch.zeros(4 * WIDTH - 1)
+        model, n = clip.TextTransformer(sd), 4 * WIDTH
+        build, held = (lambda: model._ensure(2)), (lambda: model.handle)
+    else:
+        lin = lpips.synthetic_lin_state_dict()
+        lin['lin4.model.1.weight'] = torch.zeros(511)
+        model, n = lpips.LPIPS(net='vgg', verbose=False, vgg_state_dict=lpips.synthetic_vgg_state_dict(), lin_state_dict=lin), 512
+        build, held = model._ensure, (lambda: model._handle)
+    for _ in range(2):
+        with pytest.raises(RuntimeError, match='expected %d elements, got %d' % (n, n - 1)):
+            build()
+        h = held()
+        assert h is not None and not h.loaded
+    if name != 'lpips':
+        assert ({'image': _lib.lib().aph_vit_bytes, 'text': _lib.lib().aph_text_bytes}[name])(h) > 0
     model.close()
-    assert model.handle is None
+    assert held() is None and not hasattr(h, '_as_parameter_')

@@ -24,6 +24,18 @@ def test_library_loads_and_exports_every_declared_symbol():
     assert int(re.search(r'#define APH_CROP_PARAM_FLOATS (\d+)', hdr).group(1)) == __import__('aphantasia_b200._rng', fromlist=['x']).CROP_PARAM_FLOATS
 
 
+def test_every_create_returns_its_handle_through_its_first_argument():
+    """_lib.Handle calls every `<api>_create` as (&handle, *args)."""
+    import ctypes as C
+    from aphantasia_b200 import _lib
+    hdr = open(os.path.join(ROOT, 'include', 'aphb200.h')).read()
+    creates = re.findall(r'\bint (aph_[a-z0-9_]+)_create\(([^)]*)\)', hdr)
+    assert len(creates) >= 6
+    for api, args in creates:
+        assert re.fullmatch(r'%s\*\* \w+' % api, args.split(',')[0].strip()), (api, args)
+        assert _lib._SIGS[api + '_create'][1][0] is C.POINTER(C.c_void_p), api
+
+
 def test_table_layout_matches_header():
     from aphantasia_b200 import _rng
     hdr = open(os.path.join(ROOT, 'include', 'aphb200.h')).read()
