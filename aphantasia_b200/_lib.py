@@ -37,7 +37,6 @@ _SIGS = {
     'aph_sample_fwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     'aph_sample_fwd_patches': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_void_p, C.c_int,
                                          C.POINTER(C.c_int), C.c_void_p]),
-    'aph_sample_bwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     'aph_sample_bwd_scaled': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, C.c_int, C.c_int, C.c_float, c_f32p, C.c_void_p]),
     'aph_rng_crop_tables': (C.c_int, [C.c_void_p, C.c_int64, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                       C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, C.c_int, C.c_void_p]),

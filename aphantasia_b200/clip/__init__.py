@@ -220,7 +220,7 @@ class VisionTransformer(_Tower):
         self.output_dim = sd['proj'].shape[1]
         self._sd = {k: v.detach().float().contiguous() for k, v in sd.items()}
         self._generation, self.recomputes, self._handle_epoch = 0, 0, 0        # see _EncodeImage
-        self._patch_gen, self._patch_written, self.prepatched_forwards = 0, False, 0      # see _patchlink
+        self._patch_gen, self.prepatched_forwards = 0, 0      # see _patchlink
         _patchlink.register(self)
         if max_batch:
             self._ensure(max_batch)

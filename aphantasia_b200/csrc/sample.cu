@@ -14,10 +14,9 @@
 // (rotate tap -> erase test -> perspective taps) on top of the resized crop, so every intermediate is the reference's intermediate.
 //
 // Kernels:
-//   forward : k_resize (stage 1, separable, into a library scratch image) + k_compose (stages 2-5, three channels per thread; optionally
-//             also the encoder's bf16 patch operand, aph_sample_fwd_patches). Frames whose short side is too long for k_resize's
-//             per-warp crop rows (above ~6170 px at size 224) take k_sample_fwd instead: one CTA per (crop, channel), the channel's
-//             resized crop in 196 KB of shared memory;
+//   forward : k_resize (stage 1, separable, into a library scratch image; the direct 16-tap form for frames whose short side is too
+//             long for its per-warp crop rows) + k_compose / k_compose_kornia (stages 2-5, three channels per thread; optionally also
+//             the encoder's bf16 patch operand, aph_sample_fwd_patches);
 //   backward: k_bwd_warp_adjoint (perspective crops: rotation adjoint as a gather, perspective adjoint by global reductions into a
 //             scratch image) + k_bwd_bicubic3 (every crop: rotation adjoint gathered inline, bicubic adjoint through per-warp strips
 //             and 16-byte vector reductions into the canvas gradient).
@@ -123,27 +122,6 @@ __device__ __forceinline__ bool erased(const CropParams& p, int y, int x) {
   return (unsigned)(y - p.ei) < (unsigned)p.eh && (unsigned)(x - p.ej) < (unsigned)p.ew;
 }
 
-__device__ __forceinline__ float tap_dot(const float* __restrict__ A, const Bilin& b, int size) {
-  float v = 0.f;
-  if (b.w00 != 0.f) v += b.w00 * A[b.y0 * size + b.x0];
-  if (b.w01 != 0.f) v += b.w01 * A[b.y0 * size + b.x0 + 1];
-  if (b.w10 != 0.f) v += b.w10 * A[(b.y0 + 1) * size + b.x0];
-  if (b.w11 != 0.f) v += b.w11 * A[(b.y0 + 1) * size + b.x0 + 1];
-  return v;
-}
-
-// value of the post-perspective, post-erase image B at integer pixel (y, x)
-template <bool PERSP, bool ERASE = true>
-__device__ __forceinline__ float stageB(const float* __restrict__ A, const CropParams& p, int y, int x, int size) {
-  if (ERASE && erased(p, y, x)) return 0.f;
-  if (PERSP) {
-    const Bilin b = persp_taps(p, y, x, size);
-    const float mask = b.w00 + b.w01 + b.w10 + b.w11;
-    return tap_dot(A, b, size) * mask;
-  }
-  return A[y * size + x];
-}
-
 __constant__ float c_inv_std[3] = {1.f / 0.26862954f, 1.f / 0.26130258f, 1.f / 0.27577711f};
 __constant__ float c_shift[3] = {-0.48145466f / 0.26862954f, -0.4578275f / 0.26130258f, -0.40821073f / 0.27577711f};
 
@@ -153,111 +131,14 @@ __device__ __forceinline__ bool identity_rot(const CropParams& p) { return p.r00
 __constant__ float c_mean[3] = {0.48145466f, 0.4578275f, 0.40821073f};
 __constant__ float c_std[3] = {0.26862954f, 0.26130258f, 0.27577711f};
 
-// Per-CTA tap tables: the 4 bicubic taps (canvas offset, weight) of every output row and column, computed once
-// (size entries each) instead of per pixel; wrap-around ('over*' frames) is folded into the stored canvas index.
-constexpr int STRIP = 128;     // per-warp strip (floats) used by the separable bicubic stage
-struct TapTables { int* xo; float* xw; int* yo; float* yw; };
-__device__ __forceinline__ TapTables build_taps(float* base, const CropParams& p, int size, int H, int W, int pad_top, int pad_left, float scale) {
-  TapTables t;
-  t.xo = reinterpret_cast<int*>(base); t.xw = base + 4 * size; t.yo = reinterpret_cast<int*>(base + 8 * size); t.yw = base + 12 * size;
-  for (int k = threadIdx.x; k < 2 * size; k += blockDim.x) {
-    const bool isy = k >= size;
-    const int o = isy ? k - size : k;
-    int idx[4]; float w[4];
-    cubic_taps(o, scale, p.cs, idx, w);
-#pragma unroll
-    for (int a = 0; a < 4; ++a) {
-      if (isy) { int y = p.oy + idx[a] - pad_top; y %= H; if (y < 0) y += H; t.yo[4 * o + a] = y * W; t.yw[4 * o + a] = w[a]; }
-      else { int x = p.ox + idx[a] - pad_left; x %= W; if (x < 0) x += W; t.xo[4 * o + a] = x; t.xw[4 * o + a] = w[a]; }
-    }
-  }
-  return t;
-}
-
-// rotate tap -> erase test -> perspective taps on top of the resized image A, then the CLIP normalisation as one FMA
-template <bool PERSP, bool ERASE = true>
-__device__ __forceinline__ void fwd_compose(const float* __restrict__ A, const CropParams& p, int size, int warp, int lane, int nwarps,
-                                            float inv_sd, float shift, float* __restrict__ o) {
-  for (int i = warp; i < size; i += nwarps) {
-    for (int j = lane; j < size; j += 32) {
-      const Bilin b = rot_taps(p, i, j, size);
-      const float mask = b.w00 + b.w01 + b.w10 + b.w11;
-      float s = 0.f;
-      if (b.w00 != 0.f) s += b.w00 * stageB<PERSP, ERASE>(A, p, b.y0, b.x0, size);
-      if (b.w01 != 0.f) s += b.w01 * stageB<PERSP, ERASE>(A, p, b.y0, b.x0 + 1, size);
-      if (b.w10 != 0.f) s += b.w10 * stageB<PERSP, ERASE>(A, p, b.y0 + 1, b.x0, size);
-      if (b.w11 != 0.f) s += b.w11 * stageB<PERSP, ERASE>(A, p, b.y0 + 1, b.x0 + 1, size);
-      o[i * size + j] = fmaf(s * mask, inv_sd, shift);
-    }
-  }
-}
-
-// Forward in one kernel, the path for frames too large for k_resize (sample_fwd_impl): one CTA per (crop, channel), the canvas read
-// through the per-CTA tap tables, the channel's resized crop in shared memory.
-__global__ void __launch_bounds__(1024, 1)
-k_sample_fwd(const float* __restrict__ canvas, int H, int W, int pad_top, int pad_left, const float* __restrict__ table,
-             int size, int kind, float* __restrict__ out) {
-  extern __shared__ float A[];
-  const int crop = blockIdx.x / 3, ch = blockIdx.x - crop * 3;
-  CropParams p = load_params(table + (size_t)crop * APH_CROP_PARAM_FLOATS);
-  prescale(p, size);
-  const float* cch = canvas + (size_t)ch * H * W;
-  const float scale = (size > 1) ? (float)(p.cs - 1) / (float)(size - 1) : 0.f;
-  const int n = size * size;
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
-  const TapTables tt = build_taps(A + ((n + 3) & ~3), p, size, H, W, pad_top, pad_left, scale);
-  __syncthreads();
-  // ---- stage 1: bicubic resize into shared memory (warp = output row), direct 16-tap form through the per-CTA tap tables.
-  // (A vertical-first per-warp strip variant was slower here: two extra warp barriers
-  // and a dependent shared-memory round trip per chunk outweigh the saved L1 wavefronts; the backward keeps its strip.)
-  for (int i = warp; i < size; i += nwarps) {
-    const int4 yo = *reinterpret_cast<const int4*>(tt.yo + 4 * i);
-    const float4 wy = *reinterpret_cast<const float4*>(tt.yw + 4 * i);
-    const float* r0 = cch + yo.x; const float* r1 = cch + yo.y; const float* r2 = cch + yo.z; const float* r3 = cch + yo.w;
-    for (int j0 = 0; j0 < size; j0 += 32) {
-      const int j = j0 + lane;
-      const int jc = min(j, size - 1);
-      const int4 xo = *reinterpret_cast<const int4*>(tt.xo + 4 * jc);
-      const float4 wx = *reinterpret_cast<const float4*>(tt.xw + 4 * jc);
-      const float v0 = wx.x * __ldg(r0 + xo.x) + wx.y * __ldg(r0 + xo.y) + wx.z * __ldg(r0 + xo.z) + wx.w * __ldg(r0 + xo.w);
-      const float v1 = wx.x * __ldg(r1 + xo.x) + wx.y * __ldg(r1 + xo.y) + wx.z * __ldg(r1 + xo.z) + wx.w * __ldg(r1 + xo.w);
-      const float v2 = wx.x * __ldg(r2 + xo.x) + wx.y * __ldg(r2 + xo.y) + wx.z * __ldg(r2 + xo.z) + wx.w * __ldg(r2 + xo.w);
-      const float v3 = wx.x * __ldg(r3 + xo.x) + wx.y * __ldg(r3 + xo.y) + wx.z * __ldg(r3 + xo.z) + wx.w * __ldg(r3 + xo.w);
-      float acc = wy.x * v0;
-      acc += wy.y * v1; acc += wy.z * v2; acc += wy.w * v3;
-      if (j < size) A[i * size + j] = acc;
-    }
-  }
-  __syncthreads();
-  // ---- stages 2-5 by tap composition (the perspective branch is CTA-uniform: specialised loops)
-  float* o = out + ((size_t)crop * 3 + ch) * n;
-  const float inv_sd = 1.f / c_std[ch], shift = -c_mean[ch] * inv_sd;
-  if (kind == APH_TF_FAST) {
-    const bool er = (p.flags & APH_FLAG_ERASE) != 0;      // CTA-uniform: crops without an erase hit (80 %) skip the rectangle test per tap
-    if (p.flags & APH_FLAG_PERSP) { if (er) fwd_compose<true, true>(A, p, size, warp, lane, nwarps, inv_sd, shift, o); else fwd_compose<true, false>(A, p, size, warp, lane, nwarps, inv_sd, shift, o); }
-    else if (identity_rot(p)) {
-      // angle 0 (26 % of the draws, transforms.py:168) without a perspective hit: the rotate stage resamples every pixel at its own
-      // centre (bilinear weights (1, 0, 0, 0) up to 1e-6 round-off, coverage 1), so stages 2-5 reduce to erase + normalise.
-      for (int idx = threadIdx.x; idx < n; idx += blockDim.x) {
-        const int y = idx / size, x = idx - y * size;
-        o[idx] = erased(p, y, x) ? shift : fmaf(A[idx], inv_sd, shift);
-      }
-    }
-    else if (er) fwd_compose<false, true>(A, p, size, warp, lane, nwarps, inv_sd, shift, o);
-    else fwd_compose<false, false>(A, p, size, warp, lane, nwarps, inv_sd, shift, o);
-  } else {
-    const float a = (kind != APH_TF_NONE) ? inv_sd : 1.f, b = (kind != APH_TF_NONE) ? shift : 0.f;
-    for (int idx = threadIdx.x; idx < n; idx += blockDim.x) o[idx] = fmaf(A[idx], a, b);
-  }
-}
-
-
 // ---------------------------------------------------------------------------------------------
-// Forward, two-kernel form (round 2). The one-kernel form above keeps the resized crop of ONE channel in 196 KB of shared memory and
-// recomputes the rotate / perspective geometry per channel; it is instruction-issue bound (~295 thread instructions per pixel and
-// channel). Here
+// Forward in two kernels.
 //   k_resize : stage 1 alone, SEPARABLE -- a warp owns an output row: vertical 4-tap pass over the crop's columns (coalesced row
 //              reads) into a per-warp strip, then the horizontal 4-tap pass out of the strip; 8 rows of state per CTA, 7 CTAs / SM.
+//              A frame whose short side is too long for that strip (above ~6170 px at size 224) takes the DIRECT form, launched with
+//              cap = 0 (no strip memory, 7 KB of tap tables): every output pixel reads its 16 taps straight from the canvas, four
+//              horizontal taps per source row, then the vertical combination. It is a template parameter rather than a run-time
+//              flag because the flag would cost the strip forms' output loop its unrolling.
 //              Result A [S,3,size,size] goes to a library scratch buffer (L2 / HBM), or straight to the output for transform kinds
 //              without a warp stage.
 //   k_compose: stages 2-5 for ALL THREE channels of a pixel per thread: one evaluation of the rotate (and perspective) taps,
@@ -272,12 +153,13 @@ __device__ __forceinline__ size_t patch_index(const PatchOut& po, int s, int c, 
   return ((size_t)(s * po.g + gy) * po.g + gx) * (size_t)patch_k(po.p) + (size_t)(c * po.p + py) * po.p + px;
 }
 
-template <bool WRAP>
+// DIRECT is launched with WRAP = true: the wrap is a no-op on an unpadded frame
+template <bool WRAP, bool DIRECT>
 __global__ void __launch_bounds__(256)
 k_resize(const float* __restrict__ canvas, int H, int W, int pad_top, int pad_left, const float* __restrict__ table, int size, int rows_per_cta,
          int cap, int kind, float* __restrict__ dst, PatchOut po) {
   extern __shared__ float rs[];
-  int* xi = reinterpret_cast<int*>(rs);              // [4*size] crop-relative source columns of every output column
+  int* xi = reinterpret_cast<int*>(rs);              // [4*size] source columns of every output column: crop-relative, or (direct) canvas
   float* xw = rs + 4 * size;                         // [4*size] their weights
   const int crop = blockIdx.x / 3, ch = blockIdx.x - crop * 3;
   __shared__ int s_oy, s_ox, s_cs;
@@ -291,7 +173,11 @@ k_resize(const float* __restrict__ canvas, int H, int W, int pad_top, int pad_le
     int idx[4]; float w[4];
     cubic_taps(k, scale, p.cs, idx, w);
 #pragma unroll
-    for (int a = 0; a < 4; ++a) { xi[4 * k + a] = idx[a]; xw[4 * k + a] = w[a]; }
+    for (int a = 0; a < 4; ++a) {
+      int x = idx[a];
+      if (DIRECT) { x = (p.ox + x - pad_left) % W; if (x < 0) x += W; }
+      xi[4 * k + a] = x; xw[4 * k + a] = w[a];
+    }
   }
   __syncthreads();
   float* strip = rs + 8 * size + warp * cap;
@@ -309,7 +195,9 @@ k_resize(const float* __restrict__ canvas, int H, int W, int pad_top, int pad_le
       if (WRAP) { y %= H; if (y < 0) y += H; }
       rp[a] = cch + y * W + (WRAP ? 0 : p.ox - pad_left);
     }
-    if (WRAP) {
+    if (DIRECT) {
+      // no strip: the loop below reads all 16 taps from the canvas
+    } else if (WRAP) {
       for (int x = lane; x < p.cs; x += 32) {
         int col = (p.ox + x - pad_left) % W; if (col < 0) col += W;
         float v = wy[0] * __ldg(rp[0] + col);
@@ -328,8 +216,18 @@ k_resize(const float* __restrict__ canvas, int H, int W, int pad_top, int pad_le
     for (int j = lane; j < size; j += 32) {
       const int4 xo = *reinterpret_cast<const int4*>(xi + 4 * j);
       const float4 wx = *reinterpret_cast<const float4*>(xw + 4 * j);
-      float acc = wx.x * strip[xo.x];
-      acc += wx.y * strip[xo.y]; acc += wx.z * strip[xo.z]; acc += wx.w * strip[xo.w];
+      float acc;
+      if (DIRECT) {
+        const float v0 = wx.x * __ldg(rp[0] + xo.x) + wx.y * __ldg(rp[0] + xo.y) + wx.z * __ldg(rp[0] + xo.z) + wx.w * __ldg(rp[0] + xo.w);
+        const float v1 = wx.x * __ldg(rp[1] + xo.x) + wx.y * __ldg(rp[1] + xo.y) + wx.z * __ldg(rp[1] + xo.z) + wx.w * __ldg(rp[1] + xo.w);
+        const float v2 = wx.x * __ldg(rp[2] + xo.x) + wx.y * __ldg(rp[2] + xo.y) + wx.z * __ldg(rp[2] + xo.z) + wx.w * __ldg(rp[2] + xo.w);
+        const float v3 = wx.x * __ldg(rp[3] + xo.x) + wx.y * __ldg(rp[3] + xo.y) + wx.z * __ldg(rp[3] + xo.z) + wx.w * __ldg(rp[3] + xo.w);
+        acc = wy[0] * v0;
+        acc += wy[1] * v1; acc += wy[2] * v2; acc += wy[3] * v3;
+      } else {
+        acc = wx.x * strip[xo.x];
+        acc += wx.y * strip[xo.y]; acc += wx.z * strip[xo.z]; acc += wx.w * strip[xo.w];
+      }
       const float v = (kind >= APH_TF_FAST) ? acc : fmaf(acc, na, nb);
       o[i * size + j] = v;
       if (kind < APH_TF_FAST && po.base) po.base[patch_index(po, crop, ch, i, j)] = __float2bfloat16_rn(v);
@@ -581,6 +479,7 @@ __device__ __forceinline__ void scatter3(float* __restrict__ g, int n, const Bil
   }
 }
 
+constexpr int STRIP = 128;      // per-warp strip (floats per channel) of k_bwd_bicubic3
 constexpr int BB_ROWS = 32;     // gradient rows per CTA of k_bwd_bicubic3
 constexpr int WA_ROWS = 8;      // rows per CTA of k_bwd_warp_adjoint (one per warp: the 20 % of crops it serves must still fill the machine)
 
@@ -843,14 +742,12 @@ k_bwd_bicubic3(const float* __restrict__ grad_out, float* __restrict__ gA_all, i
 
 using namespace aph;
 
-// Largest output side of the sampler. k_sample_fwd, the only forward for frames too large for k_resize, holds one channel's resized
-// crop and its tap tables in one CTA's shared memory: 210 KB of the 227 KB at this size.
+// Largest output side of the sampler: the largest crop side the image encoders take, and the largest the tests cover.
 constexpr int kMaxSampleSize = 224;
-static_assert(((size_t)kMaxSampleSize * kMaxSampleSize + 4 + 16 * kMaxSampleSize) * sizeof(float) <= 227 * 1024, "k_sample_fwd at the largest size");
 
 static int check_sample_args(const char* who, int H, int W, int S, int size, int kind) {
   APH_REQUIRE(H > 0 && W > 0 && S >= 0 && size > 0, "%s: bad shape H=%d W=%d S=%d size=%d", who, H, W, S, size);
-  APH_REQUIRE(size <= kMaxSampleSize, "%s: size=%d does not fit one CTA's shared memory (max %d)", who, size, kMaxSampleSize);
+  APH_REQUIRE(size <= kMaxSampleSize, "%s: size=%d is above %d, the largest crop side the image encoders take", who, size, kMaxSampleSize);
   APH_REQUIRE(kind >= APH_TF_NONE && kind <= APH_TF_ELASTIC, "%s: unknown transform kind %d", who, kind);
   return 0;
 }
@@ -858,11 +755,11 @@ static int check_sample_args(const char* who, int H, int W, int S, int size, int
 static Scratch g_A;                    // resized crops [S,3,size,size] between k_resize and k_compose
 
 static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int pad_left, const float* table, int S,
-                           int size, int kind, float* out, PatchOut po, int* patches_written, void* stream);
+                           int size, int kind, float* out, PatchOut po, void* stream);
 
 extern "C" int aph_sample_fwd(const float* canvas, int H, int W, int pad_top, int pad_left, const float* table, int S,
                               int size, int kind, float* out, void* stream) {
-  return sample_fwd_impl(canvas, H, W, pad_top, pad_left, table, S, size, kind, out, PatchOut{nullptr, 1, 1}, nullptr, stream);
+  return sample_fwd_impl(canvas, H, W, pad_top, pad_left, table, S, size, kind, out, PatchOut{nullptr, 1, 1}, stream);
 }
 
 extern "C" int aph_sample_fwd_patches(const float* canvas, int H, int W, int pad_top, int pad_left, const float* table, int S,
@@ -872,34 +769,23 @@ extern "C" int aph_sample_fwd_patches(const float* canvas, int H, int W, int pad
   // the kornia kinds write size + 8: the operand is the top-left (grid * patch)^2 window conv1 reads
   const int side = size + (kind >= APH_TF_CUSTOM ? 2 * KPAD : 0);
   APH_REQUIRE(kind >= APH_TF_CUSTOM ? side >= patch : size % patch == 0, "aph_sample_fwd_patches: size=%d does not fit patch=%d", size, patch);
-  *patches_written = 0;
-  return sample_fwd_impl(canvas, H, W, pad_top, pad_left, table, S, size, kind, out,
-                         PatchOut{reinterpret_cast<__nv_bfloat16*>(patches_bf16), patch, side / patch}, patches_written, stream);
+  if (int e = sample_fwd_impl(canvas, H, W, pad_top, pad_left, table, S, size, kind, out,
+                              PatchOut{reinterpret_cast<__nv_bfloat16*>(patches_bf16), patch, side / patch}, stream)) return e;
+  *patches_written = 1;
+  return 0;
 }
 
 static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int pad_left, const float* table, int S,
-                           int size, int kind, float* out, PatchOut po, int* patches_written, void* stream) {
+                           int size, int kind, float* out, PatchOut po, void* stream) {
   if (int e = check_sample_args("aph_sample_fwd", H, W, S, size, kind)) return e;
   if (S == 0) return 0;
   APH_REQUIRE(canvas && table && out, "aph_sample_fwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
-  const int cap = ((H + 2 * pad_top < W + 2 * pad_left ? H + 2 * pad_top : W + 2 * pad_left) + 1 + 3) & ~3;     // crops never exceed the short side of the frame
+  int cap = ((H + 2 * pad_top < W + 2 * pad_left ? H + 2 * pad_top : W + 2 * pad_left) + 1 + 3) & ~3;     // crops never exceed the short side of the frame
+  // k_resize holds one crop row per warp in shared memory, sized by the frame's short side; above ~6170 px (at size 224) that does not
+  // fit, and k_resize runs its direct form (cap = 0: the x tap tables alone)
+  if (((size_t)8 * size + (size_t)8 * cap) * sizeof(float) > 200 * 1024) cap = 0;
   const size_t smem2 = ((size_t)8 * size + (size_t)8 * cap) * sizeof(float);
-  const bool kornia = kind >= APH_TF_CUSTOM;
-  APH_REQUIRE(!kornia || smem2 <= 200 * 1024, "aph_sample_fwd: a %dx%d frame is too large for transform kind %d", H + 2 * pad_top, W + 2 * pad_left, kind);
-  if (smem2 > 200 * 1024) {
-    // k_resize holds one crop row per warp in shared memory, sized by the frame's short side; above ~6170 px (at size 224) that does not
-    // fit, and the one-kernel form, which reads the canvas through its tap tables, is the forward there (it writes no patch operand)
-    const size_t smem = ((size_t)size * size + 4 + 16 * (size_t)size) * sizeof(float);
-    static size_t configured = 0;
-    if (smem > configured) {
-      APH_CUDA_OK(cudaFuncSetAttribute(k_sample_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      configured = smem;
-    }
-    k_sample_fwd<<<S * 3, 1024, smem, st>>>(canvas, H, W, pad_top, pad_left, table, size, kind, out);
-    APH_LAUNCH_OK();
-    return 0;
-  }
   float* dst = out;
   if (kind >= APH_TF_FAST) {
     if (int e = g_A.grow((size_t)S * 3 * size * size * sizeof(float), st)) return e;
@@ -907,53 +793,40 @@ static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int p
   }
   static size_t conf = 0;
   if (smem2 > conf) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_resize<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_resize<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+    APH_CUDA_OK(cudaFuncSetAttribute(k_resize<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
+    APH_CUDA_OK(cudaFuncSetAttribute(k_resize<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
     conf = smem2;
   }
   const int rows_per_cta = 32;
   const dim3 g1(S * 3, (size + rows_per_cta - 1) / rows_per_cta);
-  if (pad_top || pad_left) k_resize<true><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
-  else k_resize<false><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
+  if (cap == 0) k_resize<true, true><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
+  else if (pad_top || pad_left) k_resize<true, false><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
+  else k_resize<false, false><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
   APH_LAUNCH_OK();
   if (kind == APH_TF_FAST) {
     const int tiles = ((size + 15) / 16) * ((size + 15) / 16);
     k_compose<<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
     APH_LAUNCH_OK();
-  } else if (kornia) {
+  } else if (kind >= APH_TF_CUSTOM) {
     const int s = size + 2 * KPAD, tiles = ((s + 15) / 16) * ((s + 15) / 16);
     if (kind == APH_TF_ELASTIC) k_compose_kornia<true><<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
     else k_compose_kornia<false><<<dim3(tiles, S), 256, 0, st>>>(g_A.p, table, size, out, po);
     APH_LAUNCH_OK();
   }
-  if (patches_written) *patches_written = 1;
   return 0;
 }
 
 static Scratch g_gW;                   // warp-stage adjoint scratch [S,3,size,size] of the default backward (all-zero between calls)
 static Scratch g_gR;                   // kornia kinds: d loss / d rotated image [S,3,size+8,size+8], rewritten by every backward
 
-static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int pad_left, const float* table, int S,
-                           int size, int kind, float* grad_canvas, float gscale, void* stream);
-
-extern "C" int aph_sample_bwd(const float* grad_out, int H, int W, int pad_top, int pad_left, const float* table, int S,
-                              int size, int kind, float* grad_canvas, void* stream) {
-  return sample_bwd_impl(grad_out, H, W, pad_top, pad_left, table, S, size, kind, grad_canvas, 1.f, stream);
-}
-
 extern "C" int aph_sample_bwd_scaled(const float* grad_out, int H, int W, int pad_top, int pad_left, const float* table, int S,
                                      int size, int kind, float gscale, float* grad_canvas, void* stream) {
-  return sample_bwd_impl(grad_out, H, W, pad_top, pad_left, table, S, size, kind, grad_canvas, gscale, stream);
-}
-
-static int sample_bwd_impl(const float* grad_out, int H, int W, int pad_top, int pad_left, const float* table, int S,
-                           int size, int kind, float* grad_canvas, float gscale, void* stream) {
-  if (int e = check_sample_args("aph_sample_bwd", H, W, S, size, kind)) return e;
-  APH_REQUIRE(grad_canvas, "aph_sample_bwd: null grad_canvas");
+  if (int e = check_sample_args("aph_sample_bwd_scaled", H, W, S, size, kind)) return e;
+  APH_REQUIRE(grad_canvas, "aph_sample_bwd_scaled: null grad_canvas");
   cudaStream_t st = (cudaStream_t)stream;
   APH_CUDA_OK(cudaMemsetAsync(grad_canvas, 0, (size_t)3 * H * W * sizeof(float), st));
   if (S == 0) return 0;
-  APH_REQUIRE(grad_out && table, "aph_sample_bwd: null pointer");
+  APH_REQUIRE(grad_out && table, "aph_sample_bwd_scaled: null pointer");
   const size_t smem3 = ((size_t)8 * size + 8 * 3 * STRIP) * sizeof(float);
   static size_t configured3 = 48 * 1024;
   if (smem3 > configured3) {

@@ -30,12 +30,11 @@ class _SliceImgs(torch.autograd.Function):
         if vis is not None and S > 0:
             # the encoder that will consume this batch takes its patch operand straight from the sampler's last stage (_patchlink)
             vis._ensure(S)
-            ptr, patch, grid, wrote = C.c_void_p(), C.c_int(), C.c_int(), C.c_int(0)
+            ptr, patch, grid = C.c_void_p(), C.c_int(), C.c_int()
             check(lib().aph_vit_patch_operand(vis.handle, S, C.byref(ptr), C.byref(patch), C.byref(grid)), 'aph_vit_patch_operand')
             check(lib().aph_sample_fwd_patches(x.data_ptr(), H, W, pad_top, pad_left, table_dev.data_ptr(), S, size, kind, out.data_ptr(),
-                                               ptr, patch.value, C.byref(wrote), stream_ptr()), 'aph_sample_fwd_patches')
+                                               ptr, patch.value, C.byref(C.c_int()), stream_ptr()), 'aph_sample_fwd_patches')
             vis._patch_gen += 1                     # whatever the buffer held before is gone
-            vis._patch_written = bool(wrote.value)
         else:
             check(lib().aph_sample_fwd(x.data_ptr(), H, W, pad_top, pad_left, table_dev.data_ptr(), S, size, kind, out.data_ptr(),
                                        stream_ptr()), 'aph_sample_fwd')
@@ -118,7 +117,7 @@ def slice_imgs(imgs, count, size=224, transform=None, align='uniform', macro=0.)
         vis = _patchlink.target(side, windowed=side != size) if len(imgs) == 1 else None
         gen0 = vis._patch_gen if vis is not None else 0
         out = _SliceImgs.apply(img, tdev, meta, vis)
-        if vis is not None and vis._patch_gen != gen0 and vis._patch_written:
+        if vis is not None and vis._patch_gen != gen0:
             _patchlink.stamp(out, vis, hi - lo)
         sliced.append(out)
     return sliced

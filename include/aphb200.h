@@ -166,24 +166,21 @@ int aph_cppn_bwd(aph_cppn* handle, const float* coords, int N, int H, int W, con
  * (bilinear, zeros, x coverage) -> erase -> rotate (bilinear, zeros, x coverage) -> normalise.
  * canvas [3,H,W]; the sampling frame is the canvas wrap-padded by (pad_top, pad_left)
  * ('over*' aligns, utils.py:152-187; 0,0 otherwise); table: DEVICE [S, APH_CROP_PARAM_FLOATS];
- * out [S,3,size,size] ([S,3,size+8,size+8] for APH_TF_CUSTOM / APH_TF_ELASTIC). the resized crop, its tap tables and
- * the per-warp strips must fit one CTA's shared memory (size <= 224).                                               */
+ * out [S,3,size,size] ([S,3,size+8,size+8] for APH_TF_CUSTOM / APH_TF_ELASTIC). size <= 224, the largest crop side
+ * the image encoders take; the frame may have any size.                                                             */
 int aph_sample_fwd(const float* canvas, int H, int W, int pad_top, int pad_left,
                    const float* table, int S, int size, int kind, float* out, void* stream);
 /* Same, and the last stage also writes the batch as the encoder's patch operand (bf16, patch-major: see
  * aph_vit_patch_operand below); the output side (size, or size + 8) must be a multiple of patch, or lie in
  * [res, res + patch) of an encoder with input resolution res = grid * patch: then the operand is the top-left res x res
- * window, as conv1 reads it. *patches_written = 1 when it did (0: the one-kernel fallback form ran and the caller has
- * to use aph_vit_fwd on `out`).                                                                                      */
+ * window, as conv1 reads it. The operand is written for every frame size and transform kind:
+ * *patches_written = 1 on success.                                                                                   */
 int aph_sample_fwd_patches(const float* canvas, int H, int W, int pad_top, int pad_left,
                            const float* table, int S, int size, int kind, float* out,
                            void* patches_bf16, int patch, int* patches_written, void* stream);
-/* grad_out [S,3,size,size] -> grad_canvas [3,H,W] (zeroed here, then accumulated).                 */
-int aph_sample_bwd(const float* grad_out, int H, int W, int pad_top, int pad_left,
-                   const float* table, int S, int size, int kind, float* grad_canvas, void* stream);
-
-/* Same with every contribution multiplied by gscale (the weight S_local / S of this rank's shard in the all-reduced
- * gradient under torchrun: folded into the scatter instead of a separate pass over the canvas).     */
+/* grad_out [S,3,size,size] -> grad_canvas [3,H,W] (zeroed here, then accumulated), every contribution multiplied by
+ * gscale: 1 on one GPU, the weight S_local / S of this rank's shard in the all-reduced gradient under torchrun (folded
+ * into the scatter instead of a separate pass over the canvas).                                     */
 int aph_sample_bwd_scaled(const float* grad_out, int H, int W, int pad_top, int pad_left,
                           const float* table, int S, int size, int kind, float gscale, float* grad_canvas, void* stream);
 

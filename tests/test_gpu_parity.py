@@ -12,6 +12,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
+import kornia_oracle as KO  # noqa: E402
 from oracle import restate as R  # noqa: E402
 
 
@@ -122,7 +123,7 @@ def test_sampler_vs_reference_golden(L, golden, name):
     assert _rel(canvas.grad[:, :, ::st, ::st], golden['smp_%s_gcanvas' % name]) < 1e-4
 
 
-def test_sampler_abi_non_rotation_matrix(L):
+def test_sampler_abi_non_rotation_matrix_and_shard_weight(L):
     """The C ABI takes any 2x2 inverse affine matrix per crop; the reference's sampler only draws rotations. Rows with a sheared /
     scaled matrix (with and without a perspective hit) must take the general scatter adjoint, rows with a rotation the gather:
     forward and backward vs the oracle on a table that mixes both."""
@@ -145,14 +146,14 @@ def test_sampler_abi_non_rotation_matrix(L):
     x = canvas.cuda().contiguous(); t = torch.tensor(tab).cuda(); out = torch.empty(S, 3, size, size, device='cuda'); g = torch.empty(1, 3, 300, 420, device='cuda')
     check(lib().aph_sample_fwd(x.data_ptr(), 300, 420, 0, 0, t.data_ptr(), S, size, 2, out.data_ptr(), stream_ptr()), 'fwd')
     cg = cot.cuda().contiguous()
-    check(lib().aph_sample_bwd(cg.data_ptr(), 300, 420, 0, 0, t.data_ptr(), S, size, 2, g.data_ptr(), stream_ptr()), 'bwd')
+    check(lib().aph_sample_bwd_scaled(cg.data_ptr(), 300, 420, 0, 0, t.data_ptr(), S, size, 2, 1., g.data_ptr(), stream_ptr()), 'bwd')
     torch.cuda.synchronize()
     assert _rel(out, ref) < 1e-5
     assert _rel(g, co.grad) < 1e-4
     # shard weight of the multi-GPU path (S_local / S, folded into the kernels): scales the gradient, nothing else
     g2 = torch.empty_like(g)
     check(lib().aph_sample_bwd_scaled(cg.data_ptr(), 300, 420, 0, 0, t.data_ptr(), S, size, 2, 0.375, g2.data_ptr(), stream_ptr()), 'bwd_scaled')
-    check(lib().aph_sample_bwd(cg.data_ptr(), 300, 420, 0, 0, t.data_ptr(), S, size, 2, g.data_ptr(), stream_ptr()), 'bwd')     # scratch must be clean again
+    check(lib().aph_sample_bwd_scaled(cg.data_ptr(), 300, 420, 0, 0, t.data_ptr(), S, size, 2, 1., g.data_ptr(), stream_ptr()), 'bwd')     # scratch must be clean again
     torch.cuda.synchronize()
     assert _rel(g2, 0.375 * co.grad) < 1e-4 and _rel(g, co.grad) < 1e-4
     # a frame whose rows are not 16-byte aligned takes the scalar-reduction drain
@@ -161,7 +162,7 @@ def test_sampler_abi_non_rotation_matrix(L):
     co2 = canvas_o.clone().requires_grad_(True)
     (R.sample_crops(co2, tab, size, 2) * cot).sum().backward()
     g3 = torch.empty(1, 3, 300, Wo, device='cuda')
-    check(lib().aph_sample_bwd(cg.data_ptr(), 300, Wo, 0, 0, t.data_ptr(), S, size, 2, g3.data_ptr(), stream_ptr()), 'bwd odd W')
+    check(lib().aph_sample_bwd_scaled(cg.data_ptr(), 300, Wo, 0, 0, t.data_ptr(), S, size, 2, 1., g3.data_ptr(), stream_ptr()), 'bwd odd W')
     torch.cuda.synchronize()
     assert _rel(g3, co2.grad) < 1e-4
 
@@ -192,16 +193,17 @@ def test_sampler_vs_oracle_720p(L, kind, cot_scale):
     assert _rel(cc.grad, co.grad) < 1e-4
 
 
-@pytest.mark.parametrize('kind', [0, 1, 2])
-def test_sampler_large_frame_vs_oracle(L, kind):
-    """A frame whose short side is too long for k_resize's per-warp crop rows (above ~6170 px at size 224) takes the one-kernel
-    forward, which writes no patch operand. A small canvas wrap-padded by a wide overscan makes such a frame cheaply on the device;
-    one crop is nearly as large as the frame. Forward and backward vs the oracle."""
+@pytest.mark.parametrize('kind', [0, 1, 2, 3, 4])
+def test_sampler_large_frame_every_kind_vs_oracle(L, kind):
+    """A frame whose short side is too long for k_resize's per-warp crop rows (above ~6170 px at size 224): k_resize reads each
+    output pixel's taps straight from the canvas. A small canvas wrap-padded by a wide overscan makes such a frame cheaply on the
+    device; one crop is nearly as large as the frame. Forward and backward vs the oracle (tests/kornia_oracle.py for
+    transforms_custom / _elastic), and the patch operand vs the bf16 im2col of the output's top-left 224 x 224 window."""
     from aphantasia_b200 import _rng
     from aphantasia_b200._lib import check, lib, stream_ptr
     H, W, size, pad_top, pad_left = 300, 420, 224, 3000, 2950
     fh, fw = H + 2 * pad_top, W + 2 * pad_left
-    assert 8 * (size + ((min(fh, fw) + 4) & ~3)) * 4 > 200 * 1024        # k_resize's shared memory at this frame: over its limit
+    assert 8 * (size + ((min(fh, fw) + 4) & ~3)) * 4 > 200 * 1024        # k_resize's strips at this frame: over its limit
     _seed(13)
     tab = np.zeros((4, _rng.CROP_PARAM_FLOATS), np.float32)
     for row, (oy, ox, cs) in zip(tab, [(40, 70, 6200), (3000, 2950, 300), (5100, 400, 1100), (10, 6000, 260)]):
@@ -209,30 +211,33 @@ def test_sampler_large_frame_vs_oracle(L, kind):
         row[_rng.F_ROT:_rng.F_ROT + 4] = (1., 0., 0., 1.)
         if kind == 2:
             row[_rng.F_FLAGS] = _rng.draw_fast(row, size)
+        elif kind >= 3:
+            row[_rng.F_FLAGS] = _rng.draw_kornia(row, size, kind == 4)
     if kind == 2:
         assert int(tab[0, _rng.F_FLAGS]) & 1 and tab[0, _rng.F_ANGLE] != 0, 'the largest crop should have a perspective hit and a rotation'
-    S = len(tab)
+    if kind >= 3:
+        assert tab[0, _rng.F_ANGLE] != 0, 'the largest crop should have a rotation'
+    S, side = len(tab), _rng.out_side(size, kind)
     canvas = torch.rand(1, 3, H, W)
     co = canvas.clone().requires_grad_(True)
-    ref = R.sample_crops(co, tab, size, kind, frame=(pad_top, pad_left, fh, fw))
+    ref = (KO.sample_crops if kind >= 3 else R.sample_crops)(co, tab, size, kind, frame=(pad_top, pad_left, fh, fw))
     _seed(6)
     cot = torch.randn(ref.shape)
     (ref * cot).sum().backward()
     x = canvas.cuda().contiguous(); t = torch.tensor(tab).cuda(); cg = cot.cuda().contiguous()
-    out = torch.empty(S, 3, size, size, device='cuda'); g = torch.empty(1, 3, H, W, device='cuda')
+    out = torch.empty(S, 3, side, side, device='cuda'); g = torch.empty(1, 3, H, W, device='cuda')
     patches = torch.empty(S * 7 * 7, 3 * 32 * 32, dtype=torch.bfloat16, device='cuda')
     wrote = C.c_int(-1)
     check(lib().aph_sample_fwd_patches(x.data_ptr(), H, W, pad_top, pad_left, t.data_ptr(), S, size, kind, out.data_ptr(), patches.data_ptr(),
                                        32, C.byref(wrote), stream_ptr()), 'fwd')
-    check(lib().aph_sample_bwd(cg.data_ptr(), H, W, pad_top, pad_left, t.data_ptr(), S, size, kind, g.data_ptr(), stream_ptr()), 'bwd')
+    check(lib().aph_sample_bwd_scaled(cg.data_ptr(), H, W, pad_top, pad_left, t.data_ptr(), S, size, kind, 1., g.data_ptr(), stream_ptr()), 'bwd')
     torch.cuda.synchronize()
-    assert wrote.value == 0
+    assert wrote.value == 1
     assert _rel(out, ref) < 1e-5
     assert _rel(g, co.grad) < 1e-4
-    out_k = torch.empty(S, 3, size + 8, size + 8, device='cuda')
-    for k in (3, 4):                                                    # the kornia kinds have no one-kernel form: they refuse the frame
-        assert lib().aph_sample_fwd(x.data_ptr(), H, W, pad_top, pad_left, t.data_ptr(), S, size, k, out_k.data_ptr(), stream_ptr()) != 0
-        assert b'too large' in lib().aph_last_error()
+    # row s*49 + gy*7 + gx, column c*1024 + py*32 + px
+    im2col = out[:, :, :224, :224].reshape(S, 3, 7, 32, 7, 32).permute(0, 2, 4, 1, 3, 5).reshape(S * 49, 3 * 1024)
+    assert torch.equal(patches, im2col.bfloat16())
 
 
 # ---------------------------------------------------------------------------------------------- loss / adam

@@ -80,18 +80,15 @@ def _abi(kind, S=24, size=224, H=300, W=420, seed=3):
         check(lib().aph_sample_fwd(x.data_ptr(), H, W, 0, 0, t.data_ptr(), S, size, kind, out.data_ptr(), stream_ptr()), 'fwd')
         return out
 
-    def bwd(g, gscale=None, k=kind):
+    def bwd(g, gscale=1., k=kind):
         gc_ = torch.full((1, 3, H, W), float('nan'), device='cuda')
-        if gscale is None:
-            check(lib().aph_sample_bwd(g.data_ptr(), H, W, 0, 0, t.data_ptr(), S, size, k, gc_.data_ptr(), stream_ptr()), 'bwd')
-        else:
-            check(lib().aph_sample_bwd_scaled(g.data_ptr(), H, W, 0, 0, t.data_ptr(), S, size, k, gscale, gc_.data_ptr(), stream_ptr()), 'bwd')
+        check(lib().aph_sample_bwd_scaled(g.data_ptr(), H, W, 0, 0, t.data_ptr(), S, size, k, gscale, gc_.data_ptr(), stream_ptr()), 'bwd')
         return gc_
     return fwd, bwd, (S, side, H, W)
 
 
 @pytest.mark.parametrize('kind', [3, 4])
-def test_sampler_adjoint_dot_product(kind):
+def test_sampler_backward_is_the_adjoint_of_the_forward(kind):
     """<S(x) - S(0), y> = <x, S^T y>: the backward is the exact adjoint of the forward's linear part."""
     fwd, bwd, (S, side, H, W) = _abi(kind)
     x = torch.rand(1, 3, H, W, device='cuda')
@@ -103,7 +100,7 @@ def test_sampler_adjoint_dot_product(kind):
 
 
 @pytest.mark.parametrize('kind', [3, 4])
-def test_gscale_scales_the_gradient_only_and_scratch_stays_clean(kind):
+def test_gscale_scales_the_gradient_only_and_the_scratches_stay_clean(kind):
     fwd, bwd, (S, side, H, W) = _abi(kind)
     x = torch.rand(1, 3, H, W, device='cuda')
     y = torch.randn(S, 3, side, side, device='cuda')
