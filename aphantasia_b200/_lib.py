@@ -15,6 +15,7 @@ _SIGS = {
     'aph_version': (C.c_int, []),
     'aph_last_error': (C.c_char_p, []),
     'aph_launch_count': (C.c_int64, []),
+    'aph_device_bytes': (C.c_int64, []),
     'aph_fft_plan_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int]),
     'aph_fft_plan_destroy': (C.c_int, [C.c_void_p]),
     'aph_synth_fft_fwd': (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, C.c_int, C.c_float, C.c_void_p, C.c_int,

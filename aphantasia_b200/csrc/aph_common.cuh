@@ -6,6 +6,8 @@
 #include <stdio.h>
 #include <stdarg.h>
 #include <atomic>
+#include <memory>
+#include <vector>
 
 #include "../../include/aphb200.h"
 
@@ -15,6 +17,7 @@ typedef __nv_bfloat16 bf16;
 
 void set_error(const char* fmt, ...);          // defined in api.cu (thread-local message)
 extern std::atomic<long long> g_launches;      // kernels launched by this library
+extern std::atomic<long long> g_device_bytes;  // device bytes held by DeviceAllocs, Scratch and StreamTemp
 
 inline void count_launch(int n = 1) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 
@@ -57,18 +60,56 @@ inline int num_sms() {
   return n;
 }
 
+// The three owner types below are the only code that allocates or frees device memory; aph_device_bytes() is their sum.
+struct NoCopy { NoCopy() = default; NoCopy(const NoCopy&) = delete; NoCopy& operator=(const NoCopy&) = delete; };
+
+// Device memory of a handle or plan: every allocation lives as long as its owner.
+struct DeviceAllocs : NoCopy {
+  int64_t bytes = 0;           // every allocation below
+  std::vector<void*> allocs;
+  ~DeviceAllocs() { for (void* p : allocs) cudaFree(p); g_device_bytes -= bytes; }
+  template <typename Tp>
+  int alloc(Tp** p, size_t count) {
+    APH_CUDA_OK(cudaMalloc((void**)p, count * sizeof(Tp)));
+    allocs.push_back(*p);
+    bytes += (int64_t)(count * sizeof(Tp));
+    g_device_bytes += (int64_t)(count * sizeof(Tp));
+    return 0;
+  }
+};
+
 // Library-owned device scratch (it survives torch.cuda.empty_cache()) that grows on demand. Growing waits for `st` first: work
-// already queued there may still use the old buffer.
-struct Scratch {
+// already queued there may still use the old buffer. One held for the life of the process is `static Scratch& s = *new Scratch;`,
+// never destroyed: a cudaFree from a static destructor would run after the CUDA runtime may have unloaded.
+struct Scratch : NoCopy {
   float* p = nullptr;
   size_t bytes = 0;
+  ~Scratch() { cudaFree(p); g_device_bytes -= bytes; }
   int grow(size_t need, cudaStream_t st) {
     if (need <= bytes) return 0;
     APH_CUDA_OK(cudaStreamSynchronize(st));
     if (p) cudaFree(p);
+    g_device_bytes -= bytes;
     p = nullptr; bytes = 0;
     APH_CUDA_OK(cudaMalloc(&p, need));
     bytes = need;
+    g_device_bytes += bytes;
+    return 0;
+  }
+};
+
+// A stream-ordered temporary: allocated on a stream, and freed on it behind the work queued there when it goes out of scope.
+template <typename T>
+struct StreamTemp : NoCopy {
+  T* p = nullptr;
+  size_t bytes = 0;
+  cudaStream_t st = nullptr;
+  ~StreamTemp() { if (p) cudaFreeAsync(p, st); g_device_bytes -= bytes; }
+  int alloc(size_t count, cudaStream_t s) {
+    st = s;
+    APH_CUDA_OK(cudaMallocAsync((void**)&p, count * sizeof(T), st));
+    bytes = count * sizeof(T);
+    g_device_bytes += bytes;
     return 0;
   }
 };

@@ -481,11 +481,7 @@ extern "C" int aph_cppn_create(aph_cppn** handle, int nf, int layers, int act) {
 }
 
 extern "C" int aph_cppn_destroy(aph_cppn* h) {
-  if (h) {
-    if (h->partial.p) cudaFree(h->partial.p);
-    if (h->zbuf.p) cudaFree(h->zbuf.p);
-    delete h;
-  }
+  delete h;
   return 0;
 }
 

@@ -335,7 +335,7 @@ static int vgg_forward(aph_lpips* h, const float* img, int N, int H, int W, int 
 // "lin{t}.model.1.weight" [1,C,1,1]. Other keys are refused (the Python loader drops the classifier and anything else).
 extern "C" int aph_lpips_create(aph_lpips** out) {
   APH_REQUIRE(out, "aph_lpips_create: null handle pointer");
-  aph_lpips* h = new aph_lpips();
+  std::unique_ptr<aph_lpips> h(new aph_lpips());
   int e = 0;
   for (int l = 0; l < LP_CONVS; ++l) {
     const std::string f = "features." + std::to_string(kFeatIdx[l]);
@@ -344,14 +344,12 @@ extern "C" int aph_lpips_create(aph_lpips** out) {
     e |= h->add_f32(f + ".bias", &h->bias[l], kCout[l]);
   }
   for (int t = 0; t < LP_TAPS; ++t) e |= h->add_f32("lin" + std::to_string(t) + ".model.1.weight", &h->lin[t], kCout[kTapConv[t]]);
-  if (e) { aph_lpips_destroy(h); return 1; }
-  *out = h;
+  if (e) return 1;
+  *out = h.release();
   return 0;
 }
 
 extern "C" int aph_lpips_destroy(aph_lpips* h) {
-  if (!h) return 0;
-  cudaFree(h->main_arena.p); cudaFree(h->ref_arena.p); cudaFree(h->grads.p); cudaFree(h->part.p);
   delete h;
   return 0;
 }
@@ -460,22 +458,17 @@ extern "C" int aph_lpips_conv_test(int fwd, const void* x, const float* weight, 
   APH_REQUIRE(x && weight && out && (bias || !fwd), "aph_lpips_conv_test: bad arguments");
   APH_REQUIRE(Cin % 64 == 0 && Cout % 64 == 0, "aph_lpips_conv_test: C_in=%d and C_out=%d must be multiples of 64", Cin, Cout);
   cudaStream_t st = (cudaStream_t)stream;
-  bf16* wp = nullptr;
-  const size_t n = (size_t)Cout * Cin * 9;
-  APH_CUDA_OK(cudaMallocAsync(&wp, n * sizeof(bf16), st));
-  if (int r = pack_conv3x3(weight, Cout, Cin, fwd ? wp : nullptr, fwd ? nullptr : wp, st)) return r;
+  StreamTemp<bf16> wp;
+  if (int r = wp.alloc((size_t)Cout * Cin * 9, st)) return r;
+  if (int r = pack_conv3x3(weight, Cout, Cin, fwd ? wp.p : nullptr, fwd ? nullptr : wp.p, st)) return r;
   ConvEpi e;
   e.out = reinterpret_cast<bf16*>(out);
-  int r;
   if (fwd) {
     e.bias = bias;
-    r = launch_conv3x3(x, wp, N, H, W, Cin, Cout, CONV_BIAS_RELU, e, st);
-  } else {
-    e.mask = reinterpret_cast<const bf16*>(mask);
-    r = launch_conv3x3(x, wp, N, H, W, Cout, Cin, mask ? CONV_MASK : CONV_PLAIN, e, st);
+    return launch_conv3x3(x, wp.p, N, H, W, Cin, Cout, CONV_BIAS_RELU, e, st);
   }
-  cudaFreeAsync(wp, st);
-  return r;
+  e.mask = reinterpret_cast<const bf16*>(mask);
+  return launch_conv3x3(x, wp.p, N, H, W, Cout, Cin, mask ? CONV_MASK : CONV_PLAIN, e, st);
 }
 
 // conv1_1 on caller buffers: weight fp32 [64,3,3,3], bias [64]. fwd = 1: img fp32 [N,3,H,W] -> out bf16 NHWC [N,H,W,64]

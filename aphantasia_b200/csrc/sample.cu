@@ -752,7 +752,7 @@ static int check_sample_args(const char* who, int H, int W, int S, int size, int
   return 0;
 }
 
-static Scratch g_A;                    // resized crops [S,3,size,size] between k_resize and k_compose
+static Scratch& g_A = *new Scratch;    // resized crops [S,3,size,size] between k_resize and k_compose
 
 static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int pad_left, const float* table, int S,
                            int size, int kind, float* out, PatchOut po, void* stream);
@@ -816,8 +816,8 @@ static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int p
   return 0;
 }
 
-static Scratch g_gW;                   // warp-stage adjoint scratch [S,3,size,size] of the default backward (all-zero between calls)
-static Scratch g_gR;                   // kornia kinds: d loss / d rotated image [S,3,size+8,size+8], rewritten by every backward
+static Scratch& g_gW = *new Scratch;   // warp-stage adjoint scratch [S,3,size,size] of the default backward (all-zero between calls)
+static Scratch& g_gR = *new Scratch;   // kornia kinds: d loss / d rotated image [S,3,size+8,size+8], rewritten by every backward
 
 extern "C" int aph_sample_bwd_scaled(const float* grad_out, int H, int W, int pad_top, int pad_left, const float* table, int S,
                                      int size, int kind, float gscale, float* grad_canvas, void* stream) {

@@ -21,13 +21,13 @@ constexpr int kMaxL = 40;       // filter taps (db20 = 40)
 constexpr int kMaxLevels = 16;
 struct Filt { float g0[kMaxL]; float g1[kMaxL]; int L; };
 
-struct DwtPlanImpl {
+struct DwtPlanImpl : DeviceAllocs {
   int H, W, L, J;
   int lh[kMaxLevels], lw[kMaxLevels];      // band sizes, finest (level 1) first
   int oh[kMaxLevels], ow[kMaxLevels];      // output size of each level's synthesis: 2*l - L + 2
   Filt f;
-  float* ll[kMaxLevels];                   // ll[i]: output of level i's synthesis (i = 0 is the image x_raw-sized scratch not used)
-  float* dll[kMaxLevels];                  // gradient w.r.t. ll[i]
+  float* ll[kMaxLevels] = {};              // ll[i]: output of level i's synthesis (i = 0 is the image x_raw-sized scratch not used)
+  float* dll[kMaxLevels] = {};             // gradient w.r.t. ll[i]
   float* gimg = nullptr; float* gx = nullptr;
 };
 
@@ -204,7 +204,7 @@ extern "C" int aph_dwt_plan_create(aph_dwt_plan** out, int H, int W, const float
   APH_REQUIRE(out && rec_lo_host && rec_hi_host, "aph_dwt_plan_create: null argument");
   APH_REQUIRE(L >= 2 && L <= kMaxL && L % 2 == 0, "aph_dwt_plan_create: filter length %d unsupported (even, <= %d)", L, kMaxL);
   APH_REQUIRE(H >= 2 && W >= 2, "aph_dwt_plan_create: bad size %dx%d", H, W);
-  DwtPlanImpl* p = new DwtPlanImpl();
+  std::unique_ptr<DwtPlanImpl> p(new DwtPlanImpl());
   p->H = H; p->W = W; p->L = L;
   p->f.L = L;
   for (int i = 0; i < L; ++i) { p->f.g0[i] = rec_lo_host[i]; p->f.g1[i] = rec_hi_host[i]; }
@@ -213,25 +213,20 @@ extern "C" int aph_dwt_plan_create(aph_dwt_plan** out, int H, int W, const float
   p->J = J;
   int h = H, w = W;
   for (int i = 0; i < J; ++i) { h = (h + L - 1) / 2; w = (w + L - 1) / 2; p->lh[i] = h; p->lw[i] = w; p->oh[i] = 2 * h - L + 2; p->ow[i] = 2 * w - L + 2; }
-  for (int i = 0; i < kMaxLevels; ++i) { p->ll[i] = nullptr; p->dll[i] = nullptr; }
   // ll[i] (i >= 1) = output of level (i+1)'s synthesis = low-pass input of level i (0-based level index i-1); ll[J] is Yl itself
   for (int i = 1; i < J; ++i) {
-    APH_CUDA_OK(cudaMalloc(&p->ll[i], (size_t)3 * p->oh[i] * p->ow[i] * sizeof(float)));
-    APH_CUDA_OK(cudaMalloc(&p->dll[i], (size_t)3 * p->oh[i] * p->ow[i] * sizeof(float)));
+    if (int e = p->alloc(&p->ll[i], (size_t)3 * p->oh[i] * p->ow[i])) return e;
+    if (int e = p->alloc(&p->dll[i], (size_t)3 * p->oh[i] * p->ow[i])) return e;
   }
   const size_t n = (size_t)3 * p->oh[0] * p->ow[0];
-  APH_CUDA_OK(cudaMalloc(&p->gimg, n * sizeof(float)));
-  APH_CUDA_OK(cudaMalloc(&p->gx, n * sizeof(float)));
-  *out = reinterpret_cast<aph_dwt_plan*>(p);
+  if (int e = p->alloc(&p->gimg, n)) return e;
+  if (int e = p->alloc(&p->gx, n)) return e;
+  *out = reinterpret_cast<aph_dwt_plan*>(p.release());
   return 0;
 }
 
 extern "C" int aph_dwt_plan_destroy(aph_dwt_plan* plan) {
-  if (!plan) return 0;
-  DwtPlanImpl* p = reinterpret_cast<DwtPlanImpl*>(plan);
-  for (int i = 0; i < kMaxLevels; ++i) { cudaFree(p->ll[i]); cudaFree(p->dll[i]); }
-  cudaFree(p->gimg); cudaFree(p->gx);
-  delete p;
+  delete reinterpret_cast<DwtPlanImpl*>(plan);
   return 0;
 }
 
@@ -295,7 +290,7 @@ extern "C" int aph_synth_dwt_bwd(aph_dwt_plan* plan, const float* grad_out, cons
 // Analysis (image-file resume, aphantasia/image.py:82-94): DWTForward(J, mode 'symmetric') of img [3,H,W], finest level first;
 // Ys as in aph_synth_dwt_fwd (written here), Yh_i multiplied by inv_scales_host[i]. Level i's LL lands in ll[i + 1], which
 // holds the oh[i + 1] x ow[i + 1] >= lh[i] x lw[i] synthesis output of that level, and the last one in Yl.
-// The row-filtered halves [3][2][h][ow] of each level go to a stream-ordered allocation of exactly that level's size, freed
+// The row-filtered halves [3][2][h][ow] of each level go to a stream-ordered temporary of exactly that level's size, freed
 // behind the level's two launches: the long-lived plan keeps nothing for the analysis, and no size formula can fall short
 // when lines shorter than the filter make the levels grow (h -> (h + L - 1) / 2 > h for h < L - 1).
 extern "C" int aph_dwt_analyze(aph_dwt_plan* plan, const float* img, const float* inv_scales_host, float* const* Ys, void* stream) {
@@ -307,17 +302,13 @@ extern "C" int aph_dwt_analyze(aph_dwt_plan* plan, const float* img, const float
   int h = p->H, w = p->W;
   for (int i = 0; i < J; ++i) {
     const int oh = p->lh[i], ow = p->lw[i];
-    float* rows = nullptr;
-    APH_CUDA_OK(cudaMallocAsync((void**)&rows, (size_t)3 * 2 * h * ow * sizeof(float), st));
+    StreamTemp<float> rows;
+    if (int e = rows.alloc((size_t)3 * 2 * h * ow, st)) return e;
     float* ll = (i == J - 1) ? Ys[0] : p->ll[i + 1];
-    k_dwt_afb_w<<<grid_for((size_t)3 * h * ow), 256, 0, st>>>(x, h, w, rows, ow, p->f);
-    const cudaError_t e1 = cudaGetLastError();
-    if (e1 == cudaSuccess)
-      k_dwt_afb_h<<<grid_for((size_t)3 * oh * ow), 256, 0, st>>>(rows, h, ow, ll, Ys[i + 1], inv_scales_host[i], oh, p->f);
-    const cudaError_t e2 = e1 == cudaSuccess ? cudaGetLastError() : e1;
-    APH_CUDA_OK(cudaFreeAsync(rows, st));
-    APH_CUDA_OK(e2);
-    count_launch(2);
+    k_dwt_afb_w<<<grid_for((size_t)3 * h * ow), 256, 0, st>>>(x, h, w, rows.p, ow, p->f);
+    APH_LAUNCH_OK();
+    k_dwt_afb_h<<<grid_for((size_t)3 * oh * ow), 256, 0, st>>>(rows.p, h, ow, ll, Ys[i + 1], inv_scales_host[i], oh, p->f);
+    APH_LAUNCH_OK();
     x = ll; h = oh; w = ow;
   }
   return 0;

@@ -29,7 +29,7 @@ namespace aph {
 constexpr int kMaxStages = 16;
 struct Radices { int n; int r[kMaxStages]; };
 
-struct FftPlanImpl {
+struct FftPlanImpl : DeviceAllocs {
   int H, W, Wh;
   Radices rh, rw;
   float2* twH = nullptr;   // exp(+2 pi i k / H), k in [0,H)
@@ -427,13 +427,10 @@ using namespace aph;
 
 extern "C" int aph_fft_plan_create(aph_fft_plan** plan_out, int H, int W) {
   APH_REQUIRE(plan_out && H >= 2 && W >= 2, "aph_fft_plan_create: bad arguments H=%d W=%d", H, W);
-  FftPlanImpl* p = new FftPlanImpl();
+  std::unique_ptr<FftPlanImpl> p(new FftPlanImpl());
   p->H = H; p->W = W; p->Wh = W / 2 + 1;
-  if (!factorize(H, p->rh) || !factorize(W, p->rw)) {
-    delete p;
-    set_error("aph_fft_plan_create: H=%d or W=%d has a prime factor > 13 (unsupported FFT length)", H, W);
-    return 2;
-  }
+  APH_REQUIRE(factorize(H, p->rh) && factorize(W, p->rw), "aph_fft_plan_create: H=%d or W=%d has a prime factor > 13 (unsupported FFT length)",
+              H, W);
   // tile sizes bounded by shared memory (<= ~100 KB so two CTAs fit per SM when possible, hard cap 200 KB)
   int C = 8;
   while (C > 1 && (size_t)(2 * C * (H + 1) + H) * sizeof(float2) > 100 * 1024) C >>= 1;
@@ -453,20 +450,16 @@ extern "C" int aph_fft_plan_create(aph_fft_plan** plan_out, int H, int W) {
   while (P > 1 && (size_t)(2 * P * (W + 1) + W) * sizeof(float2) > 100 * 1024) P >>= 1;
   p->rowP = P;
   p->smem_row = (size_t)(2 * P * (W + 1) + W) * sizeof(float2);
-  if (p->smem_col > 220 * 1024 || p->smem_row > 220 * 1024) {
-    delete p;
-    set_error("aph_fft_plan_create: H=%d W=%d exceeds the shared-memory FFT size", H, W);
-    return 2;
-  }
+  APH_REQUIRE(p->smem_col <= 220 * 1024 && p->smem_row <= 220 * 1024, "aph_fft_plan_create: H=%d W=%d exceeds the shared-memory FFT size", H, W);
   std::vector<float2> th(H), tw(W);
   for (int k = 0; k < H; ++k) { double a = 2.0 * M_PI * k / H; th[k] = make_float2((float)cos(a), (float)sin(a)); }
   for (int k = 0; k < W; ++k) { double a = 2.0 * M_PI * k / W; tw[k] = make_float2((float)cos(a), (float)sin(a)); }
-  APH_CUDA_OK(cudaMalloc(&p->twH, H * sizeof(float2)));
-  APH_CUDA_OK(cudaMalloc(&p->twW, W * sizeof(float2)));
+  if (int e = p->alloc(&p->twH, H)) return e;
+  if (int e = p->alloc(&p->twW, W)) return e;
   APH_CUDA_OK(cudaMemcpy(p->twH, th.data(), H * sizeof(float2), cudaMemcpyHostToDevice));
   APH_CUDA_OK(cudaMemcpy(p->twW, tw.data(), W * sizeof(float2), cudaMemcpyHostToDevice));
-  APH_CUDA_OK(cudaMalloc(&p->T, (size_t)3 * H * p->Wh * sizeof(float2)));
-  APH_CUDA_OK(cudaMalloc(&p->gimg, (size_t)3 * H * W * sizeof(float)));
+  if (int e = p->alloc(&p->T, (size_t)3 * H * p->Wh)) return e;
+  if (int e = p->alloc(&p->gimg, (size_t)3 * H * W)) return e;
   // The shared-memory limit is an attribute of the kernel, not of the plan: only ever raise it, so that creating a plan with
   // shorter lines does not break the launches of a larger plan that is still alive.
   auto raise_smem = [](const void* fn, size_t bytes) -> cudaError_t {
@@ -485,15 +478,12 @@ extern "C" int aph_fft_plan_create(aph_fft_plan** plan_out, int H, int W) {
   APH_CUDA_OK(raise_smem((const void*)k_row_c2r, p->smem_row));
   APH_CUDA_OK(raise_smem((const void*)k_row_r2c, p->smem_row));
   APH_CUDA_OK(raise_smem((const void*)k_row_rfft, p->smem_row));
-  *plan_out = reinterpret_cast<aph_fft_plan*>(p);
+  *plan_out = reinterpret_cast<aph_fft_plan*>(p.release());
   return 0;
 }
 
 extern "C" int aph_fft_plan_destroy(aph_fft_plan* plan) {
-  if (!plan) return 0;
-  FftPlanImpl* p = reinterpret_cast<FftPlanImpl*>(plan);
-  cudaFree(p->twH); cudaFree(p->twW); cudaFree(p->T); cudaFree(p->gimg);
-  delete p;
+  delete reinterpret_cast<FftPlanImpl*>(plan);
   return 0;
 }
 

@@ -128,7 +128,7 @@ extern "C" int aph_text_create(aph_text** out, const aph_text_config* cfg) {
   APH_REQUIRE(cfg->out_dim > 0 && cfg->out_dim % 128 == 0, "aph_text_create: out_dim %d must be a multiple of 128", cfg->out_dim);
   APH_REQUIRE(cfg->vocab > 0 && cfg->max_batch > 0 && cfg->layers > 0, "aph_text_create: vocab %d, max_batch %d, layers %d must be positive",
               cfg->vocab, cfg->max_batch, cfg->layers);
-  TextImpl* t = new TextImpl();
+  std::unique_ptr<TextImpl> t(new TextImpl());
   t->cfg = *cfg;
   const int D = cfg->width, O = cfg->out_dim, B = cfg->max_batch;
   const size_t M = (size_t)B * cfg->context;
@@ -137,19 +137,18 @@ extern "C" int aph_text_create(aph_text** out, const aph_text_config* cfg) {
   e |= t->add_f32("positional_embedding", &t->pos, (size_t)cfg->context * D);
   e |= t->add_f32("ln_final.weight", &t->lnf_w, D); e |= t->add_f32("ln_final.bias", &t->lnf_b, D);
   e |= t->add_bf16("text_projection", D, O, nullptr, &t->w_out);   // [D, out] -> [out, D]
-  e |= add_blocks(t, cfg->layers, D, false);
+  e |= add_blocks(t.get(), cfg->layers, D, false);
   e |= t->alloc(&t->x, M * D); e |= t->alloc(&t->x_mid, M * D); e |= t->alloc(&t->ln_out, M * D);
   e |= t->alloc(&t->qkv, M * 3 * D); e |= t->alloc(&t->attn_out, M * D);
   e |= t->alloc(&t->h_pre, M * 4 * D); e |= t->alloc(&t->h_act, M * 4 * D);
   e |= t->alloc(&t->mean, M); e |= t->alloc(&t->rstd, M);
   e |= t->alloc(&t->eot, (size_t)B); e |= t->alloc(&t->pooled, (size_t)B * D);
-  if (e) { aph_text_destroy(reinterpret_cast<aph_text*>(t)); return 1; }
-  *out = reinterpret_cast<aph_text*>(t);
+  if (e) return 1;
+  *out = reinterpret_cast<aph_text*>(t.release());
   return 0;
 }
 
 extern "C" int aph_text_destroy(aph_text* text) {
-  if (!text) return 0;
   delete reinterpret_cast<TextImpl*>(text);
   return 0;
 }

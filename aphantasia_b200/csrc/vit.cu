@@ -58,6 +58,10 @@ struct VitImpl : Encoder {
   std::map<int, int> warm_fwd, warm_bwd;
   unsigned long long stamp = 0;
   int graph_misses = 0;          // captures in a row that were never replayed (e.g. the caller re-allocates its tensors every step)
+  ~VitImpl() {
+    for (auto& g : fwd_graphs) cudaGraphExecDestroy(g.exec);
+    for (auto& g : bwd_graphs) cudaGraphExecDestroy(g.exec);
+  }
 };
 
 // LayerNorm statistics slot k: 0 = ln_pre, 1 + 2l / 2 + 2l = ln_1 / ln_2 of layer l, 2 layers + 1 = ln_post. The slots below
@@ -173,7 +177,7 @@ static int vit_attn_fwd(const bf16* qkv, bf16* out, int S, int T, int D, int hea
   return vit_attn(true, qkv, nullptr, out, nullptr, S, T, D, heads, st);
 }
 
-static Scratch g_win;   // aph_vit_bwd_sized: the R x R window gradient before k_window_expand
+static Scratch& g_win = *new Scratch;   // aph_vit_bwd_sized: the R x R window gradient before k_window_expand
 
 }  // namespace aph
 
@@ -187,7 +191,7 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
   APH_REQUIRE(cfg->patch >= 2 && cfg->patch % 2 == 0 && cfg->res % cfg->patch == 0, "aph_vit_create: res %d / patch %d (the patch must be even)",
               cfg->res, cfg->patch);
   APH_REQUIRE(cfg->out_dim % 128 == 0 && cfg->max_batch > 0 && cfg->layers > 0, "aph_vit_create: out_dim %d must be a multiple of 128", cfg->out_dim);
-  VitImpl* v = new VitImpl();
+  std::unique_ptr<VitImpl> v(new VitImpl());
   v->cfg = *cfg;
   v->g = cfg->res / cfg->patch; v->T = v->g * v->g + 1; v->D = cfg->width; v->Kp = patch_k(cfg->patch);
   const int D = v->D, T = v->T, S = cfg->max_batch, Ly = cfg->layers, O = cfg->out_dim;
@@ -201,7 +205,7 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
   e |= v->add_f32("ln_pre.weight", &v->lnpre_w, D); e |= v->add_f32("ln_pre.bias", &v->lnpre_b, D);
   e |= v->add_f32("ln_post.weight", &v->lnpost_w, D); e |= v->add_f32("ln_post.bias", &v->lnpost_b, D);
   e |= v->add_bf16("proj", D, O, &v->w_out_t, &v->w_out);
-  e |= add_blocks(v, Ly, D, true);
+  e |= add_blocks(v.get(), Ly, D, true);
   // activations
   e |= v->alloc(&v->patches, Mp * v->Kp); e |= v->alloc(&v->tok, Mp * D); e |= v->alloc(&v->e, M * D);
   v->xs.resize(2 * Ly + 1);
@@ -209,7 +213,7 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
   e |= v->alloc(&v->ln_out, M * D); e |= v->alloc(&v->attn_out, M * D); e |= v->alloc(&v->h_act, M * 4 * D);
   v->qkv.resize(Ly); v->h_pre.resize(Ly);
   for (int i = 0; i < Ly; ++i) { e |= v->alloc(&v->qkv[i], M * 3 * D); e |= v->alloc(&v->h_pre[i], (i == Ly - 1 ? (size_t)S : M) * 4 * D); }
-  e |= v->alloc(&v->st_mean, stat_off(v, 2 * Ly + 2)); e |= v->alloc(&v->st_rstd, stat_off(v, 2 * Ly + 2));
+  e |= v->alloc(&v->st_mean, stat_off(v.get(), 2 * Ly + 2)); e |= v->alloc(&v->st_rstd, stat_off(v.get(), 2 * Ly + 2));
   e |= v->alloc(&v->cls_ln, (size_t)S * D); e |= v->alloc(&v->emb_int, (size_t)S * O);
   e |= v->alloc(&v->d_emb, (size_t)S * O); e |= v->alloc(&v->d_cls, (size_t)S * D);
   e |= v->alloc(&v->dxc, (size_t)S * D); e |= v->alloc(&v->dxc_bf, (size_t)S * D);
@@ -217,7 +221,7 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
   e |= v->alloc(&v->d_ln, M * D); e |= v->alloc(&v->d_attn, M * D); e |= v->alloc(&v->d_attn_last, M * D);
   e |= v->alloc(&v->d_qkv, M * 3 * D); e |= v->alloc(&v->d_tok, Mp * D);
   if (T > kAttnResidentMaxT) e |= v->alloc(&v->attn_stats, M * cfg->heads);
-  if (e) { aph_vit_destroy(reinterpret_cast<aph_vit*>(v)); return 1; }
+  if (e) return 1;
   APH_CUDA_OK(cudaMemset(v->d_attn_last, 0, M * D * sizeof(bf16)));
   if (v->Kp != 3 * cfg->patch * cfg->patch) {   // the zero padding of the patch operand and of conv1's packed weights
     APH_CUDA_OK(cudaMemset(v->patches, 0, Mp * v->Kp * sizeof(bf16)));
@@ -225,16 +229,12 @@ extern "C" int aph_vit_create(aph_vit** out, const aph_vit_config* cfg) {
     APH_CUDA_OK(cudaMemset(v->w_conv_t, 0, (size_t)D * v->Kp * sizeof(bf16)));
   }
   APH_CUDA_OK(cudaDeviceSynchronize());     // the zeros are in place before any caller stream (blocking or not) can read them
-  *out = reinterpret_cast<aph_vit*>(v);
+  *out = reinterpret_cast<aph_vit*>(v.release());
   return 0;
 }
 
 extern "C" int aph_vit_destroy(aph_vit* vit) {
-  if (!vit) return 0;
-  VitImpl* v = reinterpret_cast<VitImpl*>(vit);
-  for (auto& g : v->fwd_graphs) cudaGraphExecDestroy(g.exec);
-  for (auto& g : v->bwd_graphs) cudaGraphExecDestroy(g.exec);
-  delete v;
+  delete reinterpret_cast<VitImpl*>(vit);
   return 0;
 }
 
@@ -449,11 +449,9 @@ extern "C" int aph_attn_long_test(int fwd, const void* qkv, const void* dout, vo
   cudaStream_t st = (cudaStream_t)stream;
   const bf16* q = reinterpret_cast<const bf16*>(qkv);
   if (fwd) return attn_stream(true, q, nullptr, reinterpret_cast<bf16*>(out), nullptr, S, T, D, heads, st);
-  float2* stats = nullptr;                   // stream-ordered scratch: freed behind the two backward launches
-  APH_CUDA_OK(cudaMallocAsync(&stats, (size_t)S * heads * T * sizeof(float2), st));
-  const int rc = attn_stream(false, q, reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(out), stats, S, T, D, heads, st);
-  APH_CUDA_OK(cudaFreeAsync(stats, st));
-  return rc;
+  StreamTemp<float2> stats;                  // freed behind the two backward launches
+  if (int e = stats.alloc((size_t)S * heads * T, st)) return e;
+  return attn_stream(false, q, reinterpret_cast<const bf16*>(dout), reinterpret_cast<bf16*>(out), stats.p, S, T, D, heads, st);
 }
 
 extern "C" int aph_ln_fwd_test(const float* x, const float* gamma, const float* beta, void* y, float* mean, float* rstd, int rows, int D,

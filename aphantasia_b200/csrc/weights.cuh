@@ -26,23 +26,11 @@ struct WeightEntry {
   bool loaded;
 };
 
-struct Weights {
+struct Weights : DeviceAllocs {
   const char* prefix = "";     // a key prefix the loader accepts and drops ("visual." for the image tower); finalize names it
-  int64_t bytes = 0;           // every allocation below, weights and activations
-  std::vector<void*> allocs;
   std::vector<WeightEntry> table;
   bool finalized = false;      // every entry loaded, and nothing loaded since
-  ~Weights() { for (void* p : allocs) cudaFree(p); }
 
-  template <typename Tp>
-  int alloc(Tp** p, size_t count) {
-    void* q = nullptr;
-    APH_CUDA_OK(cudaMalloc(&q, count * sizeof(Tp)));
-    allocs.push_back(q);
-    bytes += (int64_t)(count * sizeof(Tp));
-    *p = reinterpret_cast<Tp*>(q);
-    return 0;
-  }
   // Each allocates its destinations (null: none) and adds the entry.
   int add_f32(const std::string& key, float** dst, size_t n) {
     const int e = alloc(dst, n);

@@ -390,6 +390,10 @@ int aph_allreduce_sym(uint64_t mc_ptr, const uint64_t* peer_ptrs, const uint64_t
 /* number of kernels this library has launched since load (bench.py's gpu_launches)                 */
 int64_t aph_launch_count(void);
 
+/* device bytes this library holds right now: handles, plans, their scratch, and stream-ordered temporaries not yet freed.
+ * Unlike cudaMemGetInfo it counts no other process's memory, so a test can check that a destroy returns everything.   */
+int64_t aph_device_bytes(void);
+
 #ifdef __cplusplus
 }
 #endif
