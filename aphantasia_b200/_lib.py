@@ -77,6 +77,7 @@ _SIGS = {
     'aph_derivat_sobel_bwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, c_f32p, C.c_void_p]),
     'aph_cppn_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_int, C.c_int, C.c_int]),
     'aph_cppn_destroy': (C.c_int, [C.c_void_p]),
+    'aph_cppn_bytes': (C.c_int64, [C.c_void_p]),
     'aph_cppn_fwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), c_f32p, C.c_void_p]),
     'aph_cppn_bwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p), c_f32p, C.POINTER(C.c_void_p),
                                C.c_void_p]),

@@ -6,7 +6,8 @@
 `ConvLayer` and `CPPN` keep the original's constructor, state-dict keys (`net.{i}.conv.weight` / `.bias`) and random draws, so a
 seeded run starts from the original's weights and the script's own `load_cppn` / `export_data` work unchanged. The parameters
 stay ordinary nn.Parameters (the script's torch.optim.Adam updates them); the forward and the weight gradient run in CUDA
-(csrc/cppn.cu): one launch forward, two backward. Supported: nf_in 2, nf_out 3, nf a multiple of 8 in [8, 64], 1 to 32 layers.
+(csrc/cppn.cu): for nf <= 64 one launch forward, two backward; wider nets run layer by layer as TF32 GEMMs. Supported: nf_in 2,
+nf_out 3, nf a multiple of 8 in [8, 256], 1 to 32 layers.
 """
 import ctypes as C
 import math
@@ -38,7 +39,7 @@ class ConvLayer(nn.Module):
 
 def _unsupported(what):
     return NotImplementedError('aphantasia_b200.cppn: %s is not supported; supported is CPPN(nf_in=2, nf_hid, num_layers, nf_out=3) '
-                               'with nf_hid a multiple of 8 in [8, 64] and 1 <= num_layers <= 32' % what)
+                               'with nf_hid a multiple of 8 in [8, 256] and 1 <= num_layers <= 32' % what)
 
 
 class _CppnFn(torch.autograd.Function):

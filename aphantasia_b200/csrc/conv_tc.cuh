@@ -66,6 +66,7 @@ template <int BN, int EPI>
 struct ConvProblem {
   const ConvShape& cs;
   const ConvEpi& epi;
+  using Elem = bf16;
 
   __device__ __forceinline__ int tiles_img() const { return cs.tiles_y * cs.tiles_x; }
   __device__ __forceinline__ int cchunks() const { return cs.Cin / GEMM_BK; }

@@ -29,7 +29,32 @@
 // beside the staging buffers within CPPN_SMEM_CAP (nf 24: up to 14 layers, 61 KB at the default 10; nf 64: up to 3 layers),
 // otherwise in handle scratch (one slot per resident CTA, mostly L2-resident). Nothing else goes to global memory but the
 // coordinates, the image, its gradient and the partials.
-#include "aph_common.cuh"
+//
+// Wide nets (72 <= nf <= 256) do not fit that scheme: a warp's 16 pixels x KH activations would take KH / 2 registers per lane,
+// and per-CTA weight-gradient partials 512 KB per layer. They run layer by layer over all pixels instead, every hidden-layer
+// product a TF32 wgmma GEMM on the encoder GEMM's main loop (gemm_body, tc_gemm.cuh) with a CPPN epilogue:
+//   k_cppnw_pack     : rounds the hidden weights to TF32 once per call into the handle: W' [NF][KH] and its transpose W'^T
+//                      [KH][NF]. W' takes the input columns in the order x' = (a_0, s_0, a_1, s_1, ...) (a_j = atan(z_j) / 0.67,
+//                      s_j its square term) so that one thread holds both halves of feature j: the forward epilogue writes
+//                      them with one store, and the data-gradient epilogue applies act'(z_j) to both (relu: no reordering).
+//   k_cppnw_l0       : layer 0 (K = 2) in fp32, then the activation: x_1 [P][KH].
+//   k_cppnw_gemm FWD : z_l = x_l W'_l^T + b_l (M = pixels, N = NF, K = KH); the epilogue writes x_{l+1} = act(z_l), rounded to
+//                      TF32 when a hidden layer reads it (the output layer reads it in fp32), and in the backward also z_l
+//                      pixel-contiguous ([NF][P], the only thing the forward keeps).
+//   k_cppnw_head     : the output layer and the sigmoid in fp32, a warp per pixel.
+// The backward recomputes that forward with z_l kept, then walks down the layers:
+//   k_cppnw_head_bwd : dz_out = dy y (1 - y), dx_L = dz_out W_out and dz_{L-1} = dx_L act'(z_{L-1}) in fp32, a warp per 16
+//                      pixels; per-group partials of dW_out, db_out and db_{L-1}.
+//   k_cppnw_actT     : x_l = act(z_{l-1}) again, rounded, pixel-contiguous and split into pixel chunks ([S][KHP][chunk]).
+//   k_cppnw_gemm DW  : dW_l = dz_l^T x_l (M = NF, N = KH, K = pixels), split over S pixel chunks: partials [S][NF][KH].
+//   k_cppnw_gemm DX  : dx_l = dz_l W'_l (M = pixels, N = KH, K = NF, B = W'^T); the epilogue forms dz_{l-1} = dx act'(z_{l-1})
+//                      and writes it rounded as [P][NF] (the next DX operand) and [NF][P] (the next DW operand; layer 0's
+//                      unrounded), with per-16-pixel partials of db_{l-1}.
+//   k_cppnw_colsum   : every partial is summed in a fixed order (no float atomics: two backward calls are bit-identical).
+//   k_cppnw_l0_bwd   : dW_0, db_0 in fp32 from dz_0.
+// The rounding model is the narrow path's: both operands of every hidden-layer product rounded by cvt.rna, fp32 accumulation,
+// layer 0 / the output layer / the activations in fp32. Scratch: one handle buffer, sized by cppnw_floats().
+#include "tc_gemm.cuh"
 #include <algorithm>
 #include <math.h>
 
@@ -362,13 +387,385 @@ __global__ void __launch_bounds__(256) k_cppn_reduce(const float* __restrict__ p
   o.p[k][i - o.off[k]] = s;
 }
 
+// ================= wide nets (72 <= nf <= 256): layer by layer, TF32 wgmma GEMMs =====================================
+constexpr int CPPNW_CHUNK = 4096;       // least pixels per weight-gradient split
+constexpr int CPPNW_MAX_SPLITS = 256;
+constexpr int CPPNW_CH = 256;           // rows per k_cppnw_colsum block
+
+__device__ __forceinline__ float rna(float x) { return __uint_as_float(to_tf32(x)); }
+__device__ __forceinline__ float rna_if(float x, bool r) { return r ? rna(x) : x; }
+// column of the original [out][in] weight that column i' of W' holds (x' = a_0, s_0, a_1, s_1, ...; relu: the identity)
+__host__ __device__ __forceinline__ int cppnw_src_col(int ip, int nf, bool relu) { return relu ? ip : ((ip & 1) ? nf + (ip >> 1) : ip >> 1); }
+
+enum { CW_FWD = 0, CW_DX = 1, CW_DW = 2 };
+
+// Kernel arguments of the three GEMM kinds. Pixel-contiguous buffers ([NF][Ppad]) have rows `ld` = Ppad apart.
+struct CppnWideArgs {
+  int M, N;                       // output rows / valid columns
+  int m_tiles, n_tiles, splits, kblocks, chunk;
+  int nf, kh;
+  int64_t npix, ld;
+  float off, div;
+  const float* bias;              // FWD: b_l
+  float* x_out;                   // FWD: x_{l+1} [P][KH] in x' order
+  int round_out;                  // FWD: x_{l+1} rounded; DX: dz_{l-1} rounded
+  float* zT;                      // FWD: z_l [NF][Ppad] (backward only, else NULL)
+  const float* zT_in;             // DX: z_{l-1} [NF][Ppad]
+  float* dz_out;                  // DX: dz_{l-1} [Ppad][NF] (NULL for layer 0)
+  float* dzT_out;                 // DX: dz_{l-1} [NF][Ppad]
+  float* part;                    // DX: db_{l-1} partials [Ppad / 16][NF] (NULL for layer 0); DW: [S][NF][KH]
+};
+
+// The CPPN GEMMs as a gemm_body problem (cooperative schedule, fp32 operands rounded to TF32, mapped as 16-bit views).
+// Tile = (split, m block, n block), n fastest. The B operand of DW is split-major ([S][KHP][chunk]), so the body's n block
+// split * n_tiles + n selects the split's rows; A is offset by the split's pixels in load_a.
+template <int BN, int EPI, bool RELU>
+struct CppnProblem {
+  const CppnWideArgs& a;
+  using Elem = float;
+
+  __device__ __forceinline__ int num_tiles() const { return a.splits * a.m_tiles * a.n_tiles; }
+  __device__ __forceinline__ int k_blocks() const { return a.kblocks; }
+  __device__ __forceinline__ bool has_tile(int tile) const { return tile < num_tiles(); }
+
+  struct Tile { int m_blk, n_blk, split; };
+  __device__ __forceinline__ Tile tile(int tile) const {
+    const int per = a.m_tiles * a.n_tiles, s = tile / per, r = tile - s * per, m = r / a.n_tiles;
+    return {m, s * a.n_tiles + (r - m * a.n_tiles), s};
+  }
+  // K coordinates of the 16-bit view: 64 per 32 fp32
+  __device__ __forceinline__ void load_a(void* dst, const CUtensorMap* map_a, uint64_t* bar, Tile t, int kb) const {
+    tma_load_2d(dst, map_a, bar, (t.split * (a.chunk / 32) + kb) * GEMM_BK, t.m_blk * GEMM_BM);
+  }
+
+  __device__ __forceinline__ void epilogue(const float (&d)[1][BN / 2], Tile t, int row_in_tile, int col_in_tile, int lane) const {
+    const int row0 = t.m_blk * GEMM_BM + row_in_tile;
+    const int n0 = (t.n_blk - t.split * a.n_tiles) * BN;
+    if constexpr (EPI == CW_FWD) {
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + col_in_tile;
+        if (col >= a.N) continue;
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(a.bias + col));
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int row = row0 + 8 * r;
+          if (row >= a.M) continue;
+          const float z0 = d[0][4 * j + 2 * r] + bb.x, z1 = d[0][4 * j + 2 * r + 1] + bb.y;
+          if (a.zT) { a.zT[(size_t)col * a.ld + row] = z0; a.zT[(size_t)(col + 1) * a.ld + row] = z1; }
+          const bool rd = a.round_out;
+          if (RELU) {
+            *reinterpret_cast<float2*>(a.x_out + (size_t)row * a.kh + col) =
+                make_float2(rna_if((fmaxf(z0, 0.f) - 0.4f) / 0.58f, rd), rna_if((fmaxf(z1, 0.f) - 0.4f) / 0.58f, rd));
+          } else {
+            const float t0 = atanf(z0), t1 = atanf(z1);
+            *reinterpret_cast<float4*>(a.x_out + (size_t)row * a.kh + 2 * col) =
+                make_float4(rna_if(t0 / 0.67f, rd), rna_if((t0 * t0 - a.off) / a.div, rd), rna_if(t1 / 0.67f, rd),
+                            rna_if((t1 * t1 - a.off) / a.div, rd));
+          }
+        }
+      }
+    } else if constexpr (EPI == CW_DX) {
+      // columns (col, col + 1) of dx are (a_f, s_f) of feature f = col / 2 (relu: features col, col + 1)
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + col_in_tile;
+        const bool cv = col < a.N;
+        float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int row = row0 + 8 * r;
+          float dz0 = 0.f, dz1 = 0.f;
+          if (cv && row < a.npix) {
+            const float dx0 = d[0][4 * j + 2 * r], dx1 = d[0][4 * j + 2 * r + 1];
+            if (RELU) {
+              dz0 = __ldg(a.zT_in + (size_t)col * a.ld + row) > 0.f ? dx0 / 0.58f : 0.f;
+              dz1 = __ldg(a.zT_in + (size_t)(col + 1) * a.ld + row) > 0.f ? dx1 / 0.58f : 0.f;
+            } else {
+              const float zz = __ldg(a.zT_in + (size_t)(col >> 1) * a.ld + row), tt = atanf(zz);
+              dz0 = (dx0 / 0.67f + dx1 * (2.f * tt) / a.div) / (1.f + zz * zz);
+            }
+          }
+          if (cv && row < a.M) {     // rows past the frame get zeros: the next products read them
+            const bool rd = a.round_out;
+            if (RELU) {
+              a.dzT_out[(size_t)col * a.ld + row] = rna_if(dz0, rd);
+              a.dzT_out[(size_t)(col + 1) * a.ld + row] = rna_if(dz1, rd);
+              if (a.dz_out) *reinterpret_cast<float2*>(a.dz_out + (size_t)row * a.nf + col) = make_float2(rna(dz0), rna(dz1));
+            } else {
+              a.dzT_out[(size_t)(col >> 1) * a.ld + row] = rna_if(dz0, rd);
+              if (a.dz_out) a.dz_out[(size_t)row * a.nf + (col >> 1)] = rna(dz0);
+            }
+          }
+          s0 += dz0; s1 += dz1;
+        }
+        if (a.part) {       // db_{l-1}: the unrounded dz summed over this warp's 16 rows, in a fixed order
+#pragma unroll
+          for (int o = 4; o < 32; o <<= 1) {
+            s0 += __shfl_xor_sync(0xffffffffu, s0, o);
+            if (RELU) s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+          }
+          if (lane < 4 && cv) {
+            float* pr = a.part + (size_t)(t.m_blk * (GEMM_BM / 16) + (row_in_tile >> 4)) * a.nf;
+            if (RELU) { pr[col] = s0; pr[col + 1] = s1; }
+            else pr[col >> 1] = s0;
+          }
+        }
+      }
+    } else {   // CW_DW: this split's partial dW [NF][KH]
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = n0 + 8 * j + col_in_tile;
+        if (col >= a.N) continue;
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int row = row0 + 8 * r;
+          if (row < a.M)
+            *reinterpret_cast<float2*>(a.part + ((size_t)t.split * a.M + row) * a.N + col) = make_float2(d[0][4 * j + 2 * r], d[0][4 * j + 2 * r + 1]);
+        }
+      }
+    }
+  }
+};
+
+template <int BN, int EPI, bool RELU>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+k_cppnw_gemm(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b, CppnWideArgs a) {
+  gemm_body<BN, false>(map_a, map_b, CppnProblem<BN, EPI, RELU>{a});
+}
+
+// W' (and W'^T when wtp is given) of every hidden layer, rounded to TF32
+__global__ void __launch_bounds__(256) k_cppnw_pack(CppnWeights P, int L, int nf, int kh, bool relu, float* __restrict__ wp,
+                                                    float* __restrict__ wtp) {
+  const int64_t per = (int64_t)nf * kh, n = (L - 1) * per;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int l = (int)(i / per), r = (int)(i - l * per), o = r / kh, ip = r - o * kh;
+    const float v = rna(__ldg(P.w[l + 1] + (size_t)o * kh + cppnw_src_col(ip, nf, relu)));
+    wp[i] = v;
+    if (wtp) wtp[l * per + (int64_t)ip * nf + o] = v;
+  }
+}
+
+// layer 0 in fp32 and its activation: x_1 [P][KH] in x' order; z_0 to zT when given
+__global__ void __launch_bounds__(256) k_cppnw_l0(const float* __restrict__ coords, int64_t npix, int64_t hw, const float* __restrict__ W0,
+                                                  const float* __restrict__ b0, int nf, int kh, bool relu, float off, float div, bool round,
+                                                  float* __restrict__ x_out, float* __restrict__ zT, int64_t ld) {
+  const int64_t n = npix * nf;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t p = i / nf;
+    const int j = (int)(i - p * nf);
+    float c0, c1;
+    load_coords(coords, npix, hw, p, c0, c1);
+    const float z = fmaf(__ldg(W0 + 2 * j + 1), c1, fmaf(__ldg(W0 + 2 * j), c0, __ldg(b0 + j)));
+    if (zT) zT[(size_t)j * ld + p] = z;
+    if (relu) {
+      x_out[p * kh + j] = rna_if((fmaxf(z, 0.f) - 0.4f) / 0.58f, round);
+    } else {
+      const float t = atanf(z);
+      *reinterpret_cast<float2*>(x_out + p * kh + 2 * j) = make_float2(rna_if(t / 0.67f, round), rna_if((t * t - off) / div, round));
+    }
+  }
+}
+
+// the output layer and the sigmoid in fp32, a warp per pixel; x_L in x' order, W_out read in place
+__global__ void __launch_bounds__(256) k_cppnw_head(const float* __restrict__ x, int64_t npix, int64_t hw, const float* __restrict__ Wo,
+                                                    const float* __restrict__ bo, int nf, int kh, bool relu, float* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = (int64_t)gridDim.x * (blockDim.x >> 5);
+  for (int64_t p = blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5); p < npix; p += nw) {
+    float s[3] = {0.f, 0.f, 0.f};
+    for (int ip = 2 * lane; ip < kh; ip += 64) {
+      const float2 v = __ldg(reinterpret_cast<const float2*>(x + p * kh + ip));
+      const int i0 = cppnw_src_col(ip, nf, relu), i1 = cppnw_src_col(ip + 1, nf, relu);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) s[c] = fmaf(v.y, __ldg(Wo + c * kh + i1), fmaf(v.x, __ldg(Wo + c * kh + i0), s[c]));
+    }
+#pragma unroll
+    for (int c = 0; c < 3; ++c) s[c] = warp_sum(s[c]);
+    if (lane < 3) {
+      const int64_t n = p / hw, q = p - n * hw;
+      out[3 * n * hw + lane * hw + q] = 1.f / (1.f + expf(-(pick3(s, lane) + __ldg(bo + lane))));
+    }
+  }
+}
+
+// The output layer's backward, a warp per 16-pixel group (all Ppad / 16 groups: pixels past the frame write zeros). Lane
+// takes features j = lane + 32 k. Writes dz_{L-1} ([Ppad][NF] rounded when dz_out is given, [NF][Ppad] rounded when
+// round_dz) and the group's partial row: dW_out [3][KH] (original column order), db_out at 3 KH, db_{L-1} at 3 KH + 8.
+__global__ void __launch_bounds__(256) k_cppnw_head_bwd(const float* __restrict__ x, int64_t npix, int64_t hw, int64_t ld,
+                                                        const float* __restrict__ Wo, const float* __restrict__ bo,
+                                                        const float* __restrict__ gout, const float* __restrict__ zT, int nf, int kh,
+                                                        bool relu, float off, float div, bool round_dz, float* __restrict__ dz_out,
+                                                        float* __restrict__ dzT, float* __restrict__ part, int pw) {
+  const int lane = threadIdx.x & 31;
+  const int64_t grp = blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
+  float aw[3][2][8], ab[8], ao[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    ab[k] = 0.f;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) aw[c][0][k] = aw[c][1][k] = 0.f;
+  }
+  for (int q = 0; q < 16; ++q) {
+    const int64_t p = grp * 16 + q;
+    if (p >= npix) {
+#pragma unroll
+      for (int k = 0; k < 8; ++k) {
+        const int j = lane + 32 * k;
+        if (j < nf) {
+          dzT[(size_t)j * ld + p] = 0.f;
+          if (dz_out) dz_out[p * nf + j] = 0.f;
+        }
+      }
+      continue;
+    }
+    float xv[2][8], s[3] = {0.f, 0.f, 0.f};
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int j = lane + 32 * k;
+      xv[0][k] = xv[1][k] = 0.f;
+      if (j < nf) {
+        if (relu) {
+          xv[0][k] = __ldg(x + p * kh + j);
+        } else {
+          const float2 v = __ldg(reinterpret_cast<const float2*>(x + p * kh + 2 * j));
+          xv[0][k] = v.x; xv[1][k] = v.y;
+        }
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          s[c] = fmaf(xv[0][k], __ldg(Wo + c * kh + j), s[c]);
+          if (!relu) s[c] = fmaf(xv[1][k], __ldg(Wo + c * kh + nf + j), s[c]);
+        }
+      }
+    }
+    const int64_t n = p / hw, qq = p - n * hw;
+    float dzo[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      const float y = 1.f / (1.f + expf(-(warp_sum(s[c]) + __ldg(bo + c))));
+      dzo[c] = __ldg(gout + 3 * n * hw + c * hw + qq) * (y * (1.f - y));
+      ao[c] += dzo[c];
+    }
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+      const int j = lane + 32 * k;
+      if (j < nf) {
+        const float dx0 = dzo[0] * __ldg(Wo + j) + dzo[1] * __ldg(Wo + kh + j) + dzo[2] * __ldg(Wo + 2 * kh + j);
+        const float zz = __ldg(zT + (size_t)j * ld + p);
+        float dz;
+        if (relu) {
+          dz = zz > 0.f ? dx0 / 0.58f : 0.f;
+        } else {
+          const float dx1 = dzo[0] * __ldg(Wo + nf + j) + dzo[1] * __ldg(Wo + kh + nf + j) + dzo[2] * __ldg(Wo + 2 * kh + nf + j);
+          dz = (dx0 / 0.67f + dx1 * (2.f * atanf(zz)) / div) / (1.f + zz * zz);
+        }
+        dzT[(size_t)j * ld + p] = rna_if(dz, round_dz);
+        if (dz_out) dz_out[p * nf + j] = rna(dz);
+        ab[k] += dz;
+#pragma unroll
+        for (int c = 0; c < 3; ++c) {
+          aw[c][0][k] = fmaf(dzo[c], xv[0][k], aw[c][0][k]);
+          aw[c][1][k] = fmaf(dzo[c], xv[1][k], aw[c][1][k]);
+        }
+      }
+    }
+  }
+  float* pr = part + grp * pw;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    const int j = lane + 32 * k;
+    if (j < nf) {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        pr[c * kh + j] = aw[c][0][k];
+        if (!relu) pr[c * kh + nf + j] = aw[c][1][k];
+      }
+      pr[3 * kh + 8 + j] = ab[k];
+    }
+  }
+  if (lane < 3) pr[3 * kh + lane] = pick3(ao, lane);
+}
+
+// x_l = act(z_{l-1}) rounded, pixel-contiguous in the original column order and split-major: [S][KHP][chunk] (rows KH .. KHP
+// of a split are never read into a stored column); pixels past the frame are zeros
+__global__ void __launch_bounds__(256) k_cppnw_actT(const float* __restrict__ zT, int64_t npix, int64_t ld, int nf, int khp, int chunk,
+                                                    bool relu, float off, float div, float* __restrict__ xT) {
+  const int64_t n = (int64_t)nf * ld;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
+    const int j = (int)(i / ld);
+    const int64_t p = i - j * ld, s = p / chunk, kl = p - s * chunk;
+    float v0 = 0.f, v1 = 0.f;
+    if (p < npix) {
+      const float z = __ldg(zT + i);
+      if (relu) {
+        v0 = rna((fmaxf(z, 0.f) - 0.4f) / 0.58f);
+      } else {
+        const float t = atanf(z);
+        v0 = rna(t / 0.67f); v1 = rna((t * t - off) / div);
+      }
+    }
+    xT[(s * khp + j) * chunk + kl] = v0;
+    if (!relu) xT[(s * khp + nf + j) * chunk + kl] = v1;
+  }
+}
+
+// dW_0 [NF][2], db_0 from dz_0 [NF][Ppad] in fp32, a block per feature, summed in a fixed order
+__global__ void __launch_bounds__(256) k_cppnw_l0_bwd(const float* __restrict__ dzT, const float* __restrict__ coords, int64_t npix,
+                                                      int64_t hw, int64_t ld, float* __restrict__ dW0, float* __restrict__ db0) {
+  __shared__ float sh[3][256];
+  const int o = blockIdx.x, tid = threadIdx.x;
+  float s0 = 0.f, s1 = 0.f, sb = 0.f;
+  for (int64_t p = tid; p < npix; p += blockDim.x) {
+    const float dz = __ldg(dzT + (size_t)o * ld + p);
+    float c0, c1;
+    load_coords(coords, npix, hw, p, c0, c1);
+    s0 = fmaf(dz, c0, s0); s1 = fmaf(dz, c1, s1); sb += dz;
+  }
+  sh[0][tid] = s0; sh[1][tid] = s1; sh[2][tid] = sb;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if (tid < w) for (int k = 0; k < 3; ++k) sh[k][tid] += sh[k][tid + w];
+    __syncthreads();
+  }
+  if (tid == 0) { dW0[2 * o] = sh[0][0]; dW0[2 * o + 1] = sh[1][0]; db0[o] = sh[2][0]; }
+}
+
+// out[c] = sum over rows r of in[r][c] in a fixed order: block (32 columns x 8 row lanes) over CPPNW_CH rows. With tmp, one
+// sum per row chunk goes to tmp[chunk][c]; without, the single chunk's sum goes to the segment of `seg` holding column c
+// (a segment with a NULL pointer is not stored).
+struct CppnSegs { float* p[4]; int off[5]; int n; };
+__global__ void __launch_bounds__(256) k_cppnw_colsum(const float* __restrict__ in, int64_t rows, int cols, CppnSegs seg,
+                                                      float* __restrict__ tmp) {
+  __shared__ float sh[8][33];
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5, c = blockIdx.x * 32 + tx;
+  const int64_t r0 = (int64_t)blockIdx.y * CPPNW_CH, r1 = r0 + CPPNW_CH < rows ? r0 + CPPNW_CH : rows;
+  float s = 0.f;
+  if (c < cols)
+    for (int64_t r = r0 + ty; r < r1; r += 8) s += __ldg(in + r * cols + c);
+  sh[ty][tx] = s;
+  __syncthreads();
+  if (ty == 0 && c < cols) {
+    float v = sh[0][tx];
+#pragma unroll
+    for (int k = 1; k < 8; ++k) v += sh[k][tx];
+    if (tmp) {
+      tmp[(int64_t)blockIdx.y * cols + c] = v;
+    } else {
+      int k = 0;
+      while (k + 1 < seg.n && c >= seg.off[k + 1]) ++k;
+      if (seg.p[k]) seg.p[k][c - seg.off[k]] = v;
+    }
+  }
+}
+
 }  // namespace aph
 
 using namespace aph;
 
 struct aph_cppn {
   int nf, layers, act;
-  Scratch partial, zbuf;
+  Scratch partial, zbuf;     // nf <= 64
+  Scratch wide;              // nf >= 72: every buffer of the wide path (cppnw_floats)
 };
 
 namespace {
@@ -394,7 +791,7 @@ CppnCall make_call(aph_cppn* h, const float* coords, int N, int H, int W, const 
 }
 
 template <int NF, bool RELU>
-int cppn_fwd_t(const CppnCall& c, float* out) {
+int cppn_fwd(const CppnCall& c, float* out) {
   const int64_t mtiles = (c.npix + 15) / 16;
   const int blocks = (int)std::min<int64_t>((mtiles + CPPN_WARPS - 1) / CPPN_WARPS, (int64_t)num_sms() * 16);
   k_cppn_fwd<NF, RELU><<<blocks, 32 * CPPN_WARPS, 0, c.st>>>(c.coords, c.npix, c.hw, c.h->layers, c.P, c.off, c.div, out);
@@ -403,7 +800,7 @@ int cppn_fwd_t(const CppnCall& c, float* out) {
 }
 
 template <int NF, bool RELU>
-int cppn_bwd_t(const CppnCall& c, const float* grad_out, float* const* dparams) {
+int cppn_bwd(const CppnCall& c, const float* grad_out, float* const* dparams) {
   constexpr int KH = RELU ? NF : 2 * NF;
   aph_cppn* h = c.h;
   const int L = h->layers;
@@ -443,6 +840,209 @@ int cppn_bwd_t(const CppnCall& c, const float* grad_out, float* const* dparams) 
   return 0;
 }
 
+// ---- wide path, host side
+// Geometry of one call. Pixels are padded to Ppad = S chunk: the weight gradient splits them into S chunks of `chunk` pixels
+// (at least CPPNW_CHUNK, at most CPPNW_MAX_SPLITS chunks), and every pixel-contiguous buffer has Ppad columns.
+struct WideGeom {
+  int nf, kh, L;
+  bool relu;
+  int64_t P, Ppad, R;       // pixels, padded pixels, 16-pixel groups
+  int chunk, S;
+  int bnk, ntk, khp;        // GEMM tile width over KH, tiles, KH padded to them
+  int pw;                   // width of a head partial row: dW_out [3][KH], db_out (8 slots), db_{L-1} [NF]
+};
+
+WideGeom wide_geom(int nf, int L, int act, int64_t P) {
+  WideGeom g;
+  g.nf = nf; g.L = L; g.relu = act == CPPN_RELU; g.kh = g.relu ? nf : 2 * nf; g.P = P;
+  const int64_t per = (P + CPPNW_MAX_SPLITS - 1) / CPPNW_MAX_SPLITS;
+  g.chunk = (int)std::max<int64_t>(CPPNW_CHUNK, (per + 127) / 128 * 128);
+  g.S = (int)((P + g.chunk - 1) / g.chunk);
+  g.Ppad = (int64_t)g.S * g.chunk;
+  g.R = g.Ppad / 16;
+  g.bnk = g.kh <= 128 ? 128 : 256;
+  g.ntk = (g.kh + g.bnk - 1) / g.bnk;
+  g.khp = g.ntk * g.bnk;
+  g.pw = 3 * g.kh + 8 + nf;
+  return g;
+}
+
+// Regions of the handle buffer, in floats (include/aphb200.h states the same sum): the forward uses the first three.
+struct WideBufs { float *xa, *xb, *wp, *wtp, *zT, *xT, *dzT, *part, *tmp; };
+constexpr int CPPNW_REGIONS = 9;
+void cppnw_regions(const WideGeom& g, int64_t (&n)[CPPNW_REGIONS]) {
+  const int64_t nk = (int64_t)g.nf * g.kh;
+  n[0] = n[1] = g.Ppad * g.kh;                                      // x_l (and dz_l in the backward), ping-pong
+  n[2] = n[3] = (g.L - 1) * nk;                                     // W', W'^T
+  n[4] = (int64_t)g.L * g.nf * g.Ppad;                              // z_0 .. z_{L-1}
+  n[5] = (int64_t)g.khp * g.Ppad;                                   // x_l split-major
+  n[6] = (int64_t)g.nf * g.Ppad;                                    // dz_l pixel-contiguous
+  n[7] = std::max<int64_t>(g.R * g.pw, (int64_t)g.S * nk);          // partials
+  n[8] = 2 * ((g.R + CPPNW_CH - 1) / CPPNW_CH) * g.pw;              // column-sum passes
+}
+int64_t cppnw_floats(const WideGeom& g, bool bwd) {
+  int64_t n[CPPNW_REGIONS], total = 0;
+  cppnw_regions(g, n);
+  for (int i = 0; i < (bwd ? CPPNW_REGIONS : 3); ++i) total += n[i];
+  return total;
+}
+
+int cppnw_alloc(aph_cppn* h, const WideGeom& g, bool bwd, cudaStream_t st, WideBufs& b, const char* what) {
+  const size_t need = (size_t)cppnw_floats(g, bwd) * sizeof(float);
+  if (h->wide.grow(need, st)) {
+    cudaGetLastError();          // a failed cudaMalloc is not sticky: clear it so that later launches are not blamed
+    aph::set_error("%s: %zu bytes of device scratch could not be allocated (nf %d, %d layers, %lld pixels)", what, need, g.nf, g.L,
+                   (long long)g.P);
+    return 1;
+  }
+  int64_t n[CPPNW_REGIONS];
+  cppnw_regions(g, n);
+  float** dst[CPPNW_REGIONS] = {&b.xa, &b.xb, &b.wp, &b.wtp, &b.zT, &b.xT, &b.dzT, &b.part, &b.tmp};
+  float* p = h->wide.p;
+  for (int i = 0; i < CPPNW_REGIONS; ++i) {
+    *dst[i] = (bwd || i < 3) ? p : nullptr;
+    p += (bwd || i < 3) ? n[i] : 0;
+  }
+  return 0;
+}
+
+int grid_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)num_sms() * 8)); }
+
+// one GEMM: A [a_rows][a_k] and B [b_rows][b_k] fp32 (rows a_ld / b_ld floats apart) through their 16-bit views
+template <int BN, int EPI, bool RELU>
+int cppnw_gemm(const float* A, int a_rows, int a_k, int64_t a_ld, const float* B, int b_rows, int b_k, int64_t b_ld, const CppnWideArgs& a,
+               cudaStream_t st) {
+  auto kern = k_cppnw_gemm<BN, EPI, RELU>;
+  static bool configured = false;
+  if (!configured) {
+    APH_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<BN>::SMEM));
+    configured = true;
+  }
+  CUtensorMap ma, mb;
+  if (int e = make_tmap_bf16(&ma, A, a_rows, 2 * a_k, GEMM_BM, 2 * a_ld)) return e;
+  if (int e = make_tmap_bf16(&mb, B, b_rows, 2 * b_k, BN, 2 * b_ld)) return e;
+  const int tiles = a.splits * a.m_tiles * a.n_tiles;
+  kern<<<std::min(tiles, num_sms()), GEMM_THREADS, (size_t)GemmCfg<BN>::SMEM, st>>>(ma, mb, a);
+  APH_LAUNCH_OK();
+  return 0;
+}
+
+template <int EPI, bool RELU>
+int cppnw_gemm_bn(int bn, const float* A, int a_rows, int a_k, int64_t a_ld, const float* B, int b_rows, int b_k, int64_t b_ld,
+                  const CppnWideArgs& a, cudaStream_t st) {
+  return bn == 128 ? cppnw_gemm<128, EPI, RELU>(A, a_rows, a_k, a_ld, B, b_rows, b_k, b_ld, a, st)
+                   : cppnw_gemm<256, EPI, RELU>(A, a_rows, a_k, a_ld, B, b_rows, b_k, b_ld, a, st);
+}
+
+int cppnw_colsum(const float* in, int64_t rows, int cols, const CppnSegs& seg, float* tmp, cudaStream_t st) {
+  float* bufs[2] = {tmp, tmp + (rows + CPPNW_CH - 1) / CPPNW_CH * cols};
+  int pi = 0;
+  const unsigned gx = (unsigned)((cols + 31) / 32);
+  while (rows > CPPNW_CH) {
+    const int64_t nch = (rows + CPPNW_CH - 1) / CPPNW_CH;
+    k_cppnw_colsum<<<dim3(gx, (unsigned)nch), 256, 0, st>>>(in, rows, cols, seg, bufs[pi]);
+    APH_LAUNCH_OK();
+    in = bufs[pi]; rows = nch; pi ^= 1;
+  }
+  k_cppnw_colsum<<<dim3(gx, 1), 256, 0, st>>>(in, rows, cols, seg, nullptr);
+  APH_LAUNCH_OK();
+  return 0;
+}
+
+CppnSegs segs1(float* p, int n) {
+  CppnSegs s{};
+  s.p[0] = p; s.off[0] = 0; s.off[1] = n; s.n = 1;
+  return s;
+}
+
+// The forward of every layer but the output one: pack, layer 0, the hidden GEMMs. z_l goes to b.zT when `save`. Returns
+// the buffer holding x_L in *xl (the other one is free).
+template <bool RELU>
+int cppnw_trunk(const CppnCall& c, const WideGeom& g, const WideBufs& b, bool save, float** xl) {
+  const int L = g.L;
+  if (L > 1) {
+    k_cppnw_pack<<<grid_for((int64_t)(L - 1) * g.nf * g.kh), 256, 0, c.st>>>(c.P, L, g.nf, g.kh, RELU, b.wp, save ? b.wtp : nullptr);
+    APH_LAUNCH_OK();
+  }
+  k_cppnw_l0<<<grid_for(g.P * g.nf), 256, 0, c.st>>>(c.coords, g.P, c.hw, c.P.w[0], c.P.b[0], g.nf, g.kh, RELU, c.off, c.div, L > 1, b.xa,
+                                                     save ? b.zT : nullptr, g.Ppad);
+  APH_LAUNCH_OK();
+  float *x = b.xa, *y = b.xb;
+  const int bnf = g.nf <= 128 ? 128 : 256;
+  for (int l = 1; l < L; ++l) {
+    CppnWideArgs a{};
+    a.M = (int)g.P; a.N = g.nf; a.m_tiles = (int)((g.P + GEMM_BM - 1) / GEMM_BM); a.n_tiles = 1; a.splits = 1;
+    a.kblocks = (g.kh + 31) / 32; a.nf = g.nf; a.kh = g.kh; a.npix = g.P; a.ld = g.Ppad; a.off = c.off; a.div = c.div;
+    a.bias = c.P.b[l]; a.x_out = y; a.round_out = l + 1 < L; a.zT = save ? b.zT + (int64_t)l * g.nf * g.Ppad : nullptr;
+    if (int e = cppnw_gemm_bn<CW_FWD, RELU>(bnf, x, (int)g.P, g.kh, g.kh, b.wp + (int64_t)(l - 1) * g.nf * g.kh, g.nf, g.kh, g.kh, a, c.st))
+      return e;
+    std::swap(x, y);
+  }
+  *xl = x;
+  return 0;
+}
+
+template <bool RELU>
+int cppn_fwd_wide(const CppnCall& c, float* out) {
+  const WideGeom g = wide_geom(c.h->nf, c.h->layers, c.h->act, c.npix);
+  WideBufs b;
+  if (int e = cppnw_alloc(c.h, g, false, c.st, b, "aph_cppn_fwd")) return e;
+  float* xl = nullptr;
+  if (int e = cppnw_trunk<RELU>(c, g, b, false, &xl)) return e;
+  k_cppnw_head<<<grid_for(g.P * 32), 256, 0, c.st>>>(xl, g.P, c.hw, c.P.w[g.L], c.P.b[g.L], g.nf, g.kh, RELU, out);
+  APH_LAUNCH_OK();
+  return 0;
+}
+
+template <bool RELU>
+int cppn_bwd_wide(const CppnCall& c, const float* grad_out, float* const* dparams) {
+  const WideGeom g = wide_geom(c.h->nf, c.h->layers, c.h->act, c.npix);
+  const int L = g.L, nf = g.nf, kh = g.kh;
+  WideBufs b;
+  if (int e = cppnw_alloc(c.h, g, true, c.st, b, "aph_cppn_bwd")) return e;
+  float* x = nullptr;
+  if (int e = cppnw_trunk<RELU>(c, g, b, true, &x)) return e;
+  float* dz = x == b.xa ? b.xb : b.xa;     // dz_l [Ppad][NF] ping-pongs through the two activation buffers
+  float* dz_other = x;
+  // the output layer: dW_out, db_out, and dz_{L-1} with its db
+  k_cppnw_head_bwd<<<(unsigned)(g.R / 8), 256, 0, c.st>>>(x, g.P, c.hw, g.Ppad, c.P.w[L], c.P.b[L], grad_out,
+                                                          b.zT + (int64_t)(L - 1) * nf * g.Ppad, nf, kh, RELU, c.off, c.div, L > 1,
+                                                          L > 1 ? dz : nullptr, b.dzT, b.part, g.pw);
+  APH_LAUNCH_OK();
+  {
+    // partial row: dW_out | db_out | 5 unused slots | db_{L-1} (layer 0's db comes from k_cppnw_l0_bwd)
+    CppnSegs sg{};
+    sg.p[0] = dparams[2 * L]; sg.p[1] = dparams[2 * L + 1]; sg.p[2] = nullptr; sg.p[3] = L > 1 ? dparams[2 * L - 1] : nullptr;
+    sg.off[0] = 0; sg.off[1] = 3 * kh; sg.off[2] = 3 * kh + 3; sg.off[3] = 3 * kh + 8; sg.off[4] = g.pw;
+    sg.n = 4;
+    if (int e = cppnw_colsum(b.part, g.R, g.pw, sg, b.tmp, c.st)) return e;
+  }
+  for (int l = L - 1; l >= 1; --l) {
+    // dW_l = dz_l^T x_l over S pixel splits, then the fixed-order sum of the splits
+    k_cppnw_actT<<<grid_for((int64_t)nf * g.Ppad), 256, 0, c.st>>>(b.zT + (int64_t)(l - 1) * nf * g.Ppad, g.P, g.Ppad, nf, g.khp, g.chunk,
+                                                                   RELU, c.off, c.div, b.xT);
+    APH_LAUNCH_OK();
+    CppnWideArgs w{};
+    w.M = nf; w.N = kh; w.m_tiles = (nf + GEMM_BM - 1) / GEMM_BM; w.n_tiles = g.ntk; w.splits = g.S; w.kblocks = g.chunk / 32;
+    w.chunk = g.chunk; w.nf = nf; w.kh = kh; w.npix = g.P; w.ld = g.Ppad; w.part = b.part;
+    if (int e = cppnw_gemm_bn<CW_DW, false>(g.bnk, b.dzT, nf, (int)g.Ppad, g.Ppad, b.xT, g.S * g.khp, g.chunk, g.chunk, w, c.st)) return e;
+    if (int e = cppnw_colsum(b.part, g.S, nf * kh, segs1(dparams[2 * l], nf * kh), b.tmp, c.st)) return e;
+    // dx_l = dz_l W_l; its epilogue forms dz_{l-1} (and db_{l-1} partials above layer 0)
+    CppnWideArgs a{};
+    a.M = (int)g.Ppad; a.N = kh; a.m_tiles = (int)(g.Ppad / GEMM_BM); a.n_tiles = g.ntk; a.splits = 1; a.kblocks = (nf + 31) / 32;
+    a.nf = nf; a.kh = kh; a.npix = g.P; a.ld = g.Ppad; a.off = c.off; a.div = c.div; a.round_out = l > 1;
+    a.zT_in = b.zT + (int64_t)(l - 1) * nf * g.Ppad; a.dz_out = l > 1 ? dz_other : nullptr; a.dzT_out = b.dzT;
+    a.part = l > 1 ? b.part : nullptr;
+    if (int e = cppnw_gemm_bn<CW_DX, RELU>(g.bnk, dz, (int)g.Ppad, nf, nf, b.wtp + (int64_t)(l - 1) * nf * kh, kh, nf, nf, a, c.st)) return e;
+    if (l > 1)
+      if (int e = cppnw_colsum(b.part, g.R, nf, segs1(dparams[2 * l - 1], nf), b.tmp, c.st)) return e;
+    std::swap(dz, dz_other);
+  }
+  k_cppnw_l0_bwd<<<nf, 256, 0, c.st>>>(b.dzT, c.coords, g.P, c.hw, g.Ppad, dparams[0], dparams[1]);
+  APH_LAUNCH_OK();
+  return 0;
+}
+
 #define APH_CPPN_DISPATCH(FN, ...)                                                                \
   switch (h->nf) {                                                                                \
     case 8: return h->act == CPPN_RELU ? FN<8, true>(__VA_ARGS__) : FN<8, false>(__VA_ARGS__);    \
@@ -453,7 +1053,7 @@ int cppn_bwd_t(const CppnCall& c, const float* grad_out, float* const* dparams) 
     case 48: return h->act == CPPN_RELU ? FN<48, true>(__VA_ARGS__) : FN<48, false>(__VA_ARGS__); \
     case 56: return h->act == CPPN_RELU ? FN<56, true>(__VA_ARGS__) : FN<56, false>(__VA_ARGS__); \
     case 64: return h->act == CPPN_RELU ? FN<64, true>(__VA_ARGS__) : FN<64, false>(__VA_ARGS__); \
-    default: APH_REQUIRE(false, "aph_cppn: nf = %d is not supported", h->nf);                     \
+    default: return h->act == CPPN_RELU ? FN##_wide<true>(__VA_ARGS__) : FN##_wide<false>(__VA_ARGS__); \
   }
 
 int check_call(const aph_cppn* h, const float* coords, int N, int H, int W, const float* const* params, const char* what) {
@@ -469,7 +1069,7 @@ int check_call(const aph_cppn* h, const float* coords, int N, int H, int W, cons
 
 extern "C" int aph_cppn_create(aph_cppn** handle, int nf, int layers, int act) {
   APH_REQUIRE(handle, "aph_cppn_create: bad arguments");
-  APH_REQUIRE(nf >= 8 && nf <= 64 && nf % 8 == 0, "aph_cppn_create: nf = %d is not supported: nf must be a multiple of 8 in [8, 64]", nf);
+  APH_REQUIRE(nf >= 8 && nf <= 256 && nf % 8 == 0, "aph_cppn_create: nf = %d is not supported: nf must be a multiple of 8 in [8, 256]", nf);
   APH_REQUIRE(layers >= 1 && layers <= CPPN_MAX_LAYERS, "aph_cppn_create: layers = %d is not supported: layers must be in [1, %d]",
               layers, CPPN_MAX_LAYERS);
   APH_REQUIRE(act == CPPN_UNBIAS || act == CPPN_COMP || act == CPPN_RELU,
@@ -485,12 +1085,14 @@ extern "C" int aph_cppn_destroy(aph_cppn* h) {
   return 0;
 }
 
+extern "C" int64_t aph_cppn_bytes(const aph_cppn* h) { return h ? (int64_t)(h->partial.bytes + h->zbuf.bytes + h->wide.bytes) : 0; }
+
 extern "C" int aph_cppn_fwd(aph_cppn* h, const float* coords, int N, int H, int W, const float* const* params, float* out,
                             void* stream) {
   if (int rc = check_call(h, coords, N, H, W, params, "aph_cppn_fwd")) return rc;
   APH_REQUIRE(out, "aph_cppn_fwd: bad arguments");
   const CppnCall c = make_call(h, coords, N, H, W, params, stream);
-  APH_CPPN_DISPATCH(cppn_fwd_t, c, out);
+  APH_CPPN_DISPATCH(cppn_fwd, c, out);
 }
 
 extern "C" int aph_cppn_bwd(aph_cppn* h, const float* coords, int N, int H, int W, const float* const* params, const float* grad_out,
@@ -499,5 +1101,5 @@ extern "C" int aph_cppn_bwd(aph_cppn* h, const float* coords, int N, int H, int 
   APH_REQUIRE(grad_out && dparams, "aph_cppn_bwd: bad arguments");
   for (int i = 0; i < 2 * (h->layers + 1); ++i) APH_REQUIRE(dparams[i], "aph_cppn_bwd: gradient %d is NULL", i);
   const CppnCall c = make_call(h, coords, N, H, W, params, stream);
-  APH_CPPN_DISPATCH(cppn_bwd_t, c, grad_out, dparams);
+  APH_CPPN_DISPATCH(cppn_bwd, c, grad_out, dparams);
 }

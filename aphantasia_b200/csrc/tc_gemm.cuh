@@ -18,7 +18,13 @@
 // Rows >= M are zero-filled by TMA on load and not stored. A, the residual and the outputs may have a row stride larger than
 // their width (the encoder's last block reads and writes the class-token rows s*T of token-major matrices in place).
 // The kernel body (gemm_body: stage ring, mbarriers, producer and consumer loops) is shared with the LPIPS 3x3 convolution
-// (conv_tc.cuh), which supplies its own tile decode, A load and epilogue through a Problem type.
+// (conv_tc.cuh) and the wide CPPN layers (cppn.cu), which supply their own tile decode, A load and epilogue through a Problem
+// type. The Problem also names the operand element: bf16 (k16 per wgmma, 64 per 128-byte swizzle row) or fp32 read as TF32
+// (Elem = float: k8 per wgmma, 32 per row). Both put 32 bytes of K in one wgmma, so the stage layout, the descriptors and their
+// per-k-step offsets are the same. TMA copies bytes, so a TF32 operand is mapped as a 16-bit view [rows, 2 K] of the fp32 tensor
+// (make_tmap_bf16): its boxes land swizzled exactly as the fp32 values would, and the B coordinate kb * GEMM_BK addresses the
+// same 128-byte rows for both types. TF32 wgmma has no transpose bits, so both operands are K-major; it truncates the fp32
+// values it reads, so a TF32 Problem stores its operands already rounded to TF32.
 #pragma once
 #include "aph_common.cuh"
 #include <cuda.h>
@@ -129,8 +135,9 @@ template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wg
 template <int R> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 template <int R> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// D[64 x BN] (+)= A[64 x 16] . B[BN x 16]^T, fp32 accumulators d[BN/2] in the m64nNk16 fragment layout
-template <int BN> struct Wgmma;
+// D[64 x BN] (+)= A[64 x 16] . B[BN x 16]^T, fp32 accumulators d[BN/2] in the m64nNk16 fragment layout (bf16 operands);
+// Elem = float: A[64 x 8] . B[BN x 8]^T in TF32 (m64nNk8), the same accumulator layout
+template <int BN, class Elem = bf16> struct Wgmma;
 #define APH_WG_REGS8(o) "+f"(d[o]), "+f"(d[o + 1]), "+f"(d[o + 2]), "+f"(d[o + 3]), "+f"(d[o + 4]), "+f"(d[o + 5]), "+f"(d[o + 6]), "+f"(d[o + 7])
 template <> struct Wgmma<64> {      // the 64-channel layers of the LPIPS VGG (conv_tc.cuh)
   static __device__ __forceinline__ void mma(float (&d)[32], uint64_t da, uint64_t db, int acc) {
@@ -166,6 +173,34 @@ template <> struct Wgmma<256> {
         "%72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
         "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, "
         "%116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+        : APH_WG_REGS8(0), APH_WG_REGS8(8), APH_WG_REGS8(16), APH_WG_REGS8(24), APH_WG_REGS8(32), APH_WG_REGS8(40), APH_WG_REGS8(48), APH_WG_REGS8(56),
+          APH_WG_REGS8(64), APH_WG_REGS8(72), APH_WG_REGS8(80), APH_WG_REGS8(88), APH_WG_REGS8(96), APH_WG_REGS8(104), APH_WG_REGS8(112), APH_WG_REGS8(120)
+        : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<128, float> {
+  static __device__ __forceinline__ void mma(float (&d)[64], uint64_t da, uint64_t db, int acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1;\n\t}"
+        : APH_WG_REGS8(0), APH_WG_REGS8(8), APH_WG_REGS8(16), APH_WG_REGS8(24), APH_WG_REGS8(32), APH_WG_REGS8(40), APH_WG_REGS8(48), APH_WG_REGS8(56)
+        : "l"(da), "l"(db), "r"(acc));
+  }
+};
+template <> struct Wgmma<256, float> {
+  static __device__ __forceinline__ void mma(float (&d)[128], uint64_t da, uint64_t db, int acc) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, "
+        "%24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, "
+        "%72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+        "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, "
+        "%116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1;\n\t}"
         : APH_WG_REGS8(0), APH_WG_REGS8(8), APH_WG_REGS8(16), APH_WG_REGS8(24), APH_WG_REGS8(32), APH_WG_REGS8(40), APH_WG_REGS8(48), APH_WG_REGS8(56),
           APH_WG_REGS8(64), APH_WG_REGS8(72), APH_WG_REGS8(80), APH_WG_REGS8(88), APH_WG_REGS8(96), APH_WG_REGS8(104), APH_WG_REGS8(112), APH_WG_REGS8(120)
         : "l"(da), "l"(db), "r"(acc));
@@ -295,7 +330,8 @@ __device__ __forceinline__ void epi_store_bf16x32(const GemmEpi& epi, int row, b
 //   num_tiles(), k_blocks()                tiles; 64-wide K blocks per tile
 //   has_tile(tile)                         tile < num_tiles(), as the consumer warpgroups test it
 //   tile(tile)                             decodes a tile index into a Tile, which has the tile's N block n_blk
-//   load_a(dst, map_a, bar, t, kb)         the TMA load of the 128 x 64 A box of (Tile t, K block kb), complete_tx on bar
+//   Elem                                   the operand element: bf16, or float for TF32
+//   load_a(dst, map_a, bar, t, kb)         the TMA load of the 128-row A box of (Tile t, K block kb), complete_tx on bar
 //   epilogue(d, t, row, col, lane)         stores finished Tile t from the accumulator fragments d[h][BN / 2] of m64 row
 //                                          block h; this thread's first element is (row + 64 h, col) of the tile
 // The producer decodes each tile before its k-block loop: the compiler does not move a division across the mbarrier waits, so a
@@ -363,7 +399,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a, const CUtens
       for (int kb = 0; kb < k_blocks; ++kb, ++it) {
         const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
         mbar_wait(&full_bar[s], ph);
-        // one descriptor for the stage; offsets go into its (address >> 4) field: +2 per 16 bf16 along K inside the swizzle atom,
+        // one descriptor for the stage; offsets go into its (address >> 4) field: +2 per 32 bytes along K inside the swizzle atom,
         // +512 per 64 rows of A, +A_BYTES / 16 for B
         const uint64_t ds = make_smem_desc(smem_u32(smem + s * L::STAGE_BYTES));
         wgmma_fence();
@@ -371,7 +407,7 @@ __device__ __forceinline__ void gemm_body(const CUtensorMap& map_a, const CUtens
         for (int k = 0; k < GEMM_BK / GEMM_UK; ++k)
 #pragma unroll
           for (int h = 0; h < MMAS; ++h)
-            Wgmma<BN>::mma(d[h], ds + (uint64_t)((PINGPONG ? h : c) * 512 + 2 * k), ds + (uint64_t)(L::A_BYTES / 16 + 2 * k), (kb | k) != 0);
+            Wgmma<BN, typename Problem::Elem>::mma(d[h], ds + (uint64_t)((PINGPONG ? h : c) * 512 + 2 * k), ds + (uint64_t)(L::A_BYTES / 16 + 2 * k), (kb | k) != 0);
         wgmma_commit();
         wgmma_wait<1>();                                 // the previous stage's MMAs have retired: hand that stage back
         if (kb > 0 && tid == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
@@ -390,6 +426,7 @@ template <int BN, int EPI>
 struct GemmProblem {
   const GemmShape& shp;
   const GemmEpi& epi;
+  using Elem = bf16;
 
   __device__ __forceinline__ int num_tiles() const { return (shp.M + GEMM_BM - 1) / GEMM_BM * n_tiles(); }
   __device__ __forceinline__ int n_tiles() const { return shp.N / BN; }

@@ -145,18 +145,28 @@ int aph_affine_fwd(const float* in, int planes, int H, int W, const double* inv_
  * Layer 0: 2 -> nf; layers 1 .. layers-1: kh -> nf; output: kh -> 3, sigmoid. kh = 2 nf for act 0 `unbias`
  * (t = atan z, cat(t / 0.67, (t^2 - 0.45) / 0.396)) and act 1 `comp` (cat(t / 0.67, t^2 / 0.6)), kh = nf for act 2 `relu`
  * ((relu z - 0.4) / 0.58). The hidden layers' products run in TF32 (operands rounded by cvt.rna), everything else in fp32.
- * aph_cppn_create accepts nf a multiple of 8 in [8, 64] and layers in [1, 32] and refuses anything else (host only, no GPU
- * work). The handle owns the backward's scratch.
+ * aph_cppn_create accepts nf a multiple of 8 in [8, 256] and layers in [1, 32] and refuses anything else (host only, no GPU
+ * work). The handle owns the scratch of both calls. nf <= 64 keeps each pixel's activations in registers (no scratch for the
+ * forward; the backward's per-CTA partials). 72 <= nf <= 256 runs layer by layer over all pixels, the hidden layers as TF32
+ * wgmma GEMMs, and grows one buffer to 4 F bytes, for P = N H W pixels:
+ *   chunk = max(4096, ceil(ceil(P / 256) / 128) * 128), S = ceil(P / chunk), Pp = S chunk, R = Pp / 16,
+ *   KHP = KH rounded up to 128 (KH <= 128) or to 256, Q = 3 KH + 8 + nf,
+ *   forward:  F = 2 Pp KH + (layers - 1) nf KH
+ *   backward: F = 2 Pp KH + 2 (layers - 1) nf KH + layers nf Pp + KHP Pp + nf Pp + max(R Q, S nf KH) + 2 ceil(R / 256) Q
+ * (512 x 512, nf 256, 10 layers: 1.1 GB forward, 4.7 GB backward). A failed allocation returns an error naming the size.
  * params / dparams: HOST arrays of 2 (layers + 1) DEVICE pointers {W0, b0, W1, b1, ..., W_layers, b_layers}, W_l the
  * nn.Conv2d weight [out, in, 1, 1] (8-byte aligned), read in place by every call.
- * coords [N,2,H,W] -> out [N,3,H,W]; pixel p = n H W + h W + w. One launch.                                        */
+ * coords [N,2,H,W] -> out [N,3,H,W]; pixel p = n H W + h W + w. One launch for nf <= 64, layers + 2 above.          */
 typedef struct aph_cppn aph_cppn;
 int aph_cppn_create(aph_cppn** handle, int nf, int layers, int act);
 int aph_cppn_destroy(aph_cppn* handle);
+/* device bytes the handle holds now (its scratch grows to the largest call so far)                                    */
+int64_t aph_cppn_bytes(const aph_cppn* handle);
 int aph_cppn_fwd(aph_cppn* handle, const float* coords, int N, int H, int W, const float* const* params, float* out,
                  void* stream);
-/* grad_out [N,3,H,W] -> every dparams tensor (overwritten); no coordinate gradient. Recomputes the forward. Two launches;
- * the weight gradient is reduced in a fixed order, so repeated calls give bit-identical results.                        */
+/* grad_out [N,3,H,W] -> every dparams tensor (overwritten); no coordinate gradient. Recomputes the forward. Two launches
+ * for nf <= 64, a few per layer above; the weight gradient is reduced in a fixed order, so repeated calls give bit-identical
+ * results.                                                                                                              */
 int aph_cppn_bwd(aph_cppn* handle, const float* coords, int N, int H, int W, const float* const* params,
                  const float* grad_out, float* const* dparams, void* stream);
 
