@@ -6,7 +6,10 @@
 #include <stdio.h>
 #include <stdarg.h>
 #include <atomic>
+#include <map>
 #include <memory>
+#include <mutex>
+#include <utility>
 #include <vector>
 
 #include "../../include/aphb200.h"
@@ -58,6 +61,41 @@ inline int num_sms() {
     cache[dev].store(n, std::memory_order_relaxed);
   }
   return n;
+}
+
+// Blocks of 256 threads for a grid-stride loop over n items: one per 256 items, at least one, at most `per_sm` per SM.
+inline int stride_blocks(size_t n, int per_sm) {
+  const size_t b = (n + 255) / 256, cap = (size_t)per_sm * num_sms();
+  return (int)(b < 1 ? 1 : b < cap ? b : cap);
+}
+
+// Raises `kernel`'s dynamic shared-memory limit on the current device to at least `bytes`. It never lowers it: the limit belongs
+// to the kernel, so a launch that needs less must not break a larger one of the same kernel (two FFT plans of different sizes).
+// With `max_carveout` it also asks once for the largest shared-memory carveout. The limit is read once and then cached per
+// (kernel, device), so a launch that needs no more than before makes no attribute call.
+inline int smem_at_least(const void* kernel, size_t bytes, bool max_carveout = false) {
+  struct Conf { int smem; bool carveout; };
+  static std::mutex mu;
+  static std::map<std::pair<const void*, int>, Conf> confs;
+  int dev = 0;
+  APH_CUDA_OK(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = confs.find({kernel, dev});
+  if (it == confs.end()) {
+    cudaFuncAttributes fa;
+    APH_CUDA_OK(cudaFuncGetAttributes(&fa, kernel));
+    it = confs.insert({{kernel, dev}, Conf{fa.maxDynamicSharedSizeBytes, false}}).first;
+  }
+  Conf& c = it->second;
+  if ((int)bytes > c.smem) {
+    APH_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    c.smem = (int)bytes;
+  }
+  if (max_carveout && !c.carveout) {
+    APH_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    c.carveout = true;
+  }
+  return 0;
 }
 
 // The three owner types below are the only code that allocates or frees device memory; aph_device_bytes() is their sum.

@@ -809,7 +809,7 @@ int cppn_bwd(const CppnCall& c, const float* grad_out, float* const* dparams) {
   const bool z_in_smem = stage + zbytes <= CPPN_SMEM_CAP;
   const size_t smem = stage + (z_in_smem ? zbytes : 0);
   auto kern = k_cppn_bwd<NF, RELU>;
-  APH_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (int e = smem_at_least((const void*)kern, smem)) return e;
   int per_sm = 0;
   APH_CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 32 * CPPN_WARPS, smem));
   APH_REQUIRE(per_sm > 0, "aph_cppn_bwd: the backward kernel does not fit on this device (%zu bytes of shared memory)", smem);
@@ -906,18 +906,12 @@ int cppnw_alloc(aph_cppn* h, const WideGeom& g, bool bwd, cudaStream_t st, WideB
   return 0;
 }
 
-int grid_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, (int64_t)num_sms() * 8)); }
-
 // one GEMM: A [a_rows][a_k] and B [b_rows][b_k] fp32 (rows a_ld / b_ld floats apart) through their 16-bit views
 template <int BN, int EPI, bool RELU>
 int cppnw_gemm(const float* A, int a_rows, int a_k, int64_t a_ld, const float* B, int b_rows, int b_k, int64_t b_ld, const CppnWideArgs& a,
                cudaStream_t st) {
   auto kern = k_cppnw_gemm<BN, EPI, RELU>;
-  static bool configured = false;
-  if (!configured) {
-    APH_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GemmCfg<BN>::SMEM));
-    configured = true;
-  }
+  if (int e = smem_at_least((const void*)kern, GemmCfg<BN>::SMEM)) return e;
   CUtensorMap ma, mb;
   if (int e = make_tmap_bf16(&ma, A, a_rows, 2 * a_k, GEMM_BM, 2 * a_ld)) return e;
   if (int e = make_tmap_bf16(&mb, B, b_rows, 2 * b_k, BN, 2 * b_ld)) return e;
@@ -961,11 +955,11 @@ template <bool RELU>
 int cppnw_trunk(const CppnCall& c, const WideGeom& g, const WideBufs& b, bool save, float** xl) {
   const int L = g.L;
   if (L > 1) {
-    k_cppnw_pack<<<grid_for((int64_t)(L - 1) * g.nf * g.kh), 256, 0, c.st>>>(c.P, L, g.nf, g.kh, RELU, b.wp, save ? b.wtp : nullptr);
+    k_cppnw_pack<<<stride_blocks((int64_t)(L - 1) * g.nf * g.kh, 8), 256, 0, c.st>>>(c.P, L, g.nf, g.kh, RELU, b.wp, save ? b.wtp : nullptr);
     APH_LAUNCH_OK();
   }
-  k_cppnw_l0<<<grid_for(g.P * g.nf), 256, 0, c.st>>>(c.coords, g.P, c.hw, c.P.w[0], c.P.b[0], g.nf, g.kh, RELU, c.off, c.div, L > 1, b.xa,
-                                                     save ? b.zT : nullptr, g.Ppad);
+  k_cppnw_l0<<<stride_blocks(g.P * g.nf, 8), 256, 0, c.st>>>(c.coords, g.P, c.hw, c.P.w[0], c.P.b[0], g.nf, g.kh, RELU, c.off, c.div, L > 1, b.xa,
+                                                             save ? b.zT : nullptr, g.Ppad);
   APH_LAUNCH_OK();
   float *x = b.xa, *y = b.xb;
   const int bnf = g.nf <= 128 ? 128 : 256;
@@ -989,7 +983,7 @@ int cppn_fwd_wide(const CppnCall& c, float* out) {
   if (int e = cppnw_alloc(c.h, g, false, c.st, b, "aph_cppn_fwd")) return e;
   float* xl = nullptr;
   if (int e = cppnw_trunk<RELU>(c, g, b, false, &xl)) return e;
-  k_cppnw_head<<<grid_for(g.P * 32), 256, 0, c.st>>>(xl, g.P, c.hw, c.P.w[g.L], c.P.b[g.L], g.nf, g.kh, RELU, out);
+  k_cppnw_head<<<stride_blocks(g.P * 32, 8), 256, 0, c.st>>>(xl, g.P, c.hw, c.P.w[g.L], c.P.b[g.L], g.nf, g.kh, RELU, out);
   APH_LAUNCH_OK();
   return 0;
 }
@@ -1019,8 +1013,8 @@ int cppn_bwd_wide(const CppnCall& c, const float* grad_out, float* const* dparam
   }
   for (int l = L - 1; l >= 1; --l) {
     // dW_l = dz_l^T x_l over S pixel splits, then the fixed-order sum of the splits
-    k_cppnw_actT<<<grid_for((int64_t)nf * g.Ppad), 256, 0, c.st>>>(b.zT + (int64_t)(l - 1) * nf * g.Ppad, g.P, g.Ppad, nf, g.khp, g.chunk,
-                                                                   RELU, c.off, c.div, b.xT);
+    k_cppnw_actT<<<stride_blocks((int64_t)nf * g.Ppad, 8), 256, 0, c.st>>>(b.zT + (int64_t)(l - 1) * nf * g.Ppad, g.P, g.Ppad, nf, g.khp, g.chunk,
+                                                                           RELU, c.off, c.div, b.xT);
     APH_LAUNCH_OK();
     CppnWideArgs w{};
     w.M = nf; w.N = kh; w.m_tiles = (nf + GEMM_BM - 1) / GEMM_BM; w.n_tiles = g.ntk; w.splits = g.S; w.kblocks = g.chunk / 32;

@@ -3,7 +3,6 @@
 #pragma once
 #include "vit_ops.cuh"
 #include "weights.cuh"
-#include <map>
 
 namespace aph {
 

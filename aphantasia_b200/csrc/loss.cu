@@ -200,7 +200,7 @@ extern "C" int aph_derivat_fwd(const float* img, int C, int H, int W, double* su
   cudaStream_t st = (cudaStream_t)stream;
   APH_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * sizeof(double), st));
   const size_t n = (size_t)C * H * W;
-  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8);
+  const int blocks = stride_blocks(n, 8);
   k_derivat_fwd<<<blocks, 256, 0, st>>>(img, C, H, W, sums);
   APH_LAUNCH_OK();
   k_derivat_fin<<<1, 1, 0, st>>>(sums, (double)C * H * (W - 1), (double)C * (H - 1) * W, value);
@@ -211,7 +211,7 @@ extern "C" int aph_derivat_fwd(const float* img, int C, int H, int W, double* su
 extern "C" int aph_derivat_bwd(const float* img, int C, int H, int W, const float* upstream, float* grad_img, void* stream) {
   APH_REQUIRE(img && upstream && grad_img && C > 0 && H > 1 && W > 1, "aph_derivat_bwd: bad arguments");
   const size_t n = (size_t)C * H * W;
-  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8);
+  const int blocks = stride_blocks(n, 8);
   k_derivat_bwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(img, C, H, W, upstream, (float)(1.0 / ((double)C * H * (W - 1))),
                                                          (float)(1.0 / ((double)C * (H - 1) * W)), grad_img);
   APH_LAUNCH_OK();
@@ -223,7 +223,7 @@ extern "C" int aph_derivat_sobel_fwd(const float* img, int C, int H, int W, doub
   cudaStream_t st = (cudaStream_t)stream;
   APH_CUDA_OK(cudaMemsetAsync(sums, 0, sizeof(double), st));
   const size_t n = (size_t)C * H * W;
-  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8);
+  const int blocks = stride_blocks(n, 8);
   k_derivat_sobel_fwd<<<blocks, 256, 0, st>>>(img, C, H, W, sums);
   APH_LAUNCH_OK();
   k_derivat_sobel_fin<<<1, 1, 0, st>>>(sums, 2.0 * (double)n, value);
@@ -234,7 +234,7 @@ extern "C" int aph_derivat_sobel_fwd(const float* img, int C, int H, int W, doub
 extern "C" int aph_derivat_sobel_bwd(const float* img, int C, int H, int W, const float* upstream, float* grad_img, void* stream) {
   APH_REQUIRE(img && upstream && grad_img && C > 0 && H > 0 && W > 0, "aph_derivat_sobel_bwd: bad arguments");
   const size_t n = (size_t)C * H * W;
-  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8);
+  const int blocks = stride_blocks(n, 8);
   k_derivat_sobel_bwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(img, C, H, W, upstream, (float)(1.0 / (16.0 * (double)n)), grad_img);
   APH_LAUNCH_OK();
   return 0;
@@ -250,7 +250,7 @@ extern "C" int aph_head_fwd(const float* emb, int S, int D, const float* w, cons
 extern "C" int aph_head_bwd(const float* grad_out, const float* w, int S, int D, float* grad_emb, void* stream) {
   APH_REQUIRE(grad_out && w && grad_emb && S > 0 && D > 0, "aph_head_bwd: bad arguments");
   const size_t n = (size_t)S * D;
-  const int blocks = (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8);
+  const int blocks = stride_blocks(n, 8);
   k_head_bwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(grad_out, w, S, D, grad_emb);
   APH_LAUNCH_OK();
   return 0;
@@ -274,7 +274,7 @@ extern "C" int aph_adam_step(float* p, const float* g, float* m, float* v, int64
                              int step, void* stream) {
   APH_REQUIRE(p && g && m && v && n > 0 && step >= 1, "aph_adam_step: bad arguments");
   const double bc1 = 1.0 - pow((double)b1, step), bc2 = 1.0 - pow((double)b2, step);
-  const int blocks = (int)std::min<int64_t>((n + 255) / 256, (int64_t)num_sms() * 8);
+  const int blocks = stride_blocks((size_t)n, 8);
   k_adam<<<blocks, 256, 0, (cudaStream_t)stream>>>(p, g, m, v, (size_t)n, (float)(lr / bc1), b1, b2, eps, (float)(1.0 / sqrt(bc2)));
   APH_LAUNCH_OK();
   return 0;

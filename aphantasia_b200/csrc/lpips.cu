@@ -232,11 +232,7 @@ template <int BN, int EPI>
 static int conv_cfg(const void* x, const void* wpack, const ConvShape& cs, const ConvEpi& epi, cudaStream_t st) {
   using L = GemmCfg<BN>;
   static_assert(L::SMEM <= 227 * 1024, "conv shared-memory budget");
-  static bool configured = false;
-  if (!configured) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_conv3x3_tc<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM));
-    configured = true;
-  }
+  if (int e = smem_at_least((const void*)k_conv3x3_tc<BN, EPI>, L::SMEM)) return e;
   CUtensorMap mx, mw;
   if (int e = make_tmap_bf16_nhwc(&mx, x, cs.N, cs.H, cs.W, cs.Cin, CONV_TH, CONV_TW)) return e;
   if (int e = make_tmap_bf16(&mw, wpack, cs.Cout, 9 * cs.Cin, BN)) return e;
@@ -264,19 +260,14 @@ int launch_conv3x3(const void* x, const void* wpack, int N, int H, int W, int Ci
   return 2;
 }
 
-static int grid_for(size_t items, int block) {
-  const size_t b = (items + block - 1) / block, cap = (size_t)num_sms() * 16;
-  return (int)(b < cap ? (b > 0 ? b : 1) : cap);
-}
-
 static int launch_pool_fwd(const bf16* x, int N, int H, int W, int C, bf16* out, cudaStream_t st) {
-  k_pool_fwd<<<grid_for((size_t)N * (H / 2) * (W / 2) * (C / 8), 256), 256, 0, st>>>(x, N, H, W, C, out);
+  k_pool_fwd<<<stride_blocks((size_t)N * (H / 2) * (W / 2) * (C / 8), 16), 256, 0, st>>>(x, N, H, W, C, out);
   APH_LAUNCH_OK();
   return 0;
 }
 static int launch_tap_bwd(const bf16* f0, const bf16* f1, const float* lin, const float* up, const bf16* dpool, int N, int H, int W,
                           int C, int mask, bf16* out, cudaStream_t st) {
-  k_tap_bwd<<<grid_for((size_t)N * H * W * 32, 256), 256, 0, st>>>(f0, f1, lin, up, dpool, N, H, W, C, mask, out);
+  k_tap_bwd<<<stride_blocks((size_t)N * H * W * 32, 16), 256, 0, st>>>(f0, f1, lin, up, dpool, N, H, W, C, mask, out);
   APH_LAUNCH_OK();
   return 0;
 }

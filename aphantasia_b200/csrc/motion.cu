@@ -80,7 +80,7 @@ extern "C" int aph_affine_fwd(const float* in, int planes, int H, int W, const d
   m.a = t[0]; m.b = t[1]; m.c = t[0] * cx + t[1] * cy + t[2] + 0.5 * W - 0.5;
   m.d = t[3]; m.e = t[4]; m.f = t[3] * cx + t[4] * cy + t[5] + 0.5 * H - 0.5;
   const size_t hw = (size_t)H * W;
-  const int blocks = (int)std::min<size_t>((hw + 255) / 256, (size_t)num_sms() * 16);
+  const int blocks = stride_blocks(hw, 16);
   k_frame_affine<<<blocks, 256, 0, (cudaStream_t)stream>>>(in, planes, H, W, m, out);
   APH_LAUNCH_OK();
   return 0;

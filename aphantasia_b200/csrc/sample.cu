@@ -791,17 +791,13 @@ static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int p
     if (int e = g_A.grow((size_t)S * 3 * size * size * sizeof(float), st)) return e;
     dst = g_A.p;
   }
-  static size_t conf = 0;
-  if (smem2 > conf) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_resize<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_resize<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-    conf = smem2;
-  }
+  auto resize = k_resize<false, false>;
+  if (pad_top || pad_left) resize = k_resize<true, false>;
+  if (cap == 0) resize = k_resize<true, true>;
+  if (int e = smem_at_least((const void*)resize, smem2)) return e;
   const int rows_per_cta = 32;
   const dim3 g1(S * 3, (size + rows_per_cta - 1) / rows_per_cta);
-  if (cap == 0) k_resize<true, true><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
-  else if (pad_top || pad_left) k_resize<true, false><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
-  else k_resize<false, false><<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
+  resize<<<g1, 256, smem2, st>>>(canvas, H, W, pad_top, pad_left, table, size, rows_per_cta, cap, kind, dst, po);
   APH_LAUNCH_OK();
   if (kind == APH_TF_FAST) {
     const int tiles = ((size + 15) / 16) * ((size + 15) / 16);
@@ -828,12 +824,9 @@ extern "C" int aph_sample_bwd_scaled(const float* grad_out, int H, int W, int pa
   if (S == 0) return 0;
   APH_REQUIRE(grad_out && table, "aph_sample_bwd_scaled: null pointer");
   const size_t smem3 = ((size_t)8 * size + 8 * 3 * STRIP) * sizeof(float);
-  static size_t configured3 = 48 * 1024;
-  if (smem3 > configured3) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_bwd_bicubic3<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_bwd_bicubic3<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem3));
-    configured3 = smem3;
-  }
+  const bool vec = pad_top == 0 && pad_left == 0 && W % 4 == 0 && ((uintptr_t)grad_canvas & 15) == 0;
+  const auto bicubic = vec ? k_bwd_bicubic3<true> : k_bwd_bicubic3<false>;
+  if (int e = smem_at_least((const void*)bicubic, smem3)) return e;
   const float* bb_src = grad_out;
   if (kind >= APH_TF_CUSTOM) {
     // adjoints of normalise, jitter and the elastic stretch into gR (fully overwritten), then the rest in k_bwd_bicubic3 (mode 4)
@@ -855,10 +848,8 @@ extern "C" int aph_sample_bwd_scaled(const float* grad_out, int H, int W, int pa
     k_bwd_warp_adjoint<<<g1, 256, 0, st>>>(grad_out, table, size, gscale, g_gW.p);
     APH_LAUNCH_OK();
   }
-  const bool vec = pad_top == 0 && pad_left == 0 && W % 4 == 0 && ((uintptr_t)grad_canvas & 15) == 0;
   const dim3 g3((size + BB_ROWS - 1) / BB_ROWS, S);
-  if (vec) k_bwd_bicubic3<true><<<g3, 256, smem3, st>>>(bb_src, g_gW.p, H, W, pad_top, pad_left, table, size, kind, gscale, grad_canvas);
-  else k_bwd_bicubic3<false><<<g3, 256, smem3, st>>>(bb_src, g_gW.p, H, W, pad_top, pad_left, table, size, kind, gscale, grad_canvas);
+  bicubic<<<g3, 256, smem3, st>>>(bb_src, g_gW.p, H, W, pad_top, pad_left, table, size, kind, gscale, grad_canvas);
   APH_LAUNCH_OK();
   return 0;
 }

@@ -194,8 +194,6 @@ __global__ void __launch_bounds__(256) k_stats(const float* __restrict__ x, size
 }
 __global__ void k_fix_stats(double* stats, double n, double sigma) { stats[0] = 0.; stats[1] = sigma * sigma * (n - 1.0); stats[2] = 0.; }
 
-static inline int grid_for(size_t n) { return (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16); }
-
 }  // namespace aph
 
 using namespace aph;
@@ -252,12 +250,12 @@ extern "C" int aph_synth_dwt_fwd(aph_dwt_plan* plan, const float* const* Ys, con
     const int llh = (i == J - 1) ? p->lh[J - 1] : p->oh[i + 1], llw = (i == J - 1) ? p->lw[J - 1] : p->ow[i + 1];
     float* o = (i == 0) ? x_raw : p->ll[i];
     const size_t n = (size_t)3 * p->oh[i] * p->ow[i];
-    k_dwt_level_fwd<<<grid_for(n), 256, 0, st>>>(ll, llh, llw, Ys[i + 1], scales_host[i], p->lh[i], p->lw[i], o, p->oh[i], p->ow[i], p->f,
-                                                 i == 0 ? stats : nullptr);
+    k_dwt_level_fwd<<<stride_blocks(n, 16), 256, 0, st>>>(ll, llh, llw, Ys[i + 1], scales_host[i], p->lh[i], p->lw[i], o, p->oh[i], p->ow[i], p->f,
+                                                          i == 0 ? stats : nullptr);
     APH_LAUNCH_OK();
   }
   const size_t hw = (size_t)p->oh[0] * p->ow[0];
-  k_finish<<<grid_for(hw), 256, 0, st>>>(x_raw, stats, out, hw, contrast, make_colmat(colmat_host), apply_sigmoid);
+  k_finish<<<stride_blocks(hw, 16), 256, 0, st>>>(x_raw, stats, out, hw, contrast, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
   return 0;
 }
@@ -271,9 +269,9 @@ extern "C" int aph_synth_dwt_bwd(aph_dwt_plan* plan, const float* grad_out, cons
   cudaStream_t st = (cudaStream_t)stream;
   const size_t hw = (size_t)p->oh[0] * p->ow[0];
   APH_CUDA_OK(cudaMemsetAsync(stats + 2, 0, sizeof(double), st));
-  k_finish_bwd<<<grid_for(hw), 256, 0, st>>>(grad_out, out, x_raw, p->gimg, stats, hw, make_colmat(colmat_host), apply_sigmoid);
+  k_finish_bwd<<<stride_blocks(hw, 16), 256, 0, st>>>(grad_out, out, x_raw, p->gimg, stats, hw, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
-  k_norm_bwd<<<grid_for(3 * hw), 256, 0, st>>>(p->gimg, x_raw, stats, p->gx, 3 * hw, contrast);
+  k_norm_bwd<<<stride_blocks(3 * hw, 16), 256, 0, st>>>(p->gimg, x_raw, stats, p->gx, 3 * hw, contrast);
   APH_LAUNCH_OK();
   const int J = p->J;
   for (int i = 0; i < J; ++i) {                        // finest first
@@ -281,7 +279,7 @@ extern "C" int aph_synth_dwt_bwd(aph_dwt_plan* plan, const float* grad_out, cons
     float* dll = (i == J - 1) ? grad_Ys[0] : p->dll[i + 1];
     const int llh = (i == J - 1) ? p->lh[J - 1] : p->oh[i + 1], llw = (i == J - 1) ? p->lw[J - 1] : p->ow[i + 1];
     const size_t n = (size_t)3 * llh * llw;
-    k_dwt_level_bwd<<<grid_for(n), 256, 0, st>>>(dout, p->oh[i], p->ow[i], dll, llh, llw, grad_Ys[i + 1], scales_host[i], p->lh[i], p->lw[i], p->f);
+    k_dwt_level_bwd<<<stride_blocks(n, 16), 256, 0, st>>>(dout, p->oh[i], p->ow[i], dll, llh, llw, grad_Ys[i + 1], scales_host[i], p->lh[i], p->lw[i], p->f);
     APH_LAUNCH_OK();
   }
   return 0;
@@ -305,9 +303,9 @@ extern "C" int aph_dwt_analyze(aph_dwt_plan* plan, const float* img, const float
     StreamTemp<float> rows;
     if (int e = rows.alloc((size_t)3 * 2 * h * ow, st)) return e;
     float* ll = (i == J - 1) ? Ys[0] : p->ll[i + 1];
-    k_dwt_afb_w<<<grid_for((size_t)3 * h * ow), 256, 0, st>>>(x, h, w, rows.p, ow, p->f);
+    k_dwt_afb_w<<<stride_blocks((size_t)3 * h * ow, 16), 256, 0, st>>>(x, h, w, rows.p, ow, p->f);
     APH_LAUNCH_OK();
-    k_dwt_afb_h<<<grid_for((size_t)3 * oh * ow), 256, 0, st>>>(rows.p, h, ow, ll, Ys[i + 1], inv_scales_host[i], oh, p->f);
+    k_dwt_afb_h<<<stride_blocks((size_t)3 * oh * ow, 16), 256, 0, st>>>(rows.p, h, ow, ll, Ys[i + 1], inv_scales_host[i], oh, p->f);
     APH_LAUNCH_OK();
     x = ll; h = oh; w = ow;
   }
@@ -322,9 +320,9 @@ extern "C" int aph_pixel_fwd(const float* x, int64_t hw, float contrast, int fix
   cudaStream_t st = (cudaStream_t)stream;
   APH_CUDA_OK(cudaMemsetAsync(stats, 0, 4 * sizeof(double), st));
   if (fixcontrast) k_fix_stats<<<1, 1, 0, st>>>(stats, 3.0 * (double)hw, 3.3);       // sigma := 3.3 (image.py:115)
-  else k_stats<<<grid_for(3 * (size_t)hw), 256, 0, st>>>(x, 3 * (size_t)hw, stats);
+  else k_stats<<<stride_blocks(3 * (size_t)hw, 16), 256, 0, st>>>(x, 3 * (size_t)hw, stats);
   APH_LAUNCH_OK();
-  k_finish<<<grid_for((size_t)hw), 256, 0, st>>>(x, stats, out, (size_t)hw, contrast, make_colmat(colmat_host), apply_sigmoid);
+  k_finish<<<stride_blocks((size_t)hw, 16), 256, 0, st>>>(x, stats, out, (size_t)hw, contrast, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
   return 0;
 }
@@ -336,10 +334,10 @@ extern "C" int aph_pixel_bwd(const float* grad_out, const float* out, const floa
   cudaStream_t st = (cudaStream_t)stream;
   APH_CUDA_OK(cudaMemsetAsync(stats + 2, 0, sizeof(double), st));
   // g_img lands in grad_x, then is rewritten in place by the normalisation adjoint (with fixcontrast the std term vanishes)
-  k_finish_bwd<<<grid_for((size_t)hw), 256, 0, st>>>(grad_out, out, fixcontrast ? nullptr : x, grad_x, stats, (size_t)hw,
-                                                     make_colmat(colmat_host), apply_sigmoid);
+  k_finish_bwd<<<stride_blocks((size_t)hw, 16), 256, 0, st>>>(grad_out, out, fixcontrast ? nullptr : x, grad_x, stats, (size_t)hw,
+                                                              make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
-  k_norm_bwd<<<grid_for(3 * (size_t)hw), 256, 0, st>>>(grad_x, x, stats, grad_x, 3 * (size_t)hw, contrast);
+  k_norm_bwd<<<stride_blocks(3 * (size_t)hw, 16), 256, 0, st>>>(grad_x, x, stats, grad_x, 3 * (size_t)hw, contrast);
   APH_LAUNCH_OK();
   return 0;
 }

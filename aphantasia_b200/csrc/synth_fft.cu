@@ -460,24 +460,15 @@ extern "C" int aph_fft_plan_create(aph_fft_plan** plan_out, int H, int W) {
   APH_CUDA_OK(cudaMemcpy(p->twW, tw.data(), W * sizeof(float2), cudaMemcpyHostToDevice));
   if (int e = p->alloc(&p->T, (size_t)3 * H * p->Wh)) return e;
   if (int e = p->alloc(&p->gimg, (size_t)3 * H * W)) return e;
-  // The shared-memory limit is an attribute of the kernel, not of the plan: only ever raise it, so that creating a plan with
-  // shorter lines does not break the launches of a larger plan that is still alive.
-  auto raise_smem = [](const void* fn, size_t bytes) -> cudaError_t {
-    cudaFuncAttributes fa;
-    cudaError_t e = cudaFuncGetAttributes(&fa, fn);
-    if (e != cudaSuccess || (int)bytes <= fa.maxDynamicSharedSizeBytes) return e;
-    return cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-  };
   if (p->colSingle) {
-    APH_CUDA_OK(raise_smem((const void*)k_col_fft<true, true>, p->smem_col));
-    APH_CUDA_OK(raise_smem((const void*)k_col_fft<false, true>, p->smem_col));
+    if (int e = smem_at_least((const void*)k_col_fft<true, true>, p->smem_col)) return e;
+    if (int e = smem_at_least((const void*)k_col_fft<false, true>, p->smem_col)) return e;
   } else {
-    APH_CUDA_OK(raise_smem((const void*)k_col_fft<true>, p->smem_col));
-    APH_CUDA_OK(raise_smem((const void*)k_col_fft<false>, p->smem_col));
+    if (int e = smem_at_least((const void*)k_col_fft<true>, p->smem_col)) return e;
+    if (int e = smem_at_least((const void*)k_col_fft<false>, p->smem_col)) return e;
   }
-  APH_CUDA_OK(raise_smem((const void*)k_row_c2r, p->smem_row));
-  APH_CUDA_OK(raise_smem((const void*)k_row_r2c, p->smem_row));
-  APH_CUDA_OK(raise_smem((const void*)k_row_rfft, p->smem_row));
+  for (const void* k : {(const void*)k_row_c2r, (const void*)k_row_r2c, (const void*)k_row_rfft})
+    if (int e = smem_at_least(k, p->smem_row)) return e;
   *plan_out = reinterpret_cast<aph_fft_plan*>(p.release());
   return 0;
 }
@@ -507,7 +498,7 @@ extern "C" int aph_synth_fft_fwd(aph_fft_plan* plan, const float* params, const 
   k_row_c2r<<<3 * groups, 256, p->smem_row, st>>>(p->T, x_raw, stats, p->twW, H, W, Wh, p->rowP, norm, p->rw);
   APH_LAUNCH_OK();
   const size_t hw = (size_t)H * W;
-  const int blocks = (int)std::min<size_t>((hw + 255) / 256, (size_t)num_sms() * 8);
+  const int blocks = stride_blocks(hw, 8);
   k_finish<<<blocks, 256, 0, st>>>(x_raw, stats, out, hw, contrast, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
   return 0;
@@ -523,7 +514,7 @@ static int synth_fft_bwd_impl(aph_fft_plan* plan, const float* grad_out, const f
   const int H = p->H, W = p->W, Wh = p->Wh;
   const size_t hw = (size_t)H * W;
   APH_CUDA_OK(cudaMemsetAsync(stats + 2, 0, sizeof(double), st));
-  const int blocks = (int)std::min<size_t>((hw + 255) / 256, (size_t)num_sms() * 8);
+  const int blocks = stride_blocks(hw, 8);
   k_finish_bwd<<<blocks, 256, 0, st>>>(grad_out, out, x_raw, p->gimg, stats, hw, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
   const int groups = ((H + 1) / 2 + p->rowP - 1) / p->rowP;
@@ -580,7 +571,7 @@ extern "C" int aph_fft_analyze(aph_fft_plan* plan, const float* img, const float
 extern "C" int aph_un_rgb(const uint8_t* hwc, int H, int W, const float* inv_colmat_host, float gain, float* out, void* stream) {
   APH_REQUIRE(hwc && inv_colmat_host && out && H > 0 && W > 0, "aph_un_rgb: bad arguments");
   const size_t hw = (size_t)H * W;
-  const int blocks = (int)std::min<size_t>((hw + 255) / 256, (size_t)num_sms() * 8);
+  const int blocks = stride_blocks(hw, 8);
   k_un_rgb<<<blocks, 256, 0, (cudaStream_t)stream>>>(hwc, hw, make_colmat(inv_colmat_host), gain, out);
   APH_LAUNCH_OK();
   return 0;
@@ -603,7 +594,7 @@ __global__ void __launch_bounds__(256) k_rgb_fwd(const float* __restrict__ img, 
 
 extern "C" int aph_valid_rgb_fwd(const float* img, int64_t hw, const float* colmat_host, float* out, void* stream) {
   APH_REQUIRE(img && out && hw > 0, "aph_valid_rgb_fwd: bad arguments");
-  const int blocks = (int)std::min<size_t>(((size_t)hw + 255) / 256, (size_t)num_sms() * 8);
+  const int blocks = stride_blocks((size_t)hw, 8);
   k_rgb_fwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(img, out, (size_t)hw, make_colmat(colmat_host));
   APH_LAUNCH_OK();
   return 0;
@@ -612,7 +603,7 @@ extern "C" int aph_valid_rgb_fwd(const float* img, int64_t hw, const float* colm
 extern "C" int aph_valid_rgb_bwd(const float* grad_out, const float* out, int64_t hw, const float* colmat_host,
                                  float* grad_img, void* stream) {
   APH_REQUIRE(grad_out && out && grad_img && hw > 0, "aph_valid_rgb_bwd: bad arguments");
-  const int blocks = (int)std::min<size_t>(((size_t)hw + 255) / 256, (size_t)num_sms() * 8);
+  const int blocks = stride_blocks((size_t)hw, 8);
   k_finish_bwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(grad_out, out, nullptr, grad_img, nullptr, (size_t)hw,
                                                          make_colmat(colmat_host), 1);
   APH_LAUNCH_OK();

@@ -90,11 +90,7 @@ __global__ void __launch_bounds__(256) k_text_pool_ln(const float* __restrict__ 
 // causal tensor-core attention: the image tower's forward kernel with the mask compiled in
 template <int NW, int NT2>
 int attn_causal_launch(const bf16* qkv, bf16* out, int S, int T, int D, int heads, cudaStream_t st) {
-  static bool cfg = false;
-  if (!cfg) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd_tc<NW, NT2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_tc_fwd_smem<NW, NT2>()));
-    cfg = true;
-  }
+  if (int e = smem_at_least((const void*)k_attn_fwd_tc<NW, NT2, true>, attn_tc_fwd_smem<NW, NT2>())) return e;
   k_attn_fwd_tc<NW, NT2, true><<<S * heads, NW * 32, attn_tc_fwd_smem<NW, NT2>(), st>>>(qkv, out, T, D, heads);
   APH_LAUNCH_OK();
   return 0;

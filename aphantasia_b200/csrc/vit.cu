@@ -9,8 +9,74 @@
 #include "encoder.cuh"
 #include "vit_attn_tc.cuh"
 #include "vit_attn_stream.cuh"
+#include <set>
 
 namespace aph {
+
+bool gemm_profiling_on();      // vit_gemm.cu
+
+// CUDA-graph cache of one direction of a handle (forward or backward): the ~90 launches of a call are replayed as one graph when
+// the call repeats with the same batch size S and flag (the optimisation loop does). The first call with an S runs eagerly (lazy
+// one-time initialisations are not capturable), the next one captures and instantiates, later ones replay; a small LRU.
+struct GraphCache : NoCopy {
+  struct Entry { int S; int flag; cudaGraphExec_t exec; unsigned long long stamp; int nodes; };
+  std::vector<Entry> entries;
+  std::set<int> warm;            // batch sizes that have run eagerly
+  unsigned long long stamp = 0;
+  int misses = 0;                // captures in a row that were never replayed
+  ~GraphCache() { for (auto& e : entries) cudaGraphExecDestroy(e.exec); }
+
+  // Runs `body`, which launches on `st`, through the cache.
+  template <typename Body>
+  int run(int S, int flag, cudaStream_t& st, Body body) {
+    // GEMM profiling (aph_prof_gemm) records events around each launch, so it runs eagerly. A cache whose keys keep changing
+    // would re-capture forever: after 6 never-replayed captures in a row it stays eager
+    if (gemm_profiling_on() || misses > 6) return body();
+    for (auto& e : entries)
+      if (e.S == S && e.flag == flag) {
+        e.stamp = ++stamp;
+        misses = 0;
+        APH_CUDA_OK(cudaGraphLaunch(e.exec, st));
+        count_launch(e.nodes);         // kernels replayed by the graph
+        return 0;
+      }
+    if (warm.insert(S).second) return body();
+    // The caller's stream is often the legacy default stream (torch's default), which cannot be captured: record the launch
+    // sequence on a private stream (`st` is what the body launches on -- capture enqueues nothing), replay on the caller's.
+    static cudaStream_t cap = nullptr;
+    if (!cap) APH_CUDA_OK(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
+    cudaStream_t user = st;
+    st = cap;
+    if (cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); st = user; return body(); }
+    const int rc = body();
+    cudaGraph_t graph = nullptr;
+    const cudaError_t ce = cudaStreamEndCapture(cap, &graph);
+    st = user;
+    if (rc != 0 || ce != cudaSuccess || graph == nullptr) {
+      if (graph) cudaGraphDestroy(graph);
+      cudaGetLastError();
+      if (rc != 0) return rc;
+      return body();                                               // capture refused: stay eager
+    }
+    size_t nodes = 0;
+    cudaGraphGetNodes(graph, nullptr, &nodes);
+    g_launches.fetch_sub((long long)nodes, std::memory_order_relaxed);   // the capture pass enqueued nothing; the replay below counts
+    cudaGraphExec_t exec = nullptr;
+    if (cudaGraphInstantiate(&exec, graph, 0) != cudaSuccess) { cudaGraphDestroy(graph); cudaGetLastError(); return body(); }
+    cudaGraphDestroy(graph);
+    if (entries.size() >= 4) {                                     // evict the least recently used
+      size_t lru = 0;
+      for (size_t i = 1; i < entries.size(); ++i) if (entries[i].stamp < entries[lru].stamp) lru = i;
+      cudaGraphExecDestroy(entries[lru].exec);
+      entries.erase(entries.begin() + lru);
+    }
+    ++misses;
+    entries.push_back({S, flag, exec, ++stamp, (int)nodes});
+    APH_CUDA_OK(cudaGraphLaunch(exec, st));
+    count_launch((int)nodes);
+    return 0;
+  }
+};
 
 struct VitImpl : Encoder {
   aph_vit_config cfg;
@@ -51,17 +117,7 @@ struct VitImpl : Encoder {
   bf16* d_tok = nullptr;         // [S*g*g, D]
   float2* attn_stats = nullptr;  // [S*heads*T] (lse, delta) of the streaming attention backward (T > 256 only), reused by every layer
   int last_S = -1;
-  // CUDA-graph cache: the ~90 launches of a forward (or backward) are replayed as one graph when the call repeats with the
-  // same batch size and the same input/output pointers (the optimisation loop does); keyed, small LRU
-  struct GraphEntry { const void* in; const void* out; int S; int flag; cudaGraphExec_t exec; unsigned long long stamp; int nodes; };
-  std::vector<GraphEntry> fwd_graphs, bwd_graphs;
-  std::map<int, int> warm_fwd, warm_bwd;
-  unsigned long long stamp = 0;
-  int graph_misses = 0;          // captures in a row that were never replayed (e.g. the caller re-allocates its tensors every step)
-  ~VitImpl() {
-    for (auto& g : fwd_graphs) cudaGraphExecDestroy(g.exec);
-    for (auto& g : bwd_graphs) cudaGraphExecDestroy(g.exec);
-  }
+  GraphCache fwd_graphs, bwd_graphs;
 };
 
 // LayerNorm statistics slot k: 0 = ln_pre, 1 + 2l / 2 + 2l = ln_1 / ln_2 of layer l, 2 layers + 1 = ln_post. The slots below
@@ -69,62 +125,6 @@ struct VitImpl : Encoder {
 static size_t stat_off(const VitImpl* v, int k) {
   const size_t Mmax = (size_t)v->cfg.max_batch * v->T, k2 = 2 * (size_t)v->cfg.layers;
   return (size_t)k < k2 ? k * Mmax : k2 * Mmax + (k - k2) * (size_t)v->cfg.max_batch;
-}
-
-bool gemm_profiling_on();      // vit_gemm.cu
-
-// Runs `body` through the graph cache: 1st call with a key runs eagerly (lazy one-time initialisations are not capturable),
-// 2nd call captures + instantiates, later calls replay.
-template <typename Body>
-static int run_cached(std::vector<VitImpl::GraphEntry>& cache, std::map<int, int>& warm, unsigned long long& stamp, int& misses,
-                      const void* in, const void* out, int S, int flag, cudaStream_t& st, Body body) {
-  // GEMM profiling (aph_prof_gemm) records events around each launch, so it runs eagerly. A caller whose buffers move every
-  // step (clip_fft.py calls torch.cuda.empty_cache() per step) would re-capture forever: after 6 never-replayed captures in a
-  // row the handle stays eager
-  if (gemm_profiling_on() || misses > 6) return body();
-  for (auto& g : cache)
-    if (g.in == in && g.out == out && g.S == S && g.flag == flag) {
-      g.stamp = ++stamp;
-      misses = 0;
-      APH_CUDA_OK(cudaGraphLaunch(g.exec, st));
-      count_launch(g.nodes);           // kernels replayed by the graph
-      return 0;
-    }
-  if (!warm[S]) { warm[S] = 1; return body(); }
-  // The caller's stream is often the legacy default stream (torch's default), which cannot be captured: record the launch
-  // sequence on a private stream (`st` is what the body launches on -- capture enqueues nothing), replay on the caller's.
-  static cudaStream_t cap = nullptr;
-  if (!cap) APH_CUDA_OK(cudaStreamCreateWithFlags(&cap, cudaStreamNonBlocking));
-  cudaStream_t user = st;
-  st = cap;
-  if (cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal) != cudaSuccess) { cudaGetLastError(); st = user; return body(); }
-  const int rc = body();
-  cudaGraph_t graph = nullptr;
-  const cudaError_t ce = cudaStreamEndCapture(cap, &graph);
-  st = user;
-  if (rc != 0 || ce != cudaSuccess || graph == nullptr) {
-    if (graph) cudaGraphDestroy(graph);
-    cudaGetLastError();
-    if (rc != 0) return rc;
-    return body();                                                 // capture refused: stay eager
-  }
-  size_t nodes = 0;
-  cudaGraphGetNodes(graph, nullptr, &nodes);
-  g_launches.fetch_sub((long long)nodes, std::memory_order_relaxed);   // the capture pass enqueued nothing; the replay below counts
-  cudaGraphExec_t exec = nullptr;
-  if (cudaGraphInstantiate(&exec, graph, 0) != cudaSuccess) { cudaGraphDestroy(graph); cudaGetLastError(); return body(); }
-  cudaGraphDestroy(graph);
-  if (cache.size() >= 4) {                                         // evict the least recently used
-    size_t lru = 0;
-    for (size_t i = 1; i < cache.size(); ++i) if (cache[i].stamp < cache[lru].stamp) lru = i;
-    cudaGraphExecDestroy(cache[lru].exec);
-    cache.erase(cache.begin() + lru);
-  }
-  ++misses;
-  cache.push_back({in, out, S, flag, exec, ++stamp, (int)nodes});
-  APH_CUDA_OK(cudaGraphLaunch(exec, st));
-  count_launch((int)nodes);
-  return 0;
 }
 
 int add_blocks(Encoder* h, int layers, int D, bool dgrad) {
@@ -302,14 +302,14 @@ static int vit_fwd_impl(aph_vit* vit, const float* images, int S, int side, floa
     const int p = v->cfg.patch;
     if (v->Kp == 3 * p * p) {                // rows without padding (p = 16, 32): 8 columns per thread
       const size_t n8 = (size_t)Mp * v->Kp / 8;
-      k_patchify<false><<<(unsigned)std::min<size_t>((n8 + 255) / 256, (size_t)num_sms() * 16), 256, 0, st>>>(images, v->patches, S, p, g, side);
+      k_patchify<false><<<stride_blocks(n8, 16), 256, 0, st>>>(images, v->patches, S, p, g, side);
     } else {                                 // padded rows (p = 14): pixel pairs
       const size_t n2 = (size_t)Mp * 3 * p * p / 2;
-      k_patchify<true><<<(unsigned)std::min<size_t>((n2 + 255) / 256, (size_t)num_sms() * 16), 256, 0, st>>>(images, v->patches, S, p, g, side);
+      k_patchify<true><<<stride_blocks(n2, 16), 256, 0, st>>>(images, v->patches, S, p, g, side);
     }
     APH_LAUNCH_OK();
   }
-  const int rc = run_cached(v->fwd_graphs, v->warm_fwd, v->stamp, v->graph_misses, nullptr, nullptr, S, save_for_bwd, st, [&]() -> int {
+  const int rc = v->fwd_graphs.run(S, save_for_bwd, st, [&]() -> int {
   const int D = v->D, T = v->T, g = v->g, Ly = v->cfg.layers, O = v->cfg.out_dim, H = v->cfg.heads;
   const int M = S * T, Mp = S * g * g;
   int e;
@@ -355,10 +355,10 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
   cudaStream_t st = (cudaStream_t)stream;
   {   // caller-owned input: converted outside the cached graph (see aph_vit_fwd)
     const size_t n = (size_t)S * v->cfg.out_dim;
-    k_f32_to_bf16<<<(int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 8), 256, 0, st>>>(grad_emb, v->d_emb, n);
+    k_f32_to_bf16<<<stride_blocks(n, 8), 256, 0, st>>>(grad_emb, v->d_emb, n);
     APH_LAUNCH_OK();
   }
-  const int rc = run_cached(v->bwd_graphs, v->warm_bwd, v->stamp, v->graph_misses, nullptr, nullptr, S, 0, st, [&]() -> int {
+  const int rc = v->bwd_graphs.run(S, 0, st, [&]() -> int {
   const int D = v->D, T = v->T, Ly = v->cfg.layers, O = v->cfg.out_dim, H = v->cfg.heads;
   const int M = S * T;
   int e;
@@ -417,8 +417,8 @@ static int vit_bwd_impl(aph_vit* vit, const float* grad_emb, int S, int side, fl
     if (int e = launch_gemm(v->d_tok, v->w_conv_t, GemmShape{Mp, v->Kp, v->D}, ep, st)) return e;
     if (sized) {
       const size_t n = (size_t)S * 3 * side * side;
-      k_window_expand<<<(unsigned)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16), 256, 0, st>>>((const float*)g_win.p, grad_images,
-                                                                                                            S * 3, R, side);
+      k_window_expand<<<stride_blocks(n, 16), 256, 0, st>>>((const float*)g_win.p, grad_images,
+                                                            S * 3, R, side);
       APH_LAUNCH_OK();
     }
   }

@@ -530,24 +530,18 @@ template <int NT2>
 static int attn_launch1(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_or_dqkv, int S, int T, int D, int heads, cudaStream_t st) {
   constexpr size_t smem_f = (size_t)2 * (2 * NT2 * 16 + 64) * 128 + 1024;                                // + alignment slack
   constexpr size_t smem_b = (size_t)2 * (2 * NT2 * 16 + 128) * 128 + (size_t)2 * 64 * 128 + 1024;
-  static bool cfg = false;
-  if (!cfg) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd_tc1<NT2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_f));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_bwd_tc1<NT2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_b));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd_tc1<NT2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_bwd_tc1<NT2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    cfg = true;
-  }
   const int items = S * heads;
   CUtensorMap tm_kv, tm_q, tm_do;
   if (int e = make_tmap_bf16_tokens(&tm_kv, qkv, 3 * D, T, S, NT2 * 16)) return e;
   if (int e = make_tmap_bf16_tokens(&tm_q, qkv, 3 * D, T, S, 64)) return e;
   if (fwd) {
+    if (int e = smem_at_least((const void*)k_attn_fwd_tc1<NT2>, smem_f, true)) return e;
     const int per_sm = (int)(220 * 1024 / smem_f) < 6 ? (int)(220 * 1024 / smem_f) : 6;
     const int grid = items < num_sms() * per_sm ? items : num_sms() * per_sm;
     k_attn_fwd_tc1<NT2><<<grid, 128, smem_f, st>>>(tm_kv, tm_q, out_or_dqkv, T, D, heads, items);
   } else {
     if (int e = make_tmap_bf16_tokens(&tm_do, dout, D, T, S, 64)) return e;
+    if (int e = smem_at_least((const void*)k_attn_bwd_tc1<NT2>, smem_b, true)) return e;
     const int per_sm = (int)(220 * 1024 / smem_b) < 3 ? (int)(220 * 1024 / smem_b) : 3;
     const int grid = items < num_sms() * per_sm ? items : num_sms() * per_sm;
     k_attn_bwd_tc1<NT2><<<grid, 128, smem_b, st>>>(tm_kv, tm_q, tm_do, out_or_dqkv, T, D, heads, items);
@@ -564,16 +558,13 @@ template <int NW, int NT2> constexpr size_t attn_tc_bwd_smem() {
 // Host launch of one (warps, key-tile) shape of the one-CTA-per-(sample, head) kernels; attn_dispatch picks it from T.
 template <int NW, int NT2>
 static int attn_launch(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_or_dqkv, int S, int T, int D, int heads, cudaStream_t st) {
-  static bool cfg = false;
-  if (!cfg) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd_tc<NW, NT2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_tc_fwd_smem<NW, NT2>()));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_bwd_tc<NW, NT2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attn_tc_bwd_smem<NW, NT2>()));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_fwd_tc<NW, NT2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    APH_CUDA_OK(cudaFuncSetAttribute(k_attn_bwd_tc<NW, NT2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    cfg = true;
+  if (fwd) {
+    if (int e = smem_at_least((const void*)k_attn_fwd_tc<NW, NT2>, attn_tc_fwd_smem<NW, NT2>(), true)) return e;
+    k_attn_fwd_tc<NW, NT2><<<S * heads, NW * 32, attn_tc_fwd_smem<NW, NT2>(), st>>>(qkv, out_or_dqkv, T, D, heads);
+  } else {
+    if (int e = smem_at_least((const void*)k_attn_bwd_tc<NW, NT2>, attn_tc_bwd_smem<NW, NT2>(), true)) return e;
+    k_attn_bwd_tc<NW, NT2><<<S * heads, NW * 32, attn_tc_bwd_smem<NW, NT2>(), st>>>(qkv, dout, out_or_dqkv, T, D, heads);
   }
-  if (fwd) k_attn_fwd_tc<NW, NT2><<<S * heads, NW * 32, attn_tc_fwd_smem<NW, NT2>(), st>>>(qkv, out_or_dqkv, T, D, heads);
-  else k_attn_bwd_tc<NW, NT2><<<S * heads, NW * 32, attn_tc_bwd_smem<NW, NT2>(), st>>>(qkv, dout, out_or_dqkv, T, D, heads);
   APH_LAUNCH_OK();
   return 0;
 }

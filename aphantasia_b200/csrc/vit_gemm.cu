@@ -1,7 +1,9 @@
 // vit_gemm.cu -- host side of the wgmma GEMM (tensor-map encoding, launch) + the exported test entry.
 #include "tc_gemm.cuh"
+#include <algorithm>
 #include <atomic>
-#include <mutex>
+#include <initializer_list>
+#include <string>
 #include <vector>
 #include <utility>
 
@@ -11,67 +13,57 @@ typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                   CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-static EncodeTiledFn get_encode() {
-  static EncodeTiledFn fn = nullptr;
-  static std::once_flag once;
-  std::call_once(once, [] {
+// Encodes the tensor map of a bf16 tensor (or of the 16-bit view of an fp32 one) with the 128-byte swizzle the kernels' shared-memory
+// tiles assume. Dimensions and box are innermost first; `strides` are the byte strides of the outer dimensions. Boxes that reach
+// past the tensor's bounds arrive zero-filled.
+static int encode_tmap(CUtensorMap* out, const void* base, std::initializer_list<int64_t> dims, std::initializer_list<int64_t> strides,
+                       std::initializer_list<int> box) {
+  static const EncodeTiledFn enc = [] {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
-  });
-  return fn;
+    const bool ok = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess;
+    return ok ? reinterpret_cast<EncodeTiledFn>(p) : nullptr;
+  }();
+  APH_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
+  const int rank = (int)dims.size();
+  cuuint64_t gdim[5], gstride[4];
+  cuuint32_t gbox[5];
+  const cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  std::copy(dims.begin(), dims.end(), gdim);
+  std::copy(strides.begin(), strides.end(), gstride);
+  std::copy(box.begin(), box.end(), gbox);
+  auto shape = [&] {                 // "tensor [S x T x cols], box [1 x 64 x 64]": outermost first
+    std::string s = "tensor [";
+    for (int i = rank - 1; i >= 0; --i) s += std::to_string(gdim[i]) + (i ? " x " : "], box [");
+    for (int i = rank - 1; i >= 0; --i) s += std::to_string(gbox[i]) + (i ? " x " : "]");
+    return s;
+  };
+  bool aligned = (reinterpret_cast<uintptr_t>(base) & 15) == 0;
+  for (int i = 0; i < rank - 1; ++i) aligned = aligned && gstride[i] % 16 == 0;
+  APH_REQUIRE(aligned, "tensor map of %s: base or stride not 16-byte aligned", shape().c_str());
+  const CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, rank, const_cast<void*>(base), gdim, gstride, gbox, estr,
+                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  APH_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed: CUresult %d (%s)", (int)r, shape().c_str());
+  return 0;
 }
 
 int make_tmap_bf16(CUtensorMap* out, const void* base, int rows, int K, int box_rows, int64_t row_stride) {
-  EncodeTiledFn enc = get_encode();
-  APH_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
   if (row_stride == 0) row_stride = K;
   APH_REQUIRE(row_stride >= K, "tensor map: row stride %lld < K=%d", (long long)row_stride, K);
-  APH_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && row_stride % 8 == 0, "tensor map: base/stride not 16-byte aligned");
-  const cuuint64_t gdim[2] = {(cuuint64_t)K, (cuuint64_t)rows};
-  const cuuint64_t gstride[1] = {(cuuint64_t)row_stride * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)GEMM_BK, (cuuint32_t)box_rows};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  APH_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled failed: CUresult %d (rows=%d K=%d box_rows=%d)", (int)r, rows, K, box_rows);
-  return 0;
+  return encode_tmap(out, base, {K, rows}, {row_stride * 2}, {GEMM_BK, box_rows});
 }
 
 // 3-D view [S][T][cols] of a token-major bf16 matrix [S*T, cols]: a box of `box_rows` tokens x 64 columns of ONE sample; rows past T
 // are out of bounds in the T dimension and arrive zero-filled (the attention kernels rely on that for their padded tiles).
 int make_tmap_bf16_tokens(CUtensorMap* out, const void* base, int cols, int T, int S, int box_rows) {
-  EncodeTiledFn enc = get_encode();
-  APH_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
-  APH_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && cols % 8 == 0, "tensor map: base/stride not 16-byte aligned");
-  const cuuint64_t gdim[3] = {(cuuint64_t)cols, (cuuint64_t)T, (cuuint64_t)S};
-  const cuuint64_t gstride[2] = {(cuuint64_t)cols * 2, (cuuint64_t)T * cols * 2};
-  const cuuint32_t box[3] = {64u, (cuuint32_t)box_rows, 1u};
-  const cuuint32_t estr[3] = {1, 1, 1};
-  const CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(base), gdim, gstride, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  APH_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (tokens) failed: CUresult %d (cols=%d T=%d S=%d box_rows=%d)", (int)r, cols, T, S, box_rows);
-  return 0;
+  return encode_tmap(out, base, {cols, T, S}, {(int64_t)cols * 2, (int64_t)T * cols * 2}, {64, box_rows, 1});
 }
 
 // 4-D view of an NHWC activation for the 3x3 convolution (conv_tc.cuh): the producer loads the box at coordinates shifted by the
 // tap's (dy, dx), and the rows / columns outside the image arrive zero-filled, which is the convolution's padding 1.
 int make_tmap_bf16_nhwc(CUtensorMap* out, const void* base, int N, int H, int W, int C, int box_h, int box_w) {
-  EncodeTiledFn enc = get_encode();
-  APH_REQUIRE(enc != nullptr, "cuTensorMapEncodeTiled not available from the driver");
-  APH_REQUIRE((reinterpret_cast<uintptr_t>(base) & 15) == 0 && C % 64 == 0, "tensor map (NHWC): base not 16-byte aligned or C=%d not a multiple of 64", C);
-  const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  const cuuint64_t gstride[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-  const cuuint32_t box[4] = {64u, (cuuint32_t)box_w, (cuuint32_t)box_h, 1u};
-  const cuuint32_t estr[4] = {1, 1, 1, 1};
-  const CUresult r = enc(out, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(base), gdim, gstride, box, estr,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  APH_REQUIRE(r == CUDA_SUCCESS, "cuTensorMapEncodeTiled (NHWC) failed: CUresult %d (N=%d H=%d W=%d C=%d)", (int)r, N, H, W, C);
-  return 0;
+  return encode_tmap(out, base, {C, W, H, N}, {(int64_t)C * 2, (int64_t)W * C * 2, (int64_t)H * W * C * 2}, {64, box_w, box_h, 1});
 }
 
 // ---- optional per-launch event timing (bench.py's roofline: the GEMM kernel's real time inside a step)
@@ -90,11 +82,7 @@ static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi
   using L = GemmCfg<BN>;
   static_assert(L::SMEM <= 227 * 1024, "GEMM shared-memory budget");
   g_variant_launches[(PINGPONG || BN == 256) ? 1 : 0][EPI].fetch_add(1, std::memory_order_relaxed);
-  static bool configured = false;
-  if (!configured) {
-    APH_CUDA_OK(cudaFuncSetAttribute(k_gemm_bf16_tn<BN, PINGPONG, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, L::SMEM));
-    configured = true;
-  }
+  if (int e = smem_at_least((const void*)k_gemm_bf16_tn<BN, PINGPONG, EPI>, L::SMEM)) return e;
   CUtensorMap ma, mb;
   if (int e = make_tmap_bf16(&ma, A, shp.M, shp.K, GEMM_BM, lda)) return e;
   if (int e = make_tmap_bf16(&mb, B, shp.N, shp.K, BN)) return e;

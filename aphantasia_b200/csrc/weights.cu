@@ -6,8 +6,6 @@
 
 namespace aph {
 
-static int pack_grid(size_t n) { return (int)std::min<size_t>((n + 255) / 256, (size_t)num_sms() * 16); }
-
 // ld: row stride of the untransposed output (>= cols; the columns past cols are not written)
 __global__ void __launch_bounds__(256) k_pack_weight(const float* __restrict__ in, bf16* __restrict__ out, int rows, int cols, int transpose, int ld) {
   const size_t n = (size_t)rows * cols;
@@ -30,13 +28,13 @@ __global__ void k_pack_w(const float* __restrict__ w, int Co, int Ci, bf16* __re
 }
 
 static int pack(const float* src, bf16* dst, int rows, int cols, int transpose, int ld, cudaStream_t st) {
-  k_pack_weight<<<pack_grid((size_t)rows * cols), 256, 0, st>>>(src, dst, rows, cols, transpose, ld > 0 ? ld : cols);
+  k_pack_weight<<<stride_blocks((size_t)rows * cols, 16), 256, 0, st>>>(src, dst, rows, cols, transpose, ld > 0 ? ld : cols);
   APH_LAUNCH_OK();
   return 0;
 }
 
 int pack_conv3x3(const float* w, int co, int ci, bf16* wf, bf16* wb, cudaStream_t st) {
-  k_pack_w<<<pack_grid((size_t)co * ci * 9), 256, 0, st>>>(w, co, ci, wf, wb);
+  k_pack_w<<<stride_blocks((size_t)co * ci * 9, 16), 256, 0, st>>>(w, co, ci, wf, wb);
   APH_LAUNCH_OK();
   return 0;
 }
