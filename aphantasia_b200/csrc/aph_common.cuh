@@ -162,6 +162,31 @@ __device__ __forceinline__ double warp_sum_d(double v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// dst[k] += the block's sum of v[k], k < N, in fp64: each warp sums by shuffles, thread 0 adds the warps in index order, and one
+// atomicAdd per value. Every thread of the block must call it (it synchronises), and the block must have at most 256 threads:
+// every caller is __launch_bounds__(256) and launched with 256.
+template <int N>
+__device__ __forceinline__ void block_atomic_add_d(const double (&v)[N], double* dst) {
+  double w[N];
+#pragma unroll
+  for (int k = 0; k < N; ++k) w[k] = warp_sum_d(v[k]);
+  __shared__ double red[N][8];
+  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (lane == 0) {
+#pragma unroll
+    for (int k = 0; k < N; ++k) red[k][wid] = w[k];
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t[N] = {};
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) {
+#pragma unroll
+      for (int k = 0; k < N; ++k) t[k] += red[k][i];
+    }
+#pragma unroll
+    for (int k = 0; k < N; ++k) atomicAdd(&dst[k], t[k]);
+  }
+}
 __device__ __forceinline__ float warp_max(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));

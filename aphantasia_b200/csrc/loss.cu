@@ -76,16 +76,7 @@ __global__ void __launch_bounds__(256) k_derivat_fwd(const float* __restrict__ i
     if (x + 1 < W) sx += fabsf(img[i + 1] - v);
     if (y + 1 < H) sy += fabsf(img[i + W] - v);
   }
-  sx = warp_sum_d(sx); sy = warp_sum_d(sy);
-  __shared__ double red[2][8];
-  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) { red[0][wid] = sx; red[1][wid] = sy; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double a = 0., b = 0.;
-    for (int i = 0; i < 8; ++i) { a += red[0][i]; b += red[1][i]; }
-    atomicAdd(&sums[0], a); atomicAdd(&sums[1], b);
-  }
+  block_atomic_add_d({sx, sy}, sums);
 }
 __global__ void k_derivat_fin(const double* __restrict__ sums, double nx, double ny, float* __restrict__ value) {
   *value = (float)(0.5 * (sums[0] / nx + sums[1] / ny));
@@ -131,16 +122,7 @@ __global__ void __launch_bounds__(256) k_derivat_sobel_fwd(const float* __restri
     sobel_at(img + c * hw, H, W, y, x, gx, gy);
     s += fabsf(gx) + fabsf(gy);
   }
-  s = warp_sum_d(s);
-  __shared__ double red[8];
-  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) red[wid] = s;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double a = 0.;
-    for (int i = 0; i < 8; ++i) a += red[i];
-    atomicAdd(&sums[0], a);
-  }
+  block_atomic_add_d({s}, sums);
 }
 __global__ void k_derivat_sobel_fin(const double* __restrict__ sums, double n, float* __restrict__ value) { *value = (float)(sums[0] / n); }
 // Adjoint: pixel (yy, xx) gathers sign(g) k from every output (y, x) within one pixel whose clamped tap lands on it (several

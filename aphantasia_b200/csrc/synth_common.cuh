@@ -1,5 +1,8 @@
-// synth_common.cuh -- pointwise tail shared by the FFT and DWT synthesis: normalise by the global std, colour-
-// decorrelate, sigmoid (to_valid_rgb, /root/reference/aphantasia/image.py:21-28 fused with image.py:68,174) and its adjoint.
+// synth_common.cuh -- the pointwise tail of every image generator (FFT, DWT, pixel) and of aph_valid_rgb_*: normalise by the
+// global std, colour-decorrelate, sigmoid (to_valid_rgb, aphantasia/image.py:21-28 fused with image.py:68,174), and its adjoint.
+//   k_finish<NORM> : out = sigmoid(Mn . (x * contrast / sigma)); without NORM, out = sigmoid(Mn . x) and stats is not read
+//   k_finish_bwd   : g_img = Mn^T . (g * out * (1 - out)); accumulates sum g_img . x into stats[2]
+//   k_norm_bwd     : g_x = adjoint of the normalisation, from stats (the FFT fuses it into its row pass, k_row_r2c)
 #pragma once
 #include "aph_common.cuh"
 #include <math.h>
@@ -8,13 +11,18 @@ namespace aph {
 
 struct ColMat { float m[9]; int use; };
 
+template <bool NORM>
 static __global__ void __launch_bounds__(256) k_finish(const float* __restrict__ x_raw, const double* __restrict__ stats,
                                                 float* __restrict__ out, size_t hw, float contrast, ColMat cm, int sig) {
-  const double Nn = 3.0 * (double)hw;
-  const double var = (stats[1] - stats[0] * stats[0] / Nn) / (Nn - 1.0);
-  const float s = (float)((double)contrast / sqrt(var));
+  float s = 1.f;
+  if (NORM) {
+    const double Nn = 3.0 * (double)hw;
+    const double var = (stats[1] - stats[0] * stats[0] / Nn) / (Nn - 1.0);
+    s = (float)((double)contrast / sqrt(var));
+  }
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < hw; i += (size_t)gridDim.x * blockDim.x) {
-    const float a = x_raw[i] * s, b = x_raw[hw + i] * s, c = x_raw[2 * hw + i] * s;
+    float a = x_raw[i], b = x_raw[hw + i], c = x_raw[2 * hw + i];
+    if (NORM) { a *= s; b *= s; c *= s; }
     float o0 = a, o1 = b, o2 = c;
     if (cm.use) {
       o0 = cm.m[0] * a + cm.m[1] * b + cm.m[2] * c;
@@ -46,18 +54,20 @@ static __global__ void __launch_bounds__(256) k_finish_bwd(const float* __restri
     gimg[i] = a; gimg[hw + i] = b; gimg[2 * hw + i] = c;
     if (x_raw) dot += (double)a * x_raw[i] + (double)b * x_raw[hw + i] + (double)c * x_raw[2 * hw + i];
   }
-  if (x_raw) {
-    dot = warp_sum_d(dot);
-    __shared__ double red[8];
-    const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (lane == 0) red[wid] = dot;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double t = 0.;
-      for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += red[i];
-      atomicAdd(&stats[2], t);
-    }
-  }
+  if (x_raw) block_atomic_add_d({dot}, stats + 2);
+}
+
+// g_x = (c/sigma) (g_img - (x - mu) * dot / ((N-1) sigma^2))      (adjoint of img = x * c / std(x), SURVEY.md A1)
+static __global__ void __launch_bounds__(256) k_norm_bwd(const float* gimg, const float* __restrict__ x_raw,
+                                                  const double* __restrict__ stats, float* gx, size_t n, float contrast) {   // gimg may alias gx
+  const double Nn = (double)n;
+  const double mu = stats[0] / Nn;
+  const double var = (stats[1] - stats[0] * stats[0] / Nn) / (Nn - 1.0);
+  const float c_sig = (float)((double)contrast / sqrt(var));
+  const float kk = (float)(stats[2] / ((Nn - 1.0) * var));
+  const float muf = (float)mu;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    gx[i] = c_sig * (gimg[i] - (x_raw[i] - muf) * kk);
 }
 
 static inline ColMat make_colmat(const float* host) {

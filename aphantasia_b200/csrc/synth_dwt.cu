@@ -119,18 +119,7 @@ __global__ void __launch_bounds__(256) k_dwt_level_fwd(const float* __restrict__
     out[idx] = acc;
     if (stats) { s1 += acc; s2 += (double)acc * acc; }
   }
-  if (stats) {
-    s1 = warp_sum_d(s1); s2 = warp_sum_d(s2);
-    __shared__ double red[2][8];
-    const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    if (lane == 0) { red[0][wid] = s1; red[1][wid] = s2; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      double t1 = 0., t2 = 0.;
-      for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { t1 += red[0][i]; t2 += red[1][i]; }
-      atomicAdd(&stats[0], t1); atomicAdd(&stats[1], t2);
-    }
-  }
+  if (stats) block_atomic_add_d({s1, s2}, stats);
 }
 
 // Adjoint: d_ll [3][llh_alloc][llw] (zero outside h x w), d_bands [3][3][h][w] (already multiplied by s) from d_out [3][oh][ow].
@@ -164,33 +153,11 @@ __global__ void __launch_bounds__(256) k_dwt_level_bwd(const float* __restrict__
   }
 }
 
-// g_x = (c/sigma) (g_img - (x - mu) * dot / ((N-1) sigma^2))      (adjoint of img = x * c / std(x), SURVEY.md A1)
-__global__ void __launch_bounds__(256) k_norm_bwd(const float* gimg, const float* __restrict__ x_raw,
-                                                  const double* __restrict__ stats, float* gx, size_t n, float contrast) {   // gimg may alias gx
-  const double Nn = (double)n;
-  const double mu = stats[0] / Nn;
-  const double var = (stats[1] - stats[0] * stats[0] / Nn) / (Nn - 1.0);
-  const float c_sig = (float)((double)contrast / sqrt(var));
-  const float kk = (float)(stats[2] / ((Nn - 1.0) * var));
-  const float muf = (float)mu;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    gx[i] = c_sig * (gimg[i] - (x_raw[i] - muf) * kk);
-}
-
 // sum x, sum x^2 over n floats -> stats[0], stats[1] (fp64 atomics)
 __global__ void __launch_bounds__(256) k_stats(const float* __restrict__ x, size_t n, double* __restrict__ stats) {
   double s1 = 0., s2 = 0.;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) { const float v = x[i]; s1 += v; s2 += (double)v * v; }
-  s1 = warp_sum_d(s1); s2 = warp_sum_d(s2);
-  __shared__ double red[2][8];
-  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) { red[0][wid] = s1; red[1][wid] = s2; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t1 = 0., t2 = 0.;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { t1 += red[0][i]; t2 += red[1][i]; }
-    atomicAdd(&stats[0], t1); atomicAdd(&stats[1], t2);
-  }
+  block_atomic_add_d({s1, s2}, stats);
 }
 __global__ void k_fix_stats(double* stats, double n, double sigma) { stats[0] = 0.; stats[1] = sigma * sigma * (n - 1.0); stats[2] = 0.; }
 
@@ -255,7 +222,7 @@ extern "C" int aph_synth_dwt_fwd(aph_dwt_plan* plan, const float* const* Ys, con
     APH_LAUNCH_OK();
   }
   const size_t hw = (size_t)p->oh[0] * p->ow[0];
-  k_finish<<<stride_blocks(hw, 16), 256, 0, st>>>(x_raw, stats, out, hw, contrast, make_colmat(colmat_host), apply_sigmoid);
+  k_finish<true><<<stride_blocks(hw, 16), 256, 0, st>>>(x_raw, stats, out, hw, contrast, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
   return 0;
 }
@@ -322,7 +289,7 @@ extern "C" int aph_pixel_fwd(const float* x, int64_t hw, float contrast, int fix
   if (fixcontrast) k_fix_stats<<<1, 1, 0, st>>>(stats, 3.0 * (double)hw, 3.3);       // sigma := 3.3 (image.py:115)
   else k_stats<<<stride_blocks(3 * (size_t)hw, 16), 256, 0, st>>>(x, 3 * (size_t)hw, stats);
   APH_LAUNCH_OK();
-  k_finish<<<stride_blocks((size_t)hw, 16), 256, 0, st>>>(x, stats, out, (size_t)hw, contrast, make_colmat(colmat_host), apply_sigmoid);
+  k_finish<true><<<stride_blocks((size_t)hw, 16), 256, 0, st>>>(x, stats, out, (size_t)hw, contrast, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
   return 0;
 }

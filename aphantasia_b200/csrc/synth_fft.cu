@@ -13,8 +13,8 @@
 //                 bwd: loads dT, forward DFT, writes dP = scale * dZ.
 //   k_row_c2r   : one CTA = a few row PAIRS; two real rows are recovered from ONE complex length-W
 //                 inverse DFT (z = a + i b); writes x_raw and accumulates sum x, sum x^2 (fp64).
-//   k_finish    : out = sigmoid(Mn . (x*contrast/sigma))                       (pointwise)
-//   k_finish_bwd: g_img = Mn^T . (g*out*(1-out)); accumulates sum g_img.x      (pointwise)
+//   k_finish<true> / k_finish_bwd (synth_common.cuh): the pointwise tail, out = sigmoid(Mn . (x*contrast/sigma)) and
+//                 g_img = Mn^T . (g*out*(1-out)); accumulates sum g_img.x
 //   k_row_r2c   : g_x = (c/sigma)(g_img - (x-mu) * dot/((N-1) sigma^2)) formed on load; two real rows
 //                 per complex forward DFT; interior columns x2; writes dT.
 //   k_row_rfft  : analysis row pass (image-file resume): plain load of the image, two real rows per complex forward DFT,
@@ -314,16 +314,7 @@ __global__ void __launch_bounds__(256) k_row_c2r(const float2* __restrict__ T, f
     s1 += a; s2 += (double)a * a;
     if (r1 < H) { x_raw[((size_t)ch * H + r1) * W + n] = b; s1 += b; s2 += (double)b * b; }
   }
-  s1 = warp_sum_d(s1); s2 = warp_sum_d(s2);
-  __shared__ double red[2][8];
-  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) { red[0][wid] = s1; red[1][wid] = s2; }
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    double t1 = 0., t2 = 0.;
-    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) { t1 += red[0][i]; t2 += red[1][i]; }
-    atomicAdd(&stats[0], t1); atomicAdd(&stats[1], t2);
-  }
+  block_atomic_add_d({s1, s2}, stats);
 }
 
 // Row pass, forward (backward of the synthesis): builds g_x on load, writes dT [3][H][Wh] complex.
@@ -499,7 +490,7 @@ extern "C" int aph_synth_fft_fwd(aph_fft_plan* plan, const float* params, const 
   APH_LAUNCH_OK();
   const size_t hw = (size_t)H * W;
   const int blocks = stride_blocks(hw, 8);
-  k_finish<<<blocks, 256, 0, st>>>(x_raw, stats, out, hw, contrast, make_colmat(colmat_host), apply_sigmoid);
+  k_finish<true><<<blocks, 256, 0, st>>>(x_raw, stats, out, hw, contrast, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
   return 0;
 }
@@ -577,25 +568,10 @@ extern "C" int aph_un_rgb(const uint8_t* hwc, int H, int W, const float* inv_col
   return 0;
 }
 
-namespace aph {
-__global__ void __launch_bounds__(256) k_rgb_fwd(const float* __restrict__ img, float* __restrict__ out, size_t hw, ColMat cm) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < hw; i += (size_t)gridDim.x * blockDim.x) {
-    const float a = img[i], b = img[hw + i], c = img[2 * hw + i];
-    float o0 = a, o1 = b, o2 = c;
-    if (cm.use) {
-      o0 = cm.m[0] * a + cm.m[1] * b + cm.m[2] * c;
-      o1 = cm.m[3] * a + cm.m[4] * b + cm.m[5] * c;
-      o2 = cm.m[6] * a + cm.m[7] * b + cm.m[8] * c;
-    }
-    out[i] = 1.f / (1.f + expf(-o0)); out[hw + i] = 1.f / (1.f + expf(-o1)); out[2 * hw + i] = 1.f / (1.f + expf(-o2));
-  }
-}
-}  // namespace aph
-
 extern "C" int aph_valid_rgb_fwd(const float* img, int64_t hw, const float* colmat_host, float* out, void* stream) {
   APH_REQUIRE(img && out && hw > 0, "aph_valid_rgb_fwd: bad arguments");
   const int blocks = stride_blocks((size_t)hw, 8);
-  k_rgb_fwd<<<blocks, 256, 0, (cudaStream_t)stream>>>(img, out, (size_t)hw, make_colmat(colmat_host));
+  k_finish<false><<<blocks, 256, 0, (cudaStream_t)stream>>>(img, nullptr, out, (size_t)hw, 1.f, make_colmat(colmat_host), 1);
   APH_LAUNCH_OK();
   return 0;
 }

@@ -200,7 +200,15 @@ def _shared_fft_scale(h, w, decay_power):
     return scale
 
 
-class FFTImage:
+class _Generator:
+    """An `image_f` closure as a callable object. Its fused(colmat, sigmoid, *args, **kwargs) parses the closure's arguments
+    and runs the synthesis with to_valid_rgb's colour matrix and sigmoid fused into its last kernel; a plain call has neither."""
+
+    def __call__(self, *args, **kwargs):
+        return self.fused(None, False, *args, **kwargs)
+
+
+class FFTImage(_Generator):
     """The `image_f` closure of fft_image (image.py:164-175) as a callable object, so to_valid_rgb can fuse into it."""
 
     def __init__(self, params, h, w, decay_power):
@@ -211,13 +219,10 @@ class FFTImage:
         from .optim import register_generator
         register_generator(params, self)
 
-    def fused(self, shift, contrast, colmat, sigmoid):
+    def fused(self, colmat, sigmoid, /, shift=None, contrast=1., *noargs, **nokwargs):
         if torch.is_grad_enabled() and self.params.requires_grad:
             self.pending_fwd += 1
         return _SynthFFT.apply(self.params, self, shift, contrast, colmat, sigmoid)
-
-    def __call__(self, shift=None, contrast=1., *noargs, **nokwargs):
-        return self.fused(shift, contrast, None, False)
 
 
 def resume_fft(resume=None, shape=None, decay=None, colors=1.6, sd=0.01):
@@ -286,17 +291,14 @@ class _SynthPixel(torch.autograd.Function):
         return gx, None, None, None, None
 
 
-class PixelImage:
+class PixelImage(_Generator):
     """The `image_f` closure of pixel_image (image.py:112-118) as a callable object (fusable by to_valid_rgb)."""
 
     def __init__(self, image_t):
         self.image_t = image_t
 
-    def fused(self, shift, contrast, colmat, sigmoid, fixcontrast=False):
+    def fused(self, colmat, sigmoid, /, shift=None, contrast=1., fixcontrast=False, *noargs, **nokwargs):
         return _SynthPixel.apply(self.image_t, contrast, fixcontrast, colmat, sigmoid)
-
-    def __call__(self, shift=None, contrast=1., fixcontrast=False):
-        return self.fused(shift, contrast, None, False, fixcontrast)
 
 
 def pixel_image(shape, resume=None, sd=1., *noargs, **nokwargs):
@@ -360,12 +362,8 @@ def to_valid_rgb(image_f, colors=1., decorrelate=True):
     colmat = _color_matrix_host(colors) if decorrelate else None
 
     def inner(*args, **kwargs):
-        if isinstance(image_f, (FFTImage, DWTImage, PixelImage)):
-            shift = args[0] if len(args) > 0 else kwargs.get('shift', None)
-            contrast = args[1] if len(args) > 1 else kwargs.get('contrast', 1.)
-            if isinstance(image_f, PixelImage):
-                return _maybe_preview(image_f.fused(shift, contrast, colmat, True, args[2] if len(args) > 2 else kwargs.get('fixcontrast', False)))
-            return _maybe_preview(image_f.fused(shift, contrast, colmat, True))
+        if isinstance(image_f, _Generator):
+            return _maybe_preview(image_f.fused(colmat, True, *args, **kwargs))
         return _ValidRGB.apply(image_f(*args, **kwargs), colmat)
     return inner
 
@@ -400,7 +398,7 @@ class _SynthDWT(torch.autograd.Function):
         return (None, None, None, None) + tuple(grads)
 
 
-class DWTImage:
+class DWTImage(_Generator):
     """The `image_f` closure of dwt_image (image.py:66-69) as a callable object (fusable by to_valid_rgb)."""
 
     def __init__(self, shape, wave, sharp):
@@ -423,11 +421,8 @@ class DWTImage:
         hJ, wJ = self.level_hw[-1]
         return [(1, 3, hJ, wJ)] + [(1, 3, 3, hh, ww) for (hh, ww) in self.level_hw]
 
-    def fused(self, shift, contrast, colmat, sigmoid):
+    def fused(self, colmat, sigmoid, /, shift=None, contrast=1., *noargs, **nokwargs):
         return _SynthDWT.apply(self, contrast, colmat, sigmoid, *self.Ys)
-
-    def __call__(self, shift=None, contrast=1.):
-        return self.fused(shift, contrast, None, False)
 
 
 def _dwt_scales(level_hw, sharp):
