@@ -52,6 +52,19 @@ _SIGS = {
     'aph_vit_fwd_sized': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, C.c_void_p]),
     'aph_vit_bwd_sized': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     'aph_vit_bytes': (C.c_int64, [C.c_void_p]),
+    'aph_rn_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p]),
+    'aph_rn_destroy': (C.c_int, [C.c_void_p]),
+    'aph_rn_load_tensor': (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.c_int64, C.c_void_p]),
+    'aph_rn_finalize': (C.c_int, [C.c_void_p]),
+    'aph_rn_fwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_int, C.c_void_p]),
+    'aph_rn_bwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_void_p]),
+    'aph_rn_bytes': (C.c_int64, [C.c_void_p]),
+    'aph_rn_saved_test': (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
+    'aph_rn_stem_test': (C.c_int, [C.c_int, C.c_void_p, c_f32p, c_f32p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    'aph_rn_pool_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    'aph_rn_tokens_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    'aph_gemm_rn_epi_test': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_void_p, C.c_void_p, C.c_int,
+                                       C.c_void_p, C.c_void_p]),
     'aph_text_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p]),
     'aph_text_destroy': (C.c_int, [C.c_void_p]),
     'aph_text_load_tensor': (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.c_int64, C.c_void_p]),
@@ -104,6 +117,10 @@ EXPORTS = tuple(_SIGS)
 
 class VitConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ('patch', 'width', 'layers', 'heads', 'out_dim', 'res', 'max_batch', 'reserved')]
+
+
+class RnConfig(C.Structure):
+    _fields_ = [('layers', C.c_int32 * 4)] + [(n, C.c_int32) for n in ('width', 'heads', 'out_dim', 'res', 'max_batch', 'reserved')]
 
 
 class TextConfig(C.Structure):

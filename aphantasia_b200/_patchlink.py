@@ -1,7 +1,7 @@
 """Sampler -> encoder hand-over of the patch-embedding operand (SURVEY.md 2.4 k10-k12).
 
 The reference hands `slice_imgs`' fp32 batch to `model.encode_image` (/root/reference/clip_fft.py:250-254); the first thing the
-encoder does with it is the im2col of conv1. When exactly one image encoder is alive and its input resolution is the crop size,
+encoder does with it is the im2col of conv1. When exactly one image encoder is alive, it is a ViT and its input resolution is the crop size,
 the sampler's last stage writes that bf16 patch-major operand straight into the encoder handle's buffer (aph_sample_fwd_patches)
 and stamps the fp32 batch it returns; `encode_image` on that very tensor (same object, not modified in place, no other forward of
 the model in between) then skips k_patchify (aph_vit_fwd_prepatched). Anything else -- two encoders (--dualmod), a derived tensor,
@@ -26,7 +26,7 @@ def target(size, windowed=False):
     if os.environ.get('APH_PATCH_FUSE', '1') == '0':
         return None
     live = list(_consumers)
-    if len(live) != 1:
+    if len(live) != 1 or getattr(live[0], 'patch_size', 0) is None:      # a ResNet tower takes no patch operand
         return None
     r = live[0].input_resolution
     if not (r == size or (windowed and r <= size < r + live[0].patch_size)):

@@ -3,7 +3,8 @@
 `model.visual.input_resolution`.
 
 The image encoder (ViT-B/32, ViT-B/16, ViT-L/14) runs forward and data-gradient in libaphb200.so (csrc/vit.cu: wgmma
-GEMMs + fused kernels). Weights: an OpenAI state dict if `APH_CLIP_WEIGHTS=<file.pt>` is set (a TorchScript archive as
+GEMMs + fused kernels); the ResNet encoders RN50 and RN101 in csrc/rn.cu (the same GEMM and 3x3 convolution, BatchNorm folded
+on the host). Weights: an OpenAI state dict if `APH_CLIP_WEIGHTS=<file.pt>` is set (a TorchScript archive as
 OpenAI ships them, or a plain state dict), else seeded synthetic weights of the same architecture.
 The text encoder (csrc/text.cu, forward only) runs once per prompt before the optimisation loop when the weights hold
 the text tower; `tokenize` uses CLIP's BPE vocabulary from `APH_CLIP_BPE=<bpe_simple_vocab_16e6.txt.gz>` or from that
@@ -19,12 +20,15 @@ from collections import OrderedDict
 import torch
 
 from .. import _patchlink, _pool, _trace
-from .._lib import Handle, TextConfig, VitConfig, check, lib, require_cuda, stream_ptr
+from .._lib import Handle, RnConfig, TextConfig, VitConfig, check, lib, require_cuda, stream_ptr
 from ._bpe import SimpleTokenizer
 
 _MODELS = {'ViT-B/32': dict(patch=32, width=768, layers=12, heads=12, out_dim=512, res=224),
            'ViT-B/16': dict(patch=16, width=768, layers=12, heads=12, out_dim=512, res=224),
-           'ViT-L/14': dict(patch=14, width=1024, layers=24, heads=16, out_dim=768, res=224)}
+           'ViT-L/14': dict(patch=14, width=1024, layers=24, heads=16, out_dim=768, res=224),
+           'RN50': dict(layers=(3, 4, 6, 3), width=64, heads=32, out_dim=1024, res=224),
+           'RN101': dict(layers=(3, 4, 23, 3), width=64, heads=32, out_dim=512, res=224)}
+RN_SIDES = (223, 254)      # the crop sides whose ResNet map is 7 x 7 at the attention pool
 
 
 def available_models():
@@ -62,6 +66,96 @@ def synthetic_visual_state_dict(patch=32, width=768, layers=12, heads=12, out_di
         sd[p + 'mlp.c_proj.bias'] = uni((width,), (4 * width) ** -0.5)
         sd[p + 'ln_2.weight'] = torch.ones(width); sd[p + 'ln_2.bias'] = torch.zeros(width)
     return sd
+
+
+def synthetic_resnet_state_dict(layers=(3, 4, 6, 3), width=64, heads=32, out_dim=1024, res=224, seed=0):
+    """Seeded synthetic ModifiedResNet weights in the OpenAI key layout ("visual." prefix). Convolutions have He-normal weights
+    and every BatchNorm non-trivial running statistics and affine (so that a missing or wrong fold shows); the last BatchNorm of
+    each residual branch is scaled by 0.25 so that the residual stream stays of order one through 33 blocks."""
+    g = torch.Generator().manual_seed(seed)
+    embed = width * 32
+
+    def uni(shape, bound):
+        return (torch.rand(shape, generator=g) * 2 - 1) * bound
+
+    def conv(co, ci, k):
+        return torch.randn((co, ci, k, k), generator=g) * (2. / (ci * k * k)) ** 0.5
+
+    sd = OrderedDict()
+
+    def bn(p, c, scale=1.):
+        sd[p + '.weight'] = scale * (1 + uni((c,), 0.2))
+        sd[p + '.bias'] = uni((c,), 0.1)
+        sd[p + '.running_mean'] = uni((c,), 0.2)
+        sd[p + '.running_var'] = 1 + uni((c,), 0.5)
+        sd[p + '.num_batches_tracked'] = torch.tensor(0)
+    v = 'visual.'
+    for i, (ci, co) in enumerate(((3, width // 2), (width // 2, width // 2), (width // 2, width))):
+        sd[v + 'conv%d.weight' % (i + 1)] = conv(co, ci, 3)
+        bn(v + 'bn%d' % (i + 1), co)
+    cin = width
+    for i, n in enumerate(layers):
+        planes = width << i
+        for j in range(n):
+            p = v + 'layer%d.%d.' % (i + 1, j)
+            sd[p + 'conv1.weight'] = conv(planes, cin, 1); bn(p + 'bn1', planes)
+            sd[p + 'conv2.weight'] = conv(planes, planes, 3); bn(p + 'bn2', planes)
+            sd[p + 'conv3.weight'] = conv(4 * planes, planes, 1); bn(p + 'bn3', 4 * planes, 0.25)
+            if j == 0 and (i > 0 or cin != 4 * planes):
+                sd[p + 'downsample.0.weight'] = conv(4 * planes, cin, 1); bn(p + 'downsample.1', 4 * planes)
+            cin = 4 * planes
+    a = v + 'attnpool.'
+    sd[a + 'positional_embedding'] = torch.randn(((res // 32) ** 2 + 1, embed), generator=g) / embed ** 0.5
+    for n in ('q_proj', 'k_proj', 'v_proj'):
+        sd[a + n + '.weight'] = torch.randn((embed, embed), generator=g) * embed ** -0.5
+        sd[a + n + '.bias'] = uni((embed,), 0.02)
+    sd[a + 'c_proj.weight'] = torch.randn((out_dim, embed), generator=g) * embed ** -0.5
+    sd[a + 'c_proj.bias'] = uni((out_dim,), 0.02)
+    return sd
+
+
+def fold_resnet_state_dict(sd, eps=1e-5):
+    """The ResNet tower's device tensors (float64) from a ModifiedResNet state dict without the "visual." prefix: every
+    BatchNorm (running statistics, eps) folded into the convolution before it, w' = w g / sqrt(var + eps), b' = b - mean g /
+    sqrt(var + eps); the stem's 32-channel convolutions zero-padded to 64 channels; 1x1 weights as [C_out, C_in]; the attention
+    pool's q, k and v projections stacked into one [3 D, D] operand in that order. Keys: see aph_rn_load_tensor."""
+    out = OrderedDict()
+
+    def fold(conv, bn):
+        s = sd[bn + '.weight'].double() / torch.sqrt(sd[bn + '.running_var'].double() + eps)
+        w = sd[conv].double() * s.view(-1, 1, 1, 1)
+        return w, sd[bn + '.bias'].double() - sd[bn + '.running_mean'].double() * s
+    w1, b1 = fold('conv1.weight', 'bn1')
+    w2, b2 = fold('conv2.weight', 'bn2')
+    w3, b3 = fold('conv3.weight', 'bn3')
+    c, c2 = w1.shape[0], w3.shape[0]
+    out['conv1.weight'], out['conv1.bias'] = w1, b1
+    out['conv2.weight'] = torch.zeros(c2, c2, 3, 3, dtype=torch.float64); out['conv2.weight'][:c, :c] = w2
+    out['conv2.bias'] = torch.zeros(c2, dtype=torch.float64); out['conv2.bias'][:c] = b2
+    out['conv3.weight'] = torch.zeros(c2, c2, 3, 3, dtype=torch.float64); out['conv3.weight'][:, :c] = w3
+    out['conv3.bias'] = b3
+    blocks = sorted({k.rsplit('.', 2)[0] for k in sd if k.startswith('layer') and k.endswith('.conv1.weight')},
+                    key=lambda b: tuple(int(t) for t in b[len('layer'):].split('.')))
+    for b in blocks:
+        for n in ('conv1', 'conv2', 'conv3'):
+            w, bias = fold('%s.%s.weight' % (b, n), '%s.bn%s' % (b, n[-1]))
+            out['%s.%s.weight' % (b, n)] = w if n == 'conv2' else w.flatten(1)
+            out['%s.%s.bias' % (b, n)] = bias
+        if b + '.downsample.0.weight' in sd:
+            w, bias = fold(b + '.downsample.0.weight', b + '.downsample.1')
+            out[b + '.downsample.weight'], out[b + '.downsample.bias'] = w.flatten(1), bias
+    a = 'attnpool.'
+    out[a + 'positional_embedding'] = sd[a + 'positional_embedding'].double()
+    out[a + 'qkv.weight'] = torch.cat([sd[a + n + '_proj.weight'].double() for n in 'qkv'])
+    out[a + 'qkv.bias'] = torch.cat([sd[a + n + '_proj.bias'].double() for n in 'qkv'])
+    out[a + 'c_proj.weight'] = sd[a + 'c_proj.weight'].double()
+    out[a + 'c_proj.bias'] = sd[a + 'c_proj.bias'].double()
+    return out
+
+
+def is_resnet(state_dict):
+    """OpenAI's loader test for a ModifiedResNet image tower."""
+    return 'visual.layer1.0.conv1.weight' in state_dict
 
 
 _TEXT_KEYS = ('token_embedding.weight', 'positional_embedding', 'ln_final.weight', 'ln_final.bias', 'text_projection')
@@ -197,11 +291,7 @@ class _EncodeImage(torch.autograd.Function):
             vis._generation += 1            # the arena now belongs to this call; any other pending backward must recompute too
             vis.recomputes += 1
         gi = _pool.empty(ctx.shape)
-        side = ctx.shape[-1]
-        if side == vis.input_resolution:
-            check(lib().aph_vit_bwd(vis.handle, g.data_ptr(), ctx.S, gi.data_ptr(), stream_ptr()), 'aph_vit_bwd')
-        else:
-            check(lib().aph_vit_bwd_sized(vis.handle, g.data_ptr(), ctx.S, side, gi.data_ptr(), stream_ptr()), 'aph_vit_bwd_sized')
+        vis._bwd(g, ctx.S, ctx.shape[-1], gi)
         return gi, None, None
 
 
@@ -240,6 +330,12 @@ class VisionTransformer(_Tower):
             check(lib().aph_vit_fwd_sized(self.handle, xi.data_ptr(), S, side, emb.data_ptr(), save_for_bwd, stream_ptr()),
                   'aph_vit_fwd_sized')
 
+    def _bwd(self, g, S, side, gi):
+        if side == self.input_resolution:
+            check(lib().aph_vit_bwd(self.handle, g.data_ptr(), S, gi.data_ptr(), stream_ptr()), 'aph_vit_bwd')
+        else:
+            check(lib().aph_vit_bwd_sized(self.handle, g.data_ptr(), S, side, gi.data_ptr(), stream_ptr()), 'aph_vit_bwd_sized')
+
     def check_input(self, x):
         """conv1 (kernel = stride = patch, no padding) takes [S,3,side,side] with r <= side < r + patch (r = input_resolution) and
         reads its top-left r x r window: the size + 8 batches of transforms_custom / transforms_elastic. Anything else is refused."""
@@ -253,12 +349,57 @@ class VisionTransformer(_Tower):
         return _EncodeImage.apply(x, self, _patchlink.matches(x, self))
 
 
+class ModifiedResNet(_Tower):
+    """Handle-owning mirror of clip.model.ModifiedResNet (eval mode) through the C ABI, forward and data gradient. It reads the
+    whole crop: any side in RN_SIDES, 232 under transforms_custom / _elastic included. It has no patch operand, so the sampler
+    never writes one for it (_patchlink)."""
+    _api = 'aph_rn'
+    patch_size = None
+
+    def __init__(self, state_dict, max_batch=None):
+        sd = {k[len('visual.'):]: v for k, v in state_dict.items() if k.startswith('visual.')}
+        self.layers = tuple(len({k.split('.')[1] for k in sd if k.startswith('layer%d.' % i)}) for i in range(1, 5))
+        self.width = sd['conv3.weight'].shape[0]
+        self.heads = self.width * 32 // 64
+        self.output_dim = sd['attnpool.c_proj.weight'].shape[0]
+        self.input_resolution = 32 * round((sd['attnpool.positional_embedding'].shape[0] - 1) ** 0.5)
+        self._sd = OrderedDict((k, v.float().contiguous()) for k, v in fold_resnet_state_dict(sd).items())
+        self._generation, self.recomputes, self._handle_epoch = 0, 0, 0        # see _EncodeImage
+        self._patch_gen = 0
+        _patchlink.register(self)
+        if max_batch:
+            self._ensure(max_batch)
+
+    def _ensure(self, S):
+        if self.handle is not None and S <= self.max_batch:
+            return
+        self._build(RnConfig((C.c_int32 * 4)(*self.layers), self.width, self.heads, self.output_dim, self.input_resolution, int(S), 0), S)
+        self._handle_epoch += 1
+
+    def _fwd(self, xi, S, emb, save_for_bwd):
+        check(lib().aph_rn_fwd(self.handle, xi.data_ptr(), S, xi.shape[-1], emb.data_ptr(), save_for_bwd, stream_ptr()), 'aph_rn_fwd')
+
+    def _bwd(self, g, S, side, gi):
+        check(lib().aph_rn_bwd(self.handle, g.data_ptr(), S, side, gi.data_ptr(), stream_ptr()), 'aph_rn_bwd')
+
+    def check_input(self, x):
+        lo, hi = RN_SIDES
+        if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != x.shape[3] or not lo <= x.shape[2] <= hi:
+            raise ValueError('encode_image: the ResNet takes images [S, 3, side, side] with %d <= side <= %d (a 7 x 7 final map), '
+                             'got %s' % (lo, hi, tuple(x.shape)))
+
+    def __call__(self, x):
+        require_cuda(x, 'encode_image input')
+        self.check_input(x)
+        return _EncodeImage.apply(x, self, False)
+
+
 class CLIP:
     """What clip_fft.py needs from clip.model.CLIP."""
 
     def __init__(self, name, state_dict, synthetic):
         self.name, self.synthetic = name, synthetic
-        self.visual = VisionTransformer(state_dict)
+        self.visual = ModifiedResNet(state_dict) if is_resnet(state_dict) else VisionTransformer(state_dict)
         self.embed_dim = self.visual.output_dim
         self.transformer = TextTransformer(state_dict) if has_text_tower(state_dict) else None
         _trace.text_tower('cuda' if self.transformer is not None else 'stand-in')
@@ -375,7 +516,8 @@ def load(name, device=None, jit=False, download_root=None):
             print(' [aphantasia_b200.clip] WARNING: no BPE vocabulary (set APH_CLIP_BPE=<%s> or put it next to %s): prompts will be '
                   'byte-tokenized and the text encoder will not see CLIP tokens' % (VOCAB_FILE, path))
     else:
-        sd = synthetic_visual_state_dict(seed=int(os.environ.get('APH_CLIP_SEED', '0')), **_MODELS[name])
+        synth = synthetic_resnet_state_dict if name.startswith('RN') else synthetic_visual_state_dict
+        sd = synth(seed=int(os.environ.get('APH_CLIP_SEED', '0')), **_MODELS[name])
         synthetic = True
         print(' [aphantasia_b200.clip] no CLIP weights available: using seeded synthetic %s weights and seeded text embeddings' % name)
     return CLIP(name, sd, synthetic), None

@@ -3,6 +3,7 @@
 #pragma once
 #include "vit_ops.cuh"
 #include "weights.cuh"
+#include <functional>
 
 namespace aph {
 
@@ -41,5 +42,19 @@ typedef int (*AttnFwd)(const bf16* qkv, bf16* out, int S, int T, int D, int head
 // ln_1, qkv and attention run on all S*T rows, out_proj and what follows on Mr rows. out_proj reads its rows of attn_out and
 // x_in at row stride ld_tok (0: dense; the image tower's last block takes the class-token rows, Mr = S and ld_tok = T*D).
 int block_fwd(const BlockW& w, const BlockIO& io, int S, int T, int Mr, int ld_tok, int D, int heads, AttnFwd attn, cudaStream_t st);
+
+// The image towers' CUDA-graph cache (struct GraphCache, vit.cu) for a handle defined elsewhere (the ResNet tower, rn.cu):
+// replay() runs `body` through the cache exactly as the ViT's forward and backward do.
+struct GraphCache;
+struct GraphCacheRef : NoCopy {
+  GraphCache* cache;
+  GraphCacheRef();
+  ~GraphCacheRef();
+  int replay(int S, int flag, cudaStream_t& st, const std::function<int()>& body);
+};
+
+// The resident attention kernels (T <= 256, head dim 64) on qkv [S*T, 3D]: fwd writes out [S*T, D]; otherwise dout [S*T, D] in,
+// dqkv [S*T, 3D] out. Defined in vit.cu.
+int attn_resident(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_or_dqkv, int S, int T, int D, int heads, cudaStream_t st);
 
 }  // namespace aph

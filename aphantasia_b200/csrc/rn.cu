@@ -1,0 +1,558 @@
+// rn.cu -- CLIP ResNet image encoder handle (RN50, RN101): forward and data-gradient on bf16 NHWC activations.
+//
+// Restates CLIP's ModifiedResNet in eval mode, with every BatchNorm folded into the convolution before it (on the host, in
+// float64: aphantasia_b200/clip fold_resnet_state_dict), so each convolution here carries a weight and a bias:
+//   stem     conv 3x3 / 2 (3 -> 32) + ReLU, conv 3x3 (32 -> 32) + ReLU, conv 3x3 (32 -> 64) + ReLU, avgpool 2
+//   stages   (3, 4, 6, 3) or (3, 4, 23, 3) bottlenecks of planes 64, 128, 256, 512 (x 4 out); the first block of stages 2-4 has
+//            stride 2. Bottleneck: y = relu(conv3(pool(relu(conv2(relu(conv1 x))))) + id), pool = avgpool(stride) when stride > 1,
+//            id = downsample(pool(x)) (1x1 conv) when the stride or the width changes, else x
+//   attnpool 49 tokens of the 7 x 7 map, their mean prepended, + positional embedding; 32-head attention (head dim 64) queried by
+//            token 0; c_proj of its output
+// Kernels (sm_90a):
+//   stem conv 1         k_rn_stem_fwd / k_rn_stem_bwd: fp32 SIMT (3 input channels, stride 2); they read the caller's fp32 crops
+//                       and write its fp32 crop gradient, outside the cached graphs. Output channels 32-63 are zero, so the two
+//                       other stem convolutions run as 64-channel ones on zero-padded weights
+//   3x3 convolutions    k_conv3x3_tc (conv_tc.cuh), forward CONV_BIAS_RELU, data gradient CONV_MASK (select by the ReLU output)
+//   1x1 convolutions    launch_gemm on the NHWC tensor viewed as [pixels, C], epilogues EPI_BIAS_RELU / EPI_BIAS_RESID_RELU /
+//                       EPI_BIAS_BF16 forward, EPI_MASK / EPI_MASK_RESID / EPI_BF16 data gradient
+//   average pool        k_avgpool2_fwd, and its adjoint k_avgpool2_bwd fused with the select of the ReLU output below it
+//   attention pool      k_rn_tokens_fwd / _bwd, the q/k/v GEMM, attn_resident at T = 50, c_proj on the token-0 rows
+// The data gradient of a block's input is selected by that input being > 0 in the epilogue of the GEMM that writes it: every
+// block input is a ReLU output, except the first block's, the stem's average pool of a ReLU output, which is 0 exactly where its
+// four inputs are, whose gradient the stem's own ReLU select then drops anyway.
+#include "conv_tc.cuh"
+#include "encoder.cuh"
+
+namespace aph {
+
+constexpr int RN_T = 50, RN_GRID = 7;          // attention-pool tokens; the final map is 7 x 7
+constexpr int RN_SIDE_MIN = 223, RN_SIDE_MAX = 254;
+
+// ---- stem conv 1: 3 -> 32, 3x3, stride 2, pad 1, fp32 -------------------------------------------------------------
+// img fp32 NCHW [N,3,side,side] -> out bf16 NHWC [N,Ho,Ho,64] = relu(conv + bias) in channels 0-31, zero in 32-63.
+// w [32][3][3][3], b [32]. One thread per output pixel.
+__global__ void __launch_bounds__(128) k_rn_stem_fwd(const float* __restrict__ img, int N, int side, int Ho, const float* __restrict__ w,
+                                                     const float* __restrict__ b, bf16* __restrict__ out) {
+  __shared__ float sw[32 * 27], sb[32];
+  for (int i = threadIdx.x; i < 32 * 27; i += blockDim.x) sw[i] = w[i];
+  for (int i = threadIdx.x; i < 32; i += blockDim.x) sb[i] = b[i];
+  __syncthreads();
+  const size_t HW = (size_t)Ho * Ho, p = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (p >= (size_t)N * HW) return;
+  const int n = (int)(p / HW), rem = (int)(p - n * HW), oy = rem / Ho, ox = rem - oy * Ho;
+  const size_t plane = (size_t)side * side;
+  float in[27];
+#pragma unroll
+  for (int c = 0; c < 3; ++c)
+#pragma unroll
+    for (int t = 0; t < 9; ++t) {
+      const int y = 2 * oy + t / 3 - 1, x = 2 * ox + t % 3 - 1;
+      in[c * 9 + t] = (y >= 0 && y < side && x >= 0 && x < side) ? img[((size_t)n * 3 + c) * plane + (size_t)y * side + x] : 0.f;
+    }
+  uint4* o = reinterpret_cast<uint4*>(out + p * 64);
+#pragma unroll
+  for (int g = 0; g < 4; ++g) {
+    float acc[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float* wj = sw + (8 * g + j) * 27;
+      float s = sb[8 * g + j];
+#pragma unroll
+      for (int k = 0; k < 27; ++k) s = fmaf(wj[k], in[k], s);
+      acc[j] = fmaxf(s, 0.f);
+    }
+    o[g] = make_uint4(pack_bf16(acc[0], acc[1]), pack_bf16(acc[2], acc[3]), pack_bf16(acc[4], acc[5]), pack_bf16(acc[6], acc[7]));
+  }
+#pragma unroll
+  for (int g = 4; g < 8; ++g) o[g] = make_uint4(0u, 0u, 0u, 0u);
+}
+
+// grad fp32 NCHW [N,3,side,side] (overwritten) from dz bf16 NHWC [N,Ho,Ho,64] = d loss / d (pre-ReLU stem conv 1 output); only
+// channels 0-31 are read. One thread per input pixel: output pixel (oy, ox) read it through tap (y - 2 oy + 1, x - 2 ox + 1).
+__global__ void __launch_bounds__(128) k_rn_stem_bwd(const bf16* __restrict__ dz, int N, int side, int Ho, const float* __restrict__ w,
+                                                     float* __restrict__ grad) {
+  __shared__ float sw[32 * 27];
+  for (int i = threadIdx.x; i < 32 * 27; i += blockDim.x) sw[i] = w[i];
+  __syncthreads();
+  const size_t plane = (size_t)side * side, p = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (p >= (size_t)N * plane) return;
+  const int n = (int)(p / plane), rem = (int)(p - n * plane), y = rem / side, x = rem - y * side;
+  float g[3] = {0.f, 0.f, 0.f};
+  for (int ky = 0; ky < 3; ++ky) {
+    const int ty = y + 1 - ky;
+    if (ty < 0 || (ty & 1) || ty / 2 >= Ho) continue;
+    for (int kx = 0; kx < 3; ++kx) {
+      const int tx = x + 1 - kx;
+      if (tx < 0 || (tx & 1) || tx / 2 >= Ho) continue;
+      const int t = ky * 3 + kx;
+      const uint4* src = reinterpret_cast<const uint4*>(dz + (((size_t)n * Ho + ty / 2) * Ho + tx / 2) * 64);
+#pragma unroll
+      for (int v = 0; v < 4; ++v) {
+        const uint4 u = __ldg(src + v);
+        const uint32_t wds[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+          const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wds[h]));
+          const int co = 8 * v + 2 * h;
+#pragma unroll
+          for (int c = 0; c < 3; ++c) g[c] = fmaf(f.x, sw[co * 27 + c * 9 + t], fmaf(f.y, sw[(co + 1) * 27 + c * 9 + t], g[c]));
+        }
+      }
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 3; ++c) grad[((size_t)n * 3 + c) * plane + (size_t)y * side + x] = g[c];
+}
+
+// ---- 2x2 average pool (floor), bf16 NHWC, 8 channels per item ---------------------------------------------------------------
+__device__ __forceinline__ void rn_bf16x8(const uint4& u, float* f) {
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int h = 0; h < 4; ++h) {
+    const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[h]));
+    f[2 * h] = v.x; f[2 * h + 1] = v.y;
+  }
+}
+__device__ __forceinline__ uint4 rn_pack8(const float* f) {
+  return make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
+}
+
+__global__ void __launch_bounds__(256) k_avgpool2_fwd(const bf16* __restrict__ x, int N, int H, int W, int C, bf16* __restrict__ out) {
+  const int Ho = H / 2, Wo = W / 2, C8 = C / 8;
+  const size_t n_items = (size_t)N * Ho * Wo * C8;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n_items; i += (size_t)gridDim.x * blockDim.x) {
+    const int cv = (int)(i % C8);
+    const size_t po = i / C8;
+    const int xo = (int)(po % Wo), yo = (int)((po / Wo) % Ho), n = (int)(po / ((size_t)Wo * Ho));
+    const uint4* base = reinterpret_cast<const uint4*>(x + (((size_t)n * H + 2 * yo) * W + 2 * xo) * C) + cv;
+    const size_t row = (size_t)W * C8, col = C8;
+    float s[8], f[8];
+    rn_bf16x8(__ldg(base), s);
+    const size_t offs[3] = {col, row, row + col};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      rn_bf16x8(__ldg(base + offs[k]), f);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) s[j] += f[j];
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s[j] *= 0.25f;
+    reinterpret_cast<uint4*>(out)[i] = rn_pack8(s);
+  }
+}
+
+// out [N,H,W,C] = the adjoint of dy [N,H/2,W/2,C] (dy / 4 on each of a window's pixels, zero on the row / column floor mode
+// drops), selected by mask > 0 when mask [N,H,W,C] is not null (the ReLU output whose pool this was)
+__global__ void __launch_bounds__(256) k_avgpool2_bwd(const bf16* __restrict__ dy, const bf16* __restrict__ mask, int N, int H, int W, int C,
+                                                      bf16* __restrict__ out) {
+  const int Ho = H / 2, Wo = W / 2, C8 = C / 8;
+  const size_t n_items = (size_t)N * H * W * C8;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n_items; i += (size_t)gridDim.x * blockDim.x) {
+    const int cv = (int)(i % C8);
+    const size_t p = i / C8;
+    const int x = (int)(p % W), y = (int)((p / W) % H), n = (int)(p / ((size_t)W * H));
+    float g[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    if (y < 2 * Ho && x < 2 * Wo) {
+      rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(dy + (((size_t)n * Ho + y / 2) * Wo + x / 2) * C) + cv), g);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) g[j] *= 0.25f;
+    }
+    if (mask) {
+      float m[8];
+      rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(mask) + i), m);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) g[j] = m[j] > 0.f ? g[j] : 0.f;
+    }
+    reinterpret_cast<uint4*>(out)[i] = rn_pack8(g);
+  }
+}
+
+// ---- attention-pool tokens ----------------------------------------------------------------------------------------------
+// x bf16 [S*49, C] (the last block's output, pixel-major) -> tok bf16 [S*50, C]: row 0 = mean of the 49 rows + pos[0], row 1 + i =
+// x[i] + pos[1 + i]; pos fp32 [50, C]. One item per (sample, 8 channels); the sum runs in fp32 in pixel order.
+__global__ void __launch_bounds__(256) k_rn_tokens_fwd(const bf16* __restrict__ x, const float* __restrict__ pos, int S, int C,
+                                                       bf16* __restrict__ tok) {
+  const int C8 = C / 8, P = RN_GRID * RN_GRID;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)S * C8; i += (size_t)gridDim.x * blockDim.x) {
+    const int cv = (int)(i % C8), s = (int)(i / C8);
+    float sum[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, f[8];
+    for (int r = 0; r < P; ++r) {
+      rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(x + ((size_t)s * P + r) * C) + cv), f);
+      const float* pp = pos + (size_t)(1 + r) * C + 8 * cv;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) { sum[j] += f[j]; f[j] += pp[j]; }
+      reinterpret_cast<uint4*>(tok + ((size_t)s * RN_T + 1 + r) * C)[cv] = rn_pack8(f);
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) sum[j] = sum[j] * (1.f / P) + pos[8 * cv + j];
+    reinterpret_cast<uint4*>(tok + (size_t)s * RN_T * C)[cv] = rn_pack8(sum);
+  }
+}
+
+// the adjoint: dz bf16 [S*49, C] = x > 0 ? dtok[1 + i] + dtok[0] / 49 : 0 (x, the last block's output, is a ReLU output: the
+// select is that block's ReLU, so dz is the gradient its backward starts from)
+__global__ void __launch_bounds__(256) k_rn_tokens_bwd(const bf16* __restrict__ dtok, const bf16* __restrict__ x, int S, int C,
+                                                       bf16* __restrict__ dz) {
+  const int C8 = C / 8, P = RN_GRID * RN_GRID;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)S * P * C8; i += (size_t)gridDim.x * blockDim.x) {
+    const int cv = (int)(i % C8);
+    const size_t row = i / C8;
+    const int s = (int)(row / P), r = (int)(row % P);
+    float g0[8], g[8], m[8];
+    rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(dtok + (size_t)s * RN_T * C) + cv), g0);
+    rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(dtok + ((size_t)s * RN_T + 1 + r) * C) + cv), g);
+    rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(x) + i), m);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) g[j] = m[j] > 0.f ? g[j] + g0[j] * (1.f / P) : 0.f;
+    reinterpret_cast<uint4*>(dz)[i] = rn_pack8(g);
+  }
+}
+
+// emb [S, O] = acc + bias (c_proj's bias; the GEMM writes the fp32 product)
+__global__ void __launch_bounds__(256) k_rn_emb(const float* __restrict__ acc, const float* __restrict__ bias, int S, int O, float* __restrict__ emb) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < (size_t)S * O; i += (size_t)gridDim.x * blockDim.x)
+    emb[i] = acc[i] + bias[i % O];
+}
+
+static int avgpool_fwd(const bf16* x, int N, int H, int W, int C, bf16* out, cudaStream_t st) {
+  k_avgpool2_fwd<<<stride_blocks((size_t)N * (H / 2) * (W / 2) * (C / 8), 16), 256, 0, st>>>(x, N, H, W, C, out);
+  APH_LAUNCH_OK();
+  return 0;
+}
+static int avgpool_bwd(const bf16* dy, const bf16* mask, int N, int H, int W, int C, bf16* out, cudaStream_t st) {
+  k_avgpool2_bwd<<<stride_blocks((size_t)N * H * W * (C / 8), 16), 256, 0, st>>>(dy, mask, N, H, W, C, out);
+  APH_LAUNCH_OK();
+  return 0;
+}
+static int stem_fwd(const float* img, int N, int side, int Ho, const float* w, const float* b, bf16* out, cudaStream_t st) {
+  const size_t n = (size_t)N * Ho * Ho;
+  k_rn_stem_fwd<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(img, N, side, Ho, w, b, out);
+  APH_LAUNCH_OK();
+  return 0;
+}
+static int stem_bwd(const bf16* dz, int N, int side, int Ho, const float* w, float* grad, cudaStream_t st) {
+  const size_t n = (size_t)N * side * side;
+  k_rn_stem_bwd<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(dz, N, side, Ho, w, grad);
+  APH_LAUNCH_OK();
+  return 0;
+}
+static int tokens_fwd(const bf16* x, const float* pos, int S, int C, bf16* tok, cudaStream_t st) {
+  k_rn_tokens_fwd<<<stride_blocks((size_t)S * C / 8, 16), 256, 0, st>>>(x, pos, S, C, tok);
+  APH_LAUNCH_OK();
+  return 0;
+}
+static int tokens_bwd(const bf16* dtok, const bf16* x, int S, int C, bf16* dz, cudaStream_t st) {
+  k_rn_tokens_bwd<<<stride_blocks((size_t)S * RN_GRID * RN_GRID * C / 8, 16), 256, 0, st>>>(dtok, x, S, C, dz);
+  APH_LAUNCH_OK();
+  return 0;
+}
+
+// the stem's map side (stride-2 conv, pad 1) and the side after each 2x2 pool
+inline int rn_stem_side(int side) { return (side - 1) / 2 + 1; }
+
+struct RnBlock {
+  int cin, planes, stride, hin, hout;   // hin: the input map and the 3x3 conv's; hout = hin / stride
+  bool down;
+  bf16 *w1 = nullptr, *w1_t = nullptr, *w2 = nullptr, *w2_t = nullptr, *w3 = nullptr, *w3_t = nullptr, *wd = nullptr, *wd_t = nullptr;
+  float *b1 = nullptr, *b2 = nullptr, *b3 = nullptr, *bd = nullptr;
+  bf16 *r1 = nullptr, *r2 = nullptr, *y = nullptr;   // saved: the two ReLU outputs [S hin^2, planes], the output [S hout^2, 4 planes]
+};
+
+struct RnImpl : Weights {
+  aph_rn_config cfg;
+  int D = 0;                     // 2048: the attention pool's width
+  std::vector<RnBlock> blocks;
+  float *stem_w1 = nullptr, *stem_b1 = nullptr, *stem_b2 = nullptr, *stem_b3 = nullptr;
+  bf16 *stem_w2 = nullptr, *stem_w2_t = nullptr, *stem_w3 = nullptr, *stem_w3_t = nullptr;
+  float *pos = nullptr, *b_qkv = nullptr, *b_c = nullptr;
+  bf16 *w_qkv = nullptr, *w_qkv_t = nullptr, *w_c = nullptr, *w_c_t = nullptr;
+  // activations, sized for max_batch at side RN_SIDE_MAX
+  bf16 *s1 = nullptr, *s2 = nullptr, *s3 = nullptr, *sp = nullptr;   // stem ReLU outputs [S h1^2, 64] and its pool [S h0^2, 64]
+  bf16* scratch[6] = {};         // [S emax] each: forward temporaries and the backward's gradients
+  size_t emax = 0;               // per-crop elements of the largest map (the stem's)
+  bf16 *tok = nullptr, *qkv = nullptr, *attn = nullptr;                 // [S*50, D], [S*50, 3D], [S*50, D]
+  bf16 *d_attn = nullptr, *d_qkv = nullptr, *d_tok = nullptr;           // d_attn: zeroed at creation, only rows s*50 are written
+  float* emb_int = nullptr;      // [S, out_dim]
+  bf16* d_emb = nullptr;         // [S, out_dim]
+  int last_S = -1, last_side = -1;
+  GraphCacheRef fwd_graphs, bwd_graphs;
+};
+
+// Lays out the blocks' shapes for input side `side` (the weights' shapes do not depend on it)
+static void rn_shapes(RnImpl* h, int side) {
+  int hin = rn_stem_side(side) / 2, cin = 64;
+  size_t b = 0;
+  for (int i = 0; i < 4; ++i)
+    for (int j = 0; j < h->cfg.layers[i]; ++j, ++b) {
+      RnBlock& k = h->blocks[b];
+      k.cin = cin; k.planes = 64 << i; k.stride = (i > 0 && j == 0) ? 2 : 1;
+      k.down = k.stride > 1 || cin != 4 * k.planes;
+      k.hin = hin; k.hout = hin / k.stride;
+      hin = k.hout; cin = 4 * k.planes;
+    }
+}
+
+// the launches of the forward between the stem's first convolution (s1) and the fp32 product of c_proj (emb_int)
+static int rn_fwd_body(RnImpl* h, int S, int side, cudaStream_t st) {
+  const int h1 = rn_stem_side(side), D = h->D;
+  int e;
+  ConvEpi ce;
+  ce.bias = h->stem_b2; ce.out = h->s2;
+  if ((e = launch_conv3x3(h->s1, h->stem_w2, S, h1, h1, 64, 64, CONV_BIAS_RELU, ce, st))) return e;
+  ce.bias = h->stem_b3; ce.out = h->s3;
+  if ((e = launch_conv3x3(h->s2, h->stem_w3, S, h1, h1, 64, 64, CONV_BIAS_RELU, ce, st))) return e;
+  if ((e = avgpool_fwd(h->s3, S, h1, h1, 64, h->sp, st))) return e;
+  const bf16* x = h->sp;
+  for (const RnBlock& k : h->blocks) {
+    const int P = k.planes, E = 4 * P, Min = S * k.hin * k.hin, Mo = S * k.hout * k.hout;
+    { GemmEpi ep; ep.bias = k.b1; ep.act = 2; ep.out_bf16 = k.r1;
+      if ((e = launch_gemm(x, k.w1, GemmShape{Min, P, k.cin}, ep, st))) return e; }
+    { ConvEpi c; c.bias = k.b2; c.out = k.r2;
+      if ((e = launch_conv3x3(k.r1, k.w2, S, k.hin, k.hin, P, P, CONV_BIAS_RELU, c, st))) return e; }
+    const bf16* a3 = k.r2;
+    const bf16* id = x;
+    if (k.stride > 1) {
+      if ((e = avgpool_fwd(k.r2, S, k.hin, k.hin, P, h->scratch[0], st))) return e;
+      a3 = h->scratch[0];
+    }
+    if (k.down) {
+      const bf16* xin = x;
+      if (k.stride > 1) {
+        if ((e = avgpool_fwd(x, S, k.hin, k.hin, k.cin, h->scratch[1], st))) return e;
+        xin = h->scratch[1];
+      }
+      GemmEpi ep; ep.bias = k.bd; ep.out_bf16 = h->scratch[2];
+      if ((e = launch_gemm(xin, k.wd, GemmShape{Mo, E, k.cin}, ep, st))) return e;
+      id = h->scratch[2];
+    }
+    { GemmEpi ep; ep.bias = k.b3; ep.act = 2; ep.resid_bf16 = id; ep.out_bf16 = k.y;
+      if ((e = launch_gemm(a3, k.w3, GemmShape{Mo, E, P}, ep, st))) return e; }
+    x = k.y;
+  }
+  if ((e = tokens_fwd(x, h->pos, S, D, h->tok, st))) return e;
+  { GemmEpi ep; ep.bias = h->b_qkv; ep.out_bf16 = h->qkv;
+    if ((e = launch_gemm(h->tok, h->w_qkv, GemmShape{S * RN_T, 3 * D, D}, ep, st))) return e; }
+  if ((e = attn_resident(true, h->qkv, nullptr, h->attn, S, RN_T, D, h->cfg.heads, st))) return e;
+  // only token 0 is queried: c_proj reads rows s*50 of the attention output
+  GemmEpi ep; ep.out_f32 = h->emb_int;
+  return launch_gemm(h->attn, h->w_c, GemmShape{S, h->cfg.out_dim, D}, ep, st, RN_T * D);
+}
+
+// the launches of the backward from d_emb down to d (pre-ReLU stem conv 1 output), which it leaves in scratch[3]
+static int rn_bwd_body(RnImpl* h, int S, int side, cudaStream_t st) {
+  const int h1 = rn_stem_side(side), D = h->D;
+  bf16* const* g = h->scratch;
+  int e;
+  // attention pool: the attention-output gradient is non-zero on the token-0 rows only (d_attn's other rows stay zero)
+  { GemmEpi ep; ep.out_bf16 = h->d_attn; ep.ld_out = RN_T * D;
+    if ((e = launch_gemm(h->d_emb, h->w_c_t, GemmShape{S, D, h->cfg.out_dim}, ep, st))) return e; }
+  if ((e = attn_resident(false, h->qkv, h->d_attn, h->d_qkv, S, RN_T, D, h->cfg.heads, st))) return e;
+  { GemmEpi ep; ep.out_bf16 = h->d_tok;
+    if ((e = launch_gemm(h->d_qkv, h->w_qkv_t, GemmShape{S * RN_T, D, 3 * D}, ep, st))) return e; }
+  int cur = 0;   // g[cur]: d loss / d (the block's pre-ReLU sum), i.e. its output gradient selected by its ReLU
+  if ((e = tokens_bwd(h->d_tok, h->blocks.back().y, S, D, g[cur], st))) return e;
+  for (int b = (int)h->blocks.size() - 1; b >= 0; --b) {
+    const RnBlock& k = h->blocks[b];
+    const bf16* x = b > 0 ? h->blocks[b - 1].y : h->sp;
+    const int P = k.planes, E = 4 * P, Min = S * k.hin * k.hin, Mo = S * k.hout * k.hout;
+    const bf16* dz = g[cur];
+    bf16 *R = g[2], *U = g[3], *P1 = g[4], *T = g[5];
+    const bf16* rg = dz;                                     // the identity's gradient
+    if (k.down) {
+      GemmEpi ep; ep.out_bf16 = k.stride > 1 ? T : R;
+      if ((e = launch_gemm(dz, k.wd_t, GemmShape{Mo, k.cin, E}, ep, st))) return e;
+      if (k.stride > 1 && (e = avgpool_bwd(T, nullptr, S, k.hin, k.hin, k.cin, R, st))) return e;
+      rg = R;
+    }
+    if (k.stride > 1) {                                      // conv3's input was pool(relu2): adjoint, then relu2's select
+      GemmEpi ep; ep.out_bf16 = P1;
+      if ((e = launch_gemm(dz, k.w3_t, GemmShape{Mo, P, E}, ep, st))) return e;
+      if ((e = avgpool_bwd(P1, k.r2, S, k.hin, k.hin, P, U, st))) return e;
+    } else {
+      GemmEpi ep; ep.mask = k.r2; ep.out_bf16 = U;
+      if ((e = launch_gemm(dz, k.w3_t, GemmShape{Mo, P, E}, ep, st))) return e;
+    }
+    { ConvEpi c; c.mask = k.r1; c.out = P1;
+      if ((e = launch_conv3x3(U, k.w2_t, S, k.hin, k.hin, P, P, CONV_MASK, c, st))) return e; }
+    // the block input's gradient, selected by the input (a ReLU output; see the top of the file)
+    { GemmEpi ep; ep.mask = x; ep.resid_bf16 = rg; ep.out_bf16 = g[cur ^ 1];
+      if ((e = launch_gemm(P1, k.w1_t, GemmShape{Min, k.cin, P}, ep, st))) return e; }
+    cur ^= 1;
+  }
+  // stem: the pool's adjoint with relu3's select, then conv3 and conv2 backward with the selects of relu2 and relu1
+  if ((e = avgpool_bwd(g[cur], h->s3, S, h1, h1, 64, g[4], st))) return e;
+  ConvEpi c;
+  c.mask = h->s2; c.out = g[2];
+  if ((e = launch_conv3x3(g[4], h->stem_w3_t, S, h1, h1, 64, 64, CONV_MASK, c, st))) return e;
+  c.mask = h->s1; c.out = g[3];
+  return launch_conv3x3(g[2], h->stem_w2_t, S, h1, h1, 64, 64, CONV_MASK, c, st);
+}
+
+}  // namespace aph
+
+using namespace aph;
+
+extern "C" int aph_rn_create(aph_rn** out, const aph_rn_config* cfg) {
+  APH_REQUIRE(out && cfg, "aph_rn_create: null argument");
+  APH_REQUIRE(cfg->width == 64 && cfg->heads == 32, "aph_rn_create: width %d, heads %d unsupported (RN50 / RN101: width 64, 32 heads)",
+              cfg->width, cfg->heads);
+  APH_REQUIRE(cfg->layers[0] > 0 && cfg->layers[1] > 0 && cfg->layers[2] > 0 && cfg->layers[3] > 0, "aph_rn_create: empty stage");
+  APH_REQUIRE(cfg->out_dim % 128 == 0 && cfg->out_dim > 0 && cfg->max_batch > 0, "aph_rn_create: out_dim %d must be a multiple of 128",
+              cfg->out_dim);
+  APH_REQUIRE(cfg->res >= RN_SIDE_MIN && cfg->res <= RN_SIDE_MAX, "aph_rn_create: res %d outside [%d, %d]", cfg->res, RN_SIDE_MIN, RN_SIDE_MAX);
+  std::unique_ptr<RnImpl> h(new RnImpl());
+  h->cfg = *cfg;
+  h->D = 32 * cfg->width;
+  const int D = h->D, O = cfg->out_dim;
+  const size_t S = (size_t)cfg->max_batch, MT = S * RN_T;
+  h->blocks.resize(cfg->layers[0] + cfg->layers[1] + cfg->layers[2] + cfg->layers[3]);
+  rn_shapes(h.get(), RN_SIDE_MAX);
+  int e = 0;
+  // weights (BN folded): 1x1 convolutions [Co, Ci] and their transposes, 3x3 packed both ways, biases fp32
+  e |= h->add_f32("conv1.weight", &h->stem_w1, 32 * 27); e |= h->add_f32("conv1.bias", &h->stem_b1, 32);
+  e |= h->add_conv3x3("conv2.weight", 64, 64, &h->stem_w2, &h->stem_w2_t); e |= h->add_f32("conv2.bias", &h->stem_b2, 64);
+  e |= h->add_conv3x3("conv3.weight", 64, 64, &h->stem_w3, &h->stem_w3_t); e |= h->add_f32("conv3.bias", &h->stem_b3, 64);
+  {
+    size_t b = 0;
+    for (int i = 0; i < 4; ++i)
+      for (int j = 0; j < cfg->layers[i]; ++j, ++b) {
+        RnBlock& k = h->blocks[b];
+        const std::string p = "layer" + std::to_string(i + 1) + "." + std::to_string(j) + ".";
+        const int P = k.planes, E = 4 * P;
+        e |= h->add_bf16(p + "conv1.weight", P, k.cin, &k.w1, &k.w1_t); e |= h->add_f32(p + "conv1.bias", &k.b1, P);
+        e |= h->add_conv3x3(p + "conv2.weight", P, P, &k.w2, &k.w2_t); e |= h->add_f32(p + "conv2.bias", &k.b2, P);
+        e |= h->add_bf16(p + "conv3.weight", E, P, &k.w3, &k.w3_t); e |= h->add_f32(p + "conv3.bias", &k.b3, E);
+        if (k.down) { e |= h->add_bf16(p + "downsample.weight", E, k.cin, &k.wd, &k.wd_t); e |= h->add_f32(p + "downsample.bias", &k.bd, E); }
+        e |= h->alloc(&k.r1, S * k.hin * k.hin * P); e |= h->alloc(&k.r2, S * k.hin * k.hin * P);
+        e |= h->alloc(&k.y, S * k.hout * k.hout * E);
+      }
+  }
+  e |= h->add_f32("attnpool.positional_embedding", &h->pos, (size_t)RN_T * D);
+  e |= h->add_bf16("attnpool.qkv.weight", 3 * D, D, &h->w_qkv, &h->w_qkv_t); e |= h->add_f32("attnpool.qkv.bias", &h->b_qkv, 3 * D);
+  e |= h->add_bf16("attnpool.c_proj.weight", O, D, &h->w_c, &h->w_c_t); e |= h->add_f32("attnpool.c_proj.bias", &h->b_c, O);
+  // activations
+  const size_t h1 = rn_stem_side(RN_SIDE_MAX), h0 = h1 / 2;
+  h->emax = h1 * h1 * 64;
+  for (const RnBlock& k : h->blocks) {
+    h->emax = std::max(h->emax, (size_t)k.hin * k.hin * std::max(k.cin, k.planes));
+    h->emax = std::max(h->emax, (size_t)k.hout * k.hout * 4 * k.planes);
+  }
+  e |= h->alloc(&h->s1, S * h1 * h1 * 64); e |= h->alloc(&h->s2, S * h1 * h1 * 64); e |= h->alloc(&h->s3, S * h1 * h1 * 64);
+  e |= h->alloc(&h->sp, S * h0 * h0 * 64);
+  for (bf16*& p : h->scratch) e |= h->alloc(&p, S * h->emax);
+  e |= h->alloc(&h->tok, MT * D); e |= h->alloc(&h->qkv, MT * 3 * D); e |= h->alloc(&h->attn, MT * D);
+  e |= h->alloc(&h->d_attn, MT * D); e |= h->alloc(&h->d_qkv, MT * 3 * D); e |= h->alloc(&h->d_tok, MT * D);
+  e |= h->alloc(&h->emb_int, S * O); e |= h->alloc(&h->d_emb, S * O);
+  if (e) return 1;
+  APH_CUDA_OK(cudaMemset(h->d_attn, 0, MT * D * sizeof(bf16)));
+  APH_CUDA_OK(cudaDeviceSynchronize());     // the zeros are in place before any caller stream (blocking or not) can read them
+  *out = reinterpret_cast<aph_rn*>(h.release());
+  return 0;
+}
+
+extern "C" int aph_rn_destroy(aph_rn* h) {
+  delete reinterpret_cast<RnImpl*>(h);
+  return 0;
+}
+
+extern "C" int64_t aph_rn_bytes(const aph_rn* h) { return h ? reinterpret_cast<const RnImpl*>(h)->bytes : 0; }
+
+extern "C" int aph_rn_load_tensor(aph_rn* h, const char* key, const float* data, int64_t numel, void* stream) {
+  return load_tensor(reinterpret_cast<RnImpl*>(h), key, data, numel, (cudaStream_t)stream, "aph_rn_load_tensor");
+}
+
+extern "C" int aph_rn_finalize(aph_rn* h) { return finalize(reinterpret_cast<RnImpl*>(h), "aph_rn_finalize"); }
+
+static int rn_check(const RnImpl* h, int S, int side, const char* who) {
+  APH_REQUIRE(h->finalized, "%s: weights not finalized", who);
+  APH_REQUIRE(S > 0 && S <= h->cfg.max_batch, "%s: S=%d outside (0, max_batch=%d]", who, S, h->cfg.max_batch);
+  APH_REQUIRE(side >= RN_SIDE_MIN && side <= RN_SIDE_MAX, "%s: side=%d outside [%d, %d] (the sides whose final map is 7 x 7)", who, side,
+              RN_SIDE_MIN, RN_SIDE_MAX);
+  return 0;
+}
+
+extern "C" int aph_rn_fwd(aph_rn* rn, const float* x, int S, int side, float* emb, int save_for_bwd, void* stream) {
+  APH_REQUIRE(rn && x && emb, "aph_rn_fwd: null argument");
+  RnImpl* h = reinterpret_cast<RnImpl*>(rn);
+  if (int e = rn_check(h, S, side, "aph_rn_fwd")) return e;
+  cudaStream_t st = (cudaStream_t)stream;
+  h->last_S = h->last_side = -1;
+  rn_shapes(h, side);
+  // the kernels that touch caller memory run outside the cached graph (see aph_vit_fwd)
+  if (int e = stem_fwd(x, S, side, rn_stem_side(side), h->stem_w1, h->stem_b1, h->s1, st)) return e;
+  // the graph is keyed on the side alone: the forward's launches are the same with or without save_for_bwd
+  if (int e = h->fwd_graphs.replay(S, side, st, [&]() { return rn_fwd_body(h, S, side, st); })) return e;
+  const int O = h->cfg.out_dim;
+  k_rn_emb<<<stride_blocks((size_t)S * O, 8), 256, 0, st>>>(h->emb_int, h->b_c, S, O, emb);
+  APH_LAUNCH_OK();
+  if (save_for_bwd) { h->last_S = S; h->last_side = side; }
+  return 0;
+}
+
+extern "C" int aph_rn_bwd(aph_rn* rn, const float* grad_emb, int S, int side, float* grad_x, void* stream) {
+  APH_REQUIRE(rn && grad_emb && grad_x, "aph_rn_bwd: null argument");
+  RnImpl* h = reinterpret_cast<RnImpl*>(rn);
+  if (int e = rn_check(h, S, side, "aph_rn_bwd")) return e;
+  APH_REQUIRE(h->last_S == S && h->last_side == side, "aph_rn_bwd: no saved forward for S=%d side=%d (last saved: S=%d side=%d)", S, side,
+              h->last_S, h->last_side);
+  cudaStream_t st = (cudaStream_t)stream;
+  rn_shapes(h, side);
+  const size_t n = (size_t)S * h->cfg.out_dim;
+  k_f32_to_bf16<<<stride_blocks(n, 8), 256, 0, st>>>(grad_emb, h->d_emb, n);
+  APH_LAUNCH_OK();
+  if (int e = h->bwd_graphs.replay(S, side, st, [&]() { return rn_bwd_body(h, S, side, st); })) return e;
+  return stem_bwd(h->scratch[3], S, side, rn_stem_side(side), h->stem_w1, grad_x, st);
+}
+
+// The forward's saved ReLU outputs, for a float64 backward that takes the CUDA forward's own selects: k = 0, 1, 2 the stem's
+// [S, h1, h1, 64] (channels 32-63 zero), then 3 b + 3, 3 b + 4, 3 b + 5 block b's conv1 and conv2 outputs [S, hin, hin, P] and
+// its output [S, hout, hout, 4 P], all bf16 NHWC at the side of the last forward. *ptr is the handle's buffer (valid until the
+// next forward); *numel its element count at that side.
+extern "C" int aph_rn_saved_test(aph_rn* rn, int k, void** ptr, int64_t* numel) {
+  APH_REQUIRE(rn && ptr && numel, "aph_rn_saved_test: null argument");
+  RnImpl* h = reinterpret_cast<RnImpl*>(rn);
+  APH_REQUIRE(h->last_S > 0, "aph_rn_saved_test: no saved forward");
+  const int nb = (int)h->blocks.size();
+  APH_REQUIRE(k >= 0 && k < 3 + 3 * nb, "aph_rn_saved_test: k=%d outside [0, %d)", k, 3 + 3 * nb);
+  rn_shapes(h, h->last_side);
+  const int64_t S = h->last_S, h1 = rn_stem_side(h->last_side);
+  if (k < 3) {
+    *ptr = k == 0 ? h->s1 : k == 1 ? h->s2 : h->s3;
+    *numel = S * h1 * h1 * 64;
+    return 0;
+  }
+  const RnBlock& b = h->blocks[(k - 3) / 3];
+  const int j = (k - 3) % 3;
+  *ptr = j == 0 ? b.r1 : j == 1 ? b.r2 : b.y;
+  *numel = j < 2 ? S * b.hin * b.hin * b.planes : S * b.hout * b.hout * 4 * b.planes;
+  return 0;
+}
+
+// ---- test entries (tests/test_clip_resnet_gpu.py) ----------------------------------------------------------------
+// Stem conv 1 on caller buffers: weight fp32 [32,3,3,3], bias [32]. fwd = 1: in = crops fp32 [N,3,side,side] -> out bf16
+// [N,h,h,64] (ReLU output; channels 32-63 zero), h = (side - 1) / 2 + 1; fwd = 0: in = dz bf16 [N,h,h,64] -> out fp32 [N,3,side,side].
+extern "C" int aph_rn_stem_test(int fwd, const void* in, const float* weight, const float* bias, void* out, int N, int side, void* stream) {
+  APH_REQUIRE(in && weight && out && (bias || !fwd) && N > 0 && side > 0, "aph_rn_stem_test: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int Ho = rn_stem_side(side);
+  if (fwd) return stem_fwd(reinterpret_cast<const float*>(in), N, side, Ho, weight, bias, reinterpret_cast<bf16*>(out), st);
+  return stem_bwd(reinterpret_cast<const bf16*>(in), N, side, Ho, weight, reinterpret_cast<float*>(out), st);
+}
+
+// 2x2 average pool, bf16 NHWC, C % 8 == 0. fwd = 1: out [N,H/2,W/2,C] = pool(x); fwd = 0: x = dy [N,H/2,W/2,C] -> out [N,H,W,C]
+// = its adjoint, selected by mask [N,H,W,C] > 0 when mask is not NULL.
+extern "C" int aph_rn_pool_test(int fwd, const void* x, const void* mask, void* out, int N, int H, int W, int C, void* stream) {
+  APH_REQUIRE(x && out && N > 0 && H >= 2 && W >= 2 && C % 8 == 0 && C > 0, "aph_rn_pool_test: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (fwd) return avgpool_fwd(reinterpret_cast<const bf16*>(x), N, H, W, C, reinterpret_cast<bf16*>(out), st);
+  return avgpool_bwd(reinterpret_cast<const bf16*>(x), reinterpret_cast<const bf16*>(mask), N, H, W, C, reinterpret_cast<bf16*>(out), st);
+}
+
+// Attention-pool tokens, C % 8 == 0. fwd = 1: in = x bf16 [S*49, C], aux = pos fp32 [50, C] -> out bf16 [S*50, C]; fwd = 0:
+// in = dtok bf16 [S*50, C], aux = x bf16 [S*49, C] (the select) -> out bf16 [S*49, C].
+extern "C" int aph_rn_tokens_test(int fwd, const void* in, const void* aux, void* out, int S, int C, void* stream) {
+  APH_REQUIRE(in && aux && out && S > 0 && C % 8 == 0 && C > 0, "aph_rn_tokens_test: bad arguments");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (fwd) return tokens_fwd(reinterpret_cast<const bf16*>(in), reinterpret_cast<const float*>(aux), S, C, reinterpret_cast<bf16*>(out), st);
+  return tokens_bwd(reinterpret_cast<const bf16*>(in), reinterpret_cast<const bf16*>(aux), S, C, reinterpret_cast<bf16*>(out), st);
+}

@@ -35,10 +35,12 @@ struct GemmEpi {
   const float* bias = nullptr;     // [N]
   const float* resid = nullptr;    // fp32 [M, N], added last
   const bf16* gelu_in = nullptr;   // bf16 [M, N]: acc *= quickgelu'(gelu_in)
+  const bf16* resid_bf16 = nullptr;  // bf16 [M, N] residual of the ResNet epilogues (rows ld_out apart, like the output)
+  const bf16* mask = nullptr;      // bf16 [M, N] ReLU output selecting the data gradient (rows ld_out apart)
   float* out_f32 = nullptr;        // fp32 [M, N] (or NCHW images when unpatch_p > 0)
   bf16* out_bf16 = nullptr;        // bf16 [M, N]
   bf16* out_pre = nullptr;         // bf16 [M, N] pre-activation (acc + bias), saved for backward
-  int act = 0;                     // 1 = QuickGELU x*sigmoid(1.702x)
+  int act = 0;                     // 1 = QuickGELU x*sigmoid(1.702x), 2 = ReLU
   int unpatch_p = 0;               // >0: out_f32 is [S,3,R,R]; row = s*g*g + gy*g + gx, col = c*p*p + py*p + px (cols >= 3p^2 dropped)
   int unpatch_g = 0;
   // row strides in elements, 0 = N (dense). ld_out covers out_f32 / out_bf16 / out_pre and gelu_in, which has the output's rows.
@@ -63,7 +65,12 @@ enum : int {
   EPI_BIAS_RESID = 4,     // out_f32 = acc + bias + resid
   EPI_GELUGRAD_BF16 = 5,  // out_bf16 = acc * quickgelu'(gelu_in)
   EPI_UNPATCH = 6,        // out_f32[NCHW] = acc (patch-embed data gradient)
-  EPI_KINDS = 7
+  // the ResNet image tower's 1x1 convolutions (rn.cu), forward and data gradient
+  EPI_BIAS_RELU = 7,        // out_bf16 = relu(acc + bias)
+  EPI_BIAS_RESID_RELU = 8,  // out_bf16 = relu(acc + bias + resid_bf16)
+  EPI_MASK = 9,             // out_bf16 = mask > 0 ? acc : 0
+  EPI_MASK_RESID = 10,      // out_bf16 = mask > 0 ? acc + resid_bf16 : 0
+  EPI_KINDS = 11
 };
 
 // ---- raw PTX wrappers -------------------------------------------------------------------------
@@ -242,7 +249,10 @@ __device__ __forceinline__ void consumer_bar_arrive(int id) { asm volatile("bar.
 
 // epilogue kinds with bf16 outputs: stored 8 columns (16 B) per lane after a transpose inside each quad of lanes
 template <int EPI>
-constexpr bool epi_bf16_out() { return EPI == EPI_BF16 || EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_GELUGRAD_BF16; }
+constexpr bool epi_bf16_out() {
+  return EPI == EPI_BF16 || EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_GELUGRAD_BF16 || EPI >= EPI_BIAS_RELU;
+}
+
 
 // two adjacent output columns (col, col + 1) of one row through an fp32-output epilogue of kind EPI (launch_gemm has resolved the
 // strides: epi.ld_out and epi.ld_resid are never 0 here). out_row / res_row: the row's offsets, computed once per row and tile.
@@ -286,6 +296,14 @@ __device__ __forceinline__ void quad_transpose(uint32_t (&w)[4], int q) {
   }
 }
 
+// 8 bf16 of a row at `off` (16 B), returned in the accumulator layout of this lane (the inverse of the store's transpose)
+__device__ __forceinline__ void load_bf16x8_acc(const bf16* p, size_t off, bool valid, int q, uint32_t (&w)[4]) {
+  uint4 g = make_uint4(0u, 0u, 0u, 0u);
+  if (valid) g = __ldg(reinterpret_cast<const uint4*>(p + off));
+  w[0] = g.x; w[1] = g.y; w[2] = g.z; w[3] = g.w;
+  quad_transpose(w, q);
+}
+
 // A 32-column chunk of one row through a bf16-output epilogue of kind EPI. v[2 t + {0,1}] = accumulators at columns
 // col0 + 8 t + 2 q + {0,1}, bb[t] their bias. The math per element is that of the pairwise store; only the stores (and the
 // gelu_in loads) are 16 B per lane, so that a warp writes whole 32 B sectors. All 32 lanes must call it (shuffles); rows >= M
@@ -294,13 +312,10 @@ template <int EPI>
 __device__ __forceinline__ void epi_store_bf16x32(const GemmEpi& epi, int row, bool valid, int col0, int q, const float* v,
                                                   const float2* bb) {
   const size_t off = (size_t)row * epi.ld_out + col0 + 8 * q;  // this lane's 8 columns after the transpose
-  uint32_t w[4], w2[4];
-  if constexpr (EPI == EPI_GELUGRAD_BF16) {
-    uint4 g = make_uint4(0u, 0u, 0u, 0u);
-    if (valid) g = __ldg(reinterpret_cast<const uint4*>(epi.gelu_in + off));
-    w2[0] = g.x; w2[1] = g.y; w2[2] = g.z; w2[3] = g.w;
-    quad_transpose(w2, q);                                     // back to the accumulator layout
-  }
+  uint32_t w[4], w2[4], r2[4];
+  if constexpr (EPI == EPI_GELUGRAD_BF16) load_bf16x8_acc(epi.gelu_in, off, valid, q, w2);
+  if constexpr (EPI == EPI_MASK || EPI == EPI_MASK_RESID) load_bf16x8_acc(epi.mask, off, valid, q, w2);
+  if constexpr (EPI == EPI_BIAS_RESID_RELU || EPI == EPI_MASK_RESID) load_bf16x8_acc(epi.resid_bf16, off, valid, q, r2);
 #pragma unroll
   for (int t = 0; t < 4; ++t) {
     float v0 = v[2 * t], v1 = v[2 * t + 1];
@@ -312,9 +327,21 @@ __device__ __forceinline__ void epi_store_bf16x32(const GemmEpi& epi, int row, b
       v0 += bb[t].x; v1 += bb[t].y;
       w2[t] = pack_bf16(v0, v1);
       w[t] = pack_bf16(quickgelu(v0), quickgelu(v1));
-    } else {   // EPI_GELUGRAD_BF16
+    } else if (EPI == EPI_GELUGRAD_BF16) {
       const float2 h = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w2[t]));
       w[t] = pack_bf16(v0 * quickgelu_grad(h.x), v1 * quickgelu_grad(h.y));
+    } else {   // the ResNet kinds: + bias, + bf16 residual, then ReLU or the select by a ReLU output (never a multiply)
+      if (EPI == EPI_BIAS_RELU || EPI == EPI_BIAS_RESID_RELU) { v0 += bb[t].x; v1 += bb[t].y; }
+      if (EPI == EPI_BIAS_RESID_RELU || EPI == EPI_MASK_RESID) {
+        const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&r2[t]));
+        v0 += r.x; v1 += r.y;
+      }
+      if (EPI == EPI_MASK || EPI == EPI_MASK_RESID) {
+        const float2 m = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w2[t]));
+        w[t] = pack_bf16(m.x > 0.f ? v0 : 0.f, m.y > 0.f ? v1 : 0.f);
+      } else {
+        w[t] = pack_bf16(fmaxf(v0, 0.f), fmaxf(v1, 0.f));
+      }
     }
   }
   quad_transpose(w, q);
@@ -447,7 +474,8 @@ struct GemmProblem {
   // straight from the accumulator fragments: d[h][4j + {0,1}] = (row, col + {0,1}), d[h][4j + {2,3}] = (row + 8, ...)
   template <int MMAS>
   __device__ __forceinline__ void epilogue(const float (&d)[MMAS][BN / 2], Tile tl, int row_in_tile, int col_in_tile, int lane) const {
-    constexpr bool HAS_BIAS = (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_RESID);
+    constexpr bool HAS_BIAS = (EPI == EPI_BIAS_BF16 || EPI == EPI_BIAS_GELU || EPI == EPI_BIAS_RESID || EPI == EPI_BIAS_RELU ||
+                               EPI == EPI_BIAS_RESID_RELU);
     const int m_blk = tl.m_blk, n_blk = tl.n_blk;
 #pragma unroll
     for (int h = 0; h < MMAS; ++h) {
@@ -495,7 +523,7 @@ int make_tmap_bf16_tokens(CUtensorMap* out, const void* base, int cols, int T, i
 // 4-D view {C, W, H, N} of a bf16 NHWC activation, box {64 channels, box_w columns, box_h rows, 1 image}, 128B swizzle
 int make_tmap_bf16_nhwc(CUtensorMap* out, const void* base, int N, int H, int W, int C, int box_h, int box_w);
 // Launches the GEMM on `st`. A: [M,K] with rows `lda` elements apart (K when 0), B: [N,K] device bf16. Requires K % 64 == 0,
-// N % 128 == 0, and row strides that are multiples of 16 bytes.
+// N % 128 == 0 or N == 64 (the ResNet's 64-channel layers, on 128 x 64 tiles), and row strides that are multiples of 16 bytes.
 int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st, int lda = 0);
 
 }  // namespace aph

@@ -177,6 +177,14 @@ static int vit_attn_fwd(const bf16* qkv, bf16* out, int S, int T, int D, int hea
   return vit_attn(true, qkv, nullptr, out, nullptr, S, T, D, heads, st);
 }
 
+GraphCacheRef::GraphCacheRef() : cache(new GraphCache) {}
+GraphCacheRef::~GraphCacheRef() { delete cache; }
+int GraphCacheRef::replay(int S, int flag, cudaStream_t& st, const std::function<int()>& body) { return cache->run(S, flag, st, body); }
+
+int attn_resident(bool fwd, const bf16* qkv, const bf16* dout, bf16* out_or_dqkv, int S, int T, int D, int heads, cudaStream_t st) {
+  return attn_dispatch(fwd, qkv, dout, out_or_dqkv, S, T, D, heads, st);
+}
+
 static Scratch& g_win = *new Scratch;   // aph_vit_bwd_sized: the R x R window gradient before k_window_expand
 
 }  // namespace aph

@@ -72,7 +72,8 @@ bool gemm_profiling_on() { return g_prof; }
 static std::vector<std::pair<cudaEvent_t, cudaEvent_t>> g_prof_ev;
 static std::vector<double> g_prof_flops;
 
-// launches per (kernel variant, epilogue kind): variant 0 = the small-problem kernel (cooperative, 128 x 128 tiles),
+// launches per (kernel variant, epilogue kind): variant 0 = the small-problem kernels (cooperative, 128 x 128 tiles, or 128 x 64
+// for N = 64),
 // 1 = the large-problem kernels (ping-pong 128 x 128 tiles, or cooperative 128 x 256 tiles for long K).
 // Read by the tests to prove which kernel a shape really ran (aph_gemm_variant_launches).
 static std::atomic<long long> g_variant_launches[2][EPI_KINDS];
@@ -99,7 +100,7 @@ static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi
 int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi_in, cudaStream_t st, int lda) {
   APH_REQUIRE(A && B && shp.M > 0, "gemm: null operand or empty M");
   APH_REQUIRE(shp.K % GEMM_BK == 0 && shp.K > 0, "gemm: K=%d must be a positive multiple of %d", shp.K, GEMM_BK);
-  APH_REQUIRE(shp.N % 128 == 0 && shp.N > 0, "gemm: N=%d must be a positive multiple of 128", shp.N);
+  APH_REQUIRE((shp.N % 128 == 0 && shp.N > 0) || shp.N == 64, "gemm: N=%d must be 64 or a positive multiple of 128", shp.N);
   APH_REQUIRE(lda == 0 || lda >= shp.K, "gemm: lda=%d < K=%d", lda, shp.K);
   APH_REQUIRE((epi_in.ld_out == 0 || epi_in.ld_out >= shp.N) && (epi_in.ld_resid == 0 || epi_in.ld_resid >= shp.N),
               "gemm: output / residual row stride below N=%d", shp.N);
@@ -109,8 +110,15 @@ int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi_
   // map the requested fusion onto one of the compiled epilogue kinds
   int kind = -1;
   const bool b = epi.bias, r = epi.resid, gi = epi.gelu_in, f = epi.out_f32, h = epi.out_bf16, pre = epi.out_pre, act = epi.act == 1, un = epi.unpatch_p > 0;
+  const bool rb = epi.resid_bf16, mk = epi.mask, relu = epi.act == 2;
   APH_REQUIRE(!un || epi.ld_out == shp.N, "gemm: the un-patchify store takes no output stride");
-  if (un && f && !b && !r && !gi && !h && !pre && !act) kind = EPI_UNPATCH;
+  if (rb || mk || relu) {                     // the ResNet kinds: bf16 out, no other operand
+    if (h && !f && !r && !gi && !pre && !un) {
+      if (b && relu && !mk) kind = rb ? EPI_BIAS_RESID_RELU : EPI_BIAS_RELU;
+      else if (!b && !relu && mk) kind = rb ? EPI_MASK_RESID : EPI_MASK;
+    }
+  }
+  else if (un && f && !b && !r && !gi && !h && !pre && !act) kind = EPI_UNPATCH;
   else if (f && !h && !b && !r && !gi && !pre && !act) kind = EPI_F32;
   else if (h && !f && !b && !r && !gi && !pre && !act) kind = EPI_BF16;
   else if (h && !f && b && !r && !gi && !pre && !act) kind = EPI_BIAS_BF16;
@@ -118,7 +126,8 @@ int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi_
   else if (f && !h && b && r && !gi && !pre && !act) kind = EPI_BIAS_RESID;
   else if (h && !f && !b && !r && gi && !pre && !act) kind = EPI_GELUGRAD_BF16;
   APH_REQUIRE(kind >= 0, "gemm: unsupported epilogue combination");
-  const uintptr_t bf16_ptrs = reinterpret_cast<uintptr_t>(epi.out_bf16) | reinterpret_cast<uintptr_t>(epi.out_pre) | reinterpret_cast<uintptr_t>(epi.gelu_in);
+  const uintptr_t bf16_ptrs = reinterpret_cast<uintptr_t>(epi.out_bf16) | reinterpret_cast<uintptr_t>(epi.out_pre) | reinterpret_cast<uintptr_t>(epi.gelu_in) |
+                              reinterpret_cast<uintptr_t>(epi.resid_bf16) | reinterpret_cast<uintptr_t>(epi.mask);
   APH_REQUIRE((bf16_ptrs & 15) == 0 && ((size_t)epi.ld_out * (f ? 4 : 2)) % 16 == 0 && ((size_t)epi.ld_resid * 4) % 16 == 0 &&
               ((size_t)lda * 2) % 16 == 0,
               "gemm: bf16 epilogue operands and row strides must be 16-byte aligned (8 columns are stored per lane)");
@@ -126,16 +135,23 @@ int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi_
   // chosen when there are at least twice as many 128 x 128 tiles as SMs and K is short (K = 768 in the encoder), so that the
   // epilogue is a large share of a tile's time. With long K the mainloop dominates and the cooperative 128 x 256 tile wins: its
   // m64n256 MMAs read less shared memory per FLOP. Smaller problems (the final projection, the text tower) keep 128 x 128 tiles.
+  // N = 64 (the ResNet's first stage) runs the small-problem schedule on 128 x 64 tiles, the tile the 3x3 convolution uses there.
   const int m_tiles = (shp.M + GEMM_BM - 1) / GEMM_BM;
-  const bool pingpong = m_tiles * (shp.N / 128) >= 2 * num_sms() && shp.K <= 1024;
+  const bool narrow = shp.N == 64;
+  const bool pingpong = !narrow && m_tiles * (shp.N / 128) >= 2 * num_sms() && shp.K <= 1024;
   const bool wide = !pingpong && shp.N % 256 == 0 && m_tiles * (shp.N / 256) >= num_sms();
 #define APH_GEMM_CASE(K) case K: return pingpong ? launch_cfg<128, true, K>(A, B, shp, epi, st, lda) \
                                                  : wide ? launch_cfg<256, false, K>(A, B, shp, epi, st, lda) : launch_cfg<128, false, K>(A, B, shp, epi, st, lda);
+#define APH_GEMM_CASE_RN(K) case K: return narrow ? launch_cfg<64, false, K>(A, B, shp, epi, st, lda) : pingpong ? launch_cfg<128, true, K>(A, B, shp, epi, st, lda) \
+                                                 : wide ? launch_cfg<256, false, K>(A, B, shp, epi, st, lda) : launch_cfg<128, false, K>(A, B, shp, epi, st, lda);
+  APH_REQUIRE(!narrow || kind == EPI_BF16 || kind >= EPI_BIAS_RELU, "gemm: N=64 takes the bf16 and ResNet epilogues only");
   switch (kind) {
-    APH_GEMM_CASE(EPI_F32) APH_GEMM_CASE(EPI_BF16) APH_GEMM_CASE(EPI_BIAS_BF16) APH_GEMM_CASE(EPI_BIAS_GELU)
+    APH_GEMM_CASE(EPI_F32) APH_GEMM_CASE_RN(EPI_BF16) APH_GEMM_CASE(EPI_BIAS_BF16) APH_GEMM_CASE(EPI_BIAS_GELU)
     APH_GEMM_CASE(EPI_BIAS_RESID) APH_GEMM_CASE(EPI_GELUGRAD_BF16) APH_GEMM_CASE(EPI_UNPATCH)
+    APH_GEMM_CASE_RN(EPI_BIAS_RELU) APH_GEMM_CASE_RN(EPI_BIAS_RESID_RELU) APH_GEMM_CASE_RN(EPI_MASK) APH_GEMM_CASE_RN(EPI_MASK_RESID)
   }
 #undef APH_GEMM_CASE
+#undef APH_GEMM_CASE_RN
   return 2;
 }
 
@@ -173,8 +189,19 @@ extern "C" int aph_gemm_epi_strided_test(const void* A, int lda, const void* B, 
   return launch_gemm(A, B, GemmShape{M, N, K}, epi, (cudaStream_t)stream, lda);
 }
 
-// launches so far of kernel variant `variant` (0: the small-problem kernel, 1: the large-problem kernels) with
-// epilogue kind `epi` (EPI_* order of tc_gemm.cuh: 0 f32, 1 bf16, 2 bias-bf16, 3 bias-gelu, 4 bias-resid, 5 gelugrad, 6 unpatch; -1 = all)
+// The ResNet epilogues (rn.cu) on caller operands: relu = 1: out_bf16 = relu(acc + bias [+ resid_bf16]); relu = 0:
+// out_bf16 = mask > 0 ? acc [+ resid_bf16] : 0. N = 64 or a multiple of 128.
+extern "C" int aph_gemm_rn_epi_test(const void* A, const void* B, int M, int N, int K, const float* bias, const void* resid_bf16,
+                                    const void* mask, int relu, void* out_bf16, void* stream) {
+  GemmEpi epi;
+  epi.bias = bias; epi.resid_bf16 = reinterpret_cast<const bf16*>(resid_bf16); epi.mask = reinterpret_cast<const bf16*>(mask);
+  epi.act = relu ? 2 : 0; epi.out_bf16 = reinterpret_cast<bf16*>(out_bf16);
+  return launch_gemm(A, B, GemmShape{M, N, K}, epi, (cudaStream_t)stream);
+}
+
+// launches so far of kernel variant `variant` (0: the small-problem kernels, 1: the large-problem kernels) with
+// epilogue kind `epi` (EPI_* order of tc_gemm.cuh: 0 f32, 1 bf16, 2 bias-bf16, 3 bias-gelu, 4 bias-resid, 5 gelugrad, 6 unpatch,
+// 7 bias-relu, 8 bias-resid-relu, 9 mask, 10 mask-resid; -1 = all)
 extern "C" int64_t aph_gemm_variant_launches(int variant, int epi) {
   if (variant < 0 || variant > 1 || epi >= EPI_KINDS) return -1;
   long long n = 0;
