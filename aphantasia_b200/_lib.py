@@ -29,9 +29,11 @@ _SIGS = {
     'aph_dwt_plan_destroy': (C.c_int, [C.c_void_p]),
     'aph_dwt_plan_levels': (C.c_int, [C.c_void_p, C.POINTER(C.c_int), C.c_void_p, C.c_void_p]),
     'aph_synth_dwt_fwd': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int, c_f32p, C.c_void_p, c_f32p, C.c_void_p]),
-    'aph_synth_dwt_bwd': (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    'aph_synth_dwt_bwd': (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, C.c_void_p, C.c_void_p, C.c_float, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int]),
     'aph_pixel_fwd': (C.c_int, [c_f32p, C.c_int64, C.c_float, C.c_int, C.c_void_p, C.c_int, C.c_void_p, c_f32p, C.c_void_p]),
-    'aph_pixel_bwd': (C.c_int, [c_f32p, c_f32p, c_f32p, C.c_void_p, C.c_int64, C.c_float, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_void_p]),
+    'aph_pixel_bwd': (C.c_int, [c_f32p, c_f32p, c_f32p, C.c_void_p, C.c_int64, C.c_float, C.c_int, C.c_void_p, C.c_int, c_f32p, C.c_void_p,
+                                c_f32p, c_f32p, c_f32p, c_f32p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int]),
     'aph_valid_rgb_fwd': (C.c_int, [c_f32p, C.c_int64, C.c_void_p, c_f32p, C.c_void_p]),
     'aph_valid_rgb_bwd': (C.c_int, [c_f32p, c_f32p, C.c_int64, C.c_void_p, c_f32p, C.c_void_p]),
     'aph_affine_fwd': (C.c_int, [c_f32p, C.c_int, C.c_int, C.c_int, C.c_void_p, c_f32p, C.c_void_p]),
@@ -97,7 +99,8 @@ _SIGS = {
     'aph_head_fwd':(C.c_int, [c_f32p, C.c_int, C.c_int, c_f32p, c_f32p, c_f32p, C.c_void_p]),
     'aph_head_bwd': (C.c_int, [c_f32p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     'aph_synth_fft_bwd_adam': (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, C.c_void_p, c_f32p, C.c_float, C.c_void_p, C.c_int,
-                                         c_f32p, c_f32p, c_f32p, c_f32p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p]),
+                                         c_f32p, c_f32p, c_f32p, c_f32p, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p,
+                                         C.c_float, c_f32p]),
     'aph_lpips_create': (C.c_int, [C.POINTER(C.c_void_p)]),
     'aph_lpips_destroy': (C.c_int, [C.c_void_p]),
     'aph_lpips_load_tensor': (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.c_int64, C.c_void_p]),
@@ -110,8 +113,14 @@ _SIGS = {
     'aph_lpips_conv0_test': (C.c_int, [C.c_int, C.c_void_p, c_f32p, c_f32p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     'aph_lpips_pool_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     'aph_allreduce_sym': (C.c_int, [C.c_uint64, C.c_void_p, C.c_uint64, C.c_int, C.c_int, C.c_int64, C.c_void_p, C.c_void_p]),
-    'aph_adam_step': (C.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p]),
+    'aph_adam_step': (C.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p,
+                                C.c_float, c_f32p]),
 }
+# Entry points whose last arguments are optional (the fused / extended Adam update): a call that stops after `stream` gets
+# these values for them, so a call written for the plain form binds unchanged.
+_ADAM_OFF = (None, None, None, None, 0., 0., 0., 0., 0., 0)
+OPTIONAL_TAIL = {'aph_adam_step': (0., None), 'aph_synth_fft_bwd_adam': (0., None), 'aph_pixel_bwd': _ADAM_OFF,
+                 'aph_synth_dwt_bwd': _ADAM_OFF}
 EXPORTS = tuple(_SIGS)
 
 
@@ -138,8 +147,21 @@ def lib():
         for name, (res, args) in _SIGS.items():
             f = getattr(l, name)
             f.restype, f.argtypes = res, args
+        for name, tail in OPTIONAL_TAIL.items():
+            setattr(l, name, _with_optional_tail(getattr(l, name), tail))
         _lib = l
     return _lib
+
+
+def _with_optional_tail(f, tail):
+    full = len(f.argtypes)
+
+    def call(*args):
+        if len(args) == full - len(tail):
+            args += tail
+        return f(*args)
+    call.__name__, call.argtypes, call.restype = f.__name__, f.argtypes, f.restype
+    return call
 
 
 def check(rc, what, error=RuntimeError):

@@ -5,8 +5,8 @@
 //     cos_s = <v1,v2_s> / (|v1| |v2_s|);   mix: f = cos - 0.25 * 2*asin(|v1^ - v2^_s| / 2)^2
 //     value = mean_s f_s
 // One warp per sample; gradients w.r.t. both operands are written in the same pass.
-// aph_adam_step replaces torch.optim.Adam's single-tensor update (/root/reference/clip_fft.py:115,295).
-#include "aph_common.cuh"
+// aph_adam_step replaces torch.optim.Adam / AdamW's single-tensor update (/root/reference/clip_fft.py:108-115,295; adam.cuh).
+#include "adam.cuh"
 #include <algorithm>
 #include <math.h>
 
@@ -51,16 +51,8 @@ __global__ void __launch_bounds__(256) k_sim(const float* __restrict__ v1, int n
   }
 }
 
-__global__ void __launch_bounds__(256) k_adam(float* __restrict__ p, const float* __restrict__ g, float* __restrict__ m,
-                                              float* __restrict__ v, size_t n, float step_size, float b1, float b2, float eps,
-                                              float inv_sqrt_bc2) {
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const float gi = g[i];
-    const float mi = b1 * m[i] + (1.f - b1) * gi;
-    const float vi = b2 * v[i] + (1.f - b2) * gi * gi;
-    m[i] = mi; v[i] = vi;
-    p[i] -= step_size * mi / (sqrtf(vi) * inv_sqrt_bc2 + eps);
-  }
+__global__ void __launch_bounds__(256) k_adam(const float* __restrict__ g, size_t n, AdamArgs a) {
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) adam_elem(a, i, g[i]);
 }
 
 // ---- optional loss heads of the step (SURVEY 8 row f4) -----------------------------------------------------------
@@ -253,11 +245,10 @@ extern "C" int aph_sim_fwd(const float* v1, int n1, const float* v2, int S, int 
 }
 
 extern "C" int aph_adam_step(float* p, const float* g, float* m, float* v, int64_t n, float lr, float b1, float b2, float eps,
-                             int step, void* stream) {
+                             int step, void* stream, float weight_decay, float* vmax) {
   APH_REQUIRE(p && g && m && v && n > 0 && step >= 1, "aph_adam_step: bad arguments");
-  const double bc1 = 1.0 - pow((double)b1, step), bc2 = 1.0 - pow((double)b2, step);
   const int blocks = stride_blocks((size_t)n, 8);
-  k_adam<<<blocks, 256, 0, (cudaStream_t)stream>>>(p, g, m, v, (size_t)n, (float)(lr / bc1), b1, b2, eps, (float)(1.0 / sqrt(bc2)));
+  k_adam<<<blocks, 256, 0, (cudaStream_t)stream>>>(g, (size_t)n, make_adam(p, m, v, vmax, lr, b1, b2, eps, weight_decay, step));
   APH_LAUNCH_OK();
   return 0;
 }

@@ -4,7 +4,7 @@
 //   k_finish_bwd   : g_img = Mn^T . (g * out * (1 - out)); accumulates sum g_img . x into stats[2]
 //   k_norm_bwd     : g_x = adjoint of the normalisation, from stats (the FFT fuses it into its row pass, k_row_r2c)
 #pragma once
-#include "aph_common.cuh"
+#include "adam.cuh"
 #include <math.h>
 
 namespace aph {
@@ -58,16 +58,20 @@ static __global__ void __launch_bounds__(256) k_finish_bwd(const float* __restri
 }
 
 // g_x = (c/sigma) (g_img - (x - mu) * dot / ((N-1) sigma^2))      (adjoint of img = x * c / std(x), SURVEY.md A1)
-static __global__ void __launch_bounds__(256) k_norm_bwd(const float* gimg, const float* __restrict__ x_raw,
-                                                  const double* __restrict__ stats, float* gx, size_t n, float contrast) {   // gimg may alias gx
+// With adam.p set, g_x updates that parameter instead of being written (adam.cuh); it may be x_raw itself (the pixel generator).
+static __global__ void __launch_bounds__(256) k_norm_bwd(const float* gimg, const float* x_raw, const double* __restrict__ stats,
+                                                  float* gx, size_t n, float contrast, AdamArgs adam) {   // gimg may alias gx
   const double Nn = (double)n;
   const double mu = stats[0] / Nn;
   const double var = (stats[1] - stats[0] * stats[0] / Nn) / (Nn - 1.0);
   const float c_sig = (float)((double)contrast / sqrt(var));
   const float kk = (float)(stats[2] / ((Nn - 1.0) * var));
   const float muf = (float)mu;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    gx[i] = c_sig * (gimg[i] - (x_raw[i] - muf) * kk);
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const float g = c_sig * (gimg[i] - (x_raw[i] - muf) * kk);
+    if (adam.p) adam_elem(adam, i, g);
+    else gx[i] = g;
+  }
 }
 
 static inline ColMat make_colmat(const float* host) {

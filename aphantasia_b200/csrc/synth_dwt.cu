@@ -123,15 +123,18 @@ __global__ void __launch_bounds__(256) k_dwt_level_fwd(const float* __restrict__
 }
 
 // Adjoint: d_ll [3][llh_alloc][llw] (zero outside h x w), d_bands [3][3][h][w] (already multiplied by s) from d_out [3][oh][ow].
+// With band.p / low.p set, Adam updates the band (and, at the coarsest level, Yl = d_ll's parameter) where its gradient is formed;
+// dll / dbands may then be null and are not written.
 __global__ void __launch_bounds__(256) k_dwt_level_bwd(const float* __restrict__ dout, int oh, int ow, float* __restrict__ dll, int llh_alloc,
-                                                       int llw, float* __restrict__ dbands, float s, int h, int w, Filt f) {
+                                                       int llw, float* __restrict__ dbands, float s, int h, int w, Filt f,
+                                                       AdamArgs band, AdamArgs low) {
   const int p = f.L - 2;
   const size_t total = (size_t)3 * llh_alloc * llw;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
     const int c = (int)(idx / ((size_t)llh_alloc * llw));
     const int r = (int)(idx - (size_t)c * llh_alloc * llw);
     const int k = r / llw, l = r - k * llw;
-    if (k >= h || l >= w) { dll[idx] = 0.f; continue; }      // rows / columns trimmed before the synthesis get no gradient
+    if (k >= h || l >= w) { if (dll) dll[idx] = 0.f; continue; }      // rows / columns trimmed before the synthesis get no gradient
     const float* g = dout + (size_t)c * oh * ow;
     float a_ll = 0.f, a_lh = 0.f, a_hl = 0.f, a_hh = 0.f;
     for (int a = 0; a < f.L; ++a) {
@@ -146,10 +149,12 @@ __global__ void __launch_bounds__(256) k_dwt_level_bwd(const float* __restrict__
       }
       a_ll += f.g0[a] * r0; a_lh += f.g1[a] * r0; a_hl += f.g0[a] * r1; a_hh += f.g1[a] * r1;
     }
-    dll[idx] = a_ll;
-    dbands[((size_t)(c * 3 + 0) * h + k) * w + l] = s * a_lh;
-    dbands[((size_t)(c * 3 + 1) * h + k) * w + l] = s * a_hl;
-    dbands[((size_t)(c * 3 + 2) * h + k) * w + l] = s * a_hh;
+    const size_t b0 = ((size_t)(c * 3) * h + k) * w + l, hw = (size_t)h * w;
+    const float d0 = s * a_lh, d1 = s * a_hl, d2 = s * a_hh;
+    if (dll) dll[idx] = a_ll;
+    if (low.p) adam_elem(low, idx, a_ll);
+    if (dbands) { dbands[b0] = d0; dbands[b0 + hw] = d1; dbands[b0 + 2 * hw] = d2; }
+    if (band.p) { adam_elem(band, b0, d0); adam_elem(band, b0 + hw, d1); adam_elem(band, b0 + 2 * hw, d2); }
   }
 }
 
@@ -229,8 +234,10 @@ extern "C" int aph_synth_dwt_fwd(aph_dwt_plan* plan, const float* const* Ys, con
 
 extern "C" int aph_synth_dwt_bwd(aph_dwt_plan* plan, const float* grad_out, const float* out, const float* x_raw, double* stats,
                                  const float* scales_host, float contrast, const float* colmat_host, int apply_sigmoid,
-                                 float* const* grad_Ys, void* stream) {
-  APH_REQUIRE(plan && grad_out && x_raw && stats && scales_host && grad_Ys, "aph_synth_dwt_bwd: null pointer");
+                                 float* const* grad_Ys, void* stream, float* const* params, float* const* m, float* const* v,
+                                 float* const* vmax, float lr, float b1, float b2, float eps, float weight_decay, int step) {
+  APH_REQUIRE(plan && grad_out && x_raw && stats && scales_host && (grad_Ys || params), "aph_synth_dwt_bwd: null pointer");
+  APH_REQUIRE(!params || (m && v && step >= 1), "aph_synth_dwt_bwd: bad Adam state");
   APH_REQUIRE(!apply_sigmoid || out, "aph_synth_dwt_bwd: sigmoid backward needs the saved output");
   DwtPlanImpl* p = reinterpret_cast<DwtPlanImpl*>(plan);
   cudaStream_t st = (cudaStream_t)stream;
@@ -238,15 +245,20 @@ extern "C" int aph_synth_dwt_bwd(aph_dwt_plan* plan, const float* grad_out, cons
   APH_CUDA_OK(cudaMemsetAsync(stats + 2, 0, sizeof(double), st));
   k_finish_bwd<<<stride_blocks(hw, 16), 256, 0, st>>>(grad_out, out, x_raw, p->gimg, stats, hw, make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
-  k_norm_bwd<<<stride_blocks(3 * hw, 16), 256, 0, st>>>(p->gimg, x_raw, stats, p->gx, 3 * hw, contrast);
+  k_norm_bwd<<<stride_blocks(3 * hw, 16), 256, 0, st>>>(p->gimg, x_raw, stats, p->gx, 3 * hw, contrast, AdamArgs{});
   APH_LAUNCH_OK();
   const int J = p->J;
   for (int i = 0; i < J; ++i) {                        // finest first
     const float* dout = (i == 0) ? p->gx : p->dll[i];
-    float* dll = (i == J - 1) ? grad_Ys[0] : p->dll[i + 1];
+    float* dll = (i == J - 1) ? (grad_Ys ? grad_Ys[0] : nullptr) : p->dll[i + 1];
     const int llh = (i == J - 1) ? p->lh[J - 1] : p->oh[i + 1], llw = (i == J - 1) ? p->lw[J - 1] : p->ow[i + 1];
     const size_t n = (size_t)3 * llh * llw;
-    k_dwt_level_bwd<<<stride_blocks(n, 16), 256, 0, st>>>(dout, p->oh[i], p->ow[i], dll, llh, llw, grad_Ys[i + 1], scales_host[i], p->lh[i], p->lw[i], p->f);
+    // Yl is params[0] and Yh_(i+1) is params[i + 1], as in Ys
+    auto adam_of = [&](int t) { return params ? make_adam(params[t], m[t], v[t], vmax ? vmax[t] : nullptr, lr, b1, b2, eps, weight_decay, step)
+                                              : AdamArgs{}; };
+    k_dwt_level_bwd<<<stride_blocks(n, 16), 256, 0, st>>>(dout, p->oh[i], p->ow[i], dll, llh, llw, grad_Ys ? grad_Ys[i + 1] : nullptr,
+                                                          scales_host[i], p->lh[i], p->lw[i], p->f, adam_of(i + 1),
+                                                          i == J - 1 ? adam_of(0) : AdamArgs{});
     APH_LAUNCH_OK();
   }
   return 0;
@@ -295,16 +307,21 @@ extern "C" int aph_pixel_fwd(const float* x, int64_t hw, float contrast, int fix
 }
 
 extern "C" int aph_pixel_bwd(const float* grad_out, const float* out, const float* x, double* stats, int64_t hw, float contrast,
-                             int fixcontrast, const float* colmat_host, int apply_sigmoid, float* grad_x, void* stream) {
+                             int fixcontrast, const float* colmat_host, int apply_sigmoid, float* grad_x, void* stream, float* params,
+                             float* m, float* v, float* vmax, float lr, float b1, float b2, float eps, float weight_decay, int step) {
   APH_REQUIRE(grad_out && x && stats && grad_x && hw > 0, "aph_pixel_bwd: bad arguments");
+  APH_REQUIRE(!params || (m && v && step >= 1), "aph_pixel_bwd: bad Adam state");
   APH_REQUIRE(!apply_sigmoid || out, "aph_pixel_bwd: sigmoid backward needs the saved output");
   cudaStream_t st = (cudaStream_t)stream;
   APH_CUDA_OK(cudaMemsetAsync(stats + 2, 0, sizeof(double), st));
-  // g_img lands in grad_x, then is rewritten in place by the normalisation adjoint (with fixcontrast the std term vanishes)
+  // g_img lands in grad_x, then is rewritten in place by the normalisation adjoint (with fixcontrast the std term vanishes), or,
+  // with params, feeds the Adam update of params (which may be x itself) in that same pass
   k_finish_bwd<<<stride_blocks((size_t)hw, 16), 256, 0, st>>>(grad_out, out, fixcontrast ? nullptr : x, grad_x, stats, (size_t)hw,
                                                               make_colmat(colmat_host), apply_sigmoid);
   APH_LAUNCH_OK();
-  k_norm_bwd<<<stride_blocks(3 * (size_t)hw, 16), 256, 0, st>>>(grad_x, x, stats, grad_x, 3 * (size_t)hw, contrast);
+  k_norm_bwd<<<stride_blocks(3 * (size_t)hw, 16), 256, 0, st>>>(grad_x, x, stats, grad_x, 3 * (size_t)hw, contrast,
+                                                                params ? make_adam(params, m, v, vmax, lr, b1, b2, eps, weight_decay, step)
+                                                                       : AdamArgs{});
   APH_LAUNCH_OK();
   return 0;
 }

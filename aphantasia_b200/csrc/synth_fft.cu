@@ -211,17 +211,8 @@ __device__ void fft_lines_inreg(float2* buf, const float2* tw, int N, const Radi
 
 // ---------------------------------------------------------------------------------------------
 // Column pass. FWD: in = params [3][H][Wh] complex (+scale, +shift), out = T. !FWD: in = dT, out = dP*scale.
-// Adam state for the fused update (row f2 of SURVEY 8f): the backward's last pass already holds dP = scale * dZ in registers,
-// so p / m / v are updated right there instead of writing dP, re-reading it in torch.optim.Adam's ~12 launches.
-struct AdamArgs { float2* p; float2* m; float2* v; float step_size, b1, b2, eps, inv_sqrt_bc2; int on; };
-
-__device__ __forceinline__ float adam_elem(float& p, float& m, float& v, float g, const AdamArgs& a) {
-  m = a.b1 * m + (1.f - a.b1) * g;
-  v = a.b2 * v + (1.f - a.b2) * g * g;
-  p -= a.step_size * m / (sqrtf(v) * a.inv_sqrt_bc2 + a.eps);
-  return p;
-}
-
+// With adam.p set, the backward's last pass already holds dP = scale * dZ in registers (row f2 of SURVEY 8f): p / m / v are
+// updated right there (adam.cuh) instead of writing dP and re-reading it in the optimiser.
 template <bool FWD, bool SINGLE = false>
 __global__ void __launch_bounds__(SINGLE ? 512 : 256, SINGLE ? 1 : 2) k_col_fft(const float2* __restrict__ in, float2* __restrict__ out,
                                                  const float* __restrict__ scale, const float* __restrict__ shift,
@@ -264,11 +255,7 @@ __global__ void __launch_bounds__(SINGLE ? 512 : 256, SINGLE ? 1 : 2) k_col_fft(
       float2 v = res[c * LS + n1];
       if (!FWD) {
         const float s = scale[g]; v.x *= s; v.y *= s;
-        if (adam.on) {
-          float2 pp = adam.p[ch * plane + g], mm = adam.m[ch * plane + g], vv = adam.v[ch * plane + g];
-          adam_elem(pp.x, mm.x, vv.x, v.x, adam); adam_elem(pp.y, mm.y, vv.y, v.y, adam);
-          adam.p[ch * plane + g] = pp; adam.m[ch * plane + g] = mm; adam.v[ch * plane + g] = vv;
-        }
+        if (adam.p) { adam_elem(adam, 2 * (ch * plane + g), v.x); adam_elem(adam, 2 * (ch * plane + g) + 1, v.y); }
       }
       if (out) out[ch * plane + g] = v;
     }
@@ -498,7 +485,7 @@ extern "C" int aph_synth_fft_fwd(aph_fft_plan* plan, const float* params, const 
 static int synth_fft_bwd_impl(aph_fft_plan* plan, const float* grad_out, const float* out, const float* x_raw,
                               double* stats, const float* scale, float contrast, const float* colmat_host,
                               int apply_sigmoid, float* grad_params, const AdamArgs& adam, void* stream) {
-  APH_REQUIRE(plan && grad_out && x_raw && stats && scale && (grad_params || adam.on), "aph_synth_fft_bwd: null pointer");
+  APH_REQUIRE(plan && grad_out && x_raw && stats && scale && (grad_params || adam.p), "aph_synth_fft_bwd: null pointer");
   APH_REQUIRE(!apply_sigmoid || out, "aph_synth_fft_bwd: sigmoid backward needs the saved output");
   FftPlanImpl* p = reinterpret_cast<FftPlanImpl*>(plan);
   cudaStream_t st = (cudaStream_t)stream;
@@ -530,13 +517,10 @@ extern "C" int aph_synth_fft_bwd(aph_fft_plan* plan, const float* grad_out, cons
 extern "C" int aph_synth_fft_bwd_adam(aph_fft_plan* plan, const float* grad_out, const float* out, const float* x_raw,
                                       double* stats, const float* scale, float contrast, const float* colmat_host,
                                       int apply_sigmoid, float* grad_params, float* params, float* m, float* v,
-                                      float lr, float b1, float b2, float eps, int step, void* stream) {
+                                      float lr, float b1, float b2, float eps, int step, void* stream, float weight_decay, float* vmax) {
   APH_REQUIRE(params && m && v && step >= 1, "aph_synth_fft_bwd_adam: bad Adam state");
-  const double bc1 = 1.0 - pow((double)b1, step), bc2 = 1.0 - pow((double)b2, step);
-  AdamArgs a;
-  a.p = reinterpret_cast<float2*>(params); a.m = reinterpret_cast<float2*>(m); a.v = reinterpret_cast<float2*>(v);
-  a.step_size = (float)(lr / bc1); a.b1 = b1; a.b2 = b2; a.eps = eps; a.inv_sqrt_bc2 = (float)(1.0 / sqrt(bc2)); a.on = 1;
-  return synth_fft_bwd_impl(plan, grad_out, out, x_raw, stats, scale, contrast, colmat_host, apply_sigmoid, grad_params, a, stream);
+  return synth_fft_bwd_impl(plan, grad_out, out, x_raw, stats, scale, contrast, colmat_host, apply_sigmoid, grad_params,
+                            make_adam(params, m, v, vmax, lr, b1, b2, eps, weight_decay, step), stream);
 }
 
 // Analysis (image-file resume, aphantasia/image.py:208-220): spectrum [3,H,Wh,2] = ascale * rfftn(img [3,H,W], 'ortho'). The row

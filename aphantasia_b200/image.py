@@ -149,16 +149,13 @@ class _SynthFFT(torch.autograd.Function):
         x_raw, stats, out = ctx.saved_tensors
         gen = ctx.gen
         g = grad_out.contiguous().float()
-        fo = gen.fused_opt
-        opt = fo[0]() if (fo is not None and gen.pending_fwd == 1) else None
-        if opt is not None:
-            # row f2: exactly one grad-tracked synthesis since the last optimizer.step() -> this backward IS the whole gradient of
-            # the spectrum; Adam runs in the last FFT pass (dP never leaves registers) and step() finds nothing left to do
-            m, v, lr, b1, b2, eps, step = opt._fused_args(fo[1], fo[2])
-            p = gen.params
+        fused = gen.fused_adam([gen.params])
+        if fused is not None:
+            # Adam runs in the last FFT pass (dP never leaves registers) and step() finds nothing left to do
+            ((p, m, v, vmax),), (lr, b1, b2, eps, wd, step) = fused
             check(lib().aph_synth_fft_bwd_adam(gen.plan, g.data_ptr(), out.data_ptr(), x_raw.data_ptr(), stats.data_ptr(), gen.scale.data_ptr(),
                                                ctx.contrast, ctx.colmat, ctx.sigmoid, None, p.data_ptr(), m.data_ptr(), v.data_ptr(),
-                                               lr, b1, b2, eps, step, stream_ptr()), 'aph_synth_fft_bwd_adam')
+                                               lr, b1, b2, eps, step, stream_ptr(), wd, _ptr(vmax)), 'aph_synth_fft_bwd_adam')
             return None, None, None, None, None, None
         gp = _pool.empty((1, 3, gen.h, gen.wh, 2))
         check(lib().aph_synth_fft_bwd(gen.plan, g.data_ptr(), out.data_ptr(), x_raw.data_ptr(), stats.data_ptr(), gen.scale.data_ptr(),
@@ -203,9 +200,30 @@ def _shared_fft_scale(h, w, decay_power):
 class _Generator:
     """An `image_f` closure as a callable object. Its fused(colmat, sigmoid, *args, **kwargs) parses the closure's arguments
     and runs the synthesis with to_valid_rgb's colour matrix and sigmoid fused into its last kernel; a plain call has neither."""
+    fused_opt, pending_fwd = None, 0          # aphantasia_b200.optim hooks in here (row f2)
 
     def __call__(self, *args, **kwargs):
         return self.fused(None, False, *args, **kwargs)
+
+    def _track(self, params):
+        """Counts the grad-tracked syntheses since the optimiser's last step()."""
+        if torch.is_grad_enabled() and any(p.requires_grad for p in params):
+            self.pending_fwd += 1
+
+    def fused_adam(self, params):
+        """The optimiser step to run inside this synthesis backward, as aphantasia_b200.optim.Adam._fused_args returns it, or
+        None. Only when exactly one grad-tracked synthesis ran since the last step() is this backward the whole gradient of
+        the parameters; otherwise (--enforce synthesises twice) step() updates them from their .grad."""
+        opt = self.fused_opt() if self.fused_opt is not None and self.pending_fwd == 1 else None
+        return opt._fused_args(params) if opt is not None else None
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+def _ptrs(ts):
+    return (C.c_void_p * len(ts))(*[t.data_ptr() for t in ts])
 
 
 class FFTImage(_Generator):
@@ -215,13 +233,11 @@ class FFTImage(_Generator):
         self.params, self.h, self.w, self.wh = params, h, w, w // 2 + 1
         self.scale = _shared_fft_scale(h, w, decay_power)
         self.plan = _shared_fft_plan(h, w)
-        self.fused_opt, self.pending_fwd = None, 0          # aphantasia_b200.optim.Adam hooks in here (row f2)
         from .optim import register_generator
         register_generator(params, self)
 
     def fused(self, colmat, sigmoid, /, shift=None, contrast=1., *noargs, **nokwargs):
-        if torch.is_grad_enabled() and self.params.requires_grad:
-            self.pending_fwd += 1
+        self._track([self.params])
         return _SynthFFT.apply(self.params, self, shift, contrast, colmat, sigmoid)
 
 
@@ -267,7 +283,7 @@ def fft_image(shape, sd=0.01, decay_power=1.0, resume=None):
 
 class _SynthPixel(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, contrast, fixcontrast, colmat, sigmoid):
+    def forward(ctx, x, contrast, fixcontrast, colmat, sigmoid, gen):
         require_cuda(x, 'pixel parameters')
         xi = x.detach().contiguous().float()
         assert xi.shape[0] == 1 and xi.shape[1] == 3, 'pixel_image expects [1,3,H,W]'
@@ -277,6 +293,7 @@ class _SynthPixel(torch.autograd.Function):
         check(lib().aph_pixel_fwd(xi.data_ptr(), hw, float(contrast), int(bool(fixcontrast)), colmat, int(sigmoid), stats.data_ptr(),
                                   out.data_ptr(), stream_ptr()), 'aph_pixel_fwd')
         ctx.args = (hw, float(contrast), int(bool(fixcontrast)), colmat, int(sigmoid))
+        ctx.gen = gen
         ctx.save_for_backward(xi, stats, out)
         return out
 
@@ -286,9 +303,16 @@ class _SynthPixel(torch.autograd.Function):
         hw, contrast, fix, colmat, sig = ctx.args
         g = g.contiguous().float()
         gx = torch.empty_like(xi)
+        fused = ctx.gen.fused_adam([ctx.gen.image_t])
+        if fused is not None:          # x is updated in the normalisation adjoint's pass; gx is only scratch
+            ((p, m, v, vmax),), (lr, b1, b2, eps, wd, step) = fused
+            check(lib().aph_pixel_bwd(g.data_ptr(), out.data_ptr(), xi.data_ptr(), stats.data_ptr(), hw, contrast, fix, colmat, sig,
+                                      gx.data_ptr(), stream_ptr(), p.data_ptr(), m.data_ptr(), v.data_ptr(), _ptr(vmax), lr, b1, b2, eps,
+                                      wd, step), 'aph_pixel_bwd')
+            return None, None, None, None, None, None
         check(lib().aph_pixel_bwd(g.data_ptr(), out.data_ptr(), xi.data_ptr(), stats.data_ptr(), hw, contrast, fix, colmat, sig, gx.data_ptr(),
                                   stream_ptr()), 'aph_pixel_bwd')
-        return gx, None, None, None, None
+        return gx, None, None, None, None, None
 
 
 class PixelImage(_Generator):
@@ -296,9 +320,12 @@ class PixelImage(_Generator):
 
     def __init__(self, image_t):
         self.image_t = image_t
+        from .optim import register_generator
+        register_generator(image_t, self)
 
     def fused(self, colmat, sigmoid, /, shift=None, contrast=1., fixcontrast=False, *noargs, **nokwargs):
-        return _SynthPixel.apply(self.image_t, contrast, fixcontrast, colmat, sigmoid)
+        self._track([self.image_t])
+        return _SynthPixel.apply(self.image_t, contrast, fixcontrast, colmat, sigmoid, self)
 
 
 def pixel_image(shape, resume=None, sd=1., *noargs, **nokwargs):
@@ -391,8 +418,16 @@ class _SynthDWT(torch.autograd.Function):
         x_raw, stats, out = ctx.saved_tensors
         gen = ctx.gen
         g = grad_out.contiguous().float()
+        fused = gen.fused_adam(gen.Ys)
+        if fused is not None:          # each band, and Yl, is updated by the level adjoint that forms its gradient
+            tensors, (lr, b1, b2, eps, wd, step) = fused
+            ps, ms, vs, vmaxs = zip(*tensors)
+            check(lib().aph_synth_dwt_bwd(gen.plan, g.data_ptr(), out.data_ptr(), x_raw.data_ptr(), stats.data_ptr(), gen.scales_c, ctx.contrast,
+                                          ctx.colmat, ctx.sigmoid, None, stream_ptr(), _ptrs(ps), _ptrs(ms), _ptrs(vs),
+                                          _ptrs(vmaxs) if vmaxs[0] is not None else None, lr, b1, b2, eps, wd, step), 'aph_synth_dwt_bwd')
+            return (None,) * (4 + len(ctx.shapes))
         grads = [torch.empty(sh, device=g.device, dtype=torch.float32) for sh in ctx.shapes]
-        ptrs = (C.c_void_p * len(grads))(*[t.data_ptr() for t in grads])
+        ptrs = _ptrs(grads)
         check(lib().aph_synth_dwt_bwd(gen.plan, g.data_ptr(), out.data_ptr(), x_raw.data_ptr(), stats.data_ptr(), gen.scales_c, ctx.contrast,
                                       ctx.colmat, ctx.sigmoid, ptrs, stream_ptr()), 'aph_synth_dwt_bwd')
         return (None, None, None, None) + tuple(grads)
@@ -422,6 +457,7 @@ class DWTImage(_Generator):
         return [(1, 3, hJ, wJ)] + [(1, 3, 3, hh, ww) for (hh, ww) in self.level_hw]
 
     def fused(self, colmat, sigmoid, /, shift=None, contrast=1., *noargs, **nokwargs):
+        self._track(self.Ys)
         return _SynthDWT.apply(self, contrast, colmat, sigmoid, *self.Ys)
 
 
@@ -497,4 +533,7 @@ def dwt_image(shape, wave='coif2', sharp=0.3, colors=1., resume=None):
     assert [tuple(y.shape) for y in Ys] == gen.param_shapes(), 'dwt_image: parameter shapes do not match this size / wavelet'
     Ys = [y.requires_grad_(True) for y in Ys]
     gen.Ys = Ys
+    from .optim import register_generator
+    for y in Ys:
+        register_generator(y, gen)
     return Ys, gen, size

@@ -124,7 +124,7 @@ def main(argv=None):
     origins = install_dropin(os.path.dirname(script))
     from . import motion
     motion.install()
-    if os.environ.get('APH_FUSED_ADAM', '0') == '1':          # row f2: torch.optim.Adam over our spectrum -> fused into the synth backward
+    if os.environ.get('APH_FUSED_ADAM', '0') == '1':          # row f2: torch.optim.Adam / AdamW over our generators -> fused into their backward
         from . import optim
         optim.install()
     if os.environ.get('APH_RUN_VERBOSE', '0') == '1':

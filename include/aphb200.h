@@ -110,10 +110,15 @@ int aph_dwt_plan_levels(const aph_dwt_plan* plan, int* J, int* dims, int* out_hw
 int aph_synth_dwt_fwd(aph_dwt_plan* plan, const float* const* Ys, const float* scales_host, float contrast,
                       const float* colmat_host, int apply_sigmoid, float* x_raw, double* stats, float* out,
                       void* stream);
-/* grad_Ys: HOST array of J+1 DEVICE pointers receiving d loss / d Ys (overwritten).                               */
+/* grad_Ys: HOST array of J+1 DEVICE pointers receiving d loss / d Ys (overwritten).
+ * Adam fused into the backward (the trailing arguments; params == NULL: none): params / m / v (and vmax, may be NULL) are
+ * HOST arrays of J+1 DEVICE pointers ordered as Ys, every tensor updated in place by step `step` of aph_adam_step where
+ * its gradient is formed. grad_Ys may then be NULL (nothing is written).                                               */
 int aph_synth_dwt_bwd(aph_dwt_plan* plan, const float* grad_out, const float* out, const float* x_raw,
                       double* stats, const float* scales_host, float contrast, const float* colmat_host,
-                      int apply_sigmoid, float* const* grad_Ys, void* stream);
+                      int apply_sigmoid, float* const* grad_Ys, void* stream,
+                      float* const* params, float* const* m, float* const* v, float* const* vmax,
+                      float lr, float b1, float b2, float eps, float weight_decay, int step);
 /* Analysis of an image (img2dwt, aphantasia/image.py:82-94): DWTForward(J, wave, mode='symmetric') of img [3,H,W] (H, W of
  * the plan), rows filtered before columns, bands (LH, HL, HH). Ys: HOST array of J+1 DEVICE pointers shaped as for
  * aph_synth_dwt_fwd, overwritten; Yh_i is multiplied by inv_scales_host[i] (HOST [J]). Uses the plan's LL scratch; the
@@ -124,8 +129,13 @@ int aph_dwt_analyze(aph_dwt_plan* plan, const float* img, const float* inv_scale
  * fixcontrast), fused with to_valid_rgb. x / out / grad_x are [3,H,W]; stats as above.                             */
 int aph_pixel_fwd(const float* x, int64_t hw, float contrast, int fixcontrast, const float* colmat_host,
                   int apply_sigmoid, double* stats, float* out, void* stream);
+/* Adam fused into the backward (the trailing arguments; params == NULL: none): params / m / v (and vmax, may be NULL)
+ * [3,H,W] are updated in place by step `step` of aph_adam_step from d loss / d x; params may be x itself. grad_x is then
+ * scratch, and does not receive the gradient.                                                                        */
 int aph_pixel_bwd(const float* grad_out, const float* out, const float* x, double* stats, int64_t hw, float contrast,
-                  int fixcontrast, const float* colmat_host, int apply_sigmoid, float* grad_x, void* stream);
+                  int fixcontrast, const float* colmat_host, int apply_sigmoid, float* grad_x, void* stream,
+                  float* params, float* m, float* v, float* vmax, float lr, float b1, float b2, float eps,
+                  float weight_decay, int step);
 
 /* Stand-alone to_valid_rgb for a foreign image_f (aphantasia/image.py:21-28): img [3,H,W] -> out.  */
 int aph_valid_rgb_fwd(const float* img, int64_t hw, const float* colmat_host, float* out, void* stream);
@@ -435,17 +445,22 @@ int aph_lpips_conv0_test(int fwd, const void* in, const float* weight, const flo
 int aph_lpips_pool_test(int fwd, const void* x, const void* dy, void* out, int N, int H, int W, int C, void* stream);
 
 /* ================= step glue ==================================================================
- * torch.optim.Adam(betas=(b1,b2)) single-tensor update (clip_fft.py:108-115,295), bias-corrected. */
+ * torch.optim.Adam(betas=(b1,b2)) / AdamW(..., weight_decay, amsgrad) single-tensor update of step `step` >= 1
+ * (clip_fft.py:108-115,295), bias-corrected: weight_decay != 0 decays p by 1 - lr * weight_decay first (AdamW);
+ * vmax != NULL is AMSGrad's running maximum of v, and the denominator uses it. The trailing arguments come after the
+ * stream so that callers of the plain form bind unchanged (the Python binding passes 0 / NULL for them).           */
 int aph_adam_step(float* p, const float* g, float* m, float* v, int64_t n,
-                  float lr, float b1, float b2, float eps, int step, void* stream);
+                  float lr, float b1, float b2, float eps, int step, void* stream,
+                  float weight_decay, float* vmax);
 
 /* SURVEY.md 8 row f2: aph_synth_fft_bwd with the Adam update of the spectrum fused into its last pass (the data
- * gradient dP is in registers there): params / m / v [3,H,Wh,2] are updated in place; grad_params may be NULL
+ * gradient dP is in registers there): params / m / v (/ vmax) [3,H,Wh,2] are updated in place; grad_params may be NULL
  * (nothing is written) or receives dP as aph_synth_fft_bwd does. Same arithmetic as aph_adam_step.              */
 int aph_synth_fft_bwd_adam(aph_fft_plan* plan, const float* grad_out, const float* out, const float* x_raw,
                            double* stats, const float* scale, float contrast, const float* colmat_host,
                            int apply_sigmoid, float* grad_params, float* params, float* m, float* v,
-                           float lr, float b1, float b2, float eps, int step, void* stream);
+                           float lr, float b1, float b2, float eps, int step, void* stream,
+                           float weight_decay, float* vmax);
 
 /* ================= multi-GPU exchange (SURVEY.md 8e) ==========================================
  * In-place all-reduce(SUM) of a fp32 buffer in SYMMETRIC memory (the canvas gradient dRGB [3,H,W], replacing the
