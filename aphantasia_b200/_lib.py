@@ -67,6 +67,20 @@ _SIGS = {
     'aph_rn_tokens_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
     'aph_gemm_rn_epi_test': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_void_p, C.c_void_p, C.c_int,
                                        C.c_void_p, C.c_void_p]),
+    'aph_vqgan_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p]),
+    'aph_vqgan_destroy': (C.c_int, [C.c_void_p]),
+    'aph_vqgan_load_tensor': (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.c_int64, C.c_void_p]),
+    'aph_vqgan_finalize': (C.c_int, [C.c_void_p]),
+    'aph_vqgan_fwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_int, C.c_void_p]),
+    'aph_vqgan_bwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_void_p]),
+    'aph_vqgan_bytes': (C.c_int64, [C.c_void_p]),
+    'aph_vqgan_gn_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, c_f32p, c_f32p, C.c_int, C.c_void_p, c_f32p, C.c_void_p, C.c_int,
+                                    C.c_int, C.c_int, C.c_void_p]),
+    'aph_vqgan_conv_test': (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
+                                      C.c_void_p]),
+    'aph_vqgan_up_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    'aph_vqgan_attn_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    'aph_vqgan_ends_test': (C.c_int, [C.c_int, C.c_void_p, c_f32p, c_f32p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     'aph_text_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p]),
     'aph_text_destroy': (C.c_int, [C.c_void_p]),
     'aph_text_load_tensor': (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, C.c_int64, C.c_void_p]),
@@ -134,6 +148,11 @@ class RnConfig(C.Structure):
 
 class TextConfig(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ('width', 'layers', 'heads', 'out_dim', 'context', 'vocab', 'max_batch', 'reserved')]
+
+
+class VqganConfig(C.Structure):
+    _fields_ = [('z_channels', C.c_int32), ('ch', C.c_int32), ('ch_mult', C.c_int32 * 8)] + \
+               [(n, C.c_int32) for n in ('num_levels', 'num_res_blocks', 'attn_mask', 'out_ch', 'max_batch', 'max_tokens')]
 
 
 def lib():
@@ -217,3 +236,4 @@ def require_cuda(t, name):
     import torch
     if not (isinstance(t, torch.Tensor) and t.is_cuda):
         raise RuntimeError('aphantasia_b200: %s must be a CUDA tensor; this implementation has no CPU path' % name)
+

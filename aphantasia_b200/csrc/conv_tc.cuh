@@ -15,19 +15,24 @@
 //   CONV_BIAS_RELU  out = max(acc + bias, 0)                       forward
 //   CONV_MASK       out = mask > 0 ? acc : 0                       data gradient into a layer whose input is a ReLU output (mask):
 //                                                                  a select, so a non-finite value under a zero mask never passes
-//   CONV_PLAIN      out = acc                                      data gradient into a max-pool output (lpips.cu finishes it)
+//   CONV_PLAIN      out = acc                                      data gradient into a max-pool output (lpips.cu finishes it), and
+//                                                                  every data gradient of the VQGAN decoder (vqgan.cu)
+//   CONV_BIAS       out = acc + bias                               the VQGAN decoder's convolutions (no activation after them)
+//   CONV_BIAS_RESID out = acc + bias + resid                       its ResnetBlock's conv2, with the shortcut as a bf16 residual
 #pragma once
 #include "tc_gemm.cuh"
 
 namespace aph {
 
-enum : int { CONV_BIAS_RELU = 0, CONV_MASK = 1, CONV_PLAIN = 2 };
+enum : int { CONV_BIAS_RELU = 0, CONV_MASK = 1, CONV_PLAIN = 2, CONV_BIAS = 3, CONV_BIAS_RESID = 4 };
+template <int EPI> constexpr bool conv_has_bias() { return EPI == CONV_BIAS_RELU || EPI == CONV_BIAS || EPI == CONV_BIAS_RESID; }
 constexpr int CONV_TH = 8, CONV_TW = 16;   // the 128-pixel spatial tile
 
 struct ConvShape { int N, H, W, Cin, Cout, tiles_y, tiles_x; };
 struct ConvEpi {
-  const float* bias = nullptr;   // [Cout] (CONV_BIAS_RELU)
+  const float* bias = nullptr;   // [Cout] (CONV_BIAS_RELU, CONV_BIAS, CONV_BIAS_RESID)
   const bf16* mask = nullptr;    // bf16 NHWC [N,H,W,Cout] (CONV_MASK)
+  const bf16* resid = nullptr;   // bf16 NHWC [N,H,W,Cout] (CONV_BIAS_RESID)
   bf16* out = nullptr;           // bf16 NHWC [N,H,W,Cout]
 };
 
@@ -44,6 +49,7 @@ __device__ __forceinline__ void conv_store_bf16x32(const ConvEpi& epi, size_t pi
     m[0] = g.x; m[1] = g.y; m[2] = g.z; m[3] = g.w;
     quad_transpose(m, q);                                        // back to the accumulator layout
   }
+  if constexpr (EPI == CONV_BIAS_RESID) load_bf16x8_acc(epi.resid, off, valid, q, m);
 #pragma unroll
   for (int t = 0; t < 4; ++t) {
     const float v0 = v[2 * t], v1 = v[2 * t + 1];
@@ -52,6 +58,11 @@ __device__ __forceinline__ void conv_store_bf16x32(const ConvEpi& epi, size_t pi
     } else if (EPI == CONV_MASK) {
       const float2 h = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&m[t]));
       w[t] = pack_bf16(h.x > 0.f ? v0 : 0.f, h.y > 0.f ? v1 : 0.f);
+    } else if (EPI == CONV_BIAS) {
+      w[t] = pack_bf16(v0 + bb[t].x, v1 + bb[t].y);
+    } else if (EPI == CONV_BIAS_RESID) {
+      const float2 r = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&m[t]));
+      w[t] = pack_bf16(v0 + bb[t].x + r.x, v1 + bb[t].y + r.y);
     } else {
       w[t] = pack_bf16(v0, v1);
     }
@@ -100,7 +111,7 @@ struct ConvProblem {
       float v0[8], v1[8];
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
-        bb[i] = (EPI == CONV_BIAS_RELU) ? __ldg(reinterpret_cast<const float2*>(epi.bias + col0 + 8 * i + col_in_tile)) : make_float2(0.f, 0.f);
+        bb[i] = conv_has_bias<EPI>() ? __ldg(reinterpret_cast<const float2*>(epi.bias + col0 + 8 * i + col_in_tile)) : make_float2(0.f, 0.f);
         v0[2 * i] = d[0][4 * (j0 + i)]; v0[2 * i + 1] = d[0][4 * (j0 + i) + 1];
         v1[2 * i] = d[0][4 * (j0 + i) + 2]; v1[2 * i + 1] = d[0][4 * (j0 + i) + 3];
       }

@@ -247,14 +247,18 @@ int launch_conv3x3(const void* x, const void* wpack, int N, int H, int W, int Ci
                    cudaStream_t st) {
   APH_REQUIRE(x && wpack && epi.out && N > 0 && H > 0 && W > 0, "conv3x3: null operand or empty shape");
   APH_REQUIRE(Cin % 64 == 0 && Cout % 64 == 0 && Cin > 0 && Cout > 0, "conv3x3: C_in=%d and C_out=%d must be multiples of 64", Cin, Cout);
-  APH_REQUIRE(epi_kind != CONV_BIAS_RELU || epi.bias, "conv3x3: the forward epilogue needs a bias");
+  APH_REQUIRE((epi_kind != CONV_BIAS_RELU && epi_kind != CONV_BIAS && epi_kind != CONV_BIAS_RESID) || epi.bias,
+              "conv3x3: the forward epilogues need a bias");
+  APH_REQUIRE(epi_kind != CONV_BIAS_RESID || epi.resid, "conv3x3: the residual epilogue needs a residual");
   APH_REQUIRE(epi_kind != CONV_MASK || epi.mask, "conv3x3: the masked epilogue needs a mask");
-  APH_REQUIRE((reinterpret_cast<uintptr_t>(epi.out) & 15) == 0 && (reinterpret_cast<uintptr_t>(epi.mask) & 15) == 0,
-              "conv3x3: output and mask must be 16-byte aligned");
+  APH_REQUIRE(((reinterpret_cast<uintptr_t>(epi.out) | reinterpret_cast<uintptr_t>(epi.mask) | reinterpret_cast<uintptr_t>(epi.resid)) & 15) == 0,
+              "conv3x3: output, mask and residual must be 16-byte aligned");
   const ConvShape cs{N, H, W, Cin, Cout, (H + CONV_TH - 1) / CONV_TH, (W + CONV_TW - 1) / CONV_TW};
   const bool wide = Cout % 128 == 0;
 #define APH_CONV_CASE(K) case K: return wide ? conv_cfg<128, K>(x, wpack, cs, epi, st) : conv_cfg<64, K>(x, wpack, cs, epi, st);
-  switch (epi_kind) { APH_CONV_CASE(CONV_BIAS_RELU) APH_CONV_CASE(CONV_MASK) APH_CONV_CASE(CONV_PLAIN) }
+  switch (epi_kind) {
+    APH_CONV_CASE(CONV_BIAS_RELU) APH_CONV_CASE(CONV_MASK) APH_CONV_CASE(CONV_PLAIN) APH_CONV_CASE(CONV_BIAS) APH_CONV_CASE(CONV_BIAS_RESID)
+  }
 #undef APH_CONV_CASE
   set_error("conv3x3: unknown epilogue kind %d", epi_kind);
   return 2;

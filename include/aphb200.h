@@ -316,6 +316,67 @@ int aph_rn_tokens_test(int fwd, const void* in, const void* aux, void* out, int 
 int aph_gemm_rn_epi_test(const void* A, const void* B, int M, int N, int K, const float* bias, const void* resid_bf16,
                          const void* mask, int relu, void* out_bf16, void* stream);
 
+/* ================= VQGAN decoder (taming) ==========================================================
+ * Replaces taming.modules.diffusionmodules.model.Decoder.forward (eval mode, temb_ch = 0, dropout 0, resamp_with_conv,
+ * give_pre_end False, out_ch 3) and its data gradient d loss / d z. No weight gradients: the weights are constants.
+ * Levels i = 0 (finest) .. num_levels - 1 have width ch * ch_mult[i]; attn_mask bit i puts an AttnBlock after each ResnetBlock
+ * of level i (taming: curr_res of level i in attn_resolutions). Widths are multiples of 64; those of a nin_shortcut (a width
+ * change) or an attention (the mid block's, and the levels of attn_mask) are multiples of 128.
+ * Keys of aph_vqgan_load_tensor are taming's without "decoder.", with each AttnBlock's q, k, v stacked into
+ * "<p>.qkv.weight" [3C, C] = [q; k; v] (1x1 kernels flattened) and "<p>.qkv.bias" [3C] (aphantasia_b200.vqgan.pack_state_dict),
+ * nin_shortcut and proj_out flattened to [C_out, C_in]. aph_vqgan_finalize checks every tensor arrived.
+ * The attention materialises its T x T scores per image: T = h w (the latent's tokens when attention sits at the latent
+ * resolution, h w 4^k k levels finer) is at most APH_VQGAN_MAX_TOKENS.
+ * Device bytes (aph_vqgan_bytes) = weights + arena. S = max_batch, T = max_tokens, z = z_channels, c_top = ch ch_mult[L-1];
+ * the ops after conv_in are the ResnetBlocks (cin -> cout), AttnBlocks (width C) and Upsamples (width C) in forward order, op k
+ * running at s_k = 4^(upsamples before it) times the latent's pixels (an Upsample's output at 4 s_k), s_f the finest scale;
+ * Tp(t) = t rounded up to a multiple of 128; t_a, c_a the largest attention token count T s_k and width:
+ *   weights  2 * 2 * 9 (z c_top + sum_res (cin cout + cout^2) + sum_up C^2) + 2 * 2 (sum_nin cin cout + sum_attn 4 C^2)
+ *            + 4 (c_top + sum_res 2 cout + sum_nin cout + sum_attn 4 C + sum_up C + sum_norm 2 C + 27 c_out + 3)
+ *   arena    2 S T (z + c_top) + sum_res 2 * 2 S T s_k cout + sum_attn 2 S T s_k (5 C + Tp(T s_k)) + sum_up 2 S T 4 s_k C
+ *            + 4 * 64 S (each GroupNorm's statistics) + 4 * 2 S emax + 4 S (64 ceil(T s_f / 256) + 64)
+ *            + (with attention) 2 S t_a 3 c_a + 6 t_a Tp(t_a) + 2 Tp(t_a)^2 + 4 Tp(t_a) c_a
+ *            emax = the largest per-image T s_k * width over conv_in's z and output and every op's input and output         */
+#define APH_VQGAN_MAX_TOKENS 16384
+typedef struct aph_vqgan aph_vqgan;
+typedef struct {
+  int32_t z_channels;      /* 256                                                        */
+  int32_t ch;              /* 128                                                        */
+  int32_t ch_mult[8];      /* (1, 1, 2, 2, 4) f16, (1, 1, 2, 4) f8; num_levels used       */
+  int32_t num_levels;
+  int32_t num_res_blocks;  /* 2                                                          */
+  int32_t attn_mask;       /* bit i: AttnBlocks at level i                               */
+  int32_t out_ch;          /* 3                                                          */
+  int32_t max_batch;       /* largest N a call will pass                                 */
+  int32_t max_tokens;      /* largest latent h w a call will pass                        */
+} aph_vqgan_config;
+int aph_vqgan_create(aph_vqgan** vq, const aph_vqgan_config* cfg);
+int aph_vqgan_destroy(aph_vqgan* vq);
+int aph_vqgan_load_tensor(aph_vqgan* vq, const char* key, const float* data, int64_t numel, void* stream);
+int aph_vqgan_finalize(aph_vqgan* vq);
+/* z [N,z_channels,h,w] fp32 -> out [N,3,h 2^(L-1),w 2^(L-1)] fp32, h w <= max_tokens. save_for_bwd 0/1.                        */
+int aph_vqgan_fwd(aph_vqgan* vq, const float* z, int N, int h, int w, float* out, int save_for_bwd, void* stream);
+/* grad_out [N,3,H,W] -> grad_z [N,z_channels,h,w] (overwritten), from the last aph_vqgan_fwd(save_for_bwd = 1) of the same N, h, w. */
+int aph_vqgan_bwd(aph_vqgan* vq, const float* grad_out, int N, int h, int w, float* grad_z, void* stream);
+int64_t aph_vqgan_bytes(const aph_vqgan* vq);
+/* Test entries of the decoder's own kernels on caller buffers (bf16 NHWC activations):
+ * aph_vqgan_gn_test: GroupNorm(32, C, eps 1e-6) [+ swish], C a multiple of 64. fwd = 1: x [N,HW,C] -> out, stats fp32 [N,32,2] =
+ *   (mean, rstd); fwd = 0: dout, x, stats (of the forward) -> out = dx [+ resid unless NULL].
+ * aph_vqgan_conv_test: 3x3 convolution, weight fp32 [Cout,Cin,3,3] (packed here): out = conv(x) + bias [+ resid unless NULL].
+ * aph_vqgan_up_test: fwd = 1: in [N,H,W,C] -> out [N,2H,2W,C] (nearest); fwd = 0: in [N,2H,2W,C] -> out [N,H,W,C] (2 x 2 sums).
+ * aph_vqgan_attn_test: one head of width C (a multiple of 128) over T tokens per image. fwd = 1: qkv [N*T,3C] -> out [N*T,C];
+ *   fwd = 0: qkv, dout [N*T,C] -> out = dqkv [N*T,3C].
+ * aph_vqgan_ends_test: kind 0: in fp32 [N,C,H,W] -> out bf16 [N,H,W,C]; 1: the reverse; 2: conv_out, in bf16 [N,H,W,C], weight
+ *   fp32 [3,C,3,3], bias [3] -> out fp32 [N,3,H,W]; 3: its data gradient, in fp32 [N,3,H,W] -> out bf16 [N,H,W,C].          */
+int aph_vqgan_gn_test(int fwd, const void* x, const void* dout, const float* gamma, const float* beta, int swish, const void* resid,
+                      float* stats, void* out, int N, int HW, int C, void* stream);
+int aph_vqgan_conv_test(const void* x, const float* weight, const float* bias, const void* resid, void* out, int N, int H, int W,
+                        int Cin, int Cout, void* stream);
+int aph_vqgan_up_test(int fwd, const void* in, void* out, int N, int H, int W, int C, void* stream);
+int aph_vqgan_attn_test(int fwd, const void* qkv, const void* dout, void* out, int N, int T, int C, void* stream);
+int aph_vqgan_ends_test(int kind, const void* in, const float* weight, const float* bias, void* out, int N, int C, int H, int W,
+                        void* stream);
+
 /* ================= CLIP text encoder (forward only) ===========================================
  * Replaces clip.model.CLIP.encode_text (third-party OpenAI clip; call site clip_fft.py:150), run once per prompt
  * before the optimisation loop: token_embedding[ids] + positional_embedding -> layers x pre-LN residual block with
