@@ -127,7 +127,7 @@ k_conv3x3_tc(const __grid_constant__ CUtensorMap map_x, const __grid_constant__ 
   gemm_body<BN, false>(map_x, map_w, ConvProblem<BN, EPI>{cs, epi});
 }
 
-// Launches the convolution on `st`: x bf16 NHWC [N,H,W,Cin], wpack bf16 [Cout, 9 Cin]; Cin and Cout multiples of 64.
+// Launches the convolution on `st` (conv_tc.cu): x bf16 NHWC [N,H,W,Cin], wpack bf16 [Cout, 9 Cin]; Cin and Cout multiples of 64.
 int launch_conv3x3(const void* x, const void* wpack, int N, int H, int W, int Cin, int Cout, int epi_kind, const ConvEpi& epi,
                    cudaStream_t st);
 

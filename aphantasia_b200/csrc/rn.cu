@@ -9,163 +9,25 @@
 //   attnpool 49 tokens of the 7 x 7 map, their mean prepended, + positional embedding; 32-head attention (head dim 64) queried by
 //            token 0; c_proj of its output
 // Kernels (sm_90a):
-//   stem conv 1         k_rn_stem_fwd / k_rn_stem_bwd: fp32 SIMT (3 input channels, stride 2); they read the caller's fp32 crops
-//                       and write its fp32 crop gradient, outside the cached graphs. Output channels 32-63 are zero, so the two
-//                       other stem convolutions run as 64-channel ones on zero-padded weights
+//   stem conv 1         k_conv3in_fwd / k_conv3in_bwd<2, 32, IN_RAW> (nhwc.cu): fp32 SIMT (3 input channels, stride 2); they read
+//                       the caller's fp32 crops and write its fp32 crop gradient, outside the cached graphs. Output channels 32-63
+//                       are zero, so the two other stem convolutions run as 64-channel ones on zero-padded weights
 //   3x3 convolutions    k_conv3x3_tc (conv_tc.cuh), forward CONV_BIAS_RELU, data gradient CONV_MASK (select by the ReLU output)
 //   1x1 convolutions    launch_gemm on the NHWC tensor viewed as [pixels, C], epilogues EPI_BIAS_RELU / EPI_BIAS_RESID_RELU /
 //                       EPI_BIAS_BF16 forward, EPI_MASK / EPI_MASK_RESID / EPI_BF16 data gradient
-//   average pool        k_avgpool2_fwd, and its adjoint k_avgpool2_bwd fused with the select of the ReLU output below it
+//   average pool        k_pool2<POOL_MEAN> (nhwc.cu), and its adjoint k_unpool2 (scale 1/4) fused with the select of the ReLU
+//                       output below it
 //   attention pool      k_rn_tokens_fwd / _bwd, the q/k/v GEMM, attn_resident at T = 50, c_proj on the token-0 rows
 // The data gradient of a block's input is selected by that input being > 0 in the epilogue of the GEMM that writes it: every
 // block input is a ReLU output, except the first block's, the stem's average pool of a ReLU output, which is 0 exactly where its
 // four inputs are, whose gradient the stem's own ReLU select then drops anyway.
-#include "conv_tc.cuh"
+#include "nhwc.cuh"
 #include "encoder.cuh"
 
 namespace aph {
 
 constexpr int RN_T = 50, RN_GRID = 7;          // attention-pool tokens; the final map is 7 x 7
 constexpr int RN_SIDE_MIN = 223, RN_SIDE_MAX = 254;
-
-// ---- stem conv 1: 3 -> 32, 3x3, stride 2, pad 1, fp32 -------------------------------------------------------------
-// img fp32 NCHW [N,3,side,side] -> out bf16 NHWC [N,Ho,Ho,64] = relu(conv + bias) in channels 0-31, zero in 32-63.
-// w [32][3][3][3], b [32]. One thread per output pixel.
-__global__ void __launch_bounds__(128) k_rn_stem_fwd(const float* __restrict__ img, int N, int side, int Ho, const float* __restrict__ w,
-                                                     const float* __restrict__ b, bf16* __restrict__ out) {
-  __shared__ float sw[32 * 27], sb[32];
-  for (int i = threadIdx.x; i < 32 * 27; i += blockDim.x) sw[i] = w[i];
-  for (int i = threadIdx.x; i < 32; i += blockDim.x) sb[i] = b[i];
-  __syncthreads();
-  const size_t HW = (size_t)Ho * Ho, p = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (p >= (size_t)N * HW) return;
-  const int n = (int)(p / HW), rem = (int)(p - n * HW), oy = rem / Ho, ox = rem - oy * Ho;
-  const size_t plane = (size_t)side * side;
-  float in[27];
-#pragma unroll
-  for (int c = 0; c < 3; ++c)
-#pragma unroll
-    for (int t = 0; t < 9; ++t) {
-      const int y = 2 * oy + t / 3 - 1, x = 2 * ox + t % 3 - 1;
-      in[c * 9 + t] = (y >= 0 && y < side && x >= 0 && x < side) ? img[((size_t)n * 3 + c) * plane + (size_t)y * side + x] : 0.f;
-    }
-  uint4* o = reinterpret_cast<uint4*>(out + p * 64);
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    float acc[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const float* wj = sw + (8 * g + j) * 27;
-      float s = sb[8 * g + j];
-#pragma unroll
-      for (int k = 0; k < 27; ++k) s = fmaf(wj[k], in[k], s);
-      acc[j] = fmaxf(s, 0.f);
-    }
-    o[g] = make_uint4(pack_bf16(acc[0], acc[1]), pack_bf16(acc[2], acc[3]), pack_bf16(acc[4], acc[5]), pack_bf16(acc[6], acc[7]));
-  }
-#pragma unroll
-  for (int g = 4; g < 8; ++g) o[g] = make_uint4(0u, 0u, 0u, 0u);
-}
-
-// grad fp32 NCHW [N,3,side,side] (overwritten) from dz bf16 NHWC [N,Ho,Ho,64] = d loss / d (pre-ReLU stem conv 1 output); only
-// channels 0-31 are read. One thread per input pixel: output pixel (oy, ox) read it through tap (y - 2 oy + 1, x - 2 ox + 1).
-__global__ void __launch_bounds__(128) k_rn_stem_bwd(const bf16* __restrict__ dz, int N, int side, int Ho, const float* __restrict__ w,
-                                                     float* __restrict__ grad) {
-  __shared__ float sw[32 * 27];
-  for (int i = threadIdx.x; i < 32 * 27; i += blockDim.x) sw[i] = w[i];
-  __syncthreads();
-  const size_t plane = (size_t)side * side, p = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
-  if (p >= (size_t)N * plane) return;
-  const int n = (int)(p / plane), rem = (int)(p - n * plane), y = rem / side, x = rem - y * side;
-  float g[3] = {0.f, 0.f, 0.f};
-  for (int ky = 0; ky < 3; ++ky) {
-    const int ty = y + 1 - ky;
-    if (ty < 0 || (ty & 1) || ty / 2 >= Ho) continue;
-    for (int kx = 0; kx < 3; ++kx) {
-      const int tx = x + 1 - kx;
-      if (tx < 0 || (tx & 1) || tx / 2 >= Ho) continue;
-      const int t = ky * 3 + kx;
-      const uint4* src = reinterpret_cast<const uint4*>(dz + (((size_t)n * Ho + ty / 2) * Ho + tx / 2) * 64);
-#pragma unroll
-      for (int v = 0; v < 4; ++v) {
-        const uint4 u = __ldg(src + v);
-        const uint32_t wds[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-        for (int h = 0; h < 4; ++h) {
-          const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&wds[h]));
-          const int co = 8 * v + 2 * h;
-#pragma unroll
-          for (int c = 0; c < 3; ++c) g[c] = fmaf(f.x, sw[co * 27 + c * 9 + t], fmaf(f.y, sw[(co + 1) * 27 + c * 9 + t], g[c]));
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int c = 0; c < 3; ++c) grad[((size_t)n * 3 + c) * plane + (size_t)y * side + x] = g[c];
-}
-
-// ---- 2x2 average pool (floor), bf16 NHWC, 8 channels per item ---------------------------------------------------------------
-__device__ __forceinline__ void rn_bf16x8(const uint4& u, float* f) {
-  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-  for (int h = 0; h < 4; ++h) {
-    const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[h]));
-    f[2 * h] = v.x; f[2 * h + 1] = v.y;
-  }
-}
-__device__ __forceinline__ uint4 rn_pack8(const float* f) {
-  return make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
-}
-
-__global__ void __launch_bounds__(256) k_avgpool2_fwd(const bf16* __restrict__ x, int N, int H, int W, int C, bf16* __restrict__ out) {
-  const int Ho = H / 2, Wo = W / 2, C8 = C / 8;
-  const size_t n_items = (size_t)N * Ho * Wo * C8;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n_items; i += (size_t)gridDim.x * blockDim.x) {
-    const int cv = (int)(i % C8);
-    const size_t po = i / C8;
-    const int xo = (int)(po % Wo), yo = (int)((po / Wo) % Ho), n = (int)(po / ((size_t)Wo * Ho));
-    const uint4* base = reinterpret_cast<const uint4*>(x + (((size_t)n * H + 2 * yo) * W + 2 * xo) * C) + cv;
-    const size_t row = (size_t)W * C8, col = C8;
-    float s[8], f[8];
-    rn_bf16x8(__ldg(base), s);
-    const size_t offs[3] = {col, row, row + col};
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      rn_bf16x8(__ldg(base + offs[k]), f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) s[j] += f[j];
-    }
-#pragma unroll
-    for (int j = 0; j < 8; ++j) s[j] *= 0.25f;
-    reinterpret_cast<uint4*>(out)[i] = rn_pack8(s);
-  }
-}
-
-// out [N,H,W,C] = the adjoint of dy [N,H/2,W/2,C] (dy / 4 on each of a window's pixels, zero on the row / column floor mode
-// drops), selected by mask > 0 when mask [N,H,W,C] is not null (the ReLU output whose pool this was)
-__global__ void __launch_bounds__(256) k_avgpool2_bwd(const bf16* __restrict__ dy, const bf16* __restrict__ mask, int N, int H, int W, int C,
-                                                      bf16* __restrict__ out) {
-  const int Ho = H / 2, Wo = W / 2, C8 = C / 8;
-  const size_t n_items = (size_t)N * H * W * C8;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n_items; i += (size_t)gridDim.x * blockDim.x) {
-    const int cv = (int)(i % C8);
-    const size_t p = i / C8;
-    const int x = (int)(p % W), y = (int)((p / W) % H), n = (int)(p / ((size_t)W * H));
-    float g[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    if (y < 2 * Ho && x < 2 * Wo) {
-      rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(dy + (((size_t)n * Ho + y / 2) * Wo + x / 2) * C) + cv), g);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) g[j] *= 0.25f;
-    }
-    if (mask) {
-      float m[8];
-      rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(mask) + i), m);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) g[j] = m[j] > 0.f ? g[j] : 0.f;
-    }
-    reinterpret_cast<uint4*>(out)[i] = rn_pack8(g);
-  }
-}
 
 // ---- attention-pool tokens ----------------------------------------------------------------------------------------------
 // x bf16 [S*49, C] (the last block's output, pixel-major) -> tok bf16 [S*50, C]: row 0 = mean of the 49 rows + pos[0], row 1 + i =
@@ -177,15 +39,15 @@ __global__ void __launch_bounds__(256) k_rn_tokens_fwd(const bf16* __restrict__ 
     const int cv = (int)(i % C8), s = (int)(i / C8);
     float sum[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f}, f[8];
     for (int r = 0; r < P; ++r) {
-      rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(x + ((size_t)s * P + r) * C) + cv), f);
+      unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(x + ((size_t)s * P + r) * C) + cv), f);
       const float* pp = pos + (size_t)(1 + r) * C + 8 * cv;
 #pragma unroll
       for (int j = 0; j < 8; ++j) { sum[j] += f[j]; f[j] += pp[j]; }
-      reinterpret_cast<uint4*>(tok + ((size_t)s * RN_T + 1 + r) * C)[cv] = rn_pack8(f);
+      reinterpret_cast<uint4*>(tok + ((size_t)s * RN_T + 1 + r) * C)[cv] = pack_bf16x8(f);
     }
 #pragma unroll
     for (int j = 0; j < 8; ++j) sum[j] = sum[j] * (1.f / P) + pos[8 * cv + j];
-    reinterpret_cast<uint4*>(tok + (size_t)s * RN_T * C)[cv] = rn_pack8(sum);
+    reinterpret_cast<uint4*>(tok + (size_t)s * RN_T * C)[cv] = pack_bf16x8(sum);
   }
 }
 
@@ -199,12 +61,12 @@ __global__ void __launch_bounds__(256) k_rn_tokens_bwd(const bf16* __restrict__ 
     const size_t row = i / C8;
     const int s = (int)(row / P), r = (int)(row % P);
     float g0[8], g[8], m[8];
-    rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(dtok + (size_t)s * RN_T * C) + cv), g0);
-    rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(dtok + ((size_t)s * RN_T + 1 + r) * C) + cv), g);
-    rn_bf16x8(__ldg(reinterpret_cast<const uint4*>(x) + i), m);
+    unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(dtok + (size_t)s * RN_T * C) + cv), g0);
+    unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(dtok + ((size_t)s * RN_T + 1 + r) * C) + cv), g);
+    unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(x) + i), m);
 #pragma unroll
     for (int j = 0; j < 8; ++j) g[j] = m[j] > 0.f ? g[j] + g0[j] * (1.f / P) : 0.f;
-    reinterpret_cast<uint4*>(dz)[i] = rn_pack8(g);
+    reinterpret_cast<uint4*>(dz)[i] = pack_bf16x8(g);
   }
 }
 
@@ -214,28 +76,6 @@ __global__ void __launch_bounds__(256) k_rn_emb(const float* __restrict__ acc, c
     emb[i] = acc[i] + bias[i % O];
 }
 
-static int avgpool_fwd(const bf16* x, int N, int H, int W, int C, bf16* out, cudaStream_t st) {
-  k_avgpool2_fwd<<<stride_blocks((size_t)N * (H / 2) * (W / 2) * (C / 8), 16), 256, 0, st>>>(x, N, H, W, C, out);
-  APH_LAUNCH_OK();
-  return 0;
-}
-static int avgpool_bwd(const bf16* dy, const bf16* mask, int N, int H, int W, int C, bf16* out, cudaStream_t st) {
-  k_avgpool2_bwd<<<stride_blocks((size_t)N * H * W * (C / 8), 16), 256, 0, st>>>(dy, mask, N, H, W, C, out);
-  APH_LAUNCH_OK();
-  return 0;
-}
-static int stem_fwd(const float* img, int N, int side, int Ho, const float* w, const float* b, bf16* out, cudaStream_t st) {
-  const size_t n = (size_t)N * Ho * Ho;
-  k_rn_stem_fwd<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(img, N, side, Ho, w, b, out);
-  APH_LAUNCH_OK();
-  return 0;
-}
-static int stem_bwd(const bf16* dz, int N, int side, int Ho, const float* w, float* grad, cudaStream_t st) {
-  const size_t n = (size_t)N * side * side;
-  k_rn_stem_bwd<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(dz, N, side, Ho, w, grad);
-  APH_LAUNCH_OK();
-  return 0;
-}
 static int tokens_fwd(const bf16* x, const float* pos, int S, int C, bf16* tok, cudaStream_t st) {
   k_rn_tokens_fwd<<<stride_blocks((size_t)S * C / 8, 16), 256, 0, st>>>(x, pos, S, C, tok);
   APH_LAUNCH_OK();
@@ -301,7 +141,7 @@ static int rn_fwd_body(RnImpl* h, int S, int side, cudaStream_t st) {
   if ((e = launch_conv3x3(h->s1, h->stem_w2, S, h1, h1, 64, 64, CONV_BIAS_RELU, ce, st))) return e;
   ce.bias = h->stem_b3; ce.out = h->s3;
   if ((e = launch_conv3x3(h->s2, h->stem_w3, S, h1, h1, 64, 64, CONV_BIAS_RELU, ce, st))) return e;
-  if ((e = avgpool_fwd(h->s3, S, h1, h1, 64, h->sp, st))) return e;
+  if ((e = launch_pool2(POOL_MEAN, h->s3, S, h1, h1, 64, h->sp, st))) return e;
   const bf16* x = h->sp;
   for (const RnBlock& k : h->blocks) {
     const int P = k.planes, E = 4 * P, Min = S * k.hin * k.hin, Mo = S * k.hout * k.hout;
@@ -312,13 +152,13 @@ static int rn_fwd_body(RnImpl* h, int S, int side, cudaStream_t st) {
     const bf16* a3 = k.r2;
     const bf16* id = x;
     if (k.stride > 1) {
-      if ((e = avgpool_fwd(k.r2, S, k.hin, k.hin, P, h->scratch[0], st))) return e;
+      if ((e = launch_pool2(POOL_MEAN, k.r2, S, k.hin, k.hin, P, h->scratch[0], st))) return e;
       a3 = h->scratch[0];
     }
     if (k.down) {
       const bf16* xin = x;
       if (k.stride > 1) {
-        if ((e = avgpool_fwd(x, S, k.hin, k.hin, k.cin, h->scratch[1], st))) return e;
+        if ((e = launch_pool2(POOL_MEAN, x, S, k.hin, k.hin, k.cin, h->scratch[1], st))) return e;
         xin = h->scratch[1];
       }
       GemmEpi ep; ep.bias = k.bd; ep.out_bf16 = h->scratch[2];
@@ -361,13 +201,13 @@ static int rn_bwd_body(RnImpl* h, int S, int side, cudaStream_t st) {
     if (k.down) {
       GemmEpi ep; ep.out_bf16 = k.stride > 1 ? T : R;
       if ((e = launch_gemm(dz, k.wd_t, GemmShape{Mo, k.cin, E}, ep, st))) return e;
-      if (k.stride > 1 && (e = avgpool_bwd(T, nullptr, S, k.hin, k.hin, k.cin, R, st))) return e;
+      if (k.stride > 1 && (e = launch_unpool2(T, nullptr, S, k.hin, k.hin, k.cin, 0.25f, R, st))) return e;
       rg = R;
     }
     if (k.stride > 1) {                                      // conv3's input was pool(relu2): adjoint, then relu2's select
       GemmEpi ep; ep.out_bf16 = P1;
       if ((e = launch_gemm(dz, k.w3_t, GemmShape{Mo, P, E}, ep, st))) return e;
-      if ((e = avgpool_bwd(P1, k.r2, S, k.hin, k.hin, P, U, st))) return e;
+      if ((e = launch_unpool2(P1, k.r2, S, k.hin, k.hin, P, 0.25f, U, st))) return e;
     } else {
       GemmEpi ep; ep.mask = k.r2; ep.out_bf16 = U;
       if ((e = launch_gemm(dz, k.w3_t, GemmShape{Mo, P, E}, ep, st))) return e;
@@ -380,7 +220,7 @@ static int rn_bwd_body(RnImpl* h, int S, int side, cudaStream_t st) {
     cur ^= 1;
   }
   // stem: the pool's adjoint with relu3's select, then conv3 and conv2 backward with the selects of relu2 and relu1
-  if ((e = avgpool_bwd(g[cur], h->s3, S, h1, h1, 64, g[4], st))) return e;
+  if ((e = launch_unpool2(g[cur], h->s3, S, h1, h1, 64, 0.25f, g[4], st))) return e;
   ConvEpi c;
   c.mask = h->s2; c.out = g[2];
   if ((e = launch_conv3x3(g[4], h->stem_w3_t, S, h1, h1, 64, 64, CONV_MASK, c, st))) return e;
@@ -479,7 +319,7 @@ extern "C" int aph_rn_fwd(aph_rn* rn, const float* x, int S, int side, float* em
   h->last_S = h->last_side = -1;
   rn_shapes(h, side);
   // the kernels that touch caller memory run outside the cached graph (see aph_vit_fwd)
-  if (int e = stem_fwd(x, S, side, rn_stem_side(side), h->stem_w1, h->stem_b1, h->s1, st)) return e;
+  if (int e = launch_conv3in_fwd<2, 32, IN_RAW>(x, S, side, side, h->stem_w1, h->stem_b1, h->s1, st)) return e;
   // the graph is keyed on the side alone: the forward's launches are the same with or without save_for_bwd
   if (int e = h->fwd_graphs.replay(S, side, st, [&]() { return rn_fwd_body(h, S, side, st); })) return e;
   const int O = h->cfg.out_dim;
@@ -501,7 +341,7 @@ extern "C" int aph_rn_bwd(aph_rn* rn, const float* grad_emb, int S, int side, fl
   k_f32_to_bf16<<<stride_blocks(n, 8), 256, 0, st>>>(grad_emb, h->d_emb, n);
   APH_LAUNCH_OK();
   if (int e = h->bwd_graphs.replay(S, side, st, [&]() { return rn_bwd_body(h, S, side, st); })) return e;
-  return stem_bwd(h->scratch[3], S, side, rn_stem_side(side), h->stem_w1, grad_x, st);
+  return launch_conv3in_bwd<2, 32, IN_RAW>(h->scratch[3], S, side, side, h->stem_w1, grad_x, st);
 }
 
 // The forward's saved ReLU outputs, for a float64 backward that takes the CUDA forward's own selects: k = 0, 1, 2 the stem's
@@ -534,9 +374,8 @@ extern "C" int aph_rn_saved_test(aph_rn* rn, int k, void** ptr, int64_t* numel) 
 extern "C" int aph_rn_stem_test(int fwd, const void* in, const float* weight, const float* bias, void* out, int N, int side, void* stream) {
   APH_REQUIRE(in && weight && out && (bias || !fwd) && N > 0 && side > 0, "aph_rn_stem_test: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
-  const int Ho = rn_stem_side(side);
-  if (fwd) return stem_fwd(reinterpret_cast<const float*>(in), N, side, Ho, weight, bias, reinterpret_cast<bf16*>(out), st);
-  return stem_bwd(reinterpret_cast<const bf16*>(in), N, side, Ho, weight, reinterpret_cast<float*>(out), st);
+  if (fwd) return launch_conv3in_fwd<2, 32, IN_RAW>(reinterpret_cast<const float*>(in), N, side, side, weight, bias, reinterpret_cast<bf16*>(out), st);
+  return launch_conv3in_bwd<2, 32, IN_RAW>(reinterpret_cast<const bf16*>(in), N, side, side, weight, reinterpret_cast<float*>(out), st);
 }
 
 // 2x2 average pool, bf16 NHWC, C % 8 == 0. fwd = 1: out [N,H/2,W/2,C] = pool(x); fwd = 0: x = dy [N,H/2,W/2,C] -> out [N,H,W,C]
@@ -544,8 +383,8 @@ extern "C" int aph_rn_stem_test(int fwd, const void* in, const float* weight, co
 extern "C" int aph_rn_pool_test(int fwd, const void* x, const void* mask, void* out, int N, int H, int W, int C, void* stream) {
   APH_REQUIRE(x && out && N > 0 && H >= 2 && W >= 2 && C % 8 == 0 && C > 0, "aph_rn_pool_test: bad arguments");
   cudaStream_t st = (cudaStream_t)stream;
-  if (fwd) return avgpool_fwd(reinterpret_cast<const bf16*>(x), N, H, W, C, reinterpret_cast<bf16*>(out), st);
-  return avgpool_bwd(reinterpret_cast<const bf16*>(x), reinterpret_cast<const bf16*>(mask), N, H, W, C, reinterpret_cast<bf16*>(out), st);
+  if (fwd) return launch_pool2(POOL_MEAN, reinterpret_cast<const bf16*>(x), N, H, W, C, reinterpret_cast<bf16*>(out), st);
+  return launch_unpool2(reinterpret_cast<const bf16*>(x), reinterpret_cast<const bf16*>(mask), N, H, W, C, 0.25f, reinterpret_cast<bf16*>(out), st);
 }
 
 // Attention-pool tokens, C % 8 == 0. fwd = 1: in = x bf16 [S*49, C], aux = pos fp32 [50, C] -> out bf16 [S*50, C]; fwd = 0:

@@ -15,12 +15,13 @@
 //   attention         per image: S = Q K^T (fp32, keys padded to a multiple of 128), k_softmax_rows (P bf16, padded keys 0),
 //                     O = P V; backward dP = dO V^T, dS = P (dP - rowsum(dO O)) C^-1/2 (k_attn_ds), dQ = dS K, dK = dS^T Q,
 //                     dV = P^T dO, with the transposed operands written by k_vq_pad
-//   upsample          k_up2 (nearest x2, materialised: TMA cannot address half-pixel strides) and its adjoint k_up2_adj (2 x 2 sum)
+//   upsample          k_unpool2 (nhwc.cu) at scale 1: nearest x2, materialised (TMA cannot address half-pixel strides); its
+//                     adjoint k_pool2<POOL_SUM> (2 x 2 sum)
 //   the ends          k_nchw_to_nhwc (z), k_nhwc_to_nchw (dz), conv_out as the fp32 SIMT pair k_conv_out_fwd / _bwd on the
 //                     caller's fp32 NCHW image and its gradient
 // The kernels that touch caller memory (the two conversions and conv_out) run outside the cached graphs; everything between them
 // replays through one graph per latent shape, forward and backward.
-#include "conv_tc.cuh"
+#include "nhwc.cuh"
 #include "encoder.cuh"
 #include <memory>
 
@@ -30,17 +31,6 @@ constexpr int VQ_G = 32;              // GroupNorm groups
 constexpr int VQ_CHUNK = 256;         // pixels per GroupNorm partial
 constexpr float VQ_EPS = 1e-6f;
 
-__device__ __forceinline__ void vq_unpack8(const uint4& u, float* f) {
-  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-  for (int h = 0; h < 4; ++h) {
-    const float2 v = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w[h]));
-    f[2 * h] = v.x; f[2 * h + 1] = v.y;
-  }
-}
-__device__ __forceinline__ uint4 vq_pack8(const float* f) {
-  return make_uint4(pack_bf16(f[0], f[1]), pack_bf16(f[2], f[3]), pack_bf16(f[4], f[5]), pack_bf16(f[6], f[7]));
-}
 __device__ __forceinline__ float swishf(float y) { return y * sigmoidf_(y); }
 __device__ __forceinline__ float swish_grad(float y) {
   const float s = sigmoidf_(y);
@@ -75,13 +65,13 @@ __global__ void __launch_bounds__(256) k_gn_partials(const bf16* __restrict__ x,
     for (int p = blockIdx.x * VQ_CHUNK + pl; p < p1; p += PL) {
       const size_t off = ((size_t)n * HW + p) * C8 + cv;
       float v[8];
-      vq_unpack8(__ldg(reinterpret_cast<const uint4*>(x) + off), v);
+      unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(x) + off), v);
       if (!BWD) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) { s[j] += v[j]; q[j] = fmaf(v[j], v[j], q[j]); }
       } else {
         float d[8];
-        vq_unpack8(__ldg(reinterpret_cast<const uint4*>(dout) + off), d);
+        unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(dout) + off), d);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const float xh = (v[j] - mean[j]) * rstd[j];
@@ -130,14 +120,14 @@ __global__ void __launch_bounds__(256) k_gn_apply(const bf16* __restrict__ x, co
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n_items; i += (size_t)gridDim.x * blockDim.x) {
     const int cv = (int)(i % C8), n = (int)(i / ((size_t)HW * C8));
     float v[8];
-    vq_unpack8(__ldg(reinterpret_cast<const uint4*>(x) + i), v);
+    unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(x) + i), v);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int c = 8 * cv + j, g = c / Cg;
       const float y = fmaf(gamma[c], (v[j] - stats[(n * VQ_G + g) * 2]) * stats[(n * VQ_G + g) * 2 + 1], beta[c]);
       v[j] = swish ? swishf(y) : y;
     }
-    reinterpret_cast<uint4*>(out)[i] = vq_pack8(v);
+    reinterpret_cast<uint4*>(out)[i] = pack_bf16x8(v);
   }
 }
 
@@ -151,9 +141,9 @@ __global__ void __launch_bounds__(256) k_gn_apply_bwd(const bf16* __restrict__ d
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n_items; i += (size_t)gridDim.x * blockDim.x) {
     const int cv = (int)(i % C8), n = (int)(i / ((size_t)HW * C8));
     float v[8], d[8], r[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
-    vq_unpack8(__ldg(reinterpret_cast<const uint4*>(x) + i), v);
-    vq_unpack8(__ldg(reinterpret_cast<const uint4*>(dout) + i), d);
-    if (resid) vq_unpack8(__ldg(reinterpret_cast<const uint4*>(resid) + i), r);
+    unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(x) + i), v);
+    unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(dout) + i), d);
+    if (resid) unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(resid) + i), r);
 #pragma unroll
     for (int j = 0; j < 8; ++j) {
       const int c = 8 * cv + j, ng = n * VQ_G + c / Cg;
@@ -161,55 +151,20 @@ __global__ void __launch_bounds__(256) k_gn_apply_bwd(const bf16* __restrict__ d
       const float g = d[j] * (swish ? swish_grad(fmaf(gamma[c], xh, beta[c])) : 1.f) * gamma[c];
       v[j] = rs * (g - red[2 * ng] - xh * red[2 * ng + 1]) + r[j];
     }
-    reinterpret_cast<uint4*>(dx)[i] = vq_pack8(v);
+    reinterpret_cast<uint4*>(dx)[i] = pack_bf16x8(v);
   }
 }
 
-// ---- upsample, residual add, layout conversions --------------------------------------------------------------------------
-// out [N, 2H, 2W, C] = x [N, H, W, C] at (y / 2, x / 2)
-__global__ void __launch_bounds__(256) k_up2(const bf16* __restrict__ x, int N, int H, int W, int C, bf16* __restrict__ out) {
-  const int C8 = C / 8, W2 = 2 * W, H2 = 2 * H;
-  const size_t n_items = (size_t)N * H2 * W2 * C8;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n_items; i += (size_t)gridDim.x * blockDim.x) {
-    const int cv = (int)(i % C8);
-    const size_t p = i / C8;
-    const int xo = (int)(p % W2), yo = (int)((p / W2) % H2), n = (int)(p / ((size_t)W2 * H2));
-    reinterpret_cast<uint4*>(out)[i] = __ldg(reinterpret_cast<const uint4*>(x + (((size_t)n * H + yo / 2) * W + xo / 2) * C) + cv);
-  }
-}
-
-// the adjoint: out [N, H, W, C] = the sum of dy [N, 2H, 2W, C] over each 2 x 2 window, in (0,0) (0,1) (1,0) (1,1) order
-__global__ void __launch_bounds__(256) k_up2_adj(const bf16* __restrict__ dy, int N, int H, int W, int C, bf16* __restrict__ out) {
-  const int C8 = C / 8;
-  const size_t n_items = (size_t)N * H * W * C8;
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n_items; i += (size_t)gridDim.x * blockDim.x) {
-    const int cv = (int)(i % C8);
-    const size_t p = i / C8;
-    const int xo = (int)(p % W), yo = (int)((p / W) % H), n = (int)(p / ((size_t)W * H));
-    const size_t row = (size_t)2 * W * C8;
-    const uint4* base = reinterpret_cast<const uint4*>(dy + (((size_t)n * 2 * H + 2 * yo) * 2 * W + 2 * xo) * C) + cv;
-    float s[8], f[8];
-    vq_unpack8(__ldg(base), s);
-    const size_t offs[3] = {(size_t)C8, row, row + C8};
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-      vq_unpack8(__ldg(base + offs[k]), f);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) s[j] += f[j];
-    }
-    reinterpret_cast<uint4*>(out)[i] = vq_pack8(s);
-  }
-}
-
+// ---- residual add, layout conversions --------------------------------------------------------------------------------------
 // out = a + b, bf16, n8 items of 8 elements
 __global__ void __launch_bounds__(256) k_add_bf16(const bf16* __restrict__ a, const bf16* __restrict__ b, size_t n8, bf16* __restrict__ out) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < n8; i += (size_t)gridDim.x * blockDim.x) {
     float u[8], v[8];
-    vq_unpack8(__ldg(reinterpret_cast<const uint4*>(a) + i), u);
-    vq_unpack8(__ldg(reinterpret_cast<const uint4*>(b) + i), v);
+    unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(a) + i), u);
+    unpack_bf16x8(__ldg(reinterpret_cast<const uint4*>(b) + i), v);
 #pragma unroll
     for (int j = 0; j < 8; ++j) u[j] += v[j];
-    reinterpret_cast<uint4*>(out)[i] = vq_pack8(u);
+    reinterpret_cast<uint4*>(out)[i] = pack_bf16x8(u);
   }
 }
 
@@ -261,7 +216,7 @@ __global__ void __launch_bounds__(128) k_conv_out_fwd(const bf16* __restrict__ a
     const float* wt = sw + (size_t)t * C * 3;
     for (int cv = 0; cv < C / 8; ++cv) {
       float f[8];
-      vq_unpack8(__ldg(src + cv), f);
+      unpack_bf16x8(__ldg(src + cv), f);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         const float* wc = wt + (8 * cv + j) * 3;
@@ -303,7 +258,7 @@ __global__ void __launch_bounds__(128) k_conv_out_bwd(const float* __restrict__ 
       }
       f[j] = s;
     }
-    dst[cv] = vq_pack8(f);
+    dst[cv] = pack_bf16x8(f);
   }
 }
 
@@ -449,13 +404,6 @@ static int gn_bwd(const bf16* dout, const bf16* x, const float* stats, const flo
   return 0;
 }
 
-static int up2(bool fwd, const bf16* in, int N, int H, int W, int C, bf16* out, cudaStream_t st) {
-  if (fwd) k_up2<<<stride_blocks((size_t)N * 4 * H * W * (C / 8), 16), 256, 0, st>>>(in, N, H, W, C, out);
-  else k_up2_adj<<<stride_blocks((size_t)N * H * W * (C / 8), 16), 256, 0, st>>>(in, N, H, W, C, out);
-  APH_LAUNCH_OK();
-  return 0;
-}
-
 static int add_bf16(const bf16* a, const bf16* b, size_t n, bf16* out, cudaStream_t st) {
   k_add_bf16<<<stride_blocks(n / 8, 16), 256, 0, st>>>(a, b, n / 8, out);
   APH_LAUNCH_OK();
@@ -550,8 +498,8 @@ static int vq_fwd_body(VqImpl* h, int N, int lh, int lw, cudaStream_t st) {
         if ((e = launch_gemm(op.o, op.wp, GemmShape{Pn, C, C}, ep, st))) return e; }
       if ((e = add_bf16(x, h->sb, (size_t)Pn * C, op.out, st))) return e;
     } else {
-      if ((e = up2(true, x, N, H, W, op.cin, h->sa, st))) return e;
       H *= 2; W *= 2;
+      if ((e = launch_unpool2(x, nullptr, N, H, W, op.cin, 1.f, h->sa, st))) return e;
       ConvEpi c; c.bias = op.b1; c.out = op.out;
       if ((e = launch_conv3x3(h->sa, op.w1, N, H, W, op.cin, op.cout, CONV_BIAS, c, st))) return e;
     }
@@ -575,8 +523,8 @@ static int vq_bwd_body(VqImpl* h, int N, int lh, int lw, cudaStream_t st) {
     if (op.kind == VqOp::UP) {
       ConvEpi c; c.out = h->sa;
       if ((e = launch_conv3x3(dy, op.w1t, N, H, W, op.cout, op.cin, CONV_PLAIN, c, st))) return e;
+      if ((e = launch_pool2(POOL_SUM, h->sa, N, H, W, op.cin, dx, st))) return e;
       H /= 2; W /= 2;
-      if ((e = up2(false, h->sa, N, H, W, op.cin, dx, st))) return e;
     } else if (op.kind == VqOp::RES) {
       const int HW = H * W, Pn = N * HW;
       { ConvEpi c; c.out = h->sa;
@@ -779,9 +727,15 @@ extern "C" int aph_vqgan_conv_test(const void* x, const float* weight, const flo
   return launch_conv3x3(x, wp.p, N, H, W, Cin, Cout, resid ? CONV_BIAS_RESID : CONV_BIAS, c, st);
 }
 
+// Nearest x2 upsample, bf16 NHWC, C % 8 == 0. fwd = 1: in [N,H,W,C] -> out [N,2H,2W,C]; fwd = 0: in = dy [N,2H,2W,C] -> out
+// [N,H,W,C] = its adjoint, the sum of each 2 x 2 window.
 extern "C" int aph_vqgan_up_test(int fwd, const void* in, void* out, int N, int H, int W, int C, void* stream) {
   APH_REQUIRE(in && out && N > 0 && H > 0 && W > 0 && C % 8 == 0 && C > 0, "aph_vqgan_up_test: bad arguments");
-  return up2(fwd != 0, reinterpret_cast<const bf16*>(in), N, H, W, C, reinterpret_cast<bf16*>(out), (cudaStream_t)stream);
+  const bf16* x = reinterpret_cast<const bf16*>(in);
+  bf16* y = reinterpret_cast<bf16*>(out);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (fwd) return launch_unpool2(x, nullptr, N, 2 * H, 2 * W, C, 1.f, y, st);
+  return launch_pool2(POOL_SUM, x, N, 2 * H, 2 * W, C, y, st);
 }
 
 extern "C" int aph_vqgan_attn_test(int fwd, const void* qkv, const void* dout, void* out, int N, int T, int C, void* stream) {

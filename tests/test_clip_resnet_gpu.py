@@ -71,16 +71,20 @@ def test_stem_conv_fwd_and_crop_gradient(side):
 
 @pytest.mark.parametrize('h', [116, 112, 63, 29, 14])
 def test_average_pool_and_adjoint(h):
-    """Forward and adjoint (with and without the ReLU select), odd sides floor. The forward sums four bf16 values in fp32 and
-    rounds once; the adjoint scales by 1/4 exactly: bars 6e-3 and exact."""
+    """Forward and adjoint (with and without the ReLU select), odd sides floor. The forward sums the window's four bf16 values
+    in fp32 in (0,0) (0,1) (1,0) (1,1) order, scales by 1/4 and rounds once to nearest; the adjoint scales by 1/4 exactly: both
+    exact against an fp32 restatement of that order."""
     torch.manual_seed(h)
     N, C = 2, 64
     x = torch.randn(N, C, h, h, device='cuda').bfloat16()
     xh = _nhwc(x)
     out = torch.full((N, h // 2, h // 2, C), float('nan'), device='cuda', dtype=torch.bfloat16)
     _lib.check(_lib.lib().aph_rn_pool_test(1, xh.data_ptr(), None, out.data_ptr(), N, h, h, C, _st()), 'pool fwd')
+    e = 2 * (h // 2)
+    xf = xh[:, :e, :e].float()
+    want = ((((xf[:, 0::2, 0::2] + xf[:, 0::2, 1::2]) + xf[:, 1::2, 0::2]) + xf[:, 1::2, 1::2]) * 0.25).bfloat16()
     torch.cuda.synchronize()
-    assert torch.isfinite(out).all() and _rel(_nchw(out), F.avg_pool2d(x.double(), 2)) < 6e-3
+    assert torch.equal(out, want)
     dy = torch.randn(N, C, h // 2, h // 2, device='cuda').bfloat16()
     dyh = _nhwc(dy)
     xr = x.double().requires_grad_(True)

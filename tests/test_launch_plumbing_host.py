@@ -26,7 +26,7 @@ def test_shared_memory_limits_are_raised_only_by_the_helper():
     rest = _outside(srcs, 'aph_common.cuh', helper)
     assert [name for name, text in rest.items() if 'cudaFuncSetAttribute' in text] == []
     callers = {name for name, text in rest.items() if 'smem_at_least(' in text}
-    assert callers >= {'vit_gemm.cu', 'lpips.cu', 'cppn.cu', 'vit_attn_tc.cuh', 'text.cu', 'sample.cu', 'synth_fft.cu'}
+    assert callers >= {'vit_gemm.cu', 'conv_tc.cu', 'cppn.cu', 'vit_attn_tc.cuh', 'text.cu', 'sample.cu', 'synth_fft.cu'}
 
 
 def test_no_function_local_launch_flag_remains():
