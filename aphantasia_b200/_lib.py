@@ -62,9 +62,9 @@ _SIGS = {
     'aph_rn_bwd': (C.c_int, [C.c_void_p, c_f32p, C.c_int, C.c_int, c_f32p, C.c_void_p]),
     'aph_rn_bytes': (C.c_int64, [C.c_void_p]),
     'aph_rn_saved_test': (C.c_int, [C.c_void_p, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
-    'aph_rn_stem_test': (C.c_int, [C.c_int, C.c_void_p, c_f32p, c_f32p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    'aph_rn_stem_test': (C.c_int, [C.c_int, C.c_void_p, c_f32p, c_f32p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]),
     'aph_rn_pool_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
-    'aph_rn_tokens_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    'aph_rn_tokens_test': (C.c_int, [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]),
     'aph_gemm_rn_epi_test': (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, c_f32p, C.c_void_p, C.c_void_p, C.c_int,
                                        C.c_void_p, C.c_void_p]),
     'aph_vqgan_create': (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p]),
@@ -130,11 +130,11 @@ _SIGS = {
     'aph_adam_step': (C.c_int, [c_f32p, c_f32p, c_f32p, c_f32p, C.c_int64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_int, C.c_void_p,
                                 C.c_float, c_f32p]),
 }
-# Entry points whose last arguments are optional (the fused / extended Adam update): a call that stops after `stream` gets
-# these values for them, so a call written for the plain form binds unchanged.
+# Entry points whose last arguments are optional (the fused / extended Adam update, the ResNet stem's width and map grid): a call
+# that stops after `stream` gets these values for them, so a call written for the plain form binds unchanged.
 _ADAM_OFF = (None, None, None, None, 0., 0., 0., 0., 0., 0)
 OPTIONAL_TAIL = {'aph_adam_step': (0., None), 'aph_synth_fft_bwd_adam': (0., None), 'aph_pixel_bwd': _ADAM_OFF,
-                 'aph_synth_dwt_bwd': _ADAM_OFF}
+                 'aph_synth_dwt_bwd': _ADAM_OFF, 'aph_rn_stem_test': (0,), 'aph_rn_tokens_test': (0,)}
 EXPORTS = tuple(_SIGS)
 
 

@@ -3,9 +3,10 @@
 `model.visual.input_resolution`.
 
 The image encoder (ViT-B/32, ViT-B/16, ViT-L/14) runs forward and data-gradient in libaphb200.so (csrc/vit.cu: wgmma
-GEMMs + fused kernels); the ResNet encoders RN50 and RN101 in csrc/rn.cu (the same GEMM and 3x3 convolution, BatchNorm folded
-on the host). Weights: an OpenAI state dict if `APH_CLIP_WEIGHTS=<file.pt>` is set (a TorchScript archive as
-OpenAI ships them, or a plain state dict), else seeded synthetic weights of the same architecture.
+GEMMs + fused kernels); the ResNet encoders RN50, RN101, RN50x4, RN50x16 and RN50x64 in csrc/rn.cu (the same GEMM and 3x3
+convolution, BatchNorm folded on the host). Weights: an OpenAI state dict if `APH_CLIP_WEIGHTS_<NAME>=<file.pt>` or
+`APH_CLIP_WEIGHTS=<file.pt>` is set (a TorchScript archive as OpenAI ships them, or a plain state dict), else seeded synthetic
+weights of the same architecture. RN50x4, RN50x16 and RN50x64 have no synthetic fallback: they need a checkpoint.
 The text encoder (csrc/text.cu, forward only) runs once per prompt before the optimisation loop when the weights hold
 the text tower; `tokenize` uses CLIP's BPE vocabulary from `APH_CLIP_BPE=<bpe_simple_vocab_16e6.txt.gz>` or from that
 file next to the weights. Without text weights `encode_text` returns a deterministic seeded embedding per prompt, and
@@ -27,8 +28,24 @@ _MODELS = {'ViT-B/32': dict(patch=32, width=768, layers=12, heads=12, out_dim=51
            'ViT-B/16': dict(patch=16, width=768, layers=12, heads=12, out_dim=512, res=224),
            'ViT-L/14': dict(patch=14, width=1024, layers=24, heads=16, out_dim=768, res=224),
            'RN50': dict(layers=(3, 4, 6, 3), width=64, heads=32, out_dim=1024, res=224),
-           'RN101': dict(layers=(3, 4, 23, 3), width=64, heads=32, out_dim=512, res=224)}
-RN_SIDES = (223, 254)      # the crop sides whose ResNet map is 7 x 7 at the attention pool
+           'RN101': dict(layers=(3, 4, 23, 3), width=64, heads=32, out_dim=512, res=224),
+           'RN50x4': dict(layers=(4, 6, 10, 6), width=80, heads=40, out_dim=640, res=288),
+           'RN50x16': dict(layers=(6, 8, 18, 8), width=96, heads=48, out_dim=768, res=384),
+           'RN50x64': dict(layers=(3, 15, 36, 10), width=128, heads=64, out_dim=1024, res=448)}
+# The wide ResNets load from an OpenAI checkpoint only: no benchmark or script default needs them without one, and a synthetic
+# RN50x64 alone is 420 M parameters to draw.
+CHECKPOINT_ONLY = ('RN50x4', 'RN50x16', 'RN50x64')
+RN_SIDES = (223, 254)      # the crop sides whose ResNet map is 7 x 7 at the attention pool (RN50, RN101: resolution 224)
+
+
+def rn_sides(res):
+    """The crop sides a ResNet of input resolution `res` takes: those whose final map is res/32 x res/32."""
+    return res - 1, res + 30
+
+
+def weights_variable(name):
+    """The environment variable that names `name`'s checkpoint (APH_CLIP_WEIGHTS serves every model)."""
+    return 'APH_CLIP_WEIGHTS_' + name.replace('/', '').replace('-', '').upper()
 
 
 def available_models():
@@ -68,10 +85,11 @@ def synthetic_visual_state_dict(patch=32, width=768, layers=12, heads=12, out_di
     return sd
 
 
-def synthetic_resnet_state_dict(layers=(3, 4, 6, 3), width=64, heads=32, out_dim=1024, res=224, seed=0):
+def synthetic_resnet_state_dict(layers=(3, 4, 6, 3), width=64, heads=32, out_dim=1024, res=224, seed=0, branch_scale=0.25):
     """Seeded synthetic ModifiedResNet weights in the OpenAI key layout ("visual." prefix). Convolutions have He-normal weights
     and every BatchNorm non-trivial running statistics and affine (so that a missing or wrong fold shows); the last BatchNorm of
-    each residual branch is scaled by 0.25 so that the residual stream stays of order one through 33 blocks."""
+    each residual branch is scaled by `branch_scale`: 0.25 keeps the residual stream of order one through 33 blocks, deeper
+    towers need less."""
     g = torch.Generator().manual_seed(seed)
     embed = width * 32
 
@@ -100,7 +118,7 @@ def synthetic_resnet_state_dict(layers=(3, 4, 6, 3), width=64, heads=32, out_dim
             p = v + 'layer%d.%d.' % (i + 1, j)
             sd[p + 'conv1.weight'] = conv(planes, cin, 1); bn(p + 'bn1', planes)
             sd[p + 'conv2.weight'] = conv(planes, planes, 3); bn(p + 'bn2', planes)
-            sd[p + 'conv3.weight'] = conv(4 * planes, planes, 1); bn(p + 'bn3', 4 * planes, 0.25)
+            sd[p + 'conv3.weight'] = conv(4 * planes, planes, 1); bn(p + 'bn3', 4 * planes, branch_scale)
             if j == 0 and (i > 0 or cin != 4 * planes):
                 sd[p + 'downsample.0.weight'] = conv(4 * planes, cin, 1); bn(p + 'downsample.1', 4 * planes)
             cin = 4 * planes
@@ -114,43 +132,65 @@ def synthetic_resnet_state_dict(layers=(3, 4, 6, 3), width=64, heads=32, out_dim
     return sd
 
 
-def fold_resnet_state_dict(sd, eps=1e-5):
-    """The ResNet tower's device tensors (float64) from a ModifiedResNet state dict without the "visual." prefix: every
-    BatchNorm (running statistics, eps) folded into the convolution before it, w' = w g / sqrt(var + eps), b' = b - mean g /
-    sqrt(var + eps); the stem's 32-channel convolutions zero-padded to 64 channels; 1x1 weights as [C_out, C_in]; the attention
-    pool's q, k and v projections stacked into one [3 D, D] operand in that order. Keys: see aph_rn_load_tensor."""
+def pad64(c):
+    """The channel count the ResNet tower runs a layer of c channels at: c rounded up to a multiple of 64."""
+    return (c + 63) // 64 * 64
+
+
+def fold_resnet_state_dict(sd, eps=1e-5, dtype=torch.float64):
+    """The ResNet tower's device tensors from a ModifiedResNet state dict without the "visual." prefix: every BatchNorm (running
+    statistics, eps) folded into the convolution before it, w' = w g / sqrt(var + eps), b' = b - mean g / sqrt(var + eps), in
+    float64; every convolution but the stem's first zero-padded to pad64 output and input channels, with zero biases in the
+    padding (RN50's stem 32 -> 64; RN50x4's 40 -> 64, 80 -> 128 and planes 80 -> 128, 160 -> 192; RN50x16's 48 -> 64,
+    96 -> 128 and planes 96 -> 128), so that the padded channels stay exactly 0 through bias, ReLU, residual and pools; 1x1
+    weights as [C_out, C_in]; the attention pool's q, k and v projections stacked into one [3 D, D] operand in that order. Each
+    tensor is converted to `dtype` before the next one is folded, so the float64 working set is one tensor (RN50x64 holds 420 M
+    visual parameters). Keys: see aph_rn_load_tensor."""
     out = OrderedDict()
 
     def fold(conv, bn):
         s = sd[bn + '.weight'].double() / torch.sqrt(sd[bn + '.running_var'].double() + eps)
         w = sd[conv].double() * s.view(-1, 1, 1, 1)
         return w, sd[bn + '.bias'].double() - sd[bn + '.running_mean'].double() * s
+
+    def put(key, w, bias):
+        co, ci = w.shape[:2]
+        if (pad64(co), pad64(ci)) != (co, ci):
+            wp = torch.zeros((pad64(co), pad64(ci)) + tuple(w.shape[2:]), dtype=torch.float64)
+            wp[:co, :ci] = w
+            bp = torch.zeros(pad64(co), dtype=torch.float64)
+            bp[:co] = bias
+            w, bias = wp, bp
+        out[key + '.weight'] = (w if w.shape[-1] == 3 else w.flatten(1)).to(dtype)
+        out[key + '.bias'] = bias.to(dtype)
     w1, b1 = fold('conv1.weight', 'bn1')
-    w2, b2 = fold('conv2.weight', 'bn2')
-    w3, b3 = fold('conv3.weight', 'bn3')
-    c, c2 = w1.shape[0], w3.shape[0]
-    out['conv1.weight'], out['conv1.bias'] = w1, b1
-    out['conv2.weight'] = torch.zeros(c2, c2, 3, 3, dtype=torch.float64); out['conv2.weight'][:c, :c] = w2
-    out['conv2.bias'] = torch.zeros(c2, dtype=torch.float64); out['conv2.bias'][:c] = b2
-    out['conv3.weight'] = torch.zeros(c2, c2, 3, 3, dtype=torch.float64); out['conv3.weight'][:, :c] = w3
-    out['conv3.bias'] = b3
+    out['conv1.weight'], out['conv1.bias'] = w1.to(dtype), b1.to(dtype)
+    put('conv2', *fold('conv2.weight', 'bn2'))
+    put('conv3', *fold('conv3.weight', 'bn3'))
     blocks = sorted({k.rsplit('.', 2)[0] for k in sd if k.startswith('layer') and k.endswith('.conv1.weight')},
                     key=lambda b: tuple(int(t) for t in b[len('layer'):].split('.')))
     for b in blocks:
         for n in ('conv1', 'conv2', 'conv3'):
-            w, bias = fold('%s.%s.weight' % (b, n), '%s.bn%s' % (b, n[-1]))
-            out['%s.%s.weight' % (b, n)] = w if n == 'conv2' else w.flatten(1)
-            out['%s.%s.bias' % (b, n)] = bias
+            put('%s.%s' % (b, n), *fold('%s.%s.weight' % (b, n), '%s.bn%s' % (b, n[-1])))
         if b + '.downsample.0.weight' in sd:
-            w, bias = fold(b + '.downsample.0.weight', b + '.downsample.1')
-            out[b + '.downsample.weight'], out[b + '.downsample.bias'] = w.flatten(1), bias
+            put(b + '.downsample', *fold(b + '.downsample.0.weight', b + '.downsample.1'))
     a = 'attnpool.'
-    out[a + 'positional_embedding'] = sd[a + 'positional_embedding'].double()
-    out[a + 'qkv.weight'] = torch.cat([sd[a + n + '_proj.weight'].double() for n in 'qkv'])
-    out[a + 'qkv.bias'] = torch.cat([sd[a + n + '_proj.bias'].double() for n in 'qkv'])
-    out[a + 'c_proj.weight'] = sd[a + 'c_proj.weight'].double()
-    out[a + 'c_proj.bias'] = sd[a + 'c_proj.bias'].double()
+    out[a + 'positional_embedding'] = sd[a + 'positional_embedding'].double().to(dtype)
+    out[a + 'qkv.weight'] = torch.cat([sd[a + n + '_proj.weight'].double() for n in 'qkv']).to(dtype)
+    out[a + 'qkv.bias'] = torch.cat([sd[a + n + '_proj.bias'].double() for n in 'qkv']).to(dtype)
+    out[a + 'c_proj.weight'] = sd[a + 'c_proj.weight'].double().to(dtype)
+    out[a + 'c_proj.bias'] = sd[a + 'c_proj.bias'].double().to(dtype)
     return out
+
+
+def resnet_architecture(state_dict):
+    """(layers, width, input resolution) of a ModifiedResNet state dict with the "visual." prefix, read as OpenAI's build_model
+    reads them."""
+    sd = state_dict
+    layers = tuple(len({k.split('.')[2] for k in sd if k.startswith('visual.layer%d.' % i)}) for i in range(1, 5))
+    width = sd['visual.layer1.0.conv1.weight'].shape[0]
+    res = 32 * round((sd['visual.attnpool.positional_embedding'].shape[0] - 1) ** 0.5)
+    return layers, width, res
 
 
 def is_resnet(state_dict):
@@ -351,10 +391,11 @@ class VisionTransformer(_Tower):
 
 class ModifiedResNet(_Tower):
     """Handle-owning mirror of clip.model.ModifiedResNet (eval mode) through the C ABI, forward and data gradient. It reads the
-    whole crop: any side in RN_SIDES, 232 under transforms_custom / _elastic included. It has no patch operand, so the sampler
-    never writes one for it (_patchlink)."""
+    whole crop: any side in rn_sides(input_resolution) (RN_SIDES at 224), size + 8 under transforms_custom / _elastic included.
+    It has no patch operand, so the sampler never writes one for it (_patchlink)."""
     _api = 'aph_rn'
     patch_size = None
+    input_resolution = 224         # set per instance from the weights
 
     def __init__(self, state_dict, max_batch=None):
         sd = {k[len('visual.'):]: v for k, v in state_dict.items() if k.startswith('visual.')}
@@ -363,7 +404,7 @@ class ModifiedResNet(_Tower):
         self.heads = self.width * 32 // 64
         self.output_dim = sd['attnpool.c_proj.weight'].shape[0]
         self.input_resolution = 32 * round((sd['attnpool.positional_embedding'].shape[0] - 1) ** 0.5)
-        self._sd = OrderedDict((k, v.float().contiguous()) for k, v in fold_resnet_state_dict(sd).items())
+        self._sd = OrderedDict((k, v.contiguous()) for k, v in fold_resnet_state_dict(sd, dtype=torch.float32).items())
         self._generation, self.recomputes, self._handle_epoch = 0, 0, 0        # see _EncodeImage
         self._patch_gen = 0
         _patchlink.register(self)
@@ -383,10 +424,11 @@ class ModifiedResNet(_Tower):
         check(lib().aph_rn_bwd(self.handle, g.data_ptr(), S, side, gi.data_ptr(), stream_ptr()), 'aph_rn_bwd')
 
     def check_input(self, x):
-        lo, hi = RN_SIDES
+        lo, hi = rn_sides(self.input_resolution)
+        g = self.input_resolution // 32
         if x.dim() != 4 or x.shape[1] != 3 or x.shape[2] != x.shape[3] or not lo <= x.shape[2] <= hi:
-            raise ValueError('encode_image: the ResNet takes images [S, 3, side, side] with %d <= side <= %d (a 7 x 7 final map), '
-                             'got %s' % (lo, hi, tuple(x.shape)))
+            raise ValueError('encode_image: the ResNet takes images [S, 3, side, side] with %d <= side <= %d (a %d x %d final map), '
+                             'got %s' % (lo, hi, g, g, tuple(x.shape)))
 
     def __call__(self, x):
         require_cuda(x, 'encode_image input')
@@ -507,14 +549,26 @@ def load(name, device=None, jit=False, download_root=None):
     global _weights_dir
     if name not in _MODELS:
         raise RuntimeError('aphantasia_b200.clip: model %s not available (the CUDA hot path covers %s)' % (name, available_models()))
-    path = os.environ.get('APH_CLIP_WEIGHTS_' + name.replace('/', '').replace('-', '').upper(), os.environ.get('APH_CLIP_WEIGHTS'))
+    var = weights_variable(name)
+    path = os.environ.get(var, os.environ.get('APH_CLIP_WEIGHTS'))
     if path and os.path.isfile(path):
         sd = _read_weights(path)
         synthetic = False
+        if name in CHECKPOINT_ONLY:
+            m = _MODELS[name]
+            want = (m['layers'], m['width'], m['res'])
+            got = resnet_architecture(sd) if is_resnet(sd) else None
+            if got != want:
+                held = 'a ResNet of layers %s, width %d, resolution %d' % got if got else 'no ResNet image tower'
+                raise RuntimeError('aphantasia_b200.clip: %s holds %s, not %s (layers %s, width %d, resolution %d)'
+                                   % ((path, held, name) + want))
         _weights_dir = os.path.dirname(os.path.abspath(path))
         if has_text_tower(sd) and vocab_path() is None:
             print(' [aphantasia_b200.clip] WARNING: no BPE vocabulary (set APH_CLIP_BPE=<%s> or put it next to %s): prompts will be '
                   'byte-tokenized and the text encoder will not see CLIP tokens' % (VOCAB_FILE, path))
+    elif name in CHECKPOINT_ONLY:
+        raise RuntimeError('aphantasia_b200.clip: model %s not available without its OpenAI checkpoint: set %s=<%s.pt> (or '
+                           'APH_CLIP_WEIGHTS)' % (name, var, name))
     else:
         synth = synthetic_resnet_state_dict if name.startswith('RN') else synthetic_visual_state_dict
         sd = synth(seed=int(os.environ.get('APH_CLIP_SEED', '0')), **_MODELS[name])

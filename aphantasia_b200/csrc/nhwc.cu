@@ -3,7 +3,8 @@
 //   k_pool2<OP>         LPIPS max-pool (MAX), the ResNet average pool (MEAN), the VQGAN upsample's adjoint (SUM over the 2H x 2W map)
 //   k_unpool2           the ResNet average pool's adjoint (scale 0.25, optional ReLU select), the VQGAN nearest x2 upsample (scale 1:
 //                       bf16 -> fp32 -> x 1 -> bf16 returns every finite value unchanged)
-//   k_conv3in_fwd/_bwd  LPIPS conv1_1 <1, 64, IN_LPIPS> and the ResNet stem's conv1 <2, 32, IN_RAW>, fp32 SIMT
+//   k_conv3in_fwd/_bwd  LPIPS conv1_1 <1, 64, IN_LPIPS> and the ResNet stems' conv1 <2, COUT, IN_RAW> (COUT = width / 2: 32 RN50 /
+//                       RN101, 40 RN50x4, 48 RN50x16, 56 for width 112, 64 RN50x64), fp32 SIMT; the output row is 64 channels wide, zero above COUT
 // The 3x3 tensor-core convolution's launcher is in conv_tc.cu.
 #include "nhwc.cuh"
 
@@ -184,7 +185,11 @@ int launch_conv3in_bwd(const bf16* dz, int N, int H, int W, const float* w, floa
 
 template int launch_conv3in_fwd<1, 64, IN_LPIPS>(const float*, int, int, int, const float*, const float*, bf16*, cudaStream_t, float, float);
 template int launch_conv3in_bwd<1, 64, IN_LPIPS>(const bf16*, int, int, int, const float*, float*, cudaStream_t, float);
-template int launch_conv3in_fwd<2, 32, IN_RAW>(const float*, int, int, int, const float*, const float*, bf16*, cudaStream_t, float, float);
-template int launch_conv3in_bwd<2, 32, IN_RAW>(const bf16*, int, int, int, const float*, float*, cudaStream_t, float);
+#define APH_STEM_INSTANCES(COUT)                                                                                                   \
+  template int launch_conv3in_fwd<2, COUT, IN_RAW>(const float*, int, int, int, const float*, const float*, bf16*, cudaStream_t, float, \
+                                                   float);                                                                        \
+  template int launch_conv3in_bwd<2, COUT, IN_RAW>(const bf16*, int, int, int, const float*, float*, cudaStream_t, float);
+APH_STEM_INSTANCES(32) APH_STEM_INSTANCES(40) APH_STEM_INSTANCES(48) APH_STEM_INSTANCES(56) APH_STEM_INSTANCES(64)
+#undef APH_STEM_INSTANCES
 
 }  // namespace aph

@@ -135,8 +135,8 @@ __constant__ float c_std[3] = {0.26862954f, 0.26130258f, 0.27577711f};
 // Forward in two kernels.
 //   k_resize : stage 1 alone, SEPARABLE -- a warp owns an output row: vertical 4-tap pass over the crop's columns (coalesced row
 //              reads) into a per-warp strip, then the horizontal 4-tap pass out of the strip; 8 rows of state per CTA, 7 CTAs / SM.
-//              A frame whose short side is too long for that strip (above ~6170 px at size 224) takes the DIRECT form, launched with
-//              cap = 0 (no strip memory, 7 KB of tap tables): every output pixel reads its 16 taps straight from the canvas, four
+//              A frame whose short side is too long for that strip (above about 6400 - size px: ~6170 at size 224, ~5950 at 448)
+//              takes the DIRECT form, launched with cap = 0 (no strip memory, 32 size bytes of tap tables): every output pixel reads its 16 taps straight from the canvas, four
 //              horizontal taps per source row, then the vertical combination. It is a template parameter rather than a run-time
 //              flag because the flag would cost the strip forms' output loop its unrolling.
 //              Result A [S,3,size,size] goes to a library scratch buffer (L2 / HBM), or straight to the output for transform kinds
@@ -742,8 +742,10 @@ k_bwd_bicubic3(const float* __restrict__ grad_out, float* __restrict__ gA_all, i
 
 using namespace aph;
 
-// Largest output side of the sampler: the largest crop side the image encoders take, and the largest the tests cover.
-constexpr int kMaxSampleSize = 224;
+// Largest output side of the sampler: the largest crop side the image encoders take (RN50x64's 448; the kornia kinds write
+// size + 8), and the largest the tests cover. Every launch below is sized from `size` at run time: k_resize's tap tables take
+// 8 size floats of shared memory (14 KB at 448) and k_bwd_bicubic3's 8 size + 24 STRIP (17 KB); the grids grow with size.
+constexpr int kMaxSampleSize = 448;
 
 static int check_sample_args(const char* who, int H, int W, int S, int size, int kind) {
   APH_REQUIRE(H > 0 && W > 0 && S >= 0 && size > 0, "%s: bad shape H=%d W=%d S=%d size=%d", who, H, W, S, size);
@@ -782,8 +784,8 @@ static int sample_fwd_impl(const float* canvas, int H, int W, int pad_top, int p
   APH_REQUIRE(canvas && table && out, "aph_sample_fwd: null pointer");
   cudaStream_t st = (cudaStream_t)stream;
   int cap = ((H + 2 * pad_top < W + 2 * pad_left ? H + 2 * pad_top : W + 2 * pad_left) + 1 + 3) & ~3;     // crops never exceed the short side of the frame
-  // k_resize holds one crop row per warp in shared memory, sized by the frame's short side; above ~6170 px (at size 224) that does not
-  // fit, and k_resize runs its direct form (cap = 0: the x tap tables alone)
+  // k_resize holds one crop row per warp in shared memory, sized by the frame's short side; above about 6400 - size px (~6170 at
+  // size 224, ~5950 at 448) that does not fit, and k_resize runs its direct form (cap = 0: the x tap tables alone)
   if (((size_t)8 * size + (size_t)8 * cap) * sizeof(float) > 200 * 1024) cap = 0;
   const size_t smem2 = ((size_t)8 * size + (size_t)8 * cap) * sizeof(float);
   float* dst = out;

@@ -523,7 +523,8 @@ int make_tmap_bf16_tokens(CUtensorMap* out, const void* base, int cols, int T, i
 // 4-D view {C, W, H, N} of a bf16 NHWC activation, box {64 channels, box_w columns, box_h rows, 1 image}, 128B swizzle
 int make_tmap_bf16_nhwc(CUtensorMap* out, const void* base, int N, int H, int W, int C, int box_h, int box_w);
 // Launches the GEMM on `st`. A: [M,K] with rows `lda` elements apart (K when 0), B: [N,K] device bf16. Requires K % 64 == 0,
-// N % 128 == 0 or N == 64 (the ResNet's 64-channel layers, on 128 x 64 tiles), and row strides that are multiples of 16 bytes.
+// N % 64 == 0 (N % 128 == 64 runs 128 x 64 tiles and takes the bf16, bias-bf16 and ResNet epilogues only: the ResNet towers'
+// 64-, 192- and 320-channel layers), and row strides that are multiples of 16 bytes.
 int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi, cudaStream_t st, int lda = 0);
 
 }  // namespace aph

@@ -117,8 +117,8 @@ using namespace aph;
 extern "C" int aph_text_create(aph_text** out, const aph_text_config* cfg) {
   APH_REQUIRE(out && cfg, "aph_text_create: null argument");
   const int w128 = cfg->width / 128;
-  APH_REQUIRE(cfg->width % 128 == 0 && (w128 == 1 || w128 == 2 || w128 == 4 || w128 == 6 || w128 == 8),
-              "aph_text_create: width %d unsupported (128, 256, 512, 768, 1024)", cfg->width);
+  APH_REQUIRE(cfg->width % 128 == 0 && (w128 == 1 || w128 == 2 || w128 == 4 || w128 == 5 || w128 == 6 || w128 == 8),
+              "aph_text_create: width %d unsupported (128, 256, 512, 640, 768, 1024)", cfg->width);
   APH_REQUIRE(cfg->heads * 64 == cfg->width, "aph_text_create: head dim must be 64 (width %d, heads %d)", cfg->width, cfg->heads);
   APH_REQUIRE(cfg->context > 0 && cfg->context <= 112, "aph_text_create: context %d outside [1, 112]", cfg->context);
   APH_REQUIRE(cfg->out_dim > 0 && cfg->out_dim % 128 == 0, "aph_text_create: out_dim %d must be a multiple of 128", cfg->out_dim);
@@ -166,14 +166,14 @@ extern "C" int aph_text_fwd(aph_text* text, const int64_t* tokens, int n, float*
   const int D = t->cfg.width, C = t->cfg.context, H = t->cfg.heads, O = t->cfg.out_dim;
   const int M = n * C;
   int e;
-  NCH_DISPATCH(D, k_text_embed<NCH><<<rows_grid(M), 256, 0, st>>>(tokens, t->tok_emb, t->pos, t->x, M, C, D, t->cfg.vocab));
+  NCH_DISPATCH_TEXT(D, k_text_embed<NCH><<<rows_grid(M), 256, 0, st>>>(tokens, t->tok_emb, t->pos, t->x, M, C, D, t->cfg.vocab));
   APH_LAUNCH_OK();
   k_text_eot<<<rows_grid(n), 256, 0, st>>>(tokens, t->eot, n, C);
   APH_LAUNCH_OK();
   const BlockIO io{t->x, t->x_mid, t->x, t->ln_out, t->qkv, t->attn_out, t->h_pre, t->h_act, t->mean, t->rstd, t->mean, t->rstd};
   for (const BlockW& w : t->L)
     if ((e = block_fwd(w, io, n, C, M, 0, D, H, attn_causal, st))) return e;
-  NCH_DISPATCH(D, k_text_pool_ln<NCH><<<rows_grid(n), 256, 0, st>>>(t->x, t->eot, t->lnf_w, t->lnf_b, t->pooled, n, C, D));
+  NCH_DISPATCH_TEXT(D, k_text_pool_ln<NCH><<<rows_grid(n), 256, 0, st>>>(t->x, t->eot, t->lnf_w, t->lnf_b, t->pooled, n, C, D));
   APH_LAUNCH_OK();
   GemmEpi ep; ep.out_f32 = emb;
   return launch_gemm(t->pooled, t->w_out, GemmShape{n, O, D}, ep, st);

@@ -147,14 +147,14 @@ int add_blocks(Encoder* h, int layers, int D, bool dgrad) {
 int block_fwd(const BlockW& w, const BlockIO& io, int S, int T, int Mr, int ld_tok, int D, int heads, AttnFwd attn, cudaStream_t st) {
   const int M = S * T;
   int e;
-  NCH_DISPATCH(D, k_ln_fwd<NCH><<<rows_grid(M), 256, 0, st>>>(io.x_in, w.ln1_w, w.ln1_b, io.ln_out, io.mean1, io.rstd1, M, D));
+  NCH_DISPATCH_TEXT(D, k_ln_fwd<NCH><<<rows_grid(M), 256, 0, st>>>(io.x_in, w.ln1_w, w.ln1_b, io.ln_out, io.mean1, io.rstd1, M, D));
   APH_LAUNCH_OK();
   { GemmEpi ep; ep.bias = w.b_qkv; ep.out_bf16 = io.qkv;
     if ((e = launch_gemm(io.ln_out, w.w_qkv, GemmShape{M, 3 * D, D}, ep, st))) return e; }
   if ((e = attn(io.qkv, io.attn_out, S, T, D, heads, st))) return e;
   { GemmEpi ep; ep.bias = w.b_o; ep.resid = io.x_in; ep.ld_resid = ld_tok; ep.out_f32 = io.x_mid;
     if ((e = launch_gemm(io.attn_out, w.w_o, GemmShape{Mr, D, D}, ep, st, ld_tok))) return e; }
-  NCH_DISPATCH(D, k_ln_fwd<NCH><<<rows_grid(Mr), 256, 0, st>>>(io.x_mid, w.ln2_w, w.ln2_b, io.ln_out, io.mean2, io.rstd2, Mr, D));
+  NCH_DISPATCH_TEXT(D, k_ln_fwd<NCH><<<rows_grid(Mr), 256, 0, st>>>(io.x_mid, w.ln2_w, w.ln2_b, io.ln_out, io.mean2, io.rstd2, Mr, D));
   APH_LAUNCH_OK();
   { GemmEpi ep; ep.bias = w.b_fc; ep.out_pre = io.h_pre; ep.act = 1; ep.out_bf16 = io.h_act;
     if ((e = launch_gemm(io.ln_out, w.w_fc, GemmShape{Mr, 4 * D, D}, ep, st))) return e; }

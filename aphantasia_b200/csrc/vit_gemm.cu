@@ -73,7 +73,7 @@ static std::vector<std::pair<cudaEvent_t, cudaEvent_t>> g_prof_ev;
 static std::vector<double> g_prof_flops;
 
 // launches per (kernel variant, epilogue kind): variant 0 = the small-problem kernels (cooperative, 128 x 128 tiles, or 128 x 64
-// for N = 64),
+// where N % 128 == 64),
 // 1 = the large-problem kernels (ping-pong 128 x 128 tiles, or cooperative 128 x 256 tiles for long K).
 // Read by the tests to prove which kernel a shape really ran (aph_gemm_variant_launches).
 static std::atomic<long long> g_variant_launches[2][EPI_KINDS];
@@ -100,7 +100,7 @@ static int launch_cfg(const void* A, const void* B, GemmShape shp, const GemmEpi
 int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi_in, cudaStream_t st, int lda) {
   APH_REQUIRE(A && B && shp.M > 0, "gemm: null operand or empty M");
   APH_REQUIRE(shp.K % GEMM_BK == 0 && shp.K > 0, "gemm: K=%d must be a positive multiple of %d", shp.K, GEMM_BK);
-  APH_REQUIRE((shp.N % 128 == 0 && shp.N > 0) || shp.N == 64, "gemm: N=%d must be 64 or a positive multiple of 128", shp.N);
+  APH_REQUIRE(shp.N % 64 == 0 && shp.N > 0, "gemm: N=%d must be a positive multiple of 64", shp.N);
   APH_REQUIRE(lda == 0 || lda >= shp.K, "gemm: lda=%d < K=%d", lda, shp.K);
   APH_REQUIRE((epi_in.ld_out == 0 || epi_in.ld_out >= shp.N) && (epi_in.ld_resid == 0 || epi_in.ld_resid >= shp.N),
               "gemm: output / residual row stride below N=%d", shp.N);
@@ -135,18 +135,20 @@ int launch_gemm(const void* A, const void* B, GemmShape shp, const GemmEpi& epi_
   // chosen when there are at least twice as many 128 x 128 tiles as SMs and K is short (K = 768 in the encoder), so that the
   // epilogue is a large share of a tile's time. With long K the mainloop dominates and the cooperative 128 x 256 tile wins: its
   // m64n256 MMAs read less shared memory per FLOP. Smaller problems (the final projection, the text tower) keep 128 x 128 tiles.
-  // N = 64 (the ResNet's first stage) runs the small-problem schedule on 128 x 64 tiles, the tile the 3x3 convolution uses there.
+  // N % 128 == 64 (RN50's first stage at N = 64, the wide towers' zero-padded widths 192 and 320 and their multiples) runs the
+  // small-problem schedule on 128 x 64 tiles, the tile the 3x3 convolution uses for those widths.
   const int m_tiles = (shp.M + GEMM_BM - 1) / GEMM_BM;
-  const bool narrow = shp.N == 64;
+  const bool narrow = shp.N % 128 == 64;
   const bool pingpong = !narrow && m_tiles * (shp.N / 128) >= 2 * num_sms() && shp.K <= 1024;
   const bool wide = !pingpong && shp.N % 256 == 0 && m_tiles * (shp.N / 256) >= num_sms();
 #define APH_GEMM_CASE(K) case K: return pingpong ? launch_cfg<128, true, K>(A, B, shp, epi, st, lda) \
                                                  : wide ? launch_cfg<256, false, K>(A, B, shp, epi, st, lda) : launch_cfg<128, false, K>(A, B, shp, epi, st, lda);
 #define APH_GEMM_CASE_RN(K) case K: return narrow ? launch_cfg<64, false, K>(A, B, shp, epi, st, lda) : pingpong ? launch_cfg<128, true, K>(A, B, shp, epi, st, lda) \
                                                  : wide ? launch_cfg<256, false, K>(A, B, shp, epi, st, lda) : launch_cfg<128, false, K>(A, B, shp, epi, st, lda);
-  APH_REQUIRE(!narrow || kind == EPI_BF16 || kind >= EPI_BIAS_RELU, "gemm: N=64 takes the bf16 and ResNet epilogues only");
+  APH_REQUIRE(!narrow || kind == EPI_BF16 || kind == EPI_BIAS_BF16 || kind >= EPI_BIAS_RELU,
+              "gemm: N=%d (N %% 128 == 64) takes the bf16, bias-bf16 and ResNet epilogues only", shp.N);
   switch (kind) {
-    APH_GEMM_CASE(EPI_F32) APH_GEMM_CASE_RN(EPI_BF16) APH_GEMM_CASE(EPI_BIAS_BF16) APH_GEMM_CASE(EPI_BIAS_GELU)
+    APH_GEMM_CASE(EPI_F32) APH_GEMM_CASE_RN(EPI_BF16) APH_GEMM_CASE_RN(EPI_BIAS_BF16) APH_GEMM_CASE(EPI_BIAS_GELU)
     APH_GEMM_CASE(EPI_BIAS_RESID) APH_GEMM_CASE(EPI_GELUGRAD_BF16) APH_GEMM_CASE(EPI_UNPATCH)
     APH_GEMM_CASE_RN(EPI_BIAS_RELU) APH_GEMM_CASE_RN(EPI_BIAS_RESID_RELU) APH_GEMM_CASE_RN(EPI_MASK) APH_GEMM_CASE_RN(EPI_MASK_RESID)
   }
@@ -190,7 +192,7 @@ extern "C" int aph_gemm_epi_strided_test(const void* A, int lda, const void* B, 
 }
 
 // The ResNet epilogues (rn.cu) on caller operands: relu = 1: out_bf16 = relu(acc + bias [+ resid_bf16]); relu = 0:
-// out_bf16 = mask > 0 ? acc [+ resid_bf16] : 0. N = 64 or a multiple of 128.
+// out_bf16 = mask > 0 ? acc [+ resid_bf16] : 0. N a multiple of 64.
 extern "C" int aph_gemm_rn_epi_test(const void* A, const void* B, int M, int N, int K, const float* bias, const void* resid_bf16,
                                     const void* mask, int relu, void* out_bf16, void* stream) {
   GemmEpi epi;

@@ -11,14 +11,19 @@
 namespace aph {
 
 // Runs the statement with `constexpr int NCH = D / 128` for the row-in-registers kernels below (width 512 is the text tower's).
+#define NCH_CASE(K, ...) case K: { constexpr int NCH = K; __VA_ARGS__; } break;
 #define NCH_DISPATCH(D, ...)                                                           \
   switch ((D) / 128) {                                                                 \
-    case 1: { constexpr int NCH = 1; __VA_ARGS__; } break;                             \
-    case 2: { constexpr int NCH = 2; __VA_ARGS__; } break;                             \
-    case 4: { constexpr int NCH = 4; __VA_ARGS__; } break;                             \
-    case 6: { constexpr int NCH = 6; __VA_ARGS__; } break;                             \
-    case 8: { constexpr int NCH = 8; __VA_ARGS__; } break;                             \
+    NCH_CASE(1, __VA_ARGS__) NCH_CASE(2, __VA_ARGS__) NCH_CASE(4, __VA_ARGS__) NCH_CASE(6, __VA_ARGS__) NCH_CASE(8, __VA_ARGS__) \
     default: set_error("vit: unsupported width %d", (D)); return 2;                    \
+  }
+// The same with RN50x4's text width 640 (NCH = 5) added, for the kernels the text towers run: the shared block forward's
+// LayerNorm, the text embedding and pooling. The image towers' own kernels keep NCH_DISPATCH: aph_vit_create refuses 640.
+#define NCH_DISPATCH_TEXT(D, ...)                                                      \
+  switch ((D) / 128) {                                                                 \
+    NCH_CASE(1, __VA_ARGS__) NCH_CASE(2, __VA_ARGS__) NCH_CASE(4, __VA_ARGS__) NCH_CASE(5, __VA_ARGS__) \
+    NCH_CASE(6, __VA_ARGS__) NCH_CASE(8, __VA_ARGS__)                                 \
+    default: set_error("text: unsupported width %d", (D)); return 2;                   \
   }
 
 // ---------------------------------------------------------------------------------------------

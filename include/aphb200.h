@@ -257,32 +257,38 @@ int aph_vit_bwd_sized(aph_vit* vit, const float* grad_emb, int S, int side, floa
 /* bytes of device memory owned by the handle (weights + activation arena)                          */
 int64_t aph_vit_bytes(const aph_vit* vit);
 
-/* ================= L1: CLIP ResNet image encoder (RN50, RN101) ===================================
- * Replaces clip.model.ModifiedResNet.forward (third-party OpenAI clip) in eval mode and its data gradient: stem (three 3x3
- * convolutions, the first of stride 2, each + BatchNorm + ReLU; avgpool 2), four stages of bottlenecks (layers[i] blocks of
- * planes 64 << i, expansion 4, stride 2 in the first block of stages 2-4 as an average pool), the attention pool (mean token +
- * 49 map tokens + positional embedding, 32-head attention queried by token 0, c_proj). No weight gradients.
+/* ================= L1: CLIP ResNet image encoders (RN50, RN101, RN50x4, RN50x16, RN50x64) ============
+ * Replaces clip.model.ModifiedResNet.forward (third-party OpenAI clip) in eval mode and its data gradient, for width w and
+ * input resolution r = 32 g: stem (three 3x3 convolutions, 3 -> w/2 -> w/2 -> w, the first of stride 2, each + BatchNorm +
+ * ReLU; avgpool 2), four stages of bottlenecks (layers[i] blocks of planes w << i, expansion 4, stride 2 in the first block of
+ * stages 2-4 as an average pool), the attention pool (mean token + g^2 map tokens + positional embedding, T = g^2 + 1 tokens,
+ * w/2-head attention queried by token 0, c_proj). No weight gradients.
+ * Every channel count runs rounded up to a multiple of 64, rc(c) = 64 ceil(c / 64), on zero-padded weights and biases.
  * Keys of aph_rn_load_tensor are the OpenAI ones without "visual." after folding every BatchNorm (eps 1e-5, running statistics)
- * into its convolution (aphantasia_b200.clip.fold_resnet_state_dict): "conv{1,2,3}.weight" / ".bias" (conv1 [32,3,3,3]; conv2,
- * conv3 zero-padded to [64,64,3,3], conv2's bias to [64]), "layer{i}.{j}.conv{1,2,3}.weight" / ".bias",
- * "layer{i}.{j}.downsample.weight" / ".bias" (the 1x1 convolution of downsample.1 folded with downsample.2),
- * "attnpool.positional_embedding", "attnpool.qkv.weight" [3*2048, 2048] = [q_proj; k_proj; v_proj] and "attnpool.qkv.bias",
- * "attnpool.c_proj.weight" / ".bias". aph_rn_finalize checks every tensor arrived.
- * Device bytes (aph_rn_bytes) = weights + arena, S = max_batch, D = 2048, O = out_dim, sizes of a side-254 input
- * (h1 = 127 after the stem's convolutions, h0 = 63 after its pool; block b has input map hin_b, output map hout_b = hin_b /
- * stride_b, cin_b input channels, P_b planes, E_b = 4 P_b):
- *   weights  4 (864 + 32 + 2*64) + 2 * 2 * 2 * 9 * 64 * 64
+ * into its convolution and padding every channel count (aphantasia_b200.clip.fold_resnet_state_dict), C1 = w/2, SC = rc(w):
+ * "conv{1,2,3}.weight" / ".bias" (conv1 [C1,3,3,3], unpadded; conv2 [64,64,3,3] and its bias [64]; conv3 [SC,64,3,3] and its
+ * bias [SC]), "layer{i}.{j}.conv{1,2,3}.weight" / ".bias" (conv1 [P,cin], conv2 [P,P,3,3], conv3 [E,P]: P = rc(planes),
+ * E = 4 planes, cin the previous block's E or SC), "layer{i}.{j}.downsample.weight" / ".bias" (the 1x1 convolution of
+ * downsample.1 folded with downsample.2), "attnpool.positional_embedding" [T, D], "attnpool.qkv.weight" [3D, D] =
+ * [q_proj; k_proj; v_proj] and "attnpool.qkv.bias", "attnpool.c_proj.weight" / ".bias". aph_rn_finalize checks every tensor
+ * arrived.
+ * Device bytes (aph_rn_bytes) = weights + arena, S = max_batch, D = 32 w, O = out_dim, sizes of a side-(r + 30) input
+ * (h1 = r/2 + 15 after the stem's convolutions, h0 = h1 / 2 after its pool; block b has input map hin_b, output map hout_b =
+ * hin_b / stride_b, cin_b input channels, P_b planes and E_b output channels as above):
+ *   weights  4 (27 C1 + C1 + 64 + SC) + 2 * 2 * 9 * 64 (64 + SC)
  *            + sum_b [2 * 2 (P cin + E P (+ E cin if downsample)) + 2 * 2 * 9 P^2 + 4 (2 P + E (+ E if downsample))]
- *            + 4 * 50 D + 2 * 2 * 3 D^2 + 4 * 3 D + 2 * 2 O D + 4 O
- *   arena    2 [S (3 h1^2 64 + h0^2 64) + sum_b S (2 hin_b^2 P_b + hout_b^2 E_b) + 6 S emax + 10 * 50 S D + S O] + 4 S O
- *            emax = max(h1^2 64, max_b hin_b^2 max(cin_b, P_b), max_b hout_b^2 E_b)                                      */
+ *            + 4 T D + 2 * 2 * 3 D^2 + 4 * 3 D + 2 * 2 O D + 4 O
+ *   arena    2 [S (2 h1^2 64 + h1^2 SC + h0^2 SC) + sum_b S (2 hin_b^2 P_b + hout_b^2 E_b) + 6 S emax + 10 T S D + S O] + 4 S O
+ *            emax = max(h1^2 SC, max_b hin_b^2 max(cin_b, P_b), max_b hout_b^2 E_b)
+ * For RN50 / RN101 (w = 64, r = 224): C1 = 32, SC = 64, T = 50, h1 = 127, h0 = 63.                                      */
 typedef struct aph_rn aph_rn;
 typedef struct {
-  int32_t layers[4];  /* (3, 4, 6, 3) RN50, (3, 4, 23, 3) RN101         */
-  int32_t width;      /* 64                                            */
-  int32_t heads;      /* 32 (head dim 64)                              */
-  int32_t out_dim;    /* 1024 (RN50), 512 (RN101)                      */
-  int32_t res;        /* input resolution, 224                         */
+  int32_t layers[4];  /* (3, 4, 6, 3) RN50, (3, 4, 23, 3) RN101, (4, 6, 10, 6) RN50x4, (6, 8, 18, 8) RN50x16,
+                         (3, 15, 36, 10) RN50x64                                                                   */
+  int32_t width;      /* a multiple of 16 in [64, 128]: 64, 80 (RN50x4), 96 (RN50x16), 128 (RN50x64)          */
+  int32_t heads;      /* width / 2 (head dim 64)                                                               */
+  int32_t out_dim;    /* a multiple of 128: 1024 (RN50), 512 (RN101), 640, 768, 1024                          */
+  int32_t res;        /* input resolution, a multiple of 32 in [224, 448]: 224, 288, 384, 448                 */
   int32_t max_batch;  /* largest S a call will pass                    */
   int32_t reserved;
 } aph_rn_config;
@@ -290,29 +296,31 @@ int aph_rn_create(aph_rn** rn, const aph_rn_config* cfg);
 int aph_rn_destroy(aph_rn* rn);
 int aph_rn_load_tensor(aph_rn* rn, const char* key, const float* data, int64_t numel, void* stream);
 int aph_rn_finalize(aph_rn* rn);
-/* x [S,3,side,side] fp32 (normalised crops), 223 <= side <= 254 (the sides whose final map is 7 x 7; the whole crop is read)
- * -> emb [S,out_dim]. save_for_bwd 0/1.                                                                                   */
+/* x [S,3,side,side] fp32 (normalised crops), res - 1 <= side <= res + 30 (the sides whose final map is g x g; the whole crop is
+ * read) -> emb [S,out_dim]. save_for_bwd 0/1.                                                                             */
 int aph_rn_fwd(aph_rn* rn, const float* x, int S, int side, float* emb, int save_for_bwd, void* stream);
 /* grad_emb [S,out_dim] -> grad_x [S,3,side,side] (overwritten), from the last aph_rn_fwd(save_for_bwd = 1) of the same S, side. */
 int aph_rn_bwd(aph_rn* rn, const float* grad_emb, int S, int side, float* grad_x, void* stream);
 int64_t aph_rn_bytes(const aph_rn* rn);
 /* Test entries of the tower's own kernels on caller buffers (bf16 NHWC activations):
- * aph_rn_stem_test: stem conv 1, weight fp32 [32,3,3,3], bias [32], h = (side - 1) / 2 + 1. fwd = 1: in = crops fp32
- *   [N,3,side,side] -> out bf16 [N,h,h,64] = relu(conv + bias) in channels 0-31, zero above; fwd = 0: in = dz bf16 [N,h,h,64]
- *   (channels 0-31 read) -> out fp32 [N,3,side,side].
+ * aph_rn_stem_test: stem conv 1 of cout output channels (32, 40, 48, 56 or 64; 0 = 32), weight fp32 [cout,3,3,3], bias
+ *   [cout], h = (side - 1) / 2 + 1. fwd = 1: in = crops fp32 [N,3,side,side] -> out bf16 [N,h,h,64] = relu(conv + bias) in
+ *   channels 0 to cout-1, zero above; fwd = 0: in = dz bf16 [N,h,h,64] (channels below cout read) -> out fp32 [N,3,side,side].
  * aph_rn_pool_test: 2x2 average pool (floor), C % 8 == 0. fwd = 1: out = pool(x) [N,H/2,W/2,C]; fwd = 0: x = dy [N,H/2,W/2,C]
  *   -> out [N,H,W,C] = its adjoint, selected by mask [N,H,W,C] > 0 unless mask is NULL.
- * aph_rn_tokens_test: fwd = 1: in = x bf16 [S*49,C], aux = pos fp32 [50,C] -> out bf16 [S*50,C] (row 0 the mean of the 49 rows,
- *   + pos); fwd = 0: in = dtok bf16 [S*50,C], aux = x -> out [S*49,C] = x > 0 ? dtok[1 + i] + dtok[0] / 49 : 0.
+ * aph_rn_tokens_test: the tokens of a grid x grid map (0 = 7), P = grid^2. fwd = 1: in = x bf16 [S*P,C], aux = pos fp32
+ *   [P+1,C] -> out bf16 [S*(P+1),C] (row 0 the mean of the P rows, + pos); fwd = 0: in = dtok bf16 [S*(P+1),C], aux = x -> out
+ *   [S*P,C] = x > 0 ? dtok[1 + i] + dtok[0] / P : 0.
  * aph_rn_saved_test: the last saved forward's ReLU outputs (handle memory, valid until the next forward), bf16 NHWC: k = 0..2
- *   the stem's [S,h,h,64], then for block b (stages in order) 3 b + 3 / 3 b + 4 its conv1 / conv2 outputs [S,hin,hin,P] and
- *   3 b + 5 its output [S,hout,hout,4 P]; *numel their element count.
- * aph_gemm_rn_epi_test: the encoder GEMM with the ResNet epilogues (N = 64 or a multiple of 128): relu = 1: out_bf16 =
+ *   the stem's [S,h,h,64], [S,h,h,64], [S,h,h,SC], then for block b (stages in order) 3 b + 3 / 3 b + 4 its conv1 / conv2
+ *   outputs [S,hin,hin,P] and 3 b + 5 its output [S,hout,hout,E]; *numel their element count.
+ * aph_gemm_rn_epi_test: the encoder GEMM with the ResNet epilogues (N a multiple of 64): relu = 1: out_bf16 =
  *   relu(acc + bias [+ resid_bf16]); relu = 0: out_bf16 = mask > 0 ? acc [+ resid_bf16] : 0 (bias unused). NULL = absent.  */
 int aph_rn_saved_test(aph_rn* rn, int k, void** ptr, int64_t* numel);
-int aph_rn_stem_test(int fwd, const void* in, const float* weight, const float* bias, void* out, int N, int side, void* stream);
+int aph_rn_stem_test(int fwd, const void* in, const float* weight, const float* bias, void* out, int N, int side, void* stream,
+                     int cout);
 int aph_rn_pool_test(int fwd, const void* x, const void* mask, void* out, int N, int H, int W, int C, void* stream);
-int aph_rn_tokens_test(int fwd, const void* in, const void* aux, void* out, int S, int C, void* stream);
+int aph_rn_tokens_test(int fwd, const void* in, const void* aux, void* out, int S, int C, void* stream, int grid);
 int aph_gemm_rn_epi_test(const void* A, const void* B, int M, int N, int K, const float* bias, const void* resid_bf16,
                          const void* mask, int relu, void* out_bf16, void* stream);
 
@@ -383,7 +391,7 @@ int aph_vqgan_ends_test(int kind, const void* in, const float* weight, const flo
  * CAUSAL attention -> ln_final(x[s, argmax(ids[s])]) @ text_projection. Same kernels as the image tower.          */
 typedef struct aph_text aph_text;
 typedef struct {
-  int32_t width;      /* 512 (multiple of 128, <= 1024)              */
+  int32_t width;      /* 512: 128, 256, 512, 640, 768 or 1024        */
   int32_t layers;     /* 12                                           */
   int32_t heads;      /* 8 (head dim must be 64)                      */
   int32_t out_dim;    /* 512 (multiple of 128)                        */
